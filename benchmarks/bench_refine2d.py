@@ -4,6 +4,10 @@ csm_ceres_match2d_batch launch (host clouds: their H2D is inside the timed call)
 oracle's CPU restatement on the host threads.  Prints one JSON line.
 
   python -m benchmarks.bench_refine2d [--jobs 2000] [--submaps 4] [--iterations 10]
+                                      [--grid {probability,tsdf}]
+
+--grid tsdf refines against TSDF2D submaps (synthetic.make_tsdf2d, TSDFMatchCostFunction2D);
+its CPU baseline is the numpy restatement tests/tsdf2d_oracle.py on a smaller sample.
 """
 import argparse
 import json
@@ -22,11 +26,15 @@ def main():
     ap.add_argument("--iterations", type=int, default=10)
     ap.add_argument("--repeat", type=int, default=5)
     ap.add_argument("--no-cpu-baseline", action="store_true")
+    ap.add_argument("--grid", choices=("probability", "tsdf"), default="probability")
     args = ap.parse_args()
     from cartographer_b200 import scan_matching as sm
     worlds = []
     for s in range(args.submaps):
-        grid, occ = synthetic.make_grid2d(900 + s, size_cells=1000)
+        if args.grid == "tsdf":
+            grid, occ = synthetic.make_tsdf2d(900 + s, size_cells=1000)
+        else:
+            grid, occ = synthetic.make_grid2d(900 + s, size_cells=1000)
         rng = np.random.RandomState(900 + s)
         scans = []
         for k in range(4):
@@ -55,12 +63,28 @@ def main():
         wall.append(time.perf_counter() - t0)
         dev_ms.append(m.last_stats["device_ms"])
     out = {"metric": "refinements_per_sec", "jobs": args.jobs, "points_per_scan": 1081,
-           "grid": "1000x1000", "max_num_iterations": args.iterations,
+           "grid": "1000x1000", "grid_type": args.grid, "max_num_iterations": args.iterations,
            "value": args.jobs / float(np.median(wall)), "wall_ms": 1e3 * float(np.median(wall)),
            "device_ms": float(np.median(dev_ms)),
            "mean_iterations": float(np.mean([s["iterations"] for s in sums])),
            "h2d_bytes": int(sum(c.nbytes for c in clouds))}
-    if not args.no_cpu_baseline:
+    if not args.no_cpu_baseline and args.grid == "tsdf":
+        from tests import tsdf2d_oracle
+        ogs = {id(g): tsdf2d_oracle.TSDF2D.from_spec(g) for g, _, _ in worlds}
+        sample = cpu_jobs[:64]
+        t0 = time.perf_counter()
+        want = [tsdf2d_oracle.match(ogs[id(g)], scan, init[:2], init,
+                                    max_num_iterations=args.iterations)
+                for g, scan, init in sample]
+        secs = time.perf_counter() - t0
+        worst = max(float(np.abs(poses[i] - w["pose"]).max()) for i, w in enumerate(want))
+        out["cpu_baseline"] = {"value": len(sample) / secs, "unit": "refinements/s", "cores": 1,
+                               "kind": "numpy restatement (test oracle), not a port",
+                               "sample": "%d of the jobs, %.2f s wall" % (len(sample), secs)}
+        out["parity_checked"] = sum(float(np.abs(poses[i] - w["pose"]).max()) <= 1e-7
+                                    for i, w in enumerate(want))
+        out["max_abs_pose_difference"] = worst
+    elif not args.no_cpu_baseline:
         from concurrent.futures import ThreadPoolExecutor
         from oracle import pyoracle as oracle
         oracle.build()

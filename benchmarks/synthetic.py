@@ -110,6 +110,65 @@ def make_grid2d(seed, size_cells=1000, resolution=0.05):
     return occupancy_to_grid(occ, seed, resolution, max_x, max_y), occ
 
 
+class TSDFGridSpec:
+    """Plain record of a TSDF2D (tsd_cells[y, x], weight_cells[y, x]) + MapLimits + the
+    TSDValueConverter parameters; the fields of scan_matching.TSDF2DSpec."""
+
+    def __init__(self, tsd_cells, weight_cells, resolution, max_x, max_y, truncation_distance,
+                 max_weight):
+        self.tsd_cells = np.ascontiguousarray(tsd_cells, np.uint16)
+        self.weight_cells = np.ascontiguousarray(weight_cells, np.uint16)
+        self.num_y, self.num_x = self.tsd_cells.shape
+        self.resolution = float(resolution)
+        self.max_x = float(max_x)
+        self.max_y = float(max_y)
+        self.truncation_distance = float(truncation_distance)
+        self.max_weight = float(max_weight)
+
+
+def make_tsdf2d(seed, size_cells=1000, resolution=0.05, truncation_distance=0.3,
+                max_weight=10.0):
+    """The world of make_grid2d(seed, ...) as a TSDF2D: the signed distance to its walls
+    (positive in free space, negative inside walls), clamped to +-truncation_distance
+    (configuration_files/trajectory_builder_2d.lua: 0.3 m, max weight 10).  Cells within the
+    truncation band carry a weight that falls from max_weight at the wall to half of it at the
+    band's edge; the others are unknown (value 0, weight 0).  Values as TSDValueConverter
+    stores them (float32, lround).  Returns (spec, occ)."""
+    _, occ = make_grid2d(seed, size_cells=size_cells, resolution=resolution)
+    ny, nx = occ.shape
+    reach = int(math.ceil(truncation_distance / resolution)) + 1
+    # distance (in cells, between cell centres) to the nearest cell of the other kind
+    dist = np.full(occ.shape, np.inf)
+    pad = np.pad(occ, reach, mode="edge")
+    for dy in range(-reach, reach + 1):
+        for dx in range(-reach, reach + 1):
+            d = math.hypot(dx, dy)
+            if d == 0 or d > reach:
+                continue
+            other = pad[reach + dy:reach + dy + ny, reach + dx:reach + dx + nx] != occ
+            dist = np.where(other & (d < dist), d, dist)
+    # the surface lies half a cell from either centre
+    sd = np.where(occ, -1.0, 1.0) * (dist - 0.5) * resolution
+    band = np.abs(sd) < truncation_distance
+    trunc = np.float32(truncation_distance)
+    tsd = np.clip(sd.astype(np.float32), -trunc, trunc)
+    weight = (max_weight * (1.0 - 0.5 * np.abs(sd) / truncation_distance)).astype(np.float32)
+    weight = np.clip(weight, np.float32(0), np.float32(max_weight))
+    tsd_resolution = np.float32(32766) / (trunc - (-trunc))
+    w_resolution = np.float32(32766) / (np.float32(max_weight) - np.float32(0))
+
+    def lround(v):   # std::lround: halves away from zero
+        v = v.astype(np.float64)
+        return (np.sign(v) * np.floor(np.abs(v) + 0.5)).astype(np.int64)
+    tsd_v = lround((tsd - (-trunc)) * tsd_resolution) + 1
+    w_v = lround((weight - np.float32(0)) * w_resolution) + 1
+    tsd_cells = np.where(band, tsd_v, 0).astype(np.uint16)
+    weight_cells = np.where(band, w_v, 0).astype(np.uint16)
+    size_m = size_cells * resolution
+    return TSDFGridSpec(tsd_cells, weight_cells, resolution, size_m / 2.0, size_m / 2.0,
+                        truncation_distance, max_weight), occ
+
+
 def crop_grid(grid, occ, x0, y0, nx, ny):
     """Sub-grid of nx x ny cells starting at cell (x0, y0); limits shifted accordingly."""
     cells = grid.cells[y0:y0 + ny, x0:x0 + nx]

@@ -25,6 +25,7 @@
 // file) so that every per-point value is the one the oracle's restatement computes; sums are
 // block-tree ordered, cos / sin come from the device's double-precision routines (<= 2 ulp).
 #include <algorithm>
+#include <cfloat>
 #include <climits>
 #include <cmath>
 
@@ -48,6 +49,11 @@ struct RefJobDev {
   double resolution, max_x, max_y;
   double target[2];        // target_translation
   double init[3];          // initial_pose_estimate {x, y, angle}
+  // TSDF2D jobs only (wcells == nullptr selects the ProbabilityGrid cost, as
+  // Grid2D::GetGridType() does in ceres_scan_matcher_2d.cc:74-91): the weight cells and the
+  // TSDValueConverter constants of the job's grid (MakeTsdfConversion)
+  const uint16_t* wcells;
+  float tsd_scale, tsd_bias, w_scale, w_bias, truncation;
 };
 
 struct RefOpts {
@@ -155,10 +161,145 @@ __device__ __forceinline__ void BlockSum(double* acc, double (*s_part)[10], doub
   __syncthreads();
 }
 
-// cost, gradient and normal matrix of all three residual blocks at x (block-wide; the
-// result lands in s_tot: {cost, g[3], h[6]}).
+// ---- TSDFMatchCostFunction2D (tsdf_match_cost_function_2d.cc:42-65) through
+// InterpolatedTSDF2D (interpolated_tsdf_2d.h) -----------------------------------------------
+// r_i = n * scaling * cost_i * w_i / W with W = sum_j w_j: not point-separable, so one
+// evaluation is two block passes — W and dW/d(x, y, theta) first, then the residuals.  On dual
+// numbers every operation follows ceres/jet.h (a Jet divided by a Jet multiplies by the
+// reciprocal of the denominator's value); the interpolation's lower pixel is found on the
+// scalar part, in float, as the reference does.
+
+// TSDF2D::GetWeight (tsdf_2d.cc:85-91): 0 outside the limits and for value 0
+__device__ __forceinline__ float TsdfWeight(const RefJobDev& J, int ix, int iy) {
+  if (ix < 0 || iy < 0 || ix >= J.nx || iy >= J.ny) return 0.f;
+  const int value = __ldg(J.wcells + static_cast<size_t>(iy) * J.pitch + ix) & 0x7fff;
+  return value == 0 ? 0.f : __fadd_rn(__fmul_rn(__int2float_rn(value), J.w_scale), J.w_bias);
+}
+
+// Grid2D::GetCorrespondenceCost with the TSDF bounds +-truncation: value 0 (and outside the
+// limits) gives +truncation; the update marker is masked
+__device__ __forceinline__ float TsdfCost(const RefJobDev& J, int ix, int iy) {
+  if (ix < 0 || iy < 0 || ix >= J.nx || iy >= J.ny) return J.truncation;
+  const int value = __ldg(J.cells + static_cast<size_t>(iy) * J.pitch + ix) & 0x7fff;
+  return value == 0 ? J.truncation
+                    : __fadd_rn(__fmul_rn(__int2float_rn(value), J.tsd_scale), J.tsd_bias);
+}
+
+// MapLimits::GetCellIndex of a float point: ix from y, iy from x (double arithmetic, lround)
+__device__ __forceinline__ void TsdfCellIndex(const RefJobDev& J, float px, float py, int* ix,
+                                              int* iy) {
+  *ix = static_cast<int>(lround((J.max_y - static_cast<double>(py)) / J.resolution - 0.5));
+  *iy = static_cast<int>(lround((J.max_x - static_cast<double>(px)) / J.resolution - 0.5));
+}
+
+struct TsdfCorners {
+  float x1, y1, dx, dy;          // centre of the lower pixel, x2 - x1 and y2 - y1 (float)
+  float w11, w12, w21, w22;
+  int ix, iy;                    // index1
+};
+
+// ComputeInterpolationDataPoints + the four weights around (x, y)
+__device__ __forceinline__ void TsdfCornersAt(const RefJobDev& J, double x, double y,
+                                              TsdfCorners* c) {
+  int cx, cy;   // CenterOfLowerPixel: GetCellCenter(GetCellIndex(Vector2f(x, y)))
+  TsdfCellIndex(J, static_cast<float>(x), static_cast<float>(y), &cx, &cy);
+  float lx = static_cast<float>(J.max_x - J.resolution * (cy + 0.5));
+  float ly = static_cast<float>(J.max_y - J.resolution * (cx + 0.5));
+  if (lx > x) lx = static_cast<float>(lx - J.resolution);
+  if (ly > y) ly = static_cast<float>(ly - J.resolution);
+  const float res = static_cast<float>(J.resolution);
+  c->x1 = lx;
+  c->y1 = ly;
+  c->dx = __fadd_rn(lx, res) - lx;
+  c->dy = __fadd_rn(ly, res) - ly;
+  TsdfCellIndex(J, lx, ly, &c->ix, &c->iy);
+  c->w11 = TsdfWeight(J, c->ix, c->iy);
+  c->w12 = TsdfWeight(J, c->ix - 1, c->iy);
+  c->w21 = TsdfWeight(J, c->ix, c->iy - 1);
+  c->w22 = TsdfWeight(J, c->ix - 1, c->iy - 1);
+}
+
+// InterpolateBilinear at (x, y); kJac: also the derivatives f_v from (x_v, y_v)
 template <bool kJac>
-__device__ __forceinline__ void EvaluateAt(const RefJobDev& J, const RefOpts& P,
+__device__ __forceinline__ void TsdfBilinear(const TsdfCorners& c, float q11, float q12,
+                                             float q21, float q22, double x, const double* xv,
+                                             double y, const double* yv, double* f,
+                                             double* fv) {
+  const double c12 = static_cast<double>(q12 - q11), c22 = static_cast<double>(q22 - q21);
+  if (!kJac) {
+    const double nx = (x - static_cast<double>(c.x1)) / static_cast<double>(c.dx);
+    const double ny = (y - static_cast<double>(c.y1)) / static_cast<double>(c.dy);
+    const double q1 = c12 * ny + static_cast<double>(q11);
+    const double q2 = c22 * ny + static_cast<double>(q21);
+    *f = (q2 - q1) * nx + q1;
+    return;
+  }
+  const double inx = 1.0 / static_cast<double>(c.dx), iny = 1.0 / static_cast<double>(c.dy);
+  const double nx = (x - static_cast<double>(c.x1)) * inx;
+  const double ny = (y - static_cast<double>(c.y1)) * iny;
+  const double q1 = c12 * ny + static_cast<double>(q11);
+  const double q2 = c22 * ny + static_cast<double>(q21);
+  const double d = q2 - q1;
+  *f = d * nx + q1;
+#pragma unroll
+  for (int k = 0; k < 3; ++k) {
+    const double nxv = xv[k] * inx, nyv = yv[k] * iny;
+    const double q1v = c12 * nyv, q2v = c22 * nyv;
+    fv[k] = (d * nxv + (q2v - q1v) * nx) + q1v;
+  }
+}
+
+// Interpolated weight (and, kCost, correspondence cost) of one point at pose x
+template <bool kJac, bool kCost>
+__device__ __forceinline__ void TsdfPoint(const RefJobDev& J, const double* x, double cs,
+                                          double sn, double px, double py, double* w,
+                                          double* wv, double* cost, double* costv) {
+  const double wx = (cs * px + (-sn) * py) + x[0] * 1.0;
+  const double wy = (sn * px + cs * py) + x[1] * 1.0;
+  const double dwx[3] = {1.0, 0.0, (-sn) * px + (-cs) * py};
+  const double dwy[3] = {0.0, 1.0, cs * px + (-sn) * py};
+  TsdfCorners c;
+  TsdfCornersAt(J, wx, wy, &c);
+  TsdfBilinear<kJac>(c, c.w11, c.w12, c.w21, c.w22, wx, dwx, wy, dwy, w, wv);
+  if (!kCost) return;
+  if (c.w11 == 0.f || c.w12 == 0.f || c.w21 == 0.f || c.w22 == 0.f) {
+    *cost = static_cast<double>(J.truncation);   // GetMaxCorrespondenceCost(), no derivative
+    if (kJac) costv[0] = costv[1] = costv[2] = 0.;
+    return;
+  }
+  TsdfBilinear<kJac>(c, TsdfCost(J, c.ix, c.iy), TsdfCost(J, c.ix - 1, c.iy),
+                     TsdfCost(J, c.ix, c.iy - 1), TsdfCost(J, c.ix - 1, c.iy - 1), wx, dwx, wy,
+                     dwy, cost, costv);
+}
+
+// One TSDF residual (and Jacobian row) given W (and dW).  The functor's
+// T(n) * scaling * cost * w, then /= W.
+template <bool kJac>
+__device__ __forceinline__ void TsdfResidual(double ns, double W, const double* Wv, double w,
+                                             const double* wv, double cost,
+                                             const double* costv, double* res, double* jrow) {
+  const double a = ns * cost;
+  if (!kJac) {
+    *res = (a * w) / W;
+    return;
+  }
+  const double inv = 1.0 / W;
+  const double r = a * w;
+  *res = r * inv;
+#pragma unroll
+  for (int k = 0; k < 3; ++k) {
+    const double rv = a * wv[k] + (ns * costv[k]) * w;
+    jrow[k] = (rv - *res * Wv[k]) * inv;
+  }
+}
+
+enum { kGridProbability = 0, kGridTsdf = 1 };
+
+// cost, gradient and normal matrix of all three residual blocks at x (block-wide; the
+// result lands in s_tot: {cost, g[3], h[6]}).  false (block-uniform) where the cost function
+// returns false: a TSDF scan that sees no weight (summed_weight == 0).
+template <int kGrid, bool kJac>
+__device__ __forceinline__ bool EvaluateAt(const RefJobDev& J, const RefOpts& P,
                                            const float* __restrict__ xyz, const double* x,
                                            double (*s_part)[10], double* s_tot) {
   const double scaling = P.occupied_space_weight / sqrt(static_cast<double>(J.n));
@@ -167,11 +308,47 @@ __device__ __forceinline__ void EvaluateAt(const RefJobDev& J, const RefOpts& P,
   double acc[10];
 #pragma unroll
   for (int k = 0; k < 10; ++k) acc[k] = 0.;
+  double W = 0., Wv[3] = {0., 0., 0.};
+  if (kGrid == kGridTsdf) {
+    // pass 1: summed_weight and its derivatives
+    for (int i = threadIdx.x; i < J.n; i += kRefThreads) {
+      const double px = static_cast<double>(xyz[3 * static_cast<size_t>(i)]);
+      const double py = static_cast<double>(xyz[3 * static_cast<size_t>(i) + 1]);
+      double w, wv[3];
+      TsdfPoint<kJac, false>(J, x, cs, sn, px, py, &w, wv, nullptr, nullptr);
+      acc[0] += w;
+      if (kJac) {
+        acc[1] += wv[0];
+        acc[2] += wv[1];
+        acc[3] += wv[2];
+      }
+    }
+    BlockSum<kJac ? 4 : 1>(acc, s_part, s_tot);
+    W = s_tot[0];
+    if (kJac) {
+      Wv[0] = s_tot[1];
+      Wv[1] = s_tot[2];
+      Wv[2] = s_tot[3];
+    }
+    if (W == 0.) {   // the weights are >= 0: W == 0 whatever the order of the sum
+      __syncthreads();   // every thread has read s_tot before the caller reuses it
+      return false;
+    }
+#pragma unroll
+    for (int k = 0; k < 4; ++k) acc[k] = 0.;
+  }
+  const double ns = static_cast<double>(J.n) * scaling;
   for (int i = threadIdx.x; i < J.n; i += kRefThreads) {
     const double px = static_cast<double>(xyz[3 * static_cast<size_t>(i)]);
     const double py = static_cast<double>(xyz[3 * static_cast<size_t>(i) + 1]);
     double res, jr[3];
-    PointResidual<kJac>(J, P, scaling, x, cs, sn, px, py, &res, jr);
+    if (kGrid == kGridTsdf) {
+      double w, wv[3], cost, costv[3];
+      TsdfPoint<kJac, true>(J, x, cs, sn, px, py, &w, wv, &cost, costv);
+      TsdfResidual<kJac>(ns, W, Wv, w, wv, cost, costv, &res, jr);
+    } else {
+      PointResidual<kJac>(J, P, scaling, x, cs, sn, px, py, &res, jr);
+    }
     acc[0] += res * res;
     if (kJac) {
       acc[1] += jr[0] * res;
@@ -207,6 +384,7 @@ __device__ __forceinline__ void EvaluateAt(const RefJobDev& J, const RefOpts& P,
     }
   }
   __syncthreads();
+  return true;
 }
 
 __device__ __forceinline__ bool SolveSpd3(const double* a, const double* b, double* y) {
@@ -236,19 +414,21 @@ __device__ __forceinline__ double Norm3(const double* v) {
 enum { kCmdEvalCandidate = 0, kCmdAccept = 1, kCmdRejected = 2, kCmdDone = 3 };
 enum {
   kTermNoConvergence = 0, kTermFunctionTolerance = 1, kTermGradientTolerance = 2,
-  kTermParameterTolerance = 3, kTermMinRadius = 4, kTermInvalidSteps = 5
+  kTermParameterTolerance = 3, kTermMinRadius = 4, kTermInvalidSteps = 5,
+  kTermEvaluationFailed = 6
 };
 
-__global__ void __launch_bounds__(kRefThreads)
-k_ceres_match2d(const RefJobDev* __restrict__ jobs, RefOpts P, const float* __restrict__ cloud,
-                RefResultDev* __restrict__ results) {
-  __shared__ double s_part[kRefWarps][10];
-  __shared__ double s_tot[10];
-  __shared__ double s_pose[3];
-  __shared__ int s_cmd;
-  const RefJobDev J = jobs[blockIdx.x];
-  const float* __restrict__ xyz = cloud + J.xyz_off;
-
+// The trust-region loop of one match (one CTA), with the cost function as a compile-time
+// policy.  Where the cost function fails (TSDF, summed_weight == 0) Ceres' minimiser does:
+// at a trial point the candidate's cost is the largest double, so the step is rejected; at
+// the initial point (or at an accepted point, for its Jacobian) the solve ends as FAILURE and
+// the parameters keep the initial estimate.
+template <int kGrid>
+__device__ __forceinline__ void CeresSolve(const RefJobDev& J, const RefOpts& P,
+                                           const float* __restrict__ xyz, double (*s_part)[10],
+                                           double* s_tot, double* s_pose, int* s_cmd_p,
+                                           RefResultDev* __restrict__ result) {
+  int& s_cmd = *s_cmd_p;
   // Solver::Options defaults the reference leaves untouched
   const double kInitialRadius = 1e4, kMaxRadius = 1e16, kMinRadius = 1e-32;
   const double kMinRelativeDecrease = 1e-3, kMinLmDiagonal = 1e-6, kMaxLmDiagonal = 1e32;
@@ -272,7 +452,22 @@ k_ceres_match2d(const RefJobDev* __restrict__ jobs, RefOpts P, const float* __re
   double cand[3] = {x[0], x[1], x[2]};
   double model_cost_change = 0.;
 
-  EvaluateAt<true>(J, P, xyz, x, s_part, s_tot);
+  bool failed = !EvaluateAt<kGrid, true>(J, P, xyz, x, s_part, s_tot);
+  if (failed) {
+    if (threadIdx.x == 0) {
+      // Solver::Summary keeps its defaults (costs -1) when iteration zero fails
+      RefResultDev out;
+      out.pose[0] = J.init[0];
+      out.pose[1] = J.init[1];
+      out.pose[2] = J.init[2];
+      out.initial_cost = out.final_cost = -1.;
+      out.iterations = out.num_successful_steps = 0;
+      out.termination = kTermEvaluationFailed;
+      out.pad = 0;
+      *result = out;
+    }
+    return;
+  }
   x_cost = s_tot[0];
 #pragma unroll
   for (int k = 0; k < 3; ++k) g[k] = s_tot[1 + k];
@@ -356,7 +551,9 @@ k_ceres_match2d(const RefJobDev* __restrict__ jobs, RefOpts P, const float* __re
     {
       const double p[3] = {s_pose[0], s_pose[1], s_pose[2]};
       __syncthreads();
-      EvaluateAt<false>(J, P, xyz, p, s_part, s_tot);   // the candidate's cost, plain doubles
+      // the candidate's cost, plain doubles
+      const bool ok = EvaluateAt<kGrid, false>(J, P, xyz, p, s_part, s_tot);
+      if (threadIdx.x == 0) s_tot[0] = ok ? s_tot[0] : DBL_MAX;
     }
     // ---- thread 0: tolerances on the trial step, step quality --------------------
     if (threadIdx.x == 0) {
@@ -417,7 +614,11 @@ k_ceres_match2d(const RefJobDev* __restrict__ jobs, RefOpts P, const float* __re
     if (s_cmd == kCmdAccept) {
       const double p[3] = {s_pose[0], s_pose[1], s_pose[2]};
       __syncthreads();
-      EvaluateAt<true>(J, P, xyz, p, s_part, s_tot);   // residuals + Jacobian at the new x
+      // residuals + Jacobian at the new x
+      if (!EvaluateAt<kGrid, true>(J, P, xyz, p, s_part, s_tot)) {
+        failed = true;
+        break;
+      }
       if (threadIdx.x == 0) {
         x_cost = s_tot[0];
 #pragma unroll
@@ -431,6 +632,13 @@ k_ceres_match2d(const RefJobDev* __restrict__ jobs, RefOpts P, const float* __re
   }
   if (threadIdx.x == 0) {
     RefResultDev out;
+    if (failed) {   // FAILURE: the parameters keep the initial estimate
+      best[0] = J.init[0];
+      best[1] = J.init[1];
+      best[2] = J.init[2];
+      minimum_cost = initial_cost;
+      termination = kTermEvaluationFailed;
+    }
     out.pose[0] = best[0];
     out.pose[1] = best[1];
     out.pose[2] = best[2];
@@ -440,8 +648,25 @@ k_ceres_match2d(const RefJobDev* __restrict__ jobs, RefOpts P, const float* __re
     out.num_successful_steps = successful;
     out.termination = termination;
     out.pad = 0;
-    results[blockIdx.x] = out;
+    *result = out;
   }
+}
+
+// One CTA per match; the grid type of the job's handle selects the cost function
+// (block-uniform branch), so a batch may mix ProbabilityGrid and TSDF2D jobs.
+__global__ void __launch_bounds__(kRefThreads)
+k_ceres_match2d(const RefJobDev* __restrict__ jobs, RefOpts P, const float* __restrict__ cloud,
+                RefResultDev* __restrict__ results) {
+  __shared__ double s_part[kRefWarps][10];
+  __shared__ double s_tot[10];
+  __shared__ double s_pose[3];
+  __shared__ int s_cmd;
+  const RefJobDev J = jobs[blockIdx.x];
+  const float* __restrict__ xyz = cloud + J.xyz_off;
+  if (J.wcells == nullptr)
+    CeresSolve<kGridProbability>(J, P, xyz, s_part, s_tot, s_pose, &s_cmd, results + blockIdx.x);
+  else
+    CeresSolve<kGridTsdf>(J, P, xyz, s_part, s_tot, s_pose, &s_cmd, results + blockIdx.x);
 }
 
 // Test hook: residuals (and Jacobian rows) of one job at one pose, one thread per residual.
@@ -466,6 +691,73 @@ __global__ void k_ceres_evaluate2d(RefJobDev J, RefOpts P, const float* __restri
     }
     residuals[i] = res;
   } else if (i == J.n) {
+    const size_t n = J.n;
+    residuals[n] = P.translation_weight * (x[0] - J.target[0]);
+    residuals[n + 1] = P.translation_weight * (x[1] - J.target[1]);
+    residuals[n + 2] = P.rotation_weight * (x[2] - J.init[2]);
+    if (with_jacobian) {
+      for (int k = 0; k < 9; ++k) jacobian[3 * n + k] = 0.;
+      jacobian[3 * n + 0] = P.translation_weight;
+      jacobian[3 * (n + 1) + 1] = P.translation_weight;
+      jacobian[3 * (n + 2) + 2] = P.rotation_weight;
+    }
+  }
+}
+
+// Test hook, TSDF2D: the residuals need W first, so one CTA reduces it (block-tree order, as
+// the solver does) and then writes every residual; *valid = 0 where summed_weight == 0.
+template <bool kJac>
+__device__ __forceinline__ void EvaluateTsdf(const RefJobDev& J, const RefOpts& P,
+                                             const float* __restrict__ xyz, const double* x,
+                                             double cs, double sn, double* __restrict__ residuals,
+                                             double* __restrict__ jacobian, int* valid) {
+  __shared__ double s_part[kRefWarps][10];
+  __shared__ double s_tot[10];
+  double acc[4] = {0., 0., 0., 0.};
+  for (int i = threadIdx.x; i < J.n; i += kRefThreads) {
+    double w, wv[3];
+    TsdfPoint<kJac, false>(J, x, cs, sn, static_cast<double>(xyz[3 * static_cast<size_t>(i)]),
+                           static_cast<double>(xyz[3 * static_cast<size_t>(i) + 1]), &w, wv,
+                           nullptr, nullptr);
+    acc[0] += w;
+    if (kJac) {
+      acc[1] += wv[0];
+      acc[2] += wv[1];
+      acc[3] += wv[2];
+    }
+  }
+  BlockSum<kJac ? 4 : 1>(acc, s_part, s_tot);
+  const double W = s_tot[0];
+  const double Wv[3] = {kJac ? s_tot[1] : 0., kJac ? s_tot[2] : 0., kJac ? s_tot[3] : 0.};
+  if (threadIdx.x == 0) *valid = W == 0. ? 0 : 1;
+  if (W == 0.) return;
+  const double ns = static_cast<double>(J.n) * (P.occupied_space_weight / sqrt(static_cast<double>(J.n)));
+  for (int i = threadIdx.x; i < J.n; i += kRefThreads) {
+    double w, wv[3], cost, costv[3], res, jr[3];
+    TsdfPoint<kJac, true>(J, x, cs, sn, static_cast<double>(xyz[3 * static_cast<size_t>(i)]),
+                          static_cast<double>(xyz[3 * static_cast<size_t>(i) + 1]), &w, wv, &cost,
+                          costv);
+    TsdfResidual<kJac>(ns, W, Wv, w, wv, cost, costv, &res, jr);
+    residuals[i] = res;
+    if (kJac) {
+      jacobian[3 * static_cast<size_t>(i)] = jr[0];
+      jacobian[3 * static_cast<size_t>(i) + 1] = jr[1];
+      jacobian[3 * static_cast<size_t>(i) + 2] = jr[2];
+    }
+  }
+}
+
+__global__ void __launch_bounds__(kRefThreads)
+k_ceres_evaluate2d_tsdf(RefJobDev J, RefOpts P, const float* __restrict__ xyz, double px,
+                        double py, double pt, double cs, double sn, int with_jacobian,
+                        double* __restrict__ residuals, double* __restrict__ jacobian,
+                        int* __restrict__ valid) {
+  const double x[3] = {px, py, pt};
+  if (with_jacobian)
+    EvaluateTsdf<true>(J, P, xyz, x, cs, sn, residuals, jacobian, valid);
+  else
+    EvaluateTsdf<false>(J, P, xyz, x, cs, sn, residuals, jacobian, valid);
+  if (threadIdx.x == 0) {   // the two prior blocks, as k_ceres_evaluate2d writes them
     const size_t n = J.n;
     residuals[n] = P.translation_weight * (x[0] - J.target[0]);
     residuals[n + 1] = P.translation_weight * (x[1] - J.target[1]);
@@ -525,6 +817,15 @@ void FillJob(const csm_rt_grid2d* grid, int n, long long xyz_off, const double t
   j->init[0] = init[0];
   j->init[1] = init[1];
   j->init[2] = init[2];
+  if (grid->d_wcells != nullptr) {   // TSDF2D: TSDFMatchCostFunction2D
+    const TsdfConversion c = MakeTsdfConversion(grid->truncation, grid->max_weight);
+    j->wcells = grid->g.wcells;
+    j->tsd_scale = c.tsd_scale;
+    j->tsd_bias = c.tsd_bias;
+    j->w_scale = c.w_scale;
+    j->w_bias = c.w_bias;
+    j->truncation = grid->truncation;
+  }
 }
 
 }  // namespace
@@ -543,7 +844,6 @@ csm_status csm_ceres_match2d_batch(const csm_ceres_job2d* jobs, int32_t num_jobs
   for (int j = 0; j < num_jobs; ++j) {
     CSM_REQUIRE(jobs[j].grid != nullptr && jobs[j].xyz != nullptr, "null pointer");
     CSM_REQUIRE(jobs[j].num_points >= 1, "empty point cloud");
-    CSM_REQUIRE(jobs[j].grid->d_wcells == nullptr, "the grid must be a ProbabilityGrid");
     CSM_REQUIRE(jobs[j].grid->ctx->device == device, "grids of one batch share a device");
     floats += 3LL * jobs[j].num_points;
   }
@@ -642,6 +942,57 @@ csm_status csm_ceres_evaluate2d(const csm_rt_grid2d* grid, const float* xyz, int
     CSM_CUDA(cudaMemcpyAsync(jacobian, d_jac.p, sizeof(double) * 3 * (n + 3),
                              cudaMemcpyDeviceToHost, s));
   CSM_CUDA(cudaStreamSynchronize(s));
+  return CSM_OK;
+}
+
+csm_status csm_ceres_evaluate2d_checked(const csm_rt_grid2d* grid, const float* xyz,
+                                        int32_t num_points, const csm_ceres_options2d* options,
+                                        const double target_translation[2], double target_angle,
+                                        const double pose[3], double* residuals,
+                                        double* jacobian, int32_t* valid) {
+  CSM_REQUIRE(grid && xyz && target_translation && pose && residuals && valid, "null pointer");
+  CSM_REQUIRE(num_points >= 1, "empty point cloud");
+  if (grid->d_wcells == nullptr) {   // a ProbabilityGrid's cost function never fails
+    CSM_TRY(csm_ceres_evaluate2d(grid, xyz, num_points, options, target_translation,
+                                 target_angle, pose, residuals, jacobian));
+    *valid = 1;
+    return CSM_OK;
+  }
+  RefOpts P;
+  CSM_TRY(FillOpts(options, &P));
+  LaneGuard guard;
+  CSM_TRY(AcquireLane(grid->ctx->device, &guard));
+  Ctx* ctx = guard.lane;
+  CSM_CUDA(cudaSetDevice(ctx->device));
+  cudaStream_t s = ctx->stream;
+  const size_t n = static_cast<size_t>(num_points);
+  DevBuf& d_xyz = ctx->D("ref_eval_xyz");
+  DevBuf& d_res = ctx->D("ref_eval_res");
+  DevBuf& d_jac = ctx->D("ref_eval_jac");
+  DevBuf& d_valid = ctx->D("ref_eval_valid");
+  CSM_TRY(d_xyz.Reserve(sizeof(float) * 3 * n));
+  CSM_TRY(d_res.Reserve(sizeof(double) * (n + 3)));
+  CSM_TRY(d_jac.Reserve(sizeof(double) * 3 * (n + 3)));
+  CSM_TRY(d_valid.Reserve(sizeof(int)));
+  CSM_CUDA(cudaMemcpyAsync(d_xyz.p, xyz, sizeof(float) * 3 * n, cudaMemcpyHostToDevice, s));
+  CSM_CUDA(cudaMemsetAsync(d_res.p, 0, sizeof(double) * (n + 3), s));
+  CSM_CUDA(cudaMemsetAsync(d_jac.p, 0, sizeof(double) * 3 * (n + 3), s));
+  RefJobDev J;
+  const double init[3] = {pose[0], pose[1], target_angle};   // init[2] carries the prior's angle
+  FillJob(grid, num_points, 0, target_translation, init, &J);
+  // host cos / sin, as in csm_ceres_evaluate2d
+  k_ceres_evaluate2d_tsdf<<<1, kRefThreads, 0, s>>>(
+      J, P, d_xyz.as<float>(), pose[0], pose[1], pose[2], std::cos(pose[2]), std::sin(pose[2]),
+      jacobian != nullptr, d_res.as<double>(), d_jac.as<double>(), d_valid.as<int>());
+  CSM_LAUNCH_CHECK();
+  CSM_CUDA(cudaMemcpyAsync(residuals, d_res.p, sizeof(double) * (n + 3), cudaMemcpyDeviceToHost, s));
+  if (jacobian)
+    CSM_CUDA(cudaMemcpyAsync(jacobian, d_jac.p, sizeof(double) * 3 * (n + 3),
+                             cudaMemcpyDeviceToHost, s));
+  int v = 0;
+  CSM_CUDA(cudaMemcpyAsync(&v, d_valid.p, sizeof(int), cudaMemcpyDeviceToHost, s));
+  CSM_CUDA(cudaStreamSynchronize(s));
+  *valid = v;
   return CSM_OK;
 }
 

@@ -6,6 +6,7 @@
 #include <cuda.h>
 
 #include "common.cuh"
+#include "tsdf_conversion.h"
 
 namespace csm {
 

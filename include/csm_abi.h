@@ -232,6 +232,17 @@ csm_status csm_rt_grid2d_create(const uint16_t* cells, int32_t num_x_cells, int3
                                 double resolution, double max_x, double max_y, int32_t device,
                                 csm_rt_grid2d** out);
 csm_status csm_rt_grid2d_update(csm_rt_grid2d* grid, const uint16_t* cells);
+/* The same handle for a TSDF2D (mapping/internal/2d/tsdf_2d.h): tsd cells and weight cells
+ * (uint16, num_y x num_x, the proto's correspondence_cost_cells and tsdf_2d.weight_cells) and
+ * the TSDValueConverter parameters.  csm_rt_match2d_batch then scores with the TSDF form of
+ * csm_rt_match2d_tsdf, and csm_ceres_match2d_batch refines with TSDFMatchCostFunction2D. */
+csm_status csm_rt_grid2d_create_tsdf(const uint16_t* tsd_cells, const uint16_t* weight_cells,
+                                     int32_t num_x_cells, int32_t num_y_cells,
+                                     double resolution, double max_x, double max_y,
+                                     float truncation_distance, float max_weight,
+                                     int32_t device, csm_rt_grid2d** out);
+csm_status csm_rt_grid2d_update_tsdf(csm_rt_grid2d* grid, const uint16_t* tsd_cells,
+                                     const uint16_t* weight_cells);
 csm_status csm_rt_grid2d_destroy(csm_rt_grid2d* grid);
 
 typedef struct csm_rt_job2d {
@@ -285,8 +296,11 @@ csm_status csm_rt_score_candidates2d(const uint16_t* cells, int32_t num_x_cells,
  * itself is not linked: the solver follows Ceres' documented Levenberg-Marquardt
  * trust-region algorithm with the Solver::Options the reference sets (DENSE_QR,
  * use_nonmonotonic_steps, max_num_iterations; everything else default) — see DESIGN.md for
- * what that restatement is pinned to.  Grids are csm_rt_grid2d handles (ProbabilityGrid
- * only). */
+ * what that restatement is pinned to.  Grids are csm_rt_grid2d handles; the handle's grid
+ * type selects the cost function as Grid2D::GetGridType() does (ceres_scan_matcher_2d.cc:
+ * 74-91): a TSDF2D handle (csm_rt_grid2d_create_tsdf) gets TSDFMatchCostFunction2D
+ * (tsdf_match_cost_function_2d.cc), bilinear interpolation of the correspondence costs
+ * weighted by the interpolated weights.  One batch may mix both grid types. */
 typedef struct csm_ceres_options2d {
   double occupied_space_weight;   /* proto/scan_matching/ceres_scan_matcher_options_2d.proto */
   double translation_weight;
@@ -306,8 +320,13 @@ typedef struct csm_ceres_job2d {
 
 /* termination: 0 max_num_iterations reached (NO_CONVERGENCE), 1 function tolerance,
  * 2 gradient tolerance, 3 parameter tolerance, 4 minimum trust-region radius,
- * 5 too many consecutive invalid steps (FAILURE).  Like Ceres, 1 and 3 stop BEFORE taking the
- * step that triggered them, and the lowest-cost iterate visited is what is returned. */
+ * 5 too many consecutive invalid steps (FAILURE), 6 the cost function failed where Ceres
+ * stops (FAILURE; TSDF2D only: the scan sees no weight, summed_weight == 0, at the initial
+ * estimate or at an accepted step) — pose_estimate is then the initial estimate, and if it
+ * failed at the initial estimate initial_cost = final_cost = -1 and iterations = 0.  A trial
+ * step where the cost function fails counts as a step of infinite cost and is rejected.  Like
+ * Ceres, 1 and 3 stop BEFORE taking the step that triggered them, and the lowest-cost iterate
+ * visited is what is returned. */
 typedef struct csm_ceres_result2d {
   double pose_estimate[3];
   double initial_cost, final_cost; /* Solver::Summary::initial_cost / final_cost */
@@ -328,6 +347,15 @@ csm_status csm_ceres_evaluate2d(const csm_rt_grid2d* grid, const float* xyz, int
                                 const csm_ceres_options2d* options,
                                 const double target_translation[2], double target_angle,
                                 const double pose[3], double* residuals, double* jacobian);
+
+/* Test hook for either grid type: as csm_ceres_evaluate2d, plus *valid = 0 where the cost
+ * function returns false (TSDF2D, summed_weight == 0; the scan's residuals and Jacobian rows
+ * are then 0, the priors' are still written).  ProbabilityGrid handles always give 1. */
+csm_status csm_ceres_evaluate2d_checked(const csm_rt_grid2d* grid, const float* xyz,
+                                        int32_t num_points, const csm_ceres_options2d* options,
+                                        const double target_translation[2], double target_angle,
+                                        const double pose[3], double* residuals,
+                                        double* jacobian, int32_t* valid);
 
 /* ==== 3D: FastCorrelativeScanMatcher3D ====================================== */
 /* A HybridGrid crosses the ABI in the flat form of proto::HybridGrid
