@@ -1188,7 +1188,43 @@ k_q_scatter(const Node* __restrict__ queue, const int* __restrict__ ctl,
 #define CSM_LAT_THREADS 128
 #endif
 constexpr int kLatThreads = CSM_LAT_THREADS;   // every warp works on its own item
-constexpr int kLatChunk = 256;
+// Points staged per chunk, and the spacing of the early-exit tests below: on the config-2
+// workload, with the bound at the optimum, tests every 128 points skip 31 % of the h = 6
+// words and 48-52 % of the h = 5 words, every 256 points 27 % and 44-48 %
+// (benchmarks/prototypes/early_exit_counts.py).
+constexpr int kLatChunk = 128;
+
+// Largest integer sum whose score is <= `score` (the node's own sum when `score` is
+// ToScore of it), and smallest sum whose score passes both survival tests of a child
+// (score > min_score and score >= bound; 255 n + 1 if none does).  ToScore is monotone in
+// the sum, so a walk from the rounded estimate ends at the exact integer, in one or two
+// steps in practice.  Without a score range (k255 = 0) they give the loosest values, which
+// never rule a parent out.
+__device__ __forceinline__ int SumAtMost(const StackDev& st, float score, int n) {
+  const int top = 255 * n;
+  if (!(st.k255 > 0.f)) return top;
+  int e = __float2int_rn((score - st.min_score) / st.k255 * static_cast<float>(n));
+  e = min(max(e, 0), top);
+  while (e < top && ToScore(st, e + 1, n) <= score) ++e;
+  while (e > 0 && ToScore(st, e, n) > score) --e;
+  return e;
+}
+__device__ __forceinline__ int SumToSurvive(const StackDev& st, float min_score, float bound,
+                                            int n) {
+  const int top = 255 * n;
+  auto pass = [&](int t) {
+    const float sc = ToScore(st, t, n);
+    return sc > min_score && sc >= bound;
+  };
+  if (!(st.k255 > 0.f)) return 0;
+  int t = __float2int_rn((fmaxf(min_score, bound) - st.min_score) / st.k255 *
+                         static_cast<float>(n));
+  t = min(max(t, 0), top + 1);
+  while (t > 0 && pass(t - 1)) --t;
+  while (t <= top && !pass(t)) ++t;
+  return t;
+}
+
 template <int kUnroll>
 __global__ void __launch_bounds__(kLatThreads, CSM_LAT_MINB)
 k_expand_lattice(const JobDev* __restrict__ jobs, const ScanInfo* __restrict__ info,
@@ -1230,11 +1266,22 @@ k_expand_lattice(const JobDev* __restrict__ jobs, const ScanInfo* __restrict__ i
   Node nd = Node{it.scan, si.min_x, si.min_y, 0.f};
   if (active) nd = sorted[it.start + pidx];
   // the bound may have risen since the node was queued
-  const bool live = active && nd.score >= OrderedToFloat(lb[si.job]);
+  const float bound0 = OrderedToFloat(lb[si.job]);
+  const bool live = active && nd.score >= bound0;
   const int i0 = (nd.xo - si.min_x) >> h, j0 = (nd.yo - si.min_y) >> h;  // parent lattice coords
   const int toff = j0 * ids + i0;
   const bool x2 = !(nd.xo + s > si.max_x), y2 = !(nd.yo + s > si.max_y);
   unsigned sum0 = 0, sum1 = 0, sum2 = 0, sum3 = 0;  // slots 2*ix+iy: 00, 01, 10, 11
+  // Early exit.  Every child window lies inside the parent's, so at each point the
+  // largest byte of the word is <= the parent's level-h value there, and the parent's
+  // sum is <= p_hi.  After some points, with partial child sums c_t and `mx` the partial
+  // sum of the largest bytes, child t ends at most at c_t + p_hi - mx.  Once that is below
+  // t_min (no sum below it survives: the bound only rises) for every valid child, the
+  // parent is decided and its remaining words are not read.
+  const int p_hi = SumAtMost(st, nd.score, jb.n);
+  const int t_min = SumToSurvive(st, jb.min_score, bound0, jb.n);
+  unsigned mx = 0;
+  bool run = live;       // live and not yet ruled out
   for (int p0 = 0; p0 < jb.n; p0 += kLatChunk) {
     __syncwarp();
     for (int t = lane; t < kLatChunk; t += 32) {
@@ -1255,9 +1302,16 @@ k_expand_lattice(const JobDev* __restrict__ jobs, const ScanInfo* __restrict__ i
       s_pt[t] = d;
     }
     __syncwarp();
-    if (live) {
+    if (run) {
       const int cnt = min(kLatChunk, jb.n - p0);
       unsigned r0 = 0, r1 = 0;  // packed u16 pairs: (ix 0, ix 1) of iy 0 / iy 1
+      auto add = [&](unsigned w) {
+        const unsigned a = __byte_perm(w, 0u, 0x4140), b = __byte_perm(w, 0u, 0x4342);
+        r0 += a;
+        r1 += b;
+        const unsigned ab = __vmaxu2(a, b);   // u16 pair (max(b0, b2), max(b1, b3))
+        mx += max(ab & 0xffffu, ab >> 16);
+      };
       // two staged points per 16-byte shared load (entries past cnt never pass the range test)
 #pragma unroll(kUnroll / 2)
       for (int t = 2 * sub; t < cnt; t += 2 * G) {
@@ -1267,28 +1321,39 @@ k_expand_lattice(const JobDev* __restrict__ jobs, const ScanInfo* __restrict__ i
         if (static_cast<unsigned>(Ia) < static_cast<unsigned>(ids) &&
             static_cast<unsigned>(Ja) < static_cast<unsigned>(jd)) {
 #ifdef CSM_WIN_TILED
-          const unsigned w = __ldg(win + (d.x + WinCell(Ia, Ja, ids)));
+          add(__ldg(win + (d.x + WinCell(Ia, Ja, ids))));
 #else
-          const unsigned w = __ldg(win + (d.x + toff));
+          add(__ldg(win + (d.x + toff)));
 #endif
-          r0 += __byte_perm(w, 0u, 0x4140);
-          r1 += __byte_perm(w, 0u, 0x4342);
         }
         if (static_cast<unsigned>(Ib) < static_cast<unsigned>(ids) &&
             static_cast<unsigned>(Jb) < static_cast<unsigned>(jd)) {
 #ifdef CSM_WIN_TILED
-          const unsigned w = __ldg(win + (d.z + WinCell(Ib, Jb, ids)));
+          add(__ldg(win + (d.z + WinCell(Ib, Jb, ids))));
 #else
-          const unsigned w = __ldg(win + (d.z + toff));
+          add(__ldg(win + (d.z + toff)));
 #endif
-          r0 += __byte_perm(w, 0u, 0x4140);
-          r1 += __byte_perm(w, 0u, 0x4342);
         }
       }
       sum0 += r0 & 0xffffu;   // (ix 0, iy 0)
       sum2 += r0 >> 16;       // (ix 1, iy 0)
       sum1 += r1 & 0xffffu;   // (ix 0, iy 1)
       sum3 += r1 >> 16;       // (ix 1, iy 1)
+    }
+    if (p0 + kLatChunk < jb.n) {
+      // c_t - mx summed over the G sub-lanes of the parent (G is the same on every lane)
+      int d0 = static_cast<int>(sum0 - mx), d1 = static_cast<int>(sum1 - mx);
+      int d2 = static_cast<int>(sum2 - mx), d3 = static_cast<int>(sum3 - mx);
+      for (int o = 1; o < G; o <<= 1) {
+        d0 += __shfl_xor_sync(0xffffffffu, d0, o);
+        d1 += __shfl_xor_sync(0xffffffffu, d1, o);
+        d2 += __shfl_xor_sync(0xffffffffu, d2, o);
+        d3 += __shfl_xor_sync(0xffffffffu, d3, o);
+      }
+      const int lim = t_min - p_hi;
+      run = run && (d0 >= lim || (y2 && d1 >= lim) || (x2 && d2 >= lim) ||
+                    (x2 && y2 && d3 >= lim));
+      if (!__any_sync(0xffffffffu, run)) break;
     }
   }
   // totals of the G sub-lanes (all lanes of the warp take part)
@@ -1301,9 +1366,11 @@ k_expand_lattice(const JobDev* __restrict__ jobs, const ScanInfo* __restrict__ i
   const bool lead = live && sub == 0;   // one lane per parent carries on
   const unsigned valid = lead ? (1u | (y2 ? 2u : 0u) | (x2 ? 4u : 0u) | ((x2 && y2) ? 8u : 0u)) : 0u;
   if (lead) {
+    // a parent ruled out early still counts: the bound decided all its children
     atomicAdd(&counters[0], (unsigned long long)__popc(valid));
     atomicAdd(&counters[1], 1ull);
   }
+  const unsigned emit = run ? valid : 0u;   // its partial sums never reach the queues
   const int sums[4] = {static_cast<int>(sum0), static_cast<int>(sum1), static_cast<int>(sum2),
                        static_cast<int>(sum3)};
   float sc[4];
@@ -1313,7 +1380,7 @@ k_expand_lattice(const JobDev* __restrict__ jobs, const ScanInfo* __restrict__ i
     if (!lead) return;
 #pragma unroll
     for (int t = 0; t < 4; ++t) {
-      if (!((valid >> t) & 1u) || !(sc[t] > jb.min_score)) continue;
+      if (!((emit >> t) & 1u) || !(sc[t] > jb.min_score)) continue;
       const unsigned o = FloatToOrdered(sc[t]);
       const unsigned old = atomicMax(&lb[si.job], o);
       if (o >= old) {
@@ -1332,7 +1399,7 @@ k_expand_lattice(const JobDev* __restrict__ jobs, const ScanInfo* __restrict__ i
   unsigned keep = 0;
 #pragma unroll
   for (int t = 0; t < 4; ++t)
-    if (((valid >> t) & 1u) && sc[t] > jb.min_score && sc[t] >= bound) keep |= 1u << t;
+    if (((emit >> t) & 1u) && sc[t] > jb.min_score && sc[t] >= bound) keep |= 1u << t;
   // slot t = 2*ix + iy
   const unsigned m00 = __ballot_sync(0xffffffffu, keep & 1u), m10 = __ballot_sync(0xffffffffu, keep & 4u);
   const unsigned m01 = __ballot_sync(0xffffffffu, keep & 2u), m11 = __ballot_sync(0xffffffffu, keep & 8u);
