@@ -1191,7 +1191,9 @@ constexpr int kLatThreads = CSM_LAT_THREADS;   // every warp works on its own it
 // Points staged per chunk, and the spacing of the early-exit tests below: on the config-2
 // workload, with the bound at the optimum, tests every 128 points skip 31 % of the h = 6
 // words and 48-52 % of the h = 5 words, every 256 points 27 % and 44-48 %
-// (benchmarks/prototypes/early_exit_counts.py).
+// (benchmarks/prototypes/early_exit_counts.py).  With the lanes re-mapped, tests every 64
+// points would cut the warp passes by only about 5 % more, for twice the tests
+// (benchmarks/prototypes/lane_remap_counts.py).
 constexpr int kLatChunk = 128;
 
 // Largest integer sum whose score is <= `score` (the node's own sum when `score` is
@@ -1245,10 +1247,12 @@ k_expand_lattice(const JobDev* __restrict__ jobs, const ScanInfo* __restrict__ i
   const WorkItem it = items[item];
   // With few parents, G = 2^lg lanes share one parent and split the scan points
   // (lane = parent * G + sub, sub-lane `sub` takes the point pairs sub, sub + G, ...).
+  // G grows when the early exit below leaves few parents running.
   int lg = 0;
   while ((it.count << (lg + 1)) <= 32) ++lg;
-  const int G = 1 << lg;
-  const int pidx = lane >> lg, sub = lane & (G - 1);
+  int G = 1 << lg;
+  int sub = lane & (G - 1);
+  const int pidx = lane >> lg;
   const ScanInfo si = info[it.scan];
   const JobDev& jb = jobs[si.job];
   const StackDev& st = *jb.stack;
@@ -1268,9 +1272,14 @@ k_expand_lattice(const JobDev* __restrict__ jobs, const ScanInfo* __restrict__ i
   // the bound may have risen since the node was queued
   const float bound0 = OrderedToFloat(lb[si.job]);
   const bool live = active && nd.score >= bound0;
-  const int i0 = (nd.xo - si.min_x) >> h, j0 = (nd.yo - si.min_y) >> h;  // parent lattice coords
-  const int toff = j0 * ids + i0;
-  const bool x2 = !(nd.xo + s > si.max_x), y2 = !(nd.yo + s > si.max_y);
+  int i0 = (nd.xo - si.min_x) >> h, j0 = (nd.yo - si.min_y) >> h;  // parent lattice coords
+  int toff = j0 * ids + i0;
+  bool x2 = !(nd.xo + s > si.max_x), y2 = !(nd.yo + s > si.max_y);
+  if (live && sub == 0) {
+    // a parent ruled out early still counts: the bound decided all its children
+    atomicAdd(&counters[0], 1ull + y2 + x2 + (x2 && y2));
+    atomicAdd(&counters[1], 1ull);
+  }
   unsigned sum0 = 0, sum1 = 0, sum2 = 0, sum3 = 0;  // slots 2*ix+iy: 00, 01, 10, 11
   // Early exit.  Every child window lies inside the parent's, so at each point the
   // largest byte of the word is <= the parent's level-h value there, and the parent's
@@ -1278,7 +1287,7 @@ k_expand_lattice(const JobDev* __restrict__ jobs, const ScanInfo* __restrict__ i
   // sum of the largest bytes, child t ends at most at c_t + p_hi - mx.  Once that is below
   // t_min (no sum below it survives: the bound only rises) for every valid child, the
   // parent is decided and its remaining words are not read.
-  const int p_hi = SumAtMost(st, nd.score, jb.n);
+  int p_hi = SumAtMost(st, nd.score, jb.n);
   const int t_min = SumToSurvive(st, jb.min_score, bound0, jb.n);
   unsigned mx = 0;
   bool run = live;       // live and not yet ruled out
@@ -1353,7 +1362,47 @@ k_expand_lattice(const JobDev* __restrict__ jobs, const ScanInfo* __restrict__ i
       const int lim = t_min - p_hi;
       run = run && (d0 >= lim || (y2 && d1 >= lim) || (x2 && d2 >= lim) ||
                     (x2 && y2 && d3 >= lim));
-      if (!__any_sync(0xffffffffu, run)) break;
+      const unsigned leads = __ballot_sync(0xffffffffu, run && sub == 0);  // running parents
+      if (!leads) break;
+      const int L = __popc(leads);
+      if ((L << (lg + 1)) <= 32) {
+        // Re-map: the L running parents move, in lane (lattice) order, to groups of the
+        // largest G with L * G <= 32, so the lanes of ruled-out parents share the remaining
+        // points.  A group's partials are first summed over its old sub-lanes; the new
+        // sub-lane 0 takes the totals over and the other sub-lanes start from zero.  Lanes
+        // left without a running parent hold nothing.
+        for (int o = 1; o < G; o <<= 1) {
+          sum0 += __shfl_xor_sync(0xffffffffu, sum0, o);
+          sum1 += __shfl_xor_sync(0xffffffffu, sum1, o);
+          sum2 += __shfl_xor_sync(0xffffffffu, sum2, o);
+          sum3 += __shfl_xor_sync(0xffffffffu, sum3, o);
+          mx += __shfl_xor_sync(0xffffffffu, mx, o);
+        }
+        ++lg;
+        while ((L << (lg + 1)) <= 32) ++lg;
+        G = 1 << lg;
+        sub = lane & (G - 1);
+        const int k = lane >> lg;       // rank of the lane's new parent among the running ones
+        unsigned m = leads;
+        for (int i = 0; i < k && m; ++i) m &= m - 1;   // lowest bit: the k-th leader's lane
+        const int src = m ? __ffs(m) - 1 : 0;
+        const bool own = m && sub == 0;
+        const unsigned v0 = __shfl_sync(0xffffffffu, sum0, src), v1 = __shfl_sync(0xffffffffu, sum1, src);
+        const unsigned v2 = __shfl_sync(0xffffffffu, sum2, src), v3 = __shfl_sync(0xffffffffu, sum3, src);
+        const unsigned vm = __shfl_sync(0xffffffffu, mx, src);
+        sum0 = own ? v0 : 0u; sum1 = own ? v1 : 0u; sum2 = own ? v2 : 0u; sum3 = own ? v3 : 0u;
+        mx = own ? vm : 0u;
+        nd.xo = __shfl_sync(0xffffffffu, nd.xo, src);
+        nd.yo = __shfl_sync(0xffffffffu, nd.yo, src);
+        p_hi = __shfl_sync(0xffffffffu, p_hi, src);
+        const int f = __shfl_sync(0xffffffffu, (x2 ? 1 : 0) | (y2 ? 2 : 0), src);
+        x2 = f & 1;
+        y2 = f & 2;
+        run = m != 0;
+        i0 = (nd.xo - si.min_x) >> h;
+        j0 = (nd.yo - si.min_y) >> h;
+        toff = j0 * ids + i0;
+      }
     }
   }
   // totals of the G sub-lanes (all lanes of the warp take part)
@@ -1363,14 +1412,10 @@ k_expand_lattice(const JobDev* __restrict__ jobs, const ScanInfo* __restrict__ i
     const unsigned v2 = __shfl_xor_sync(0xffffffffu, sum2, o), v3 = __shfl_xor_sync(0xffffffffu, sum3, o);
     if (o < G) { sum0 += v0; sum1 += v1; sum2 += v2; sum3 += v3; }
   }
-  const bool lead = live && sub == 0;   // one lane per parent carries on
-  const unsigned valid = lead ? (1u | (y2 ? 2u : 0u) | (x2 ? 4u : 0u) | ((x2 && y2) ? 8u : 0u)) : 0u;
-  if (lead) {
-    // a parent ruled out early still counts: the bound decided all its children
-    atomicAdd(&counters[0], (unsigned long long)__popc(valid));
-    atomicAdd(&counters[1], 1ull);
-  }
-  const unsigned emit = run ? valid : 0u;   // its partial sums never reach the queues
+  // one lane per running parent carries on (the lanes of a parent ruled out early hold
+  // partial sums that never reach the queues)
+  const bool lead = run && sub == 0;
+  const unsigned emit = lead ? (1u | (y2 ? 2u : 0u) | (x2 ? 4u : 0u) | ((x2 && y2) ? 8u : 0u)) : 0u;
   const int sums[4] = {static_cast<int>(sum0), static_cast<int>(sum1), static_cast<int>(sum2),
                        static_cast<int>(sum3)};
   float sc[4];
@@ -2155,6 +2200,21 @@ static csm_status RunBatch2D(Ctx* ctx, const csm_stack2d* const* stacks, int num
   const int sort_grid = ctx->sm_count * 8;
   const int max_items = kChunk / 32 + std::min(kChunk, total_scans) + 1;
   static const int lat_unroll = getenv("CSM_LAT_UNROLL") ? atoi(getenv("CSM_LAT_UNROLL")) : 8;
+  {
+    // The lattice kernel's shared-memory carve-out: just what CSM_LAT_MINB CTAs need, so the
+    // rest of the unified L1 caches the window tables, which its loads are bound by.  On an
+    // H100 80GB HBM3 (700 W) this took k_expand_lattice from 26.64-26.81 ms per config-2 step
+    // with the driver's own choice to 26.42-26.53 ms; the largest carve-out gave 31.1 ms.
+    int dev = 0, smem_sm = 0, rsv = 0;
+    CSM_CUDA(cudaGetDevice(&dev));
+    CSM_CUDA(cudaDeviceGetAttribute(&smem_sm, cudaDevAttrMaxSharedMemoryPerMultiprocessor, dev));
+    CSM_CUDA(cudaDeviceGetAttribute(&rsv, cudaDevAttrReservedSharedMemoryPerBlock, dev));
+    const int need = CSM_LAT_MINB * (static_cast<int>(sizeof(int2)) * kLatThreads / 32 * kLatChunk + rsv);
+    const int pct = std::min(100, DivUp(100LL * need, std::max(1, smem_sm)));
+    CSM_CUDA(cudaFuncSetAttribute(k_expand_lattice<4>, cudaFuncAttributePreferredSharedMemoryCarveout, pct));
+    CSM_CUDA(cudaFuncSetAttribute(k_expand_lattice<8>, cudaFuncAttributePreferredSharedMemoryCarveout, pct));
+    CSM_CUDA(cudaFuncSetAttribute(k_expand_lattice<16>, cudaFuncAttributePreferredSharedMemoryCarveout, pct));
+  }
   auto level_step = [&](int h) -> csm_status {
     int* scan_cnt = d_scan_cnt.as<int>();
     int* cursor = scan_cnt + total_scans;
