@@ -12,10 +12,10 @@
 // interpolation of interpolated_grid.h:49-96 on dual numbers over (x, y, z)
 // (occupied_space_cost_function_3d.h:68-78), then the residual row in the 6-dimensional
 // tangent space (ambient row times the parameterisation's 4 x 3 plus-Jacobian).  The block
-// reduces cost, J^T r and the upper triangle of J^T J (28 doubles); thread 0 keeps the
-// minimiser's state in shared memory and does the Levenberg-Marquardt step exactly as
-// refine2d.cu does, with 6 parameters, x (+) delta = {t + dt, exp(dq) * q} and the gradient
-// tolerance measured as |x - (x (+) -g)|_inf.  Doubles, no FMA contraction (-fmad=false).
+// reduces cost, J^T r and the upper triangle of J^T J (28 doubles); thread 0 runs the
+// trust-region minimiser of trust_region.cuh (the one refine2d.cu runs), its state in shared
+// memory, with 6 parameters, x (+) delta = {t + dt, exp(dq) * q} and the gradient tolerance
+// measured as |x - (x (+) -g)|_inf.  Doubles, no FMA contraction (-fmad=false).
 #include <algorithm>
 #include <cmath>
 
@@ -23,11 +23,10 @@
 #ifndef CSM_REFINE_DEVICE_ONLY
 #include "grid3d.cuh"
 #endif
+#include "trust_region.cuh"
 
 namespace csm {
 
-constexpr int kRef3Threads = 256;
-constexpr int kRef3Warps = kRef3Threads / 32;
 constexpr int kRef3N = 6;                              // tangent-space parameters
 constexpr int kRef3H = kRef3N * (kRef3N + 1) / 2;      // upper triangle of J^T J
 constexpr int kRef3Acc = 1 + kRef3N + kRef3H;          // 28
@@ -54,11 +53,7 @@ struct Ref3Opts {
   int use_nonmonotonic_steps, max_num_iterations;
 };
 
-struct Ref3ResultDev {
-  double pose[7];
-  double initial_cost, final_cost;
-  int iterations, num_successful_steps, termination, pad;
-};
+using Ref3ResultDev = ResultDev<7>;   // trust_region.cuh
 
 // ---- dual numbers over (x, y, z) with ceres/jet.h's arithmetic ------------------------
 struct D3 {
@@ -252,31 +247,6 @@ __device__ __forceinline__ void PriorRows(const Ref3JobDev& J, const Ref3Opts& P
   }
 }
 
-__device__ __forceinline__ int Tri6(int i, int j) {   // i <= j
-  return i * kRef3N - i * (i - 1) / 2 + (j - i);
-}
-
-template <int kCount>
-__device__ __forceinline__ void BlockSum3(double* acc, double (*s_part)[kRef3Acc],
-                                          double* s_tot) {
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-#pragma unroll
-  for (int k = 0; k < kCount; ++k) {
-    double v = acc[k];
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) v += __shfl_down_sync(0xffffffffu, v, o);
-    if (lane == 0) s_part[warp][k] = v;
-  }
-  __syncthreads();
-  if (threadIdx.x < kCount) {
-    double v = 0.;
-#pragma unroll
-    for (int w = 0; w < kRef3Warps; ++w) v += s_part[w][threadIdx.x];
-    s_tot[threadIdx.x] = v;
-  }
-  __syncthreads();
-}
-
 // Block-wide evaluation at `pose`: s_tot = {cost, g[6], h[21]} (g, h only with kJac).
 template <bool kJac>
 __device__ __forceinline__ void EvaluateAt3(const Ref3JobDev& J, const Ref3Opts& P,
@@ -291,7 +261,7 @@ __device__ __forceinline__ void EvaluateAt3(const Ref3JobDev& J, const Ref3Opts&
     const Ref3Cloud& G = J.c[b];
     const float* __restrict__ xyz = cloud + G.xyz_off;
     const double scaling = P.occupied_space_weight[b] / sqrt(static_cast<double>(G.npts));
-    for (int i = threadIdx.x; i < G.npts; i += kRef3Threads) {
+    for (int i = threadIdx.x; i < G.npts; i += kRefThreads) {
       const double px = static_cast<double>(xyz[3 * static_cast<size_t>(i)]);
       const double py = static_cast<double>(xyz[3 * static_cast<size_t>(i) + 1]);
       const double pz = static_cast<double>(xyz[3 * static_cast<size_t>(i) + 2]);
@@ -303,12 +273,12 @@ __device__ __forceinline__ void EvaluateAt3(const Ref3JobDev& J, const Ref3Opts&
         for (int a = 0; a < kRef3N; ++a) {
           acc[1 + a] += row[a] * res;
 #pragma unroll
-          for (int c = a; c < kRef3N; ++c) acc[1 + kRef3N + Tri6(a, c)] += row[a] * row[c];
+          for (int c = a; c < kRef3N; ++c) acc[1 + kRef3N + Tri<kRef3N>(a, c)] += row[a] * row[c];
         }
       }
     }
   }
-  BlockSum3<kJac ? kRef3Acc : 1>(acc, s_part, s_tot);
+  BlockSum<kJac ? kRef3Acc : 1>(acc, s_part, s_tot);
   if (threadIdx.x == 0) {
     double res[6], rows[6][kRef3N];
     PriorRows(J, P, pose, pj, res, rows);
@@ -319,268 +289,55 @@ __device__ __forceinline__ void EvaluateAt3(const Ref3JobDev& J, const Ref3Opts&
       for (int k = 0; k < 6; ++k)
         for (int a = 0; a < kRef3N; ++a) {
           s_tot[1 + a] += rows[k][a] * res[k];
-          for (int c = a; c < kRef3N; ++c) s_tot[1 + kRef3N + Tri6(a, c)] += rows[k][a] * rows[k][c];
+          for (int c = a; c < kRef3N; ++c) s_tot[1 + kRef3N + Tri<kRef3N>(a, c)] += rows[k][a] * rows[k][c];
         }
     }
   }
   __syncthreads();
 }
 
-// Cholesky solve of A y = b, A symmetric positive definite (upper triangle, row-major)
-__device__ __forceinline__ bool SolveSpd6(const double* a, const double* b, double* y) {
-  double l[kRef3N][kRef3N];
-  for (int i = 0; i < kRef3N; ++i)
-    for (int j = 0; j < kRef3N; ++j) l[i][j] = 0.;
-  for (int i = 0; i < kRef3N; ++i) {
-    for (int j = 0; j <= i; ++j) {
-      double s = a[Tri6(j, i)];
-      for (int k = 0; k < j; ++k) s -= l[i][k] * l[j][k];
-      if (i == j) {
-        if (!(s > 0.)) return false;
-        l[i][i] = sqrt(s);
-      } else {
-        l[i][j] = s / l[j][j];
-      }
-    }
-  }
-  double z[kRef3N];
-  for (int i = 0; i < kRef3N; ++i) {
-    double s = b[i];
-    for (int k = 0; k < i; ++k) s -= l[i][k] * z[k];
-    z[i] = s / l[i][i];
-  }
-  for (int i = kRef3N - 1; i >= 0; --i) {
-    double s = z[i];
-    for (int k = i + 1; k < kRef3N; ++k) s -= l[k][i] * y[k];
-    y[i] = s / l[i][i];
-  }
-  for (int i = 0; i < kRef3N; ++i)
-    if (!isfinite(y[i])) return false;
-  return true;
-}
+// The 3D match for the minimiser: {t, q} moved in the tangent space of
+// QuaternionParameterization; the gradient tolerance is measured as |x - (x (+) -g)|_inf.
+struct Match3D {
+  static constexpr int kAmbient = 7, kN = kRef3N;
+  const Ref3JobDev& J;
+  const Ref3Opts& P;
+  const float* __restrict__ cloud;
+  double (*s_part)[kRef3Acc];
 
-__device__ __forceinline__ double NormN(const double* v, int n) {
-  double s = 0.;
-  for (int i = 0; i < n; ++i) s += v[i] * v[i];
-  return sqrt(s);
-}
-
-// State of the minimiser; lives in shared memory, touched by thread 0 only.
-struct Solver3 {
-  double x[7], best[7], cand[7];
-  double g[kRef3N], h[kRef3H], scale[kRef3N], diagonal[kRef3N];
-  double x_cost, x_norm, minimum_cost, initial_cost;
-  double radius, decrease_factor;
-  double current_cost, reference_cost, candidate_cost_ev, ev_minimum_cost;
-  double acc_reference, acc_candidate, model_cost_change;
-  int reuse_diagonal, last_step_successful;
-  int num_nonmonotonic, num_invalid, iteration, successful, termination;
+  template <bool kJac>
+  __device__ __forceinline__ bool Evaluate(const double* x, double* s_tot) const {
+    EvaluateAt3<kJac>(J, P, cloud, x, s_part, s_tot);
+    return true;
+  }
+  __device__ __forceinline__ static void Plus(const double* x, const double* delta,
+                                              double* out) {
+    Plus7(x, delta, out);
+  }
+  __device__ __forceinline__ static double GradientMaxNorm(const double* x, const double* g) {
+    double neg[kRef3N], moved[7], gmax = 0.;
+#pragma unroll
+    for (int a = 0; a < kRef3N; ++a) neg[a] = -g[a];
+    Plus7(x, neg, moved);
+#pragma unroll
+    for (int k = 0; k < 7; ++k) gmax = fmax(gmax, fabs(x[k] - moved[k]));
+    return gmax;
+  }
 };
 
-enum { kCmd3EvalCandidate = 0, kCmd3Accept = 1, kCmd3Rejected = 2, kCmd3Done = 3 };
-enum {
-  kTerm3NoConvergence = 0, kTerm3FunctionTolerance = 1, kTerm3GradientTolerance = 2,
-  kTerm3ParameterTolerance = 3, kTerm3MinRadius = 4, kTerm3InvalidSteps = 5
-};
-
-__global__ void __launch_bounds__(kRef3Threads)
+__global__ void __launch_bounds__(kRefThreads)
 k_ceres_match3d(const Ref3JobDev* __restrict__ jobs, Ref3Opts P, const float* __restrict__ cloud,
                 Ref3ResultDev* __restrict__ results) {
-  __shared__ double s_part[kRef3Warps][kRef3Acc];
+  __shared__ double s_part[kRefWarps][kRef3Acc];
   __shared__ double s_tot[kRef3Acc];
   __shared__ double s_pose[7];
   __shared__ int s_cmd;
-  __shared__ Solver3 S;
+  __shared__ TrustRegionState<7, kRef3N> S;
   __shared__ Ref3JobDev J;
   if (threadIdx.x == 0) J = jobs[blockIdx.x];
   __syncthreads();
-
-  const double kInitialRadius = 1e4, kMaxRadius = 1e16, kMinRadius = 1e-32;
-  const double kMinRelativeDecrease = 1e-3, kMinLmDiagonal = 1e-6, kMaxLmDiagonal = 1e32;
-  const int kMaxConsecutiveInvalidSteps = 5;
-  const double kFunctionTolerance = 1e-6, kGradientTolerance = 1e-10, kParameterTolerance = 1e-8;
-  const int max_nonmonotonic = P.use_nonmonotonic_steps ? 5 : 0;
-
-  {
-    double p[7];
-    for (int k = 0; k < 7; ++k) p[k] = J.init[k];
-    EvaluateAt3<true>(J, P, cloud, p, s_part, s_tot);
-  }
-  if (threadIdx.x == 0) {
-    for (int k = 0; k < 7; ++k) S.x[k] = S.best[k] = S.cand[k] = J.init[k];
-    S.x_cost = s_tot[0];
-    for (int a = 0; a < kRef3N; ++a) S.g[a] = s_tot[1 + a];
-    for (int a = 0; a < kRef3H; ++a) S.h[a] = s_tot[1 + kRef3N + a];
-    S.x_norm = NormN(S.x, 7);
-    S.initial_cost = S.minimum_cost = S.x_cost;
-    S.current_cost = S.reference_cost = S.candidate_cost_ev = S.ev_minimum_cost = S.x_cost;
-    for (int a = 0; a < kRef3N; ++a) {
-      S.scale[a] = 1.0 / (1.0 + sqrt(S.h[Tri6(a, a)]));
-      S.diagonal[a] = 0.;
-    }
-    S.radius = kInitialRadius;
-    S.decrease_factor = 2.0;
-    S.reuse_diagonal = 0;
-    S.last_step_successful = 0;
-    S.acc_reference = S.acc_candidate = S.model_cost_change = 0.;
-    S.num_nonmonotonic = S.num_invalid = S.iteration = S.successful = 0;
-    S.termination = kTerm3NoConvergence;
-  }
-  __syncthreads();
-
-  while (true) {
-    if (threadIdx.x == 0) {
-      int cmd = kCmd3EvalCandidate;
-      while (true) {   // (repeats only after an invalid step)
-        if (S.last_step_successful) {
-          ++S.successful;
-          if (S.x_cost < S.minimum_cost) {
-            S.minimum_cost = S.x_cost;
-            for (int k = 0; k < 7; ++k) S.best[k] = S.x[k];
-          }
-          S.last_step_successful = 0;
-        }
-        if (S.iteration >= P.max_num_iterations) { S.termination = kTerm3NoConvergence; cmd = kCmd3Done; break; }
-        {
-          double neg[kRef3N], moved[7], gmax = 0.;
-          for (int a = 0; a < kRef3N; ++a) neg[a] = -S.g[a];
-          Plus7(S.x, neg, moved);
-          for (int k = 0; k < 7; ++k) gmax = fmax(gmax, fabs(S.x[k] - moved[k]));
-          if (gmax <= kGradientTolerance) { S.termination = kTerm3GradientTolerance; cmd = kCmd3Done; break; }
-        }
-        if (S.radius <= kMinRadius) { S.termination = kTerm3MinRadius; cmd = kCmd3Done; break; }
-        ++S.iteration;
-        double hs[kRef3H], gs[kRef3N];
-        for (int a = 0; a < kRef3N; ++a) {
-          gs[a] = S.g[a] * S.scale[a];
-          for (int c = a; c < kRef3N; ++c) hs[Tri6(a, c)] = S.h[Tri6(a, c)] * S.scale[a] * S.scale[c];
-        }
-        if (!S.reuse_diagonal)
-          for (int a = 0; a < kRef3N; ++a)
-            S.diagonal[a] = fmin(fmax(hs[Tri6(a, a)], kMinLmDiagonal), kMaxLmDiagonal);
-        double am[kRef3H];
-        for (int i = 0; i < kRef3H; ++i) am[i] = hs[i];
-        for (int a = 0; a < kRef3N; ++a) am[Tri6(a, a)] = hs[Tri6(a, a)] + S.diagonal[a] / S.radius;
-        double y[kRef3N];
-        bool valid = SolveSpd6(am, gs, y);
-        S.reuse_diagonal = 1;
-        double step[kRef3N];
-        for (int a = 0; a < kRef3N; ++a) step[a] = 0.;
-        if (valid) {
-          for (int a = 0; a < kRef3N; ++a) step[a] = -y[a];
-          double sg = 0., shs = 0.;
-          for (int a = 0; a < kRef3N; ++a) {
-            sg += step[a] * gs[a];
-            double row = 0.;
-            for (int c = 0; c < kRef3N; ++c) row += hs[a <= c ? Tri6(a, c) : Tri6(c, a)] * step[c];
-            shs += step[a] * row;
-          }
-          S.model_cost_change = -(sg + 0.5 * shs);
-          valid = !(S.model_cost_change < 0.0);
-        }
-        if (!valid) {
-          if (++S.num_invalid >= kMaxConsecutiveInvalidSteps) { S.termination = kTerm3InvalidSteps; cmd = kCmd3Done; break; }
-          S.radius = S.radius / S.decrease_factor;
-          S.decrease_factor *= 2.0;
-          S.reuse_diagonal = 0;
-          continue;
-        }
-        S.num_invalid = 0;
-        double delta[kRef3N];
-        for (int a = 0; a < kRef3N; ++a) delta[a] = step[a] * S.scale[a];
-        Plus7(S.x, delta, S.cand);
-        break;
-      }
-      for (int k = 0; k < 7; ++k) s_pose[k] = S.cand[k];
-      s_cmd = cmd;
-    }
-    __syncthreads();
-    if (s_cmd == kCmd3Done) break;
-    {
-      double p[7];
-      for (int k = 0; k < 7; ++k) p[k] = s_pose[k];
-      __syncthreads();
-      EvaluateAt3<false>(J, P, cloud, p, s_part, s_tot);
-    }
-    if (threadIdx.x == 0) {
-      const double candidate_cost = s_tot[0];
-      int cmd = kCmd3Rejected;
-      double diff[7];
-      for (int k = 0; k < 7; ++k) diff[k] = S.x[k] - S.cand[k];
-      if (NormN(diff, 7) <= kParameterTolerance * (S.x_norm + kParameterTolerance)) {
-        S.termination = kTerm3ParameterTolerance;
-        cmd = kCmd3Done;
-      } else if (fabs(S.x_cost - candidate_cost) <= kFunctionTolerance * S.x_cost) {
-        S.termination = kTerm3FunctionTolerance;
-        cmd = kCmd3Done;
-      } else {
-        const double relative_decrease = (S.current_cost - candidate_cost) / S.model_cost_change;
-        const double historical_decrease =
-            (S.reference_cost - candidate_cost) / (S.acc_reference + S.model_cost_change);
-        const double step_quality = fmax(relative_decrease, historical_decrease);
-        if (step_quality > kMinRelativeDecrease) {
-          cmd = kCmd3Accept;
-          for (int k = 0; k < 7; ++k) S.x[k] = S.cand[k];
-          S.x_norm = NormN(S.x, 7);
-          const double t = 2.0 * step_quality - 1.0;
-          S.radius = S.radius / fmax(1.0 / 3.0, 1.0 - t * t * t);
-          S.radius = fmin(kMaxRadius, S.radius);
-          S.decrease_factor = 2.0;
-          S.reuse_diagonal = 0;
-          S.current_cost = candidate_cost;
-          S.acc_candidate += S.model_cost_change;
-          S.acc_reference += S.model_cost_change;
-          if (S.current_cost < S.ev_minimum_cost) {
-            S.ev_minimum_cost = S.current_cost;
-            S.num_nonmonotonic = 0;
-            S.candidate_cost_ev = S.current_cost;
-            S.acc_candidate = 0.;
-          } else {
-            ++S.num_nonmonotonic;
-            if (S.current_cost > S.candidate_cost_ev) {
-              S.candidate_cost_ev = S.current_cost;
-              S.acc_candidate = 0.;
-            }
-          }
-          if (S.num_nonmonotonic == max_nonmonotonic) {
-            S.reference_cost = S.candidate_cost_ev;
-            S.acc_reference = S.acc_candidate;
-          }
-        } else {
-          S.radius = S.radius / S.decrease_factor;
-          S.decrease_factor *= 2.0;
-          S.reuse_diagonal = 1;
-        }
-      }
-      s_cmd = cmd;
-    }
-    __syncthreads();
-    if (s_cmd == kCmd3Done) break;
-    if (s_cmd == kCmd3Accept) {
-      double p[7];
-      for (int k = 0; k < 7; ++k) p[k] = s_pose[k];
-      __syncthreads();
-      EvaluateAt3<true>(J, P, cloud, p, s_part, s_tot);
-      if (threadIdx.x == 0) {
-        S.x_cost = s_tot[0];
-        for (int a = 0; a < kRef3N; ++a) S.g[a] = s_tot[1 + a];
-        for (int a = 0; a < kRef3H; ++a) S.h[a] = s_tot[1 + kRef3N + a];
-        S.last_step_successful = 1;
-      }
-    }
-    __syncthreads();
-  }
-  if (threadIdx.x == 0) {
-    Ref3ResultDev out;
-    for (int k = 0; k < 7; ++k) out.pose[k] = S.best[k];
-    out.initial_cost = S.initial_cost;
-    out.final_cost = S.minimum_cost;
-    out.iterations = S.iteration;
-    out.num_successful_steps = S.successful;
-    out.termination = S.termination;
-    out.pad = 0;
-    results[blockIdx.x] = out;
-  }
+  TrustRegionMinimize(Match3D{J, P, cloud, s_part}, J.init, P.max_num_iterations,
+                      P.use_nonmonotonic_steps, S, s_tot, s_pose, s_cmd, results + blockIdx.x);
 }
 
 // Test hook: residuals (and tangent-space Jacobian rows) of one job at one pose.
@@ -732,7 +489,7 @@ csm_status csm_ceres_match3d_batch(const csm_ceres_job3d* jobs, int32_t num_jobs
   CSM_CUDA(cudaEventRecord(ctx->ev0, s));
   CSM_CUDA(cudaMemcpyAsync(d_up.p, h, up_bytes, cudaMemcpyHostToDevice, s));
   ProfBegin(ctx);
-  k_ceres_match3d<<<num_jobs, kRef3Threads, 0, s>>>(
+  k_ceres_match3d<<<num_jobs, kRefThreads, 0, s>>>(
       reinterpret_cast<const Ref3JobDev*>(d_up.as<char>() + off_jobs), P, d_up.as<float>(),
       d_out.as<Ref3ResultDev>());
   CSM_LAUNCH_CHECK();

@@ -22,9 +22,9 @@ SO = os.path.join(HERE, "_build", "librefine2d_emulation.so")
 @pytest.fixture(scope="module")
 def emu():
     src = os.path.join(HERE, "refine2d_emulation.cc")
-    cu = os.path.join(HERE, "..", "..", "cartographer_b200", "csrc", "refine2d.cu")
-    if not os.path.exists(SO) or os.path.getmtime(SO) < max(os.path.getmtime(src),
-                                                           os.path.getmtime(cu)):
+    csrc = os.path.join(HERE, "..", "..", "cartographer_b200", "csrc")
+    deps = [src] + [os.path.join(csrc, f) for f in ("refine2d.cu", "trust_region.cuh")]
+    if not os.path.exists(SO) or os.path.getmtime(SO) < max(map(os.path.getmtime, deps)):
         os.makedirs(os.path.dirname(SO), exist_ok=True)
         subprocess.check_call(["g++", "-std=c++17", "-O2", "-ffp-contract=off", "-fPIC", "-shared",
                                "-pthread", "-w", "-x", "c++", src, "-o", SO])
