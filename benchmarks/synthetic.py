@@ -433,3 +433,43 @@ def make_node3d(world, rng, rings=16, azimuths=2048, max_range=20.0, seed=0, his
                           max_range=max_range, seed=seed)
     return dict(pose=yaw_pose7(*pose), cloud=cloud, low=voxel_downsample(cloud, lo_res),
                 hist=rotational_histogram(cloud, hist_size))
+
+
+def surface_intensity(world, points_world, seed=0, bright_fraction=0.01):
+    """Per-point intensities of world-frame points on the building's surfaces: each 0.5 m
+    block of the occupancy volume has one seeded reflectivity in [10, 90), each return adds
+    N(0, 2) noise, and `bright_fraction` of them are retroreflections at 200.  Draws from its
+    own RNG streams, so no other generator's output depends on it."""
+    occ, cell, origin = world[0], world[1], world[2]
+    block = max(1, int(round(0.5 / cell)))
+    shape = tuple(-(-s // block) for s in occ.shape)
+    table = np.random.RandomState(seed + 60013).uniform(10.0, 90.0, shape).astype(np.float32)
+    c = np.floor((np.asarray(points_world, np.float64) - origin) / cell).astype(np.int64) // block
+    for a, s in zip((0, 1, 2), (shape[2], shape[1], shape[0])):
+        c[:, a] = np.clip(c[:, a], 0, s - 1)
+    rng = np.random.RandomState(seed + 60017)
+    v = table[c[:, 2], c[:, 1], c[:, 0]] + rng.normal(0.0, 2.0, len(c)).astype(np.float32)
+    v[rng.uniform(size=len(c)) < bright_fraction] = 200.0
+    return np.maximum(v, 0.0).astype(np.float32)
+
+
+def make_intensity_grid3d(hybrid_grid, world, seed=0):
+    """An IntensityHybridGrid over the voxels of `hybrid_grid` (the submap's high-resolution
+    grid): each voxel averages 1-3 returns of its surface's intensity (surface_intensity
+    without retroreflections), as AverageIntensityData {sum, count}."""
+    from cartographer_b200.scan_matching import IntensityGridSpec
+    idx = hybrid_grid.indices
+    centres = idx.astype(np.float64) * hybrid_grid.resolution
+    counts = np.random.RandomState(seed + 60019).randint(1, 4, len(idx)).astype(np.int32)
+    mean = surface_intensity(world, centres, seed, bright_fraction=0.0)
+    sums = (mean * counts).astype(np.float32)
+    return IntensityGridSpec(hybrid_grid.resolution, idx, sums, counts)
+
+
+def node_intensities(world, node, seed=0):
+    """PointCloud::intensities() of a make_node3d scan: surface_intensity at its world points."""
+    p = node["pose"]
+    yaw = 2.0 * math.atan2(p[6], p[3])
+    c, s = math.cos(yaw), math.sin(yaw)
+    w = node["cloud"].astype(np.float64) @ np.array([[c, -s, 0], [s, c, 0], [0, 0, 1]]).T + p[:3]
+    return surface_intensity(world, w, seed)

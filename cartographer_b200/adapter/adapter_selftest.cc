@@ -325,6 +325,32 @@ int main() {
                 refined_pose.rotation().z(), summary3.initial_cost, summary3.final_cost,
                 summary3.iterations, summary3.num_successful_steps, summary3.termination);
     if (!(summary3.final_cost <= summary3.initial_cost)) return 1;
+
+    // ... with an intensity block on the pair (ceres_scan_matcher_3d.cc:123-139): intensity
+    // 50 at the cloud's cells, one retroreflection above the threshold
+    mapping::IntensityHybridGrid intensity_grid(0.05f);
+    for (const auto& v : hybrid.voxels()) intensity_grid.AddIntensity(v.x, v.y, v.z, 50.f);
+    std::vector<float> intensities(data.high_resolution_point_cloud.size(), 50.f);
+    intensities[3] = 150.f;
+    const sensor::PointCloud cloud_i(data.high_resolution_point_cloud.points(), intensities);
+    const mapping::scan_matching::DeviceIntensityGrid device_intensity(intensity_grid);
+    mapping::scan_matching::proto::CeresScanMatcherOptions3D oi =
+        bo.ceres_scan_matcher_options_3d();
+    oi.mutable_intensity_cost_function_options(0)->set_weight(0.5);
+    oi.mutable_intensity_cost_function_options(0)->set_huber_scale(0.3);
+    oi.mutable_intensity_cost_function_options(0)->set_intensity_threshold(100.f);
+    mapping::scan_matching::CeresScanMatcher3D ceres3i(oi);
+    ceres3i.Match(start.translation(), start, {{&cloud_i, &device_grid, &device_intensity}},
+                  &refined_pose, &summary3);
+    std::printf(
+        "RESULT ceres3d_intensity %.17g %.17g %.17g %.17g %.17g %.17g %.17g %.17g %.17g %d %d "
+        "%d\n",
+        refined_pose.translation().x(), refined_pose.translation().y(),
+        refined_pose.translation().z(), refined_pose.rotation().w(), refined_pose.rotation().x(),
+        refined_pose.rotation().y(), refined_pose.rotation().z(), summary3.initial_cost,
+        summary3.final_cost, summary3.iterations, summary3.num_successful_steps,
+        summary3.termination);
+    if (!(summary3.final_cost <= summary3.initial_cost)) return 1;
   }
   return 0;
 }

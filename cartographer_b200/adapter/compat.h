@@ -13,6 +13,7 @@
 #include <cstdint>
 #include <functional>
 #include <memory>
+#include <utility>
 #include <vector>
 
 namespace cartographer {
@@ -54,11 +55,16 @@ namespace sensor {
 struct RangefinderPoint { struct { float v[3]; float x() const { return v[0]; } float y() const { return v[1]; } float z() const { return v[2]; } } position; };
 class PointCloud {
  public:
+  PointCloud() = default;
+  PointCloud(std::vector<RangefinderPoint> points, std::vector<float> intensities)
+      : points_(std::move(points)), intensities_(std::move(intensities)) {}
   void push_back(const RangefinderPoint& p) { points_.push_back(p); }
   size_t size() const { return points_.size(); }
   const std::vector<RangefinderPoint>& points() const { return points_; }
+  const std::vector<float>& intensities() const { return intensities_; }
  private:
   std::vector<RangefinderPoint> points_;
+  std::vector<float> intensities_;
 };
 }  // namespace sensor
 
@@ -102,6 +108,27 @@ class HybridGrid {
  private:
   float resolution_;
   int grid_size_ = 128;
+  std::vector<Voxel> voxels_;
+};
+// mapping/3d/hybrid_grid.h:547-570: AddIntensity and iteration over the voxels'
+// AverageIntensityData {sum, count}.
+class IntensityHybridGrid {
+ public:
+  struct Voxel { int x, y, z; float sum; int count; };
+  explicit IntensityHybridGrid(float resolution) : resolution_(resolution) {}
+  float resolution() const { return resolution_; }
+  void AddIntensity(int x, int y, int z, float intensity) {
+    for (Voxel& v : voxels_)
+      if (v.x == x && v.y == y && v.z == z) {
+        v.count += 1;
+        v.sum += intensity;
+        return;
+      }
+    voxels_.push_back(Voxel{x, y, z, intensity, 1});
+  }
+  const std::vector<Voxel>& voxels() const { return voxels_; }
+ private:
+  float resolution_;
   std::vector<Voxel> voxels_;
 };
 // mapping/trajectory_node.h:45-63 (the fields the 3D matcher reads).
@@ -257,10 +284,29 @@ class CeresScanMatcherOptions2D {
   double occupied_ = 20., translation_ = 10., rotation_ = 1.;
   CeresSolverOptions solver_;
 };
+// proto/scan_matching/ceres_scan_matcher_options_3d.proto:21-26
+class IntensityCostFunctionOptions {
+ public:
+  double weight() const { return weight_; }
+  double huber_scale() const { return huber_scale_; }
+  float intensity_threshold() const { return intensity_threshold_; }
+  void set_weight(double v) { weight_ = v; }
+  void set_huber_scale(double v) { huber_scale_ = v; }
+  void set_intensity_threshold(float v) { intensity_threshold_ = v; }
+ private:
+  double weight_ = 0., huber_scale_ = 0.;
+  float intensity_threshold_ = 0.f;
+};
 // proto/scan_matching/ceres_scan_matcher_options_3d.proto (defaults: pose_graph.lua:49-60)
 class CeresScanMatcherOptions3D {
  public:
   int occupied_space_weight_size() const { return 2; }
+  const IntensityCostFunctionOptions& intensity_cost_function_options(int i) const {
+    return intensity_[i];
+  }
+  IntensityCostFunctionOptions* mutable_intensity_cost_function_options(int i) {
+    return &intensity_[i];
+  }
   double occupied_space_weight(int i) const { return occupied_[i]; }
   double translation_weight() const { return translation_; }
   double rotation_weight() const { return rotation_; }
@@ -276,6 +322,7 @@ class CeresScanMatcherOptions3D {
   void set_rotation_weight(double v) { rotation_ = v; }
  private:
   double occupied_[2] = {5., 30.};
+  IntensityCostFunctionOptions intensity_[2];
   double translation_ = 10., rotation_ = 1.;
   bool only_optimize_yaw_ = false;
   CeresScanMatcherOptions2D::CeresSolverOptions solver_{false, 10, 1};

@@ -23,4 +23,15 @@ struct csm_grid3d {
   ~csm_grid3d() { cudaFree(d_vol); }
 };
 
+// The dense device copy of an IntensityHybridGrid (refine3d.cu): GetIntensity per voxel of
+// the bounding box of the voxels it was made from, 0 elsewhere.
+struct csm_intensity_grid3d {
+  csm::Ctx* ctx = nullptr;
+  float* d_vol = nullptr;
+  int lo[3] = {0, 0, 0};
+  int n[3] = {0, 0, 0};
+  float resolution = 0.f;
+  ~csm_intensity_grid3d() { cudaFree(d_vol); }
+};
+
 #endif  // CSM_GRID3D_CUH_

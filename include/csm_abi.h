@@ -497,8 +497,9 @@ csm_status csm_rt_match3d(const csm_grid3d* grid, const float* xyz, int32_t num_
  * smoothstep-interpolated grid (occupied_space_cost_function_3d.h:68-78,
  * interpolated_grid.h:49-96), a translation prior and a rotation prior
  * (translation_delta_cost_functor_3d.h, rotation_delta_cost_functor_3d.h:42-53), minimised over
- * {translation[3], rotation[4]} with ceres::QuaternionParameterization.  No intensity grids
- * (the constraint builder passes none) and only_optimize_yaw must be 0.  Same solver notes as
+ * {translation[3], rotation[4]} with ceres::QuaternionParameterization.  Intensity grids
+ * (which the constraint builder does not pass): csm_ceres_match3d_intensity_batch below.
+ * only_optimize_yaw must be 0.  Same solver notes as
  * csm_ceres_match2d_batch; grids are csm_grid3d handles.  Poses are {t xyz, q wxyz}. */
 typedef struct csm_ceres_options3d {
   double occupied_space_weight[2]; /* occupied_space_weight_0 / _1 */
@@ -536,6 +537,57 @@ csm_status csm_ceres_match3d_batch(const csm_ceres_job3d* jobs, int32_t num_jobs
  * {dt[3], dq[3]}; the rotation prior's target is job->initial_pose's rotation. */
 csm_status csm_ceres_evaluate3d(const csm_ceres_job3d* job, const csm_ceres_options3d* options,
                                 const double pose[7], double* residuals, double* jacobian);
+
+/* ---- intensity residuals in 3D: IntensityCostFunction3D under HuberLoss ---------- */
+/* An IntensityHybridGrid resident on the device (mapping/3d/hybrid_grid.h:547-570), from the
+ * flat form HybridGridBase<AverageIntensityData>::Iterator gives: voxel indices (n x 3, as
+ * csm_grid3d_create), sum[n] and count[n] of each voxel's AverageIntensityData, no index
+ * twice.  Each voxel holds GetIntensity (sum / count in float, 0 where count == 0); reads
+ * outside the voxels' bounding box return 0, and a grid of no voxels reads 0 everywhere. */
+typedef struct csm_intensity_grid3d csm_intensity_grid3d;
+csm_status csm_intensity_grid3d_create(const int32_t* indices, const float* sum,
+                                       const int32_t* count, int64_t num_voxels,
+                                       float resolution, int32_t device,
+                                       csm_intensity_grid3d** out);
+csm_status csm_intensity_grid3d_destroy(csm_intensity_grid3d* grid);
+
+/* Per csm_ceres_job3d: PointCloudAndHybridGridsPointers::intensity_hybrid_grid of each cloud
+ * (NULL: that cloud has no intensity block) and its PointCloud::intensities()
+ * (num_points[b] floats, host memory; required where the grid is set). */
+typedef struct csm_ceres_intensity_job3d {
+  const csm_intensity_grid3d* intensity_grid[2];
+  const float* intensities[2];
+} csm_ceres_intensity_job3d;
+
+/* intensity_cost_function_options_0 / _1 (ceres_scan_matcher_options_3d.proto:24-25,42-43);
+ * each must be positive for a cloud that has an intensity block in the batch. */
+typedef struct csm_ceres_intensity_options3d {
+  double weight[2];
+  double huber_scale[2];
+  float intensity_threshold[2];    /* returns brighter than this are left out */
+} csm_ceres_intensity_options3d;
+
+/* csm_ceres_match3d_batch where cloud b of job j may carry an intensity block
+ * (ceres_scan_matcher_3d.cc:123-139): IntensityCostFunction3D with scaling weight / sqrt(n)
+ * under ceres::HuberLoss(huber_scale), after that cloud's occupied-space block.  Jobs with
+ * and without intensity blocks may share a batch; a job without one gives what
+ * csm_ceres_match3d_batch gives, bit for bit. */
+csm_status csm_ceres_match3d_intensity_batch(
+    const csm_ceres_job3d* jobs, const csm_ceres_intensity_job3d* intensity_jobs,
+    int32_t num_jobs, const csm_ceres_options3d* options,
+    const csm_ceres_intensity_options3d* intensity_options, csm_ceres_result3d* results,
+    csm_stats* stats /* may be NULL */);
+
+/* Test hook: as csm_ceres_evaluate3d, in the problem's residual-block order — per cloud its
+ * occupied-space residuals, then its intensity residuals if it has a grid; then 3
+ * translation and 3 rotation residuals.  Residuals and rows are uncorrected by the loss, as
+ * CostFunction::Evaluate returns them. */
+csm_status csm_ceres_evaluate3d_intensity(const csm_ceres_job3d* job,
+                                          const csm_ceres_intensity_job3d* intensity_job,
+                                          const csm_ceres_options3d* options,
+                                          const csm_ceres_intensity_options3d* intensity_options,
+                                          const double pose[7], double* residuals,
+                                          double* jacobian);
 
 /* ==== multi-GPU: one process per GPU, the sharded ConstraintBuilder queue ==== */
 /* Every (submap, node) search only depends on its submap's matcher
