@@ -1801,15 +1801,39 @@ struct BatchPlan {
 
 struct TieLeaf { int scan, xo, yo; };
 
+// Test hooks csm_score_top2d / csm_branch_step2d: a batch of one job that stops after its
+// lowest-resolution pass (level == 0), or that runs one branch step over caller-given
+// parents in place of the level loop (level >= 1).  The form fields override the
+// CSM_TOP_KERNEL / CSM_NO_LATTICE / CSM_LAT_UNROLL switches for this call only.
+struct Probe2D {
+  int level = 0;
+  const char* top_form = nullptr;  // as CSM_TOP_KERNEL; nullptr = the size-based choice
+  bool lattice = false;
+  int unroll = 8;
+  const csm_node2d* parents = nullptr;
+  int num_parents = 0;
+  float bound = 0.f;
+  // results
+  std::vector<int> top_sums;
+  int cap = 0;  // slots per scan in top_sums
+  std::vector<ScanInfo> info;
+  int top_kernel = 0;  // form that ran: 1 small, 2 gather, 3 tile, 4 dense
+  int tile_iters = 0;  // K of k_score_top_tile<K> (0 for the other forms)
+  std::vector<Node> out;  // pushed children (level >= 2) or recorded leaves (level 1)
+  float final_bound = 0.f;
+  unsigned long long counters[2] = {0, 0};
+};
+
 }  // namespace
 
-// Runs a batch of independent matches.  `with_search` == false stops after
-// discretisation (test hook csm_discretize2d).
+// Runs a batch of independent matches.  `discretize_only` stops after discretisation
+// (test hook csm_discretize2d); `probe` (may be null) turns the call into a Probe2D.
 static csm_status RunBatch2D(Ctx* ctx, const csm_stack2d* const* stacks, int num_stacks,
                              const csm_cloud* const* clouds, int num_clouds,
                              const csm_job2d* jobs, int num_jobs, double linear_window,
                              double angular_window, csm_result2d* results, csm_stats* total,
-                             bool discretize_only, int32_t* out_dscan, int32_t* out_bounds) {
+                             bool discretize_only, int32_t* out_dscan, int32_t* out_bounds,
+                             Probe2D* probe = nullptr) {
   CSM_CUDA(cudaSetDevice(ctx->device));
   cudaStream_t s = ctx->stream;
   static const bool timing = getenv("CSM_TIMING") != nullptr;
@@ -2011,7 +2035,8 @@ static csm_status RunBatch2D(Ctx* ctx, const csm_stack2d* const* stacks, int num
   CSM_TRY(d_top.Reserve(sizeof(int) * plan.total_slots));
   // Wide lattices (MatchFullSubmap) take the dense decimated-grid kernel; narrow
   // ones (local windows: a few dozen candidates per scan) the gather kernel.
-  static const char* force = getenv("CSM_TOP_KERNEL");  // "small" | "gather" | "tile" | "dense" (debug)
+  static const char* env_force = getenv("CSM_TOP_KERNEL");  // "small" | "gather" | "tile" | "dense" (debug)
+  const char* force = probe ? probe->top_form : env_force;
   int max_cap = 0, max_cap_x = 0, max_cap_y = 0;
   for (const JobDev& d : plan.jobs) {
     max_cap = std::max(max_cap, d.cap);
@@ -2069,6 +2094,7 @@ static csm_status RunBatch2D(Ctx* ctx, const csm_stack2d* const* stacks, int num
       k_score_top_tile<K><<<grid, kTileThreads, smem, s>>>(                                  \
           d_jobs.as<JobDev>(), d_info.as<ScanInfo>(), d_dscan.as<short2>(), d_top.as<int>(), \
           d_slot_base.as<long long>(), total_scans, lat_ints);                               \
+      if (probe) probe->tile_iters = K;                                                      \
     } while (0)
     if (tile_words <= 32) CSM_TILE(1);
     else if (tile_words <= 64) CSM_TILE(2);
@@ -2085,12 +2111,30 @@ static csm_status RunBatch2D(Ctx* ctx, const csm_stack2d* const* stacks, int num
         d_slot_base.as<long long>(), total_scans);
   }
   CSM_LAUNCH_CHECK();
+  if (probe) probe->top_kernel = use_small_top ? 1 : use_gather_top ? 2 : use_tile_top ? 3 : 4;
   if (g_profile_on.load()) {
     unsigned long long c3 = 0;
     ProfStop(ctx);
     CSM_CUDA(cudaStreamSynchronize(s));
     CSM_CUDA(cudaMemcpy(&c3, ctr + 3, sizeof(c3), cudaMemcpyDeviceToHost));
     ProfCommit(ctx, top_name, static_cast<double>(c3));
+  }
+  if (probe && probe->level == 0) {
+    unsigned long long err[2] = {0, 0};
+    probe->cap = plan.jobs[0].cap;
+    probe->top_sums.resize(plan.total_slots);
+    probe->info.resize(total_scans);
+    CSM_CUDA(cudaMemcpyAsync(probe->top_sums.data(), d_top.p, sizeof(int) * plan.total_slots,
+                             cudaMemcpyDeviceToHost, s));
+    CSM_CUDA(cudaMemcpyAsync(probe->info.data(), d_info.p, sizeof(ScanInfo) * total_scans,
+                             cudaMemcpyDeviceToHost, s));
+    CSM_CUDA(cudaMemcpyAsync(err, ctr + 6, sizeof(err), cudaMemcpyDeviceToHost, s));
+    CSM_CUDA(cudaStreamSynchronize(s));
+    if (err[0] || err[1]) {
+      SetError("a scan's lattice or cell indices exceed the engine's limits");
+      return CSM_E_CAPACITY;
+    }
+    return CSM_OK;
   }
 
   phase("top pass");
@@ -2162,6 +2206,8 @@ static csm_status RunBatch2D(Ctx* ctx, const csm_stack2d* const* stacks, int num
   CSM_TRY(d_items.Reserve(sizeof(WorkItem) * (static_cast<size_t>(kChunk) / 32 + total_scans + 2)));
   CSM_TRY(d_sorted.Reserve(sizeof(Node) * static_cast<size_t>(kChunk)));
   static const bool use_lattice = getenv("CSM_NO_LATTICE") == nullptr;
+  const int lattice_min = probe ? (probe->lattice ? 1 : INT_MAX)
+                                : (use_lattice ? kLatticeMin : INT_MAX);
   auto queue_ptr = [&](int h) -> Node* {
     return h == hmax ? d_qtop.as<Node>() : d_q.as<Node>() + static_cast<size_t>(kQueueCap) * h;
   };
@@ -2199,7 +2245,8 @@ static csm_status RunBatch2D(Ctx* ctx, const csm_stack2d* const* stacks, int num
   const int nb = DivUp(total_scans, 1024);
   const int sort_grid = ctx->sm_count * 8;
   const int max_items = kChunk / 32 + std::min(kChunk, total_scans) + 1;
-  static const int lat_unroll = getenv("CSM_LAT_UNROLL") ? atoi(getenv("CSM_LAT_UNROLL")) : 8;
+  static const int env_unroll = getenv("CSM_LAT_UNROLL") ? atoi(getenv("CSM_LAT_UNROLL")) : 8;
+  const int lat_unroll = probe ? probe->unroll : env_unroll;
   {
     // The lattice kernel's shared-memory carve-out: just what CSM_LAT_MINB CTAs need, so the
     // rest of the unified L1 caches the window tables, which its loads are bound by.  On an
@@ -2223,7 +2270,7 @@ static csm_status RunBatch2D(Ctx* ctx, const csm_stack2d* const* stacks, int num
     int* part_b = part_a + nb;
     Node* next = h - 1 >= 1 ? queue_ptr(h - 1) : nullptr;
     int* next_count = ictr + (h - 1 >= 1 ? h - 1 : 31);
-    k_level_begin<<<1, 32, 0, s>>>(ictr, h, kChunk, use_lattice ? kLatticeMin : INT_MAX);
+    k_level_begin<<<1, 32, 0, s>>>(ictr, h, kChunk, lattice_min);
     CSM_LAUNCH_CHECK();
     CSM_CUDA(cudaMemsetAsync(d_scan_cnt.p, 0, sizeof(int) * 2 * total_scans, s));
     ProfBegin(ctx);
@@ -2292,6 +2339,61 @@ static csm_status RunBatch2D(Ctx* ctx, const csm_stack2d* const* stacks, int num
     return CSM_OK;
   };
 
+  if (probe) {
+    // one level_step over the caller's parents: the level-loop state is reset to them
+    const int h = probe->level, n = probe->num_parents;
+    CSM_REQUIRE(h >= 1 && h <= hmax, "level out of range");
+    CSM_REQUIRE(n >= 0 && n <= std::min(queue_cap(h), kChunk), "number of parents");
+    h_info.resize(total_scans);
+    CSM_CUDA(cudaMemcpyAsync(h_info.data(), d_info.p, sizeof(ScanInfo) * total_scans,
+                             cudaMemcpyDeviceToHost, s));
+    CSM_CUDA(cudaStreamSynchronize(s));
+    std::vector<Node> parents(n);
+    for (int i = 0; i < n; ++i) {
+      const csm_node2d& p = probe->parents[i];
+      CSM_REQUIRE(p.scan_index >= 0 && p.scan_index < total_scans, "parent scan_index");
+      const ScanInfo& si = h_info[p.scan_index];
+      const int dx = p.x_index_offset - si.min_x, dy = p.y_index_offset - si.min_y;
+      CSM_REQUIRE(dx >= 0 && dy >= 0 && (dx & ((1 << h) - 1)) == 0 && (dy & ((1 << h) - 1)) == 0 &&
+                  p.x_index_offset <= si.max_x && p.y_index_offset <= si.max_y,
+                  "parent is not a node of its scan's level lattice");
+      parents[i] = Node{p.scan_index, p.x_index_offset, p.y_index_offset, p.score};
+    }
+    const unsigned bound = HostFloatToOrdered(probe->bound);
+    CSM_CUDA(cudaMemsetAsync(ictr, 0, sizeof(int) * kCtlInts, s));
+    CSM_CUDA(cudaMemsetAsync(ctr, 0, sizeof(unsigned long long) * 2, s));
+    CSM_CUDA(cudaMemcpyAsync(ictr + h, &n, sizeof(int), cudaMemcpyHostToDevice, s));
+    CSM_CUDA(cudaMemcpyAsync(d_lb.p, &bound, sizeof(unsigned), cudaMemcpyHostToDevice, s));
+    if (n)
+      CSM_CUDA(cudaMemcpyAsync(queue_ptr(h), parents.data(), sizeof(Node) * n,
+                               cudaMemcpyHostToDevice, s));
+    prof_c0 = 0;
+    CSM_TRY(level_step(h));
+    int ctl[kCtlInts];
+    unsigned long long c[8];
+    unsigned lb_out = 0;
+    CSM_CUDA(cudaMemcpyAsync(ctl, ictr, sizeof(ctl), cudaMemcpyDeviceToHost, s));
+    CSM_CUDA(cudaMemcpyAsync(c, ctr, sizeof(c), cudaMemcpyDeviceToHost, s));
+    CSM_CUDA(cudaMemcpyAsync(&lb_out, d_lb.p, sizeof(unsigned), cudaMemcpyDeviceToHost, s));
+    CSM_CUDA(cudaStreamSynchronize(s));
+    if (c[6] || c[7]) {
+      SetError("a scan's lattice or cell indices exceed the engine's limits");
+      return CSM_E_CAPACITY;
+    }
+    const int cnt = h >= 2 ? ctl[h - 1] : ctl[kCtlLeaf];
+    if (ctl[kCtlOverflow] || cnt > 4 * n) {
+      SetError("internal: more children than 4 per parent");
+      return CSM_E_CAPACITY;
+    }
+    probe->out.resize(cnt);
+    if (cnt)
+      CSM_CUDA(cudaMemcpy(probe->out.data(), h >= 2 ? queue_ptr(h - 1) : d_leaves.as<Node>(),
+                          sizeof(Node) * cnt, cudaMemcpyDeviceToHost));
+    probe->final_bound = HostOrderedToFloat(lb_out);
+    probe->counters[0] = c[0];
+    probe->counters[1] = c[1];
+    return CSM_OK;
+  }
   for (int h = hmax; h >= 1; --h) CSM_TRY(level_step(h));
   CSM_TRY(collect());
   // frontiers larger than one chunk (rare): continue deepest non-empty level first
@@ -2610,6 +2712,94 @@ csm_status csm_discretize2d(const csm_stack2d* stack, const float* xyz, int32_t 
   }
   csm_cloud_destroy(cloud);
   return st;
+}
+
+}  // extern "C"
+
+// Runs `probe` on the match csm_match2d would run with these arguments.
+static csm_status RunProbe2D(const csm_stack2d* stack, const float* xyz, int32_t n,
+                             const double initial_pose[3], int32_t full_submap,
+                             double linear_window, double angular_window, float min_score,
+                             Probe2D* probe) {
+  CSM_REQUIRE(stack && xyz, "null pointer");
+  CSM_REQUIRE(full_submap || initial_pose, "null initial pose");
+  csm_cloud* cloud = nullptr;
+  CSM_TRY(csm_cloud_create(xyz, n, stack->ctx->device, &cloud));
+  csm_job2d job;
+  std::memset(&job, 0, sizeof(job));
+  job.full_submap = full_submap;
+  if (initial_pose) std::memcpy(job.initial_pose, initial_pose, sizeof(double) * 3);
+  job.min_score = min_score;
+  const csm_cloud* cl = cloud;
+  LaneGuard guard;
+  csm_status st = AcquireLane(stack->ctx->device, &guard);
+  if (st == CSM_OK)
+    st = RunBatch2D(guard.lane, &stack, 1, &cl, 1, &job, 1, linear_window, angular_window,
+                    nullptr, nullptr, false, nullptr, nullptr, probe);
+  csm_cloud_destroy(cloud);
+  return st;
+}
+
+extern "C" {
+
+csm_status csm_score_top2d(const csm_stack2d* stack, const float* xyz, int32_t n,
+                           const double initial_pose[3], int32_t full_submap,
+                           double linear_window, double angular_window, int32_t form,
+                           int32_t* num_scans, int32_t* slots_per_scan, int32_t* sums,
+                           int32_t* lattices, int32_t* kernel) {
+  static const char* const kForms[] = {nullptr, "small", "gather", "tile", "dense"};
+  CSM_REQUIRE(num_scans && slots_per_scan, "null pointer");
+  CSM_REQUIRE(form >= 0 && form <= 4, "form");
+  Probe2D probe;
+  probe.top_form = kForms[form];
+  CSM_TRY(RunProbe2D(stack, xyz, n, initial_pose, full_submap, linear_window, angular_window,
+                     0.f, &probe));
+  const int S = static_cast<int>(probe.info.size());
+  *num_scans = S;
+  *slots_per_scan = probe.cap;
+  if (sums) std::memcpy(sums, probe.top_sums.data(), sizeof(int) * probe.top_sums.size());
+  if (lattices)
+    for (int i = 0; i < S; ++i) {
+      const ScanInfo& si = probe.info[i];
+      const int32_t v[6] = {si.min_x, si.max_x, si.min_y, si.max_y, si.nxc, si.nyc};
+      std::memcpy(lattices + 6 * i, v, sizeof(v));
+    }
+  if (kernel) {
+    kernel[0] = probe.top_kernel;
+    kernel[1] = probe.tile_iters;
+  }
+  return CSM_OK;
+}
+
+csm_status csm_branch_step2d(const csm_stack2d* stack, const float* xyz, int32_t n,
+                             const double initial_pose[3], int32_t full_submap,
+                             double linear_window, double angular_window, float min_score,
+                             int32_t level, const csm_node2d* parents, int32_t num_parents,
+                             float bound, int32_t form, int32_t unroll, csm_node2d* children,
+                             int32_t* num_children, float* final_bound, int64_t counters[2]) {
+  CSM_REQUIRE(children && num_children && final_bound && counters, "null pointer");
+  CSM_REQUIRE(parents || num_parents == 0, "null parents");
+  CSM_REQUIRE(level >= 1, "level out of range");
+  CSM_REQUIRE(form == 0 || form == 1, "form");
+  CSM_REQUIRE(unroll == 4 || unroll == 8 || unroll == 16, "unroll");
+  Probe2D probe;
+  probe.level = level;
+  probe.lattice = form == 1;
+  probe.unroll = unroll;
+  probe.parents = parents;
+  probe.num_parents = num_parents;
+  probe.bound = bound;
+  CSM_TRY(RunProbe2D(stack, xyz, n, initial_pose, full_submap, linear_window, angular_window,
+                     min_score, &probe));
+  *num_children = static_cast<int32_t>(probe.out.size());
+  for (size_t i = 0; i < probe.out.size(); ++i) {
+    const Node& c = probe.out[i];
+    children[i] = csm_node2d{c.scan, c.xo, c.yo, c.score};
+  }
+  *final_bound = probe.final_bound;
+  counters[0] = static_cast<int64_t>(probe.counters[0]);
+  counters[1] = static_cast<int64_t>(probe.counters[1]);
+  return CSM_OK;
 }
 
 csm_status csm_score_candidates2d(const csm_stack2d* stack, int32_t level,

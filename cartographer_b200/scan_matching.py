@@ -13,6 +13,9 @@ import numpy as np
 from . import _lib
 from ._lib import CsmStats, JOB2D_DTYPE, RESULT2D_DTYPE, check, lib, ptr
 
+# csm_node2d: a branch-and-bound frontier node
+NODE2D_DTYPE = np.dtype([("scan", "<i4"), ("xo", "<i4"), ("yo", "<i4"), ("score", "<f4")])
+
 
 @dataclass
 class FastCorrelativeScanMatcherOptions2D:
@@ -167,6 +170,51 @@ class FastCorrelativeScanMatcher2D:
         bounds = np.empty((S.value, 4), np.int32)
         check(lib().csm_discretize2d(*args, ptr(ds, C.c_int32), ptr(bounds, C.c_int32)))
         return ds, bounds
+
+    TOP_FORMS = ("auto", "small", "gather", "tile", "dense")
+
+    def score_top(self, point_cloud, initial_pose_estimate=(0.0, 0.0, 0.0), full_submap=False,
+                  form="auto"):
+        """csm_score_top2d: the lowest-resolution sums of the match's candidates.
+        -> (sums, lattices, kernel): sums[scan] is the scan's nxc * nyc sums in slot order
+        (slot = i * nyc + j), lattices is num_scans x (min_x, max_x, min_y, max_y, nxc, nyc),
+        kernel = (form that ran, K of k_score_top_tile<K> or 0)."""
+        xyz = _f32(point_cloud)
+        ip = np.ascontiguousarray(initial_pose_estimate, dtype=np.float64)
+        S, cap = C.c_int32(0), C.c_int32(0)
+        args = (self._h, ptr(xyz, C.c_float), C.c_int32(len(xyz)), ptr(ip, C.c_double),
+                C.c_int32(int(full_submap)), C.c_double(self.options.linear_search_window),
+                C.c_double(self.options.angular_search_window),
+                C.c_int32(self.TOP_FORMS.index(form)), C.byref(S), C.byref(cap))
+        check(lib().csm_score_top2d(*args, None, None, None))
+        sums = np.zeros((S.value, cap.value), np.int32)
+        lattices = np.zeros((S.value, 6), np.int32)
+        kernel = np.zeros(2, np.int32)
+        check(lib().csm_score_top2d(*args, ptr(sums, C.c_int32), ptr(lattices, C.c_int32),
+                                    ptr(kernel, C.c_int32)))
+        return ([sums[k, :nxc * nyc] for k, (_, _, _, _, nxc, nyc) in enumerate(lattices)],
+                lattices, (self.TOP_FORMS[kernel[0]], int(kernel[1])))
+
+    def branch_step(self, point_cloud, initial_pose_estimate, full_submap, min_score, level,
+                    parents, bound, form, unroll=8):
+        """csm_branch_step2d: one branch step over `parents` (NODE2D_DTYPE records) at
+        `level` with the job's bound set to `bound`; form "warp" or "lattice".
+        -> (children in queue order, final bound, (candidates scored, parents expanded))."""
+        xyz = _f32(point_cloud)
+        ip = np.ascontiguousarray(initial_pose_estimate, dtype=np.float64)
+        par = np.ascontiguousarray(parents, dtype=NODE2D_DTYPE)
+        out = np.zeros(max(1, 4 * len(par)), NODE2D_DTYPE)
+        count, final = C.c_int32(0), C.c_float(0.0)
+        ctr = np.zeros(2, np.int64)
+        check(lib().csm_branch_step2d(
+            self._h, ptr(xyz, C.c_float), C.c_int32(len(xyz)), ptr(ip, C.c_double),
+            C.c_int32(int(full_submap)), C.c_double(self.options.linear_search_window),
+            C.c_double(self.options.angular_search_window), C.c_float(min_score),
+            C.c_int32(level), par.ctypes.data_as(C.c_void_p), C.c_int32(len(par)),
+            C.c_float(bound), C.c_int32(("warp", "lattice").index(form)), C.c_int32(unroll),
+            out.ctypes.data_as(C.c_void_p), C.byref(count), C.byref(final),
+            ptr(ctr, C.c_int64)))
+        return out[:count.value].copy(), np.float32(final.value), (int(ctr[0]), int(ctr[1]))
 
 
 def load_pbstream_matchers2d(path, options, device=0):
@@ -468,7 +516,7 @@ def device_count():
 __all__ = ["FastCorrelativeScanMatcherOptions2D", "RealTimeCorrelativeScanMatcherOptions",
            "FastCorrelativeScanMatcher2D", "RealTimeCorrelativeScanMatcher2D", "DeviceCloud",
            "match_batch", "load_pbstream_matchers2d", "match_batch_sharded", "MultiGpuContext", "RealTimeGrid2D",
-           "kernel_launch_count", "device_count", "JOB2D_DTYPE",
+           "kernel_launch_count", "device_count", "JOB2D_DTYPE", "NODE2D_DTYPE",
            "RESULT2D_DTYPE", "_lib"]
 
 

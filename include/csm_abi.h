@@ -193,6 +193,40 @@ csm_status csm_discretize2d(const csm_stack2d* stack, const float* xyz, int32_t 
                             const double initial_pose[3], int32_t full_submap,
                             double linear_search_window, double angular_search_window,
                             int32_t* num_scans, int32_t* discrete_scans, int32_t* bounds);
+/* The lowest-resolution pass of the same match (ScoreCandidates at depth - 1 over every
+ * candidate GenerateLowestResolutionCandidates makes, fast...2d.cc:281-312), run by the
+ * batch's own launch code.  form: 0 = the size-based choice a match makes, 1 = small,
+ * 2 = gather, 3 = tile, 4 = dense; a form that cannot serve the shape returns
+ * CSM_E_INVALID.  Call with sums == NULL to get *num_scans and *slots_per_scan first.
+ * sums is num_scans x slots_per_scan: the integer sum of candidate
+ * (min_x + i * 2^(depth-1), min_y + j * 2^(depth-1)) at slot i * nyc + j, slots past
+ * nxc * nyc unspecified.  lattices (may be NULL) is num_scans x
+ * {min_x, max_x, min_y, max_y, nxc, nyc}.  kernel (may be NULL) receives the form that
+ * ran (1 .. 4 as above) and, for the tile form, K of k_score_top_tile<K> (else 0). */
+csm_status csm_score_top2d(const csm_stack2d* stack, const float* xyz, int32_t num_points,
+                           const double initial_pose[3], int32_t full_submap,
+                           double linear_search_window, double angular_search_window,
+                           int32_t form, int32_t* num_scans, int32_t* slots_per_scan,
+                           int32_t* sums, int32_t* lattices, int32_t* kernel);
+/* A node of the branch-and-bound frontier: Candidate2D identity and score. */
+typedef struct csm_node2d {
+  int32_t scan_index, x_index_offset, y_index_offset;
+  float score;
+} csm_node2d;
+/* One branch step of the same match (the children loop of BranchAndBound,
+ * fast...2d.cc:335-376) over caller-given parents of level `level` (1 .. depth-1, on
+ * their scan's lattice of stride 2^level), with the job's bound set to `bound` first,
+ * run by the batch's own launch code.  form: 0 = one warp per parent, 1 = scan-grouped
+ * lattice kernel with `unroll` 4, 8 or 16.  children (4 * num_parents records) receives
+ * the pushed children in queue order (level >= 2) or the recorded leaves (level 1);
+ * final_bound the job's bound afterwards, counters {candidates scored, parents expanded}. */
+csm_status csm_branch_step2d(const csm_stack2d* stack, const float* xyz, int32_t num_points,
+                             const double initial_pose[3], int32_t full_submap,
+                             double linear_search_window, double angular_search_window,
+                             float min_score, int32_t level, const csm_node2d* parents,
+                             int32_t num_parents, float bound, int32_t form, int32_t unroll,
+                             csm_node2d* children, int32_t* num_children, float* final_bound,
+                             int64_t counters[2]);
 
 /* ---- RealTimeCorrelativeScanMatcher2D::Match ------------------------------ */
 /* real_time_correlative_scan_matcher_2d.cc:117-149 on a ProbabilityGrid (the
