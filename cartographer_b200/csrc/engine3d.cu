@@ -614,15 +614,20 @@ k3_collect(const Leaf3* __restrict__ leaves, const Scan3* __restrict__ scans,
   }
 }
 
-// scores an explicit candidate list (tie resolution): one CTA per candidate
+// scores an explicit candidate list (tie resolution): one CTA per candidate; `sums` (may be
+// null) also receives the integer sums (test hook csm_score_candidates3d)
 struct List3 { int scan, ox, oy, oz, depth; };
 __global__ void __launch_bounds__(kT3)
-k3_score_list(Job3 jb, const List3* __restrict__ cands, float* __restrict__ scores) {
+k3_score_list(Job3 jb, const List3* __restrict__ cands, float* __restrict__ scores,
+              int* __restrict__ sums_out) {
   __shared__ int s_red[kT3 / 32 * 8];
   const List3 c = cands[blockIdx.x];
   int sums[8];
   ScoreOct(jb, c.scan, c.depth, c.ox, c.oy, c.oz, 0, 1u, sums, s_red);
-  if (threadIdx.x == 0) scores[blockIdx.x] = ToScore3(sums[0], jb.n_hi);
+  if (threadIdx.x == 0) {
+    scores[blockIdx.x] = ToScore3(sums[0], jb.n_hi);
+    if (sums_out) sums_out[blockIdx.x] = sums[0];
+  }
 }
 
 }  // namespace csm
@@ -730,6 +735,33 @@ struct ScanPlan {
   std::vector<float> angles;
   std::vector<float> all_scores;
   int num_angles = 0;
+};
+
+// Test hooks csm_score_candidates3d / csm_score_top3d / csm_branch_step3d: a match that
+// scores a caller-given candidate list after discretisation (kList), stops after its dives
+// (kTop), or runs one level of the branch step over caller-given parents in place of the
+// level loop (kStep).
+struct Probe3D {
+  enum Mode { kList, kTop, kStep } mode = kTop;
+  // kList
+  const List3* list = nullptr;
+  int list_n = 0;
+  std::vector<int> sums;
+  std::vector<float> scores;
+  // kTop
+  int num_scans = 0, nxc = 0, nzc = 0, top_best = 0;
+  std::vector<int> angle, top_sums;
+  std::vector<float> rot;
+  // kStep
+  int level = 0;
+  const Node3* parents = nullptr;
+  int num_parents = 0;
+  float bound = 0.f;
+  std::vector<Node3> children;   // level >= 2
+  std::vector<Leaf3> leaves;     // level 1
+  // kTop and kStep: the bound afterwards, {candidates scored, parents expanded, gate evaluations}
+  float final_bound = 0.f;
+  unsigned long long counters[3] = {0, 0, 0};
 };
 
 }  // namespace
@@ -1055,13 +1087,13 @@ static csm_status MakeSearch3(const csm_matcher3d* m, float max_range, const dou
 }
 
 // One match = one stream of launches + one synchronisation.  `dev` (optional) carries the
-// node's clouds already on the device.
+// node's clouds already on the device.  `probe` (may be null) turns the call into a Probe3D.
 static csm_status Run3D(Ctx* ctx, const csm_matcher3d* m, const csm_node3d* node,
                         const NodeDev3* dev, const double node_pose[7],
                         const double submap_pose[7], int full, float min_score,
                         csm_result3d* result, csm_stats* stats, bool discretize_only,
                         int32_t* out_num_scans, int32_t* out_cells, float* out_poses,
-                        float* out_rot) {
+                        float* out_rot, Probe3D* probe = nullptr) {
   CSM_CUDA(cudaSetDevice(ctx->device));
   cudaStream_t s = ctx->stream;
   const float max_range = dev ? dev->max_range : MaxRange3(node);
@@ -1197,6 +1229,38 @@ static csm_status Run3D(Ctx* ctx, const csm_matcher3d* m, const csm_node3d* node
     return CSM_OK;
   }
 
+  if (probe && probe->mode == Probe3D::kList) {
+    const int n = probe->list_n;
+    CSM_CUDA(cudaMemcpyAsync(hp, ictr, rb_ctr, cudaMemcpyDeviceToHost, s));
+    CSM_CUDA(cudaStreamSynchronize(s));
+    for (int i = 0; i < n; ++i) {
+      const List3& c = probe->list[i];
+      CSM_REQUIRE(c.scan >= 0 && c.scan < hp[kC3Scans], "candidate scan_index");
+      CSM_REQUIRE(c.depth >= 0 && c.depth <= hmax, "candidate depth");
+    }
+    probe->num_scans = hp[kC3Scans];
+    probe->sums.resize(n);
+    probe->scores.resize(n);
+    if (n == 0) return CSM_OK;
+    DevBuf& d_lc = ctx->D("m3_tie_c");
+    DevBuf& d_ls = ctx->D("m3_tie_s");
+    DevBuf& d_li = ctx->D("m3_probe_sums");
+    CSM_TRY(d_lc.Reserve(sizeof(List3) * n));
+    CSM_TRY(d_ls.Reserve(sizeof(float) * n));
+    CSM_TRY(d_li.Reserve(sizeof(int) * n));
+    CSM_CUDA(cudaMemcpyAsync(d_lc.p, probe->list, sizeof(List3) * n, cudaMemcpyHostToDevice, s));
+    ProfBegin(ctx);
+    k3_score_list<<<n, kT3, 0, s>>>(jb, d_lc.as<List3>(), d_ls.as<float>(), d_li.as<int>());
+    CSM_LAUNCH_CHECK();
+    ProfEnd(ctx, "k3_score_list", n);
+    CSM_CUDA(cudaMemcpyAsync(probe->scores.data(), d_ls.p, sizeof(float) * n,
+                             cudaMemcpyDeviceToHost, s));
+    CSM_CUDA(cudaMemcpyAsync(probe->sums.data(), d_li.p, sizeof(int) * n, cudaMemcpyDeviceToHost,
+                             s));
+    CSM_CUDA(cudaStreamSynchronize(s));
+    return CSM_OK;
+  }
+
   // ---- lowest-resolution pass + dives (grids sized for all angles; filtered-out scans exit) ----
   CSM_TRY(d_top.Reserve(sizeof(int) * max_top));
   ProfBegin(ctx);
@@ -1208,6 +1272,33 @@ static csm_status Run3D(Ctx* ctx, const csm_matcher3d* m, const csm_node3d* node
   k3_dive<<<A, kT3, 0, s>>>(jb, d_top.as<int>(), dive_ratio, lb, ctr);
   CSM_LAUNCH_CHECK();
   ProfEnd(ctx, "k3_dive", static_cast<double>(A) * 8 * hmax);
+  if (probe && probe->mode == Probe3D::kTop) {
+    CSM_CUDA(cudaMemcpyAsync(hp, ictr, rb_ctr, cudaMemcpyDeviceToHost, s));
+    unsigned long long c[8];
+    CSM_CUDA(cudaMemcpyAsync(c, ctr, sizeof(c), cudaMemcpyDeviceToHost, s));
+    CSM_CUDA(cudaStreamSynchronize(s));
+    const int S = hp[kC3Scans];
+    probe->num_scans = S;
+    probe->nxc = jb.nxc;
+    probe->nzc = jb.nzc;
+    probe->top_best = hp[kC3TopBest];
+    probe->final_bound = HostUnord(static_cast<unsigned>(hp[kC3Bound]));
+    probe->counters[0] = c[0];
+    probe->counters[1] = c[1];
+    probe->counters[2] = c[2];
+    probe->angle.resize(S);
+    probe->top_sums.resize(per_scan * S);
+    std::vector<Scan3> hs(S);
+    if (S) {
+      CSM_CUDA(cudaMemcpy(probe->angle.data(), d_sel.p, sizeof(int) * S, cudaMemcpyDeviceToHost));
+      CSM_CUDA(cudaMemcpy(hs.data(), d_scans.p, sizeof(Scan3) * S, cudaMemcpyDeviceToHost));
+      CSM_CUDA(cudaMemcpy(probe->top_sums.data(), d_top.p, sizeof(int) * per_scan * S,
+                          cudaMemcpyDeviceToHost));
+    }
+    probe->rot.resize(S);
+    for (int k = 0; k < S; ++k) probe->rot[k] = hs[k].rot_score;
+    return CSM_OK;
+  }
 
   // ---- branch and bound: device-driven level loop (see engine2d.cu) ----
   const int kChunk = 1 << 16;
@@ -1217,7 +1308,8 @@ static csm_status Run3D(Ctx* ctx, const csm_matcher3d* m, const csm_node3d* node
   DevBuf& d_q = ctx->D("m3_queues");
   DevBuf& d_leaves = ctx->D("m3_leaves");
   DevBuf& d_best = ctx->D("m3_best");
-  CSM_TRY(d_qtop.Reserve(sizeof(Node3) * static_cast<size_t>(max_top)));
+  CSM_TRY(d_qtop.Reserve(sizeof(Node3) * static_cast<size_t>(
+                                               std::max<long long>(max_top, probe ? probe->num_parents : 0))));
   CSM_TRY(d_q.Reserve(sizeof(Node3) * static_cast<size_t>(kQueueCap) * std::max(1, hmax)));
   CSM_TRY(d_leaves.Reserve(sizeof(Leaf3) * static_cast<size_t>(kLeafCap)));
   CSM_TRY(d_best.Reserve(sizeof(BestLeaf3) * static_cast<size_t>(kLeafCap)));
@@ -1240,6 +1332,53 @@ static csm_status Run3D(Ctx* ctx, const csm_matcher3d* m, const csm_node3d* node
     ProfEnd(ctx, "k3_expand", 0.);
     return CSM_OK;
   };
+  if (probe) {
+    // the level loop over the caller's parents only: its state is reset to them
+    const int h = probe->level, n = probe->num_parents;
+    CSM_REQUIRE(h >= 1 && h <= hmax, "level out of range");
+    CSM_REQUIRE(n >= 0 && (h == hmax || n <= kQueueCap), "number of parents");
+    CSM_CUDA(cudaMemcpyAsync(hp, ictr, rb_ctr, cudaMemcpyDeviceToHost, s));
+    CSM_CUDA(cudaStreamSynchronize(s));
+    const int S = hp[kC3Scans];
+    for (int i = 0; i < n; ++i) {
+      const Node3& p = probe->parents[i];
+      CSM_REQUIRE(p.scan >= 0 && p.scan < S, "parent scan_index");
+      const int dx = p.ox + sp.wxy, dy = p.oy + sp.wxy, dz = p.oz + sp.wz;
+      CSM_REQUIRE(dx >= 0 && dy >= 0 && dz >= 0 && ((dx | dy | dz) & ((1 << h) - 1)) == 0 &&
+                      p.ox <= sp.wxy && p.oy <= sp.wxy && p.oz <= sp.wz,
+                  "parent is not a node of its level's lattice");
+    }
+    for (int l = 1; l <= hmax; ++l) hp[l] = 0;
+    hp[h] = n;
+    hp[kC3Leaf] = 0;
+    hp[kC3Overflow] = 0;
+    hp[kC3Bound] = static_cast<int>(HostOrd(probe->bound));
+    CSM_CUDA(cudaMemcpyAsync(ictr, hp, rb_ctr, cudaMemcpyHostToDevice, s));
+    CSM_CUDA(cudaMemsetAsync(ctr, 0, 8 * 8, s));
+    if (n)
+      CSM_CUDA(cudaMemcpyAsync(queue_ptr(h), probe->parents, sizeof(Node3) * n,
+                               cudaMemcpyHostToDevice, s));
+    for (int done = 0; done < n; done += kChunk) CSM_TRY(level_step(h));
+    unsigned long long c[8];
+    CSM_CUDA(cudaMemcpyAsync(hp, ictr, rb_ctr, cudaMemcpyDeviceToHost, s));
+    CSM_CUDA(cudaMemcpyAsync(c, ctr, sizeof(c), cudaMemcpyDeviceToHost, s));
+    CSM_CUDA(cudaStreamSynchronize(s));
+    if (hp[kC3Overflow]) { SetError("3D branch-and-bound capacity exceeded"); return CSM_E_CAPACITY; }
+    if (h >= 2) {
+      probe->children.resize(hp[h - 1]);
+      if (hp[h - 1])
+        CSM_CUDA(cudaMemcpy(probe->children.data(), queue_ptr(h - 1), sizeof(Node3) * hp[h - 1],
+                            cudaMemcpyDeviceToHost));
+    } else {
+      probe->leaves.resize(hp[kC3Leaf]);
+      if (hp[kC3Leaf])
+        CSM_CUDA(cudaMemcpy(probe->leaves.data(), d_leaves.p, sizeof(Leaf3) * hp[kC3Leaf],
+                            cudaMemcpyDeviceToHost));
+    }
+    probe->final_bound = HostUnord(static_cast<unsigned>(hp[kC3Bound]));
+    for (int k = 0; k < 3; ++k) probe->counters[k] = c[k];
+    return CSM_OK;
+  }
   int host_syncs = 0;
   auto collect = [&]() -> csm_status {
     CSM_CUDA(cudaMemsetAsync(ictr + kC3Best, 0, 4, s));
@@ -1298,7 +1437,7 @@ static csm_status Run3D(Ctx* ctx, const csm_matcher3d* m, const csm_node3d* node
     CSM_CUDA(cudaMemcpyAsync(d_lc.p, lc.data(), sizeof(List3) * lc.size(),
                              cudaMemcpyHostToDevice, s));
     k3_score_list<<<static_cast<int>(lc.size()), kT3, 0, s>>>(jb, d_lc.as<List3>(),
-                                                               d_ls.as<float>());
+                                                               d_ls.as<float>(), nullptr);
     CSM_LAUNCH_CHECK();
     CSM_CUDA(cudaMemcpyAsync(anc.data(), d_ls.p, sizeof(float) * lc.size(),
                              cudaMemcpyDeviceToHost, s));
@@ -1537,6 +1676,96 @@ csm_status csm_discretize3d(const csm_matcher3d* m, const csm_node3d* node,
   CSM_TRY(AcquireLane(m->ctx->device, &guard));
   return Run3D(guard.lane, m, node, nullptr, node_pose, submap_pose, full, 0.f, nullptr, nullptr,
                true, num_scans, cells, poses, rot);
+}
+
+}  // extern "C"
+
+// Runs `probe` on the match csm_match3d would run with these arguments.
+static csm_status RunProbe3D(const csm_matcher3d* m, const csm_node3d* node,
+                             const double node_pose[7], const double submap_pose[7], int32_t full,
+                             float min_score, Probe3D* probe) {
+  CSM_REQUIRE(m && node && node_pose && submap_pose, "null pointer");
+  CSM_REQUIRE(node->num_high >= 1 && node->high_resolution_point_cloud, "high-resolution cloud");
+  CSM_REQUIRE(node->num_low >= 0 && (node->num_low == 0 || node->low_resolution_point_cloud),
+              "low-resolution cloud");
+  LaneGuard guard;
+  CSM_TRY(AcquireLane(m->ctx->device, &guard));
+  return Run3D(guard.lane, m, node, nullptr, node_pose, submap_pose, full, min_score, nullptr,
+               nullptr, false, nullptr, nullptr, nullptr, nullptr, probe);
+}
+
+extern "C" {
+
+csm_status csm_score_candidates3d(const csm_matcher3d* m, const csm_node3d* node,
+                                  const double node_pose[7], const double submap_pose[7],
+                                  int32_t full_submap, const csm_candidate3d* candidates,
+                                  int32_t num_candidates, int32_t* sums, float* scores) {
+  static_assert(sizeof(csm_candidate3d) == sizeof(List3), "csm_candidate3d is List3");
+  CSM_REQUIRE(sums && scores && (candidates || num_candidates == 0) && num_candidates >= 0,
+              "candidates");
+  Probe3D probe;
+  probe.mode = Probe3D::kList;
+  probe.list = reinterpret_cast<const List3*>(candidates);
+  probe.list_n = num_candidates;
+  CSM_TRY(RunProbe3D(m, node, node_pose, submap_pose, full_submap, 0.f, &probe));
+  std::memcpy(sums, probe.sums.data(), sizeof(int) * num_candidates);
+  std::memcpy(scores, probe.scores.data(), sizeof(float) * num_candidates);
+  return CSM_OK;
+}
+
+csm_status csm_score_top3d(const csm_matcher3d* m, const csm_node3d* node,
+                           const double node_pose[7], const double submap_pose[7],
+                           int32_t full_submap, float min_score, int32_t* num_scans,
+                           int32_t lattice[2], int32_t* angle_index, float* rotational_scores,
+                           int32_t* sums, int32_t* top_best, float* bound, int64_t counters[2]) {
+  CSM_REQUIRE(num_scans && lattice, "null pointer");
+  Probe3D probe;
+  probe.mode = Probe3D::kTop;
+  CSM_TRY(RunProbe3D(m, node, node_pose, submap_pose, full_submap, min_score, &probe));
+  const int S = probe.num_scans;
+  *num_scans = S;
+  lattice[0] = probe.nxc;
+  lattice[1] = probe.nzc;
+  if (angle_index) std::memcpy(angle_index, probe.angle.data(), sizeof(int) * S);
+  if (rotational_scores) std::memcpy(rotational_scores, probe.rot.data(), sizeof(float) * S);
+  if (sums) std::memcpy(sums, probe.top_sums.data(), sizeof(int) * probe.top_sums.size());
+  if (top_best) *top_best = probe.top_best;
+  if (bound) *bound = probe.final_bound;
+  if (counters) {
+    counters[0] = static_cast<int64_t>(probe.counters[0]);
+    counters[1] = static_cast<int64_t>(probe.counters[2]);
+  }
+  return CSM_OK;
+}
+
+csm_status csm_branch_step3d(const csm_matcher3d* m, const csm_node3d* node,
+                             const double node_pose[7], const double submap_pose[7],
+                             int32_t full_submap, float min_score, int32_t level,
+                             const csm_bnb_node3d* parents, int32_t num_parents, float bound,
+                             csm_bnb_node3d* children, csm_bnb_leaf3d* leaves, int32_t* num_out,
+                             float* final_bound, int64_t counters[3]) {
+  static_assert(sizeof(csm_bnb_node3d) == sizeof(Node3), "csm_bnb_node3d is Node3");
+  static_assert(sizeof(csm_bnb_leaf3d) == sizeof(Leaf3), "csm_bnb_leaf3d is Leaf3");
+  CSM_REQUIRE(num_out && final_bound && counters, "null pointer");
+  CSM_REQUIRE(num_parents >= 0 && (parents || num_parents == 0), "parents");
+  CSM_REQUIRE(level >= 2 ? children != nullptr : leaves != nullptr, "output records");
+  Probe3D probe;
+  probe.mode = Probe3D::kStep;
+  probe.level = level;
+  probe.parents = reinterpret_cast<const Node3*>(parents);
+  probe.num_parents = num_parents;
+  probe.bound = bound;
+  CSM_TRY(RunProbe3D(m, node, node_pose, submap_pose, full_submap, min_score, &probe));
+  if (level >= 2) {
+    *num_out = static_cast<int32_t>(probe.children.size());
+    std::memcpy(children, probe.children.data(), sizeof(Node3) * probe.children.size());
+  } else {
+    *num_out = static_cast<int32_t>(probe.leaves.size());
+    std::memcpy(leaves, probe.leaves.data(), sizeof(Leaf3) * probe.leaves.size());
+  }
+  *final_bound = probe.final_bound;
+  for (int k = 0; k < 3; ++k) counters[k] = static_cast<int64_t>(probe.counters[k]);
+  return CSM_OK;
 }
 
 }  // extern "C"

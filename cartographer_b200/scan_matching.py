@@ -537,6 +537,13 @@ class CsmNode3D(C.Structure):
                 ("histogram_size", C.c_int32), ("gravity_alignment", C.c_double * 4)]
 
 
+# csm_bnb_node3d / csm_bnb_leaf3d: a 3D branch-and-bound frontier node and a recorded leaf
+BNB_NODE3D_DTYPE = np.dtype([("scan", "<i4"), ("x", "<i4"), ("y", "<i4"), ("z", "<i4"),
+                             ("score", "<f4")])
+BNB_LEAF3D_DTYPE = np.dtype([("scan", "<i4"), ("x", "<i4"), ("y", "<i4"), ("z", "<i4"),
+                             ("score", "<f4"), ("low", "<f4")])
+
+
 class CsmResult3D(C.Structure):
     _fields_ = [("found", C.c_int32), ("score", C.c_float), ("pose_estimate", C.c_double * 7),
                 ("rotational_score", C.c_float), ("low_resolution_score", C.c_float),
@@ -698,6 +705,68 @@ class FastCorrelativeScanMatcher3D:
             check(lib().csm_discretize3d(*args, ptr(cells, C.c_int32), ptr(poses, C.c_float),
                                          ptr(rot, C.c_float)))
         return cells, poses, rot
+
+    def _probe_args(self, full, node_pose, submap_pose, holder):
+        npose = np.ascontiguousarray(node_pose, np.float64)
+        spose = np.ascontiguousarray(submap_pose, np.float64)
+        return (self._h, C.byref(holder.c), ptr(npose, C.c_double), ptr(spose, C.c_double),
+                C.c_int32(int(full)))
+
+    def score_candidates(self, full, node_pose, submap_pose, constant_data, candidates):
+        """csm_score_candidates3d: `candidates` is n x {scan, x, y, z, depth}.
+        -> (sums int32, scores float32) in the given order."""
+        holder = _NodeHolder(constant_data)
+        cand = np.ascontiguousarray(candidates, np.int32).reshape(-1, 5)
+        sums = np.zeros(len(cand), np.int32)
+        scores = np.zeros(len(cand), np.float32)
+        check(lib().csm_score_candidates3d(
+            *self._probe_args(full, node_pose, submap_pose, holder), ptr(cand, C.c_int32),
+            C.c_int32(len(cand)), ptr(sums, C.c_int32), ptr(scores, C.c_float)))
+        return sums, scores
+
+    def score_top(self, full, node_pose, submap_pose, constant_data, min_score):
+        """csm_score_top3d: the match up to and including its dives.  -> dict with
+        angle (angle index per kept scan), rot (rotational scores), nxc, nzc,
+        sums (num_scans x nzc x nxc x nxc: [scan, z, y, x]), top_best, bound and
+        counters (candidates scored by the dives, gate evaluations)."""
+        holder = _NodeHolder(constant_data)
+        args = self._probe_args(full, node_pose, submap_pose, holder) + (C.c_float(min_score),)
+        S = C.c_int32(0)
+        lat = np.zeros(2, np.int32)
+        check(lib().csm_score_top3d(*args, C.byref(S), ptr(lat, C.c_int32), None, None, None,
+                                    None, None, None))
+        S, nxc, nzc = S.value, int(lat[0]), int(lat[1])
+        angle = np.zeros(S, np.int32)
+        rot = np.zeros(S, np.float32)
+        sums = np.zeros((S, nzc, nxc, nxc), np.int32)
+        best, bound = C.c_int32(0), C.c_float(0)
+        ctr = np.zeros(2, np.int64)
+        S2 = C.c_int32(0)
+        check(lib().csm_score_top3d(*args, C.byref(S2), ptr(lat, C.c_int32), ptr(angle, C.c_int32),
+                                    ptr(rot, C.c_float), ptr(sums, C.c_int32), C.byref(best),
+                                    C.byref(bound), ptr(ctr, C.c_int64)))
+        assert S2.value == S
+        return dict(angle=angle, rot=rot, nxc=nxc, nzc=nzc, sums=sums, top_best=best.value,
+                    bound=np.float32(bound.value), counters=(int(ctr[0]), int(ctr[1])))
+
+    def branch_step(self, full, node_pose, submap_pose, constant_data, min_score, level,
+                    parents, bound):
+        """csm_branch_step3d over `parents` (BNB_NODE3D_DTYPE records) of `level` with the
+        bound set to `bound`.  -> (children in queue order (level >= 2) or leaves
+        (BNB_LEAF3D_DTYPE, level 1), final bound, (candidates scored, parents expanded,
+        gate evaluations))."""
+        holder = _NodeHolder(constant_data)
+        par = np.ascontiguousarray(parents, dtype=BNB_NODE3D_DTYPE)
+        out = np.zeros(max(1, 8 * len(par)), BNB_NODE3D_DTYPE if level >= 2 else BNB_LEAF3D_DTYPE)
+        count, final = C.c_int32(0), C.c_float(0.0)
+        ctr = np.zeros(3, np.int64)
+        optr = out.ctypes.data_as(C.c_void_p)
+        check(lib().csm_branch_step3d(
+            *self._probe_args(full, node_pose, submap_pose, holder), C.c_float(min_score),
+            C.c_int32(level), par.ctypes.data_as(C.c_void_p), C.c_int32(len(par)),
+            C.c_float(bound), optr if level >= 2 else None, None if level >= 2 else optr,
+            C.byref(count), C.byref(final), ptr(ctr, C.c_int64)))
+        return out[:count.value].copy(), np.float32(final.value), tuple(int(c) for c in ctr)
 
 
 class CsmJob3D(C.Structure):

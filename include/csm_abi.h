@@ -504,6 +504,55 @@ csm_status csm_discretize3d(const csm_matcher3d* matcher, const csm_node3d* node
                             const double global_submap_pose[7], int32_t full_submap,
                             int32_t* num_scans, int32_t* cells, float* poses,
                             float* rotational_scores);
+/* A candidate of ScoreCandidates (:332-355): a discrete scan (index after the rotational
+ * filter), a linear offset in voxels and the precomputation depth it is scored at. */
+typedef struct csm_candidate3d {
+  int32_t scan_index, x, y, z, depth;
+} csm_candidate3d;
+/* ScoreCandidates of the same match's discrete scans over a caller-given list (no sort),
+ * run by the match's own scoring kernel: sums and scores receive num_candidates values,
+ * the integer sum and ToProbability(sum / n). */
+csm_status csm_score_candidates3d(const csm_matcher3d* matcher, const csm_node3d* node,
+                                  const double global_node_pose[7],
+                                  const double global_submap_pose[7], int32_t full_submap,
+                                  const csm_candidate3d* candidates, int32_t num_candidates,
+                                  int32_t* sums, float* scores);
+/* The same match up to and including its greedy dives: *num_scans after the rotational
+ * filter and lattice = {nxc, nzc} (lowest-resolution candidates per axis, x == y).  The
+ * other outputs may be NULL (call with sums == NULL to size them first): the angle index
+ * and rotational score of each kept scan, every lowest-resolution sum (scan-major, then
+ * z, y, x), the largest of them, the bound after the dives and
+ * counters {candidates scored by the dives, low-resolution gate evaluations}. */
+csm_status csm_score_top3d(const csm_matcher3d* matcher, const csm_node3d* node,
+                           const double global_node_pose[7], const double global_submap_pose[7],
+                           int32_t full_submap, float min_score, int32_t* num_scans,
+                           int32_t lattice[2], int32_t* angle_index, float* rotational_scores,
+                           int32_t* sums, int32_t* top_best, float* bound, int64_t counters[2]);
+/* A node of the 3D branch-and-bound frontier, and a recorded leaf with its low-resolution
+ * (gate) score. */
+typedef struct csm_bnb_node3d {
+  int32_t scan_index, x, y, z;
+  float score;
+} csm_bnb_node3d;
+typedef struct csm_bnb_leaf3d {
+  int32_t scan_index, x, y, z;
+  float score, low_resolution_score;
+} csm_bnb_leaf3d;
+/* One level of the same match's branch step (BranchAndBound's children loop, :403-437)
+ * over caller-given parents of `level` (1 .. depth-1, nodes of that level's lattice), with
+ * the bound set to `bound` first, run by the match's own launch code until the level's
+ * queue is drained (in chunks, from its end).  Level >= 2: children (8 * num_parents
+ * records) receives the pushed children in queue order; level 1: leaves (8 * num_parents
+ * records) the recorded gate-passing leaves.  *num_out is their number, *final_bound the
+ * bound afterwards, counters {candidates scored, parents expanded, gate evaluations}.  A
+ * full queue or leaf list returns CSM_E_CAPACITY, as in a match. */
+csm_status csm_branch_step3d(const csm_matcher3d* matcher, const csm_node3d* node,
+                             const double global_node_pose[7],
+                             const double global_submap_pose[7], int32_t full_submap,
+                             float min_score, int32_t level, const csm_bnb_node3d* parents,
+                             int32_t num_parents, float bound, csm_bnb_node3d* children,
+                             csm_bnb_leaf3d* leaves, int32_t* num_out, float* final_bound,
+                             int64_t counters[3]);
 
 /* ==== RealTimeCorrelativeScanMatcher3D ======================================== */
 /* A HybridGrid resident on the device (dense uint16 box over its non-zero voxels; reads

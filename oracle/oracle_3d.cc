@@ -471,22 +471,30 @@ FastCorrelativeScanMatcher3D::GenerateLowestResolutionCandidates(
   return candidates;
 }
 
+// :338-346, the sum of one candidate (shared by ScoreCandidates and ScoreCandidatesForTest)
+int FastCorrelativeScanMatcher3D::CandidateSum(const int depth,
+                                               const DiscreteScan3D& discrete_scan,
+                                               const Array3i& candidate_offset) const {
+  const int reduction_exponent = std::max(0, depth - options_.full_resolution_depth + 1);
+  const PrecomputationGrid3D& grid = stack_->Get(depth);
+  int sum = 0;
+  const Array3i offset{candidate_offset.x >> reduction_exponent,
+                       candidate_offset.y >> reduction_exponent,
+                       candidate_offset.z >> reduction_exponent};
+  for (const Array3i& cell_index : discrete_scan.cell_indices_per_depth[depth]) {
+    sum += grid.value(
+        Array3i{cell_index.x + offset.x, cell_index.y + offset.y, cell_index.z + offset.z});
+  }
+  return sum;
+}
+
 // :332-355
 void FastCorrelativeScanMatcher3D::ScoreCandidates(
     const int depth, const std::vector<DiscreteScan3D>& discrete_scans,
     std::vector<Candidate3D>* const candidates) const {
-  const int reduction_exponent = std::max(0, depth - options_.full_resolution_depth + 1);
-  const PrecomputationGrid3D& grid = stack_->Get(depth);
   for (Candidate3D& candidate : *candidates) {
-    int sum = 0;
     const DiscreteScan3D& discrete_scan = discrete_scans[candidate.scan_index];
-    const Array3i offset{candidate.offset.x >> reduction_exponent,
-                         candidate.offset.y >> reduction_exponent,
-                         candidate.offset.z >> reduction_exponent};
-    for (const Array3i& cell_index : discrete_scan.cell_indices_per_depth[depth]) {
-      sum += grid.value(
-          Array3i{cell_index.x + offset.x, cell_index.y + offset.y, cell_index.z + offset.z});
-    }
+    const int sum = CandidateSum(depth, discrete_scan, candidate.offset);
     candidate.score = ToProbability3D(
         sum / static_cast<float>(discrete_scan.cell_indices_per_depth[depth].size()));
   }
@@ -582,6 +590,27 @@ FastCorrelativeScanMatcher3D::GenerateDiscreteScansForTest(bool full,
   return GenerateDiscreteScans(sp, data.high_resolution_point_cloud,
                                data.rotational_scan_matcher_histogram, data.gravity_alignment,
                                node, submap, nullptr);
+}
+
+void FastCorrelativeScanMatcher3D::ScoreCandidatesForTest(
+    bool full, const Rigid3d& global_node_pose, const Rigid3d& global_submap_pose,
+    const NodeData3D& data, int depth, const std::vector<std::array<int, 4>>& candidates,
+    int* sums, float* scores, float* low_resolution_scores) const {
+  const std::vector<DiscreteScan3D> discrete_scans =
+      GenerateDiscreteScansForTest(full, global_node_pose, global_submap_pose, data);
+  const auto low_resolution_matcher =
+      CreateLowResolutionMatcher(low_resolution_hybrid_grid_, &data.low_resolution_point_cloud);
+  for (size_t i = 0; i < candidates.size(); ++i) {
+    const std::array<int, 4>& c = candidates[i];
+    Candidate3D candidate(c[0], Array3i{c[1], c[2], c[3]});
+    const DiscreteScan3D& discrete_scan = discrete_scans.at(candidate.scan_index);
+    sums[i] = CandidateSum(depth, discrete_scan, candidate.offset);
+    scores[i] = ToProbability3D(
+        sums[i] / static_cast<float>(discrete_scan.cell_indices_per_depth[depth].size()));
+    if (depth == 0 && low_resolution_scores)
+      low_resolution_scores[i] =
+          low_resolution_matcher(GetPoseFromCandidate(discrete_scans, candidate));
+  }
 }
 
 // ---- real_time_correlative_scan_matcher_3d.cc ---------------------------------------

@@ -174,8 +174,16 @@ class FastCorrelativeScanMatcher3D {  // fast_correlative_scan_matcher_3d.{h,cc}
   std::vector<DiscreteScan3D> GenerateDiscreteScansForTest(
       bool full, const Rigid3d& global_node_pose, const Rigid3d& global_submap_pose,
       const NodeData3D& data) const;
+  // test hook: the sums and scores of caller-given candidates {scan_index, x, y, z} at
+  // `depth` on those discrete scans (no sort); at depth 0 also the low-resolution
+  // matcher's score of GetPoseFromCandidate (low_resolution_scores may be null)
+  void ScoreCandidatesForTest(bool full, const Rigid3d& global_node_pose,
+                              const Rigid3d& global_submap_pose, const NodeData3D& data,
+                              int depth, const std::vector<std::array<int, 4>>& candidates,
+                              int* sums, float* scores, float* low_resolution_scores) const;
 
  private:
+  int CandidateSum(int depth, const DiscreteScan3D& discrete_scan, const Array3i& offset) const;
   std::unique_ptr<Result3D> MatchWithSearchParameters(
       const SearchParameters& sp, const Rigid3f& global_node_pose,
       const Rigid3f& global_submap_pose, const PointCloud& point_cloud,

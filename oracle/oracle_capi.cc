@@ -509,6 +509,25 @@ int orc_fast3d_discrete_scans(void* h, int full, const double* node_pose,
   return static_cast<int>(scans.size());
 }
 
+// ScoreCandidates of caller-given candidates (n x {scan, x, y, z}) at `depth` on the same
+// discrete scans (test hook): sums, scores and, at depth 0, low-resolution scores (may be null).
+void orc_fast3d_score_candidates(void* h, int full, const double* node_pose,
+                                 const double* submap_pose, const double* gravity,
+                                 const float* hi_xyz, int n_hi, const float* lo_xyz, int n_lo,
+                                 const float* hist, int hist_n, int depth,
+                                 const int32_t* candidates, int n, int32_t* sums, float* scores,
+                                 float* low_scores) {
+  Fast3DHandle* f = static_cast<Fast3DHandle*>(h);
+  const NodeData3D data = MakeNode(gravity, hi_xyz, n_hi, lo_xyz, n_lo, hist, hist_n);
+  std::vector<std::array<int, 4>> c(n);
+  for (int i = 0; i < n; ++i)
+    c[i] = {candidates[4 * i], candidates[4 * i + 1], candidates[4 * i + 2], candidates[4 * i + 3]};
+  std::vector<int> s(n);
+  f->matcher->ScoreCandidatesForTest(full != 0, MakeRigid3d(node_pose), MakeRigid3d(submap_pose),
+                                     data, depth, c, s.data(), scores, low_scores);
+  std::copy(s.begin(), s.end(), sums);
+}
+
 void orc_rotational_match(const float* submap_hist, const float* hist, int n, float initial_angle,
                           const float* angles, int m, float* out) {
   const std::vector<float> a(submap_hist, submap_hist + n), b(hist, hist + n);

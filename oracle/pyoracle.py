@@ -430,6 +430,28 @@ class FastCorrelativeScanMatcher3D:
                                             _p(rot, C.c_float))
         return cells, poses, rot
 
+    def score_candidates(self, full, node_pose, submap_pose, node, depth, candidates):
+        """ScoreCandidates of `candidates` (n x {scan, x, y, z}) at `depth` on the discrete
+        scans of this match, unsorted -> (sums int32, scores float32, low-resolution scores
+        float32 of GetPoseFromCandidate at depth 0, else None)."""
+        npose = np.ascontiguousarray(node_pose, np.float64)
+        spose = np.ascontiguousarray(submap_pose, np.float64)
+        grav = np.ascontiguousarray(node["gravity_alignment"], np.float64)
+        hi, lo = _f32(node["high_resolution_point_cloud"]), _f32(node["low_resolution_point_cloud"])
+        hist = _f32(node["rotational_scan_matcher_histogram"]).reshape(-1)
+        cand = _i32(candidates).reshape(-1, 4)
+        n = len(cand)
+        sums = np.zeros(n, np.int32)
+        scores = np.zeros(n, np.float32)
+        low = np.zeros(n, np.float32)
+        lib().orc_fast3d_score_candidates(
+            self._h, C.c_int(int(full)), _p(npose, C.c_double), _p(spose, C.c_double),
+            _p(grav, C.c_double), _p(hi, C.c_float), C.c_int(len(hi)), _p(lo, C.c_float),
+            C.c_int(len(lo)), _p(hist, C.c_float), C.c_int(len(hist)), C.c_int(depth),
+            _p(cand, C.c_int32), C.c_int(n), _p(sums, C.c_int32), _p(scores, C.c_float),
+            _p(low, C.c_float) if depth == 0 else None)
+        return sums, scores, (low if depth == 0 else None)
+
 
 def rotational_match(submap_hist, hist, initial_angle, angles):
     a, b = _f32(submap_hist).reshape(-1), _f32(hist).reshape(-1)

@@ -84,6 +84,87 @@ def node_data(hi, low=None, hist=None, gravity=(1.0, 0.0, 0.0, 0.0)):
                 rotational_scan_matcher_histogram=np.zeros(10, np.float32) if hist is None else hist)
 
 
+def random_voxels(rng, n, extent, resolution, values=None, center=(0, 0, 0)):
+    """n random voxels (unique) in center + [-extent, extent)^3 with random values in
+    1 .. 32767, or `values` (a scalar or an array), as a HybridGridSpec."""
+    idx = np.unique(rng.randint(-extent, extent, size=(n, 3)) + np.asarray(center), axis=0)
+    if values is None:
+        vals = rng.randint(1, 32768, size=len(idx))
+    elif np.ndim(values):
+        vals = np.asarray(values)[:len(idx)]
+    else:
+        vals = np.full(len(idx), values)
+    return synthetic.HybridGridSpec(resolution, idx.astype(np.int32), vals.astype(np.uint16))
+
+
+def random_cloud(rng, n, radius, center=(0.0, 0.0, 0.0)):
+    """n points uniform in a cube of half-width `radius` around `center` (float32)."""
+    return (rng.uniform(-radius, radius, size=(n, 3)) + np.asarray(center)).astype(np.float32)
+
+
+def fast_options(depth=5, frd=3, xy=0.7, z=0.3, angular=0.05, min_rot=0.0, min_low=0.0):
+    return dict(branch_and_bound_depth=depth, full_resolution_depth=frd,
+                min_rotational_score=min_rot, min_low_resolution_score=min_low,
+                linear_xy_search_window=xy, linear_z_search_window=z,
+                angular_search_window=angular)
+
+
+def search_window(options, resolution):
+    """SearchParameters of Match (:127-144): (wxy, wz) = lround(window / resolution)."""
+    res = np.float32(resolution)
+    return (int(np.floor(options["linear_xy_search_window"] / res + 0.5)),
+            int(np.floor(options["linear_z_search_window"] / res + 0.5)))
+
+
+def to_score(sums, n):
+    """PrecomputationGrid3D::ToProbability(sum / float(n)) (precomputation_grid_3d.h:32-35)."""
+    k_min = np.float32(0.1)
+    k = (np.float32(1.0) - k_min - k_min) / np.float32(255.0)
+    return (k_min + (np.asarray(sums).astype(np.float32) / np.float32(n)) * k).astype(np.float32)
+
+
+def make_pair(oracle, sm, hi, lo, od, hist=None):
+    """The oracle's and the engine's FastCorrelativeScanMatcher3D on the same grids, the
+    engine given the oracle's grid size (MatchFullSubmap's window depends on it)."""
+    hist = np.zeros(10, np.float32) if hist is None else np.asarray(hist, np.float32)
+    ohi = oracle.HybridGrid(hi.resolution, hi.indices, hi.values)
+    olo = oracle.HybridGrid(lo.resolution, lo.indices, lo.values)
+    om = oracle.FastCorrelativeScanMatcher3D(ohi, olo, hist, od)
+    opts = sm.FastCorrelativeScanMatcherOptions3D(
+        od["branch_and_bound_depth"], od["full_resolution_depth"], od["min_rotational_score"],
+        od["min_low_resolution_score"], od["linear_xy_search_window"],
+        od["linear_z_search_window"], od["angular_search_window"])
+    m = sm.FastCorrelativeScanMatcher3D(hi, lo, hist, opts, grid_size_in_voxels=ohi.grid_size())
+    return om, m
+
+
+def engine_node(sm, d):
+    return sm.TrajectoryNodeData3D(d["high_resolution_point_cloud"],
+                                   d["low_resolution_point_cloud"],
+                                   d["rotational_scan_matcher_histogram"], d["gravity_alignment"])
+
+
+def numpy_sums(om, cells, depth, frd, wxy, wz, candidates):
+    """ScoreCandidates' sums (fast_correlative_scan_matcher_3d.cc:332-355) in numpy over the
+    oracle's level box: the per-depth cell indices of DiscretizeScan (:200-244), the
+    candidate offset >> reduction_exponent, 0 outside the box.  cells: the full-resolution
+    cells of the discrete scans (S x n x 3); candidates: m x {scan, x, y, z}."""
+    cand = np.asarray(candidates, np.int64).reshape(-1, 4)
+    e = max(0, depth - frd + 1)
+    start = np.array([-wxy, -wxy, -wz], np.int64)
+    c = np.asarray(cells, np.int64)
+    if e:
+        c = ((c + start) >> e) - (start >> e)
+    pts = c[cand[:, 0]] + (cand[:, 1:4] >> e)[:, None, :]
+    lo, box = om.level(depth)
+    rel = pts - np.asarray(lo, np.int64)
+    dims = np.array(box.shape[::-1], np.int64)
+    inside = np.all((rel >= 0) & (rel < dims), axis=-1)
+    rel = np.where(inside[..., None], rel, 0)
+    v = np.where(inside, box[rel[..., 2], rel[..., 1], rel[..., 0]] if box.size else 0, 0)
+    return v.astype(np.int64).sum(axis=1)
+
+
 def _mat(p):
     t, (w, x, y, z) = p[:3], p[3:]
     M = np.eye(4, dtype=np.float32)
