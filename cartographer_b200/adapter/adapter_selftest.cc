@@ -352,5 +352,43 @@ int main() {
         summary3.termination);
     if (!(summary3.final_cost <= summary3.initial_cost)) return 1;
   }
+  // ---- RangeDataInserter3D on device grids: the reference's InsertPointCloudWithIntensities
+  // (range_data_inserter_3d_test.cc:57-69), twice, into empty 1 m grids ----
+  {
+    mapping::proto::RangeDataInserterOptions3D io;
+    io.set_hit_probability(0.7);
+    io.set_miss_probability(0.4);
+    io.set_num_free_space_voxels(1000);
+    io.set_intensity_threshold(100.f);
+    const mapping::scan_matching::RangeDataInserter3D inserter(io);
+    mapping::scan_matching::DeviceHybridGrid grid(1.f, 0);
+    mapping::scan_matching::DeviceIntensityGrid intensity(1.f, 0);
+    sensor::RangeData range_data;
+    range_data.origin = {{0.f, 0.f, -4.f}};
+    range_data.returns = sensor::PointCloud(
+        {{{{-3.f, -1.f, 4.f}}}, {{{-2.f, 0.f, 4.f}}}, {{{-1.f, 1.f, 4.f}}}, {{{0.f, 2.f, 4.f}}}},
+        {7.f, 8.f, 9.f, 10.f});
+    for (int i = 0; i < 2; ++i) inserter.Insert(range_data, &grid, &intensity);
+    int32_t lo[3], dims[3];
+    if (csm_grid3d_read(grid.handle(), lo, dims, nullptr) != CSM_OK) return 1;
+    std::vector<uint16_t> values(static_cast<size_t>(dims[0]) * dims[1] * dims[2]);
+    if (csm_grid3d_read(grid.handle(), lo, dims, values.data()) != CSM_OK) return 1;
+    std::printf("RESULT insert3d %d %d %d %d %d %d", lo[0], lo[1], lo[2], dims[0], dims[1], dims[2]);
+    for (uint16_t v : values) std::printf(" %u", v);
+    std::printf("\n");
+    if (csm_intensity_grid3d_read(intensity.handle(), lo, dims, nullptr, nullptr, nullptr) != CSM_OK)
+      return 1;
+    const size_t vox = static_cast<size_t>(dims[0]) * dims[1] * dims[2];
+    std::vector<float> mean(vox), sum(vox);
+    std::vector<int32_t> count(vox);
+    if (csm_intensity_grid3d_read(intensity.handle(), lo, dims, mean.data(), sum.data(),
+                                  count.data()) != CSM_OK)
+      return 1;
+    std::printf("RESULT insert3d_intensity %d %d %d %d %d %d", lo[0], lo[1], lo[2], dims[0],
+                dims[1], dims[2]);
+    for (size_t i = 0; i < vox; ++i)
+      std::printf(" %08x:%08x:%d", Bits(mean[i]), Bits(sum[i]), count[i]);
+    std::printf("\n");
+  }
   return 0;
 }

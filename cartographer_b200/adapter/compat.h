@@ -66,7 +66,34 @@ class PointCloud {
   std::vector<RangefinderPoint> points_;
   std::vector<float> intensities_;
 };
+// sensor/range_data.h:28-35 (origin is an Eigen::Vector3f there).
+struct RangeData {
+  struct { float v[3]; float x() const { return v[0]; } float y() const { return v[1]; } float z() const { return v[2]; } } origin;
+  PointCloud returns;
+  PointCloud misses;
+};
 }  // namespace sensor
+
+namespace mapping {
+namespace proto {
+// mapping/proto/range_data_inserter_options_3d.proto
+class RangeDataInserterOptions3D {
+ public:
+  double hit_probability() const { return hit_; }
+  double miss_probability() const { return miss_; }
+  int num_free_space_voxels() const { return nfsv_; }
+  float intensity_threshold() const { return threshold_; }
+  void set_hit_probability(double v) { hit_ = v; }
+  void set_miss_probability(double v) { miss_ = v; }
+  void set_num_free_space_voxels(int v) { nfsv_ = v; }
+  void set_intensity_threshold(float v) { threshold_ = v; }
+ private:
+  double hit_ = 0., miss_ = 0.;
+  int nfsv_ = 0;
+  float threshold_ = 0.f;
+};
+}  // namespace proto
+}  // namespace mapping
 
 namespace transform {
 // transform/rigid_transform.h:116-196 (Rigid3<double>) and Eigen::Quaterniond as used

@@ -29,7 +29,9 @@
 #include "cartographer/mapping/proto/scan_matching/ceres_scan_matcher_options_2d.pb.h"
 #include "cartographer/mapping/proto/scan_matching/fast_correlative_scan_matcher_options_2d.pb.h"
 #include "cartographer/mapping/proto/scan_matching/real_time_correlative_scan_matcher_options.pb.h"
+#include "cartographer/mapping/proto/range_data_inserter_options_3d.pb.h"
 #include "cartographer/sensor/point_cloud.h"
+#include "cartographer/sensor/range_data.h"
 #include "cartographer/transform/rigid_transform.h"
 #define CSM_ADAPTER_REAL_CARTOGRAPHER 1
 #else
@@ -455,10 +457,15 @@ class DeviceHybridGrid {
                                            static_cast<int64_t>(val.size()), grid.resolution(),
                                            device, &grid_));
   }
+  // The grid of a fresh submap (HybridGrid(resolution)), filled by RangeDataInserter3D below.
+  DeviceHybridGrid(float resolution, int device) {
+    b200_internal::Check(csm_grid3d_create(nullptr, nullptr, 0, resolution, device, &grid_));
+  }
   ~DeviceHybridGrid() { csm_grid3d_destroy(grid_); }
   DeviceHybridGrid(const DeviceHybridGrid&) = delete;
   DeviceHybridGrid& operator=(const DeviceHybridGrid&) = delete;
   const csm_grid3d* handle() const { return grid_; }
+  csm_grid3d* mutable_handle() { return grid_; }
 
  private:
   csm_grid3d* grid_ = nullptr;
@@ -483,13 +490,55 @@ class DeviceIntensityGrid {
                                                      static_cast<int64_t>(sum.size()),
                                                      grid.resolution(), device, &grid_));
   }
+  // The intensity grid of a fresh submap (IntensityHybridGrid(resolution)).
+  DeviceIntensityGrid(float resolution, int device) {
+    b200_internal::Check(
+        csm_intensity_grid3d_create(nullptr, nullptr, nullptr, 0, resolution, device, &grid_));
+  }
   ~DeviceIntensityGrid() { csm_intensity_grid3d_destroy(grid_); }
   DeviceIntensityGrid(const DeviceIntensityGrid&) = delete;
   DeviceIntensityGrid& operator=(const DeviceIntensityGrid&) = delete;
   const csm_intensity_grid3d* handle() const { return grid_; }
+  csm_intensity_grid3d* mutable_handle() { return grid_; }
 
  private:
   csm_intensity_grid3d* grid_ = nullptr;
+};
+
+// mapping/3d/range_data_inserter_3d.h:28-45 on device grids: Submap3D::InsertData
+// (submap_3d.cc:271-290) keeps its submap's high-resolution, low-resolution and intensity
+// grids as DeviceHybridGrid / DeviceIntensityGrid and inserts every scan in place, so the
+// real-time matcher and CeresScanMatcher3D read the updated submap without a re-upload.
+class RangeDataInserter3D {
+ public:
+  explicit RangeDataInserter3D(const mapping::proto::RangeDataInserterOptions3D& options,
+                               int device = 0) {
+    csm_range_inserter_options3d o;
+    o.hit_probability = options.hit_probability();
+    o.miss_probability = options.miss_probability();
+    o.num_free_space_voxels = options.num_free_space_voxels();
+    o.intensity_threshold = options.intensity_threshold();
+    b200_internal::Check(csm_range_inserter3d_create(&o, device, &inserter_));
+  }
+  ~RangeDataInserter3D() { csm_range_inserter3d_destroy(inserter_); }
+  RangeDataInserter3D(const RangeDataInserter3D&) = delete;
+  RangeDataInserter3D& operator=(const RangeDataInserter3D&) = delete;
+
+  // range_data_inserter_3d.cc:87-114; range_data in the grids' frame.
+  void Insert(const sensor::RangeData& range_data, DeviceHybridGrid* hybrid_grid,
+              DeviceIntensityGrid* intensity_hybrid_grid) const {
+    if (hybrid_grid == nullptr) std::abort();  // CHECK_NOTNULL (:90)
+    const std::vector<float> xyz = b200_internal::Flatten(range_data.returns);
+    const float origin[3] = {range_data.origin.x(), range_data.origin.y(), range_data.origin.z()};
+    const std::vector<float>& intensities = range_data.returns.intensities();
+    b200_internal::Check(csm_range_inserter3d_insert(
+        inserter_, origin, xyz.data(), intensities.empty() ? nullptr : intensities.data(),
+        static_cast<int32_t>(range_data.returns.size()), hybrid_grid->mutable_handle(),
+        intensity_hybrid_grid ? intensity_hybrid_grid->mutable_handle() : nullptr, nullptr));
+  }
+
+ private:
+  csm_range_inserter3d* inserter_ = nullptr;
 };
 
 class RealTimeCorrelativeScanMatcher3D {

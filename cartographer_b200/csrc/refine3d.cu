@@ -944,7 +944,10 @@ csm_status csm_intensity_grid3d_create(const int32_t* idx, const float* sum, con
     CSM_REQUIRE(lo[a] >= -8192 && hi[a] < 8192, "voxel index outside the 2^14 cube");  // hybrid_grid.h:387
     g->lo[a] = lo[a];
     g->n[a] = hi[a] - lo[a] + 1;
+    g->tight.lo[a] = lo[a];
+    g->tight.hi[a] = hi[a];
   }
+  g->tight.empty = n == 0;
   const size_t vox = static_cast<size_t>(g->n[0]) * g->n[1] * g->n[2];
   CSM_REQUIRE(vox < (size_t(4) << 30), "dense volume too large");
   // IntensityHybridGrid::GetIntensity (hybrid_grid.h:562-569): the float mean, 0 where no
@@ -969,6 +972,10 @@ csm_status csm_intensity_grid3d_create(const int32_t* idx, const float* sum, con
     CSM_LAUNCH_CHECK();
   }
   CSM_CUDA(cudaStreamSynchronize(s));
+  // what a first insert fills its sum / count volumes from (insert3d.cu)
+  g->made_idx.assign(idx, idx + 3 * n);
+  g->made_sum.assign(sum, sum + n);
+  g->made_count.assign(count, count + n);
   *out = g.release();
   return CSM_OK;
 }

@@ -188,11 +188,16 @@ csm_status csm_grid3d_create(const int32_t* idx, const uint16_t* values, int64_t
     CSM_REQUIRE(lo[a] >= -8192 && hi[a] < 8192, "voxel index outside the 2^14 cube");  // hybrid_grid.h:387
     d.lo[a] = lo[a];
     d.n[a] = hi[a] - lo[a] + 1;
+    g->tight.lo[a] = lo[a];
+    g->tight.hi[a] = hi[a];
   }
+  g->tight.empty = n == 0;
   const size_t vox = static_cast<size_t>(d.n[0]) * d.n[1] * d.n[2];
   CSM_REQUIRE(vox < (size_t(8) << 30), "dense volume too large");
-  CSM_CUDA(cudaMalloc(&g->d_vol, std::max<size_t>(vox * 2, 256)));
-  CSM_CUDA(cudaMemsetAsync(g->d_vol, 0, std::max<size_t>(vox * 2, 256), s));
+  // whole 32-bit words: the inserter clears update markers with 32-bit atomics (insert3d.cu)
+  const size_t bytes = std::max<size_t>((vox * 2 + 3) / 4 * 4, 256);
+  CSM_CUDA(cudaMalloc(&g->d_vol, bytes));
+  CSM_CUDA(cudaMemsetAsync(g->d_vol, 0, bytes, s));
   d.p = g->d_vol;
   d.resolution = resolution;
   {

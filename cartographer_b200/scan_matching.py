@@ -852,12 +852,34 @@ class DeviceHybridGrid:
                                       C.c_int64(len(val)), C.c_float(self.resolution),
                                       C.c_int32(device), C.byref(self._h)))
 
+    @classmethod
+    def empty(cls, resolution, device=0):
+        """The grid of a fresh submap: no voxels, filled by RangeDataInserter3D.Insert."""
+        return cls(_EmptyGrid(resolution, np.zeros((0, 3), np.int32), np.zeros(0, np.uint16)),
+                   device)
+
+    def read(self):
+        """(lo, values): the dense box, values[z, y, x] of voxel lo + (x, y, z)."""
+        lo, dims = np.zeros(3, np.int32), np.zeros(3, np.int32)
+        check(lib().csm_grid3d_read(self._h, ptr(lo, C.c_int32), ptr(dims, C.c_int32), None))
+        out = np.zeros(tuple(dims[::-1]), np.uint16)
+        check(lib().csm_grid3d_read(self._h, ptr(lo, C.c_int32), ptr(dims, C.c_int32),
+                                    ptr(out, C.c_uint16)))
+        return lo, out
+
     def close(self):
         if getattr(self, "_h", None):
             lib().csm_grid3d_destroy(self._h)
             self._h = None
 
     __del__ = close
+
+
+@dataclass
+class _EmptyGrid:
+    resolution: float
+    indices: np.ndarray
+    values: np.ndarray
 
 
 @dataclass
@@ -888,9 +910,88 @@ class DeviceIntensityGrid:
             C.c_int64(len(counts)), C.c_float(self.resolution), C.c_int32(device),
             C.byref(self._h)))
 
+    @classmethod
+    def empty(cls, resolution, device=0):
+        """The intensity grid of a fresh submap: no voxels."""
+        return cls(IntensityGridSpec(resolution, np.zeros((0, 3), np.int32),
+                                     np.zeros(0, np.float32), np.zeros(0, np.int32)), device)
+
+    def read(self):
+        """(lo, mean, sum, count): the dense box, each indexed [z, y, x] from voxel lo;
+        mean is GetIntensity, sum / count each voxel's AverageIntensityData."""
+        lo, dims = np.zeros(3, np.int32), np.zeros(3, np.int32)
+        check(lib().csm_intensity_grid3d_read(self._h, ptr(lo, C.c_int32), ptr(dims, C.c_int32),
+                                              None, None, None))
+        shape = tuple(dims[::-1])
+        mean, sums = np.zeros(shape, np.float32), np.zeros(shape, np.float32)
+        counts = np.zeros(shape, np.int32)
+        check(lib().csm_intensity_grid3d_read(
+            self._h, ptr(lo, C.c_int32), ptr(dims, C.c_int32), ptr(mean, C.c_float),
+            ptr(sums, C.c_float), ptr(counts, C.c_int32)))
+        return lo, mean, sums, counts
+
     def close(self):
         if getattr(self, "_h", None):
             lib().csm_intensity_grid3d_destroy(self._h)
+            self._h = None
+
+    __del__ = close
+
+
+# ===========================================================================
+# RangeDataInserter3D (mapping/3d/range_data_inserter_3d.h)
+# ===========================================================================
+class CsmRangeInserterOptions3D(C.Structure):
+    _fields_ = [("hit_probability", C.c_double), ("miss_probability", C.c_double),
+                ("num_free_space_voxels", C.c_int32), ("intensity_threshold", C.c_float)]
+
+
+@dataclass
+class RangeDataInserterOptions3D:
+    """proto RangeDataInserterOptions3D (mapping/proto/range_data_inserter_options_3d.proto);
+    defaults are configuration_files/trajectory_builder_3d.lua's submaps.range_data_inserter."""
+    hit_probability: float = 0.55
+    miss_probability: float = 0.49
+    num_free_space_voxels: int = 2
+    intensity_threshold: float = 40.0
+
+    def _c(self):
+        return CsmRangeInserterOptions3D(self.hit_probability, self.miss_probability,
+                                         self.num_free_space_voxels, self.intensity_threshold)
+
+
+class RangeDataInserter3D:
+    """Insert(origin, returns, intensities, grid, intensity_grid=None) writes one scan into a
+    DeviceHybridGrid and, with intensities, a DeviceIntensityGrid, as the reference's
+    RangeDataInserter3D::Insert writes a HybridGrid / IntensityHybridGrid.  origin (3) and
+    returns (n x 3) are in the grid's frame; intensities (n) may be None."""
+
+    def __init__(self, options, device=0):
+        self.options = options
+        self.last_stats = None
+        self._h = C.c_void_p()
+        o = options._c()
+        check(lib().csm_range_inserter3d_create(C.byref(o), C.c_int32(device),
+                                                C.byref(self._h)))
+
+    def Insert(self, origin, returns, intensities, grid, intensity_grid=None):
+        org = np.ascontiguousarray(origin, dtype=np.float32).reshape(3)
+        xyz = _f32(returns)
+        inten = None
+        if intensities is not None:
+            inten = np.ascontiguousarray(intensities, dtype=np.float32).reshape(-1)
+            if len(inten) != len(xyz):
+                raise ValueError("intensities and returns differ in length")
+        stats = CsmStats()
+        check(lib().csm_range_inserter3d_insert(
+            self._h, ptr(org, C.c_float), ptr(xyz, C.c_float),
+            None if inten is None else ptr(inten, C.c_float), C.c_int32(len(xyz)), grid._h,
+            None if intensity_grid is None else intensity_grid._h, C.byref(stats)))
+        self.last_stats = stats.as_dict()
+
+    def close(self):
+        if getattr(self, "_h", None):
+            lib().csm_range_inserter3d_destroy(self._h)
             self._h = None
 
     __del__ = close

@@ -661,6 +661,45 @@ csm_status csm_ceres_match3d_intensity_batch(
     const csm_ceres_intensity_options3d* intensity_options, csm_ceres_result3d* results,
     csm_stats* stats /* may be NULL */);
 
+/* ---- map writing in 3D: RangeDataInserter3D on device grids --------------------------- */
+/* RangeDataInserter3D (mapping/3d/range_data_inserter_3d.cc:71-114) applied in place to a
+ * csm_grid3d and, optionally, a csm_intensity_grid3d, so that the handles the 3D matchers read
+ * follow the submap without a rebuild.  Every voxel ends bit-equal to what the reference's
+ * Insert + FinishUpdate leaves: hits apply the hit table, misses (the last
+ * num_free_space_voxels samples of each ray) the miss table, each cell at most once per insert
+ * and hits first; intensities (returns not brighter than intensity_threshold) are added per
+ * voxel in return order.  A handle's dense box grows as an insert reaches past it (DESIGN §9).
+ * No match may be in flight on a handle being inserted into. */
+typedef struct csm_range_inserter_options3d {   /* proto RangeDataInserterOptions3D */
+  double hit_probability;                       /* in (0.5, 1) */
+  double miss_probability;                      /* in [0, 0.5) */
+  int32_t num_free_space_voxels;                /* >= 0 */
+  float intensity_threshold;
+} csm_range_inserter_options3d;
+/* Owns the hit and miss tables (ComputeLookupTableToApplyOdds, probability_values.cc:76-87)
+ * on one device. */
+typedef struct csm_range_inserter3d csm_range_inserter3d;
+csm_status csm_range_inserter3d_create(const csm_range_inserter_options3d* options,
+                                       int32_t device, csm_range_inserter3d** out);
+csm_status csm_range_inserter3d_destroy(csm_range_inserter3d* inserter);
+/* RangeDataInserter3D::Insert.  origin and returns (num_returns x {x, y, z}) are in the grid's
+ * frame; intensities (num_returns floats) may be NULL, and intensity_grid may be NULL.
+ * CSM_E_INVALID, with every handle unchanged, for an origin, hit or intensity cell outside
+ * [-8192, 8192)^3 or grids on another device than the inserter.  stats (may be NULL) gets
+ * host_syncs and device_ms. */
+csm_status csm_range_inserter3d_insert(const csm_range_inserter3d* inserter,
+                                       const float origin[3], const float* returns,
+                                       const float* intensities, int32_t num_returns,
+                                       csm_grid3d* grid, csm_intensity_grid3d* intensity_grid,
+                                       csm_stats* stats /* may be NULL */);
+/* Test hooks: a handle's current dense box.  With out / mean == NULL only lo and dims are
+ * written; otherwise the box is copied out (((z - lo.z) * dims.y + (y - lo.y)) * dims.x +
+ * (x - lo.x)).  For an intensity grid, sum and count (each may be NULL) are every voxel's
+ * AverageIntensityData and mean its GetIntensity. */
+csm_status csm_grid3d_read(const csm_grid3d* grid, int32_t lo[3], int32_t dims[3], uint16_t* out);
+csm_status csm_intensity_grid3d_read(const csm_intensity_grid3d* grid, int32_t lo[3],
+                                     int32_t dims[3], float* mean, float* sum, int32_t* count);
+
 /* Test hook: as csm_ceres_evaluate3d, in the problem's residual-block order — per cloud its
  * occupied-space residuals, then its intensity residuals if it has a grid; then 3
  * translation and 3 rotation residuals.  Residuals and rows are uncorrected by the loss, as
