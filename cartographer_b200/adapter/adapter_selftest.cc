@@ -390,5 +390,52 @@ int main() {
       std::printf(" %08x:%08x:%d", Bits(mean[i]), Bits(sum[i]), count[i]);
     std::printf("\n");
   }
+  // ---- ProbabilityGridRangeDataInserter2D on a device grid: the reference's InsertPointCloud
+  // (range_data_inserter_2d_test.cc:47-58) with one miss, then a return that makes the grid
+  // grow; the cropped grid and a stack built from it ----
+  {
+    mapping::proto::ProbabilityGridRangeDataInserterOptions2D io;
+    io.set_hit_probability(0.7);
+    io.set_miss_probability(0.4);
+    io.set_insert_free_space(true);
+    const mapping::scan_matching::ProbabilityGridRangeDataInserter2D inserter(io);
+    mapping::scan_matching::DeviceGrid2D grid(
+        mapping::MapLimits(1., 1., 5., mapping::CellLimits{5, 5}), 0);
+    sensor::RangeData range_data;
+    range_data.origin = {{-0.5f, 0.5f, 0.f}};
+    range_data.returns = sensor::PointCloud(
+        {{{{-3.5f, 0.5f, 0.f}}}, {{{-2.5f, 1.5f, 0.f}}}, {{{-1.5f, 2.5f, 0.f}}},
+         {{{-0.5f, 3.5f, 0.f}}}},
+        {});
+    range_data.misses = sensor::PointCloud({{{{0.5f, 4.5f, 0.f}}}}, {});
+    inserter.Insert(range_data, &grid);
+    sensor::RangeData far;
+    far.origin = {{-0.5f, 0.5f, 0.f}};
+    far.returns = sensor::PointCloud({{{{-6.5f, 0.5f, 0.f}}}}, {});
+    inserter.Insert(far, &grid);
+    const std::unique_ptr<mapping::scan_matching::DeviceGrid2D> cropped = grid.ComputeCroppedGrid();
+    for (const mapping::scan_matching::DeviceGrid2D* g : {&grid, cropped.get()}) {
+      std::vector<uint16_t> cells;
+      const csm_rt_grid2d_info info = g->Read(&cells);
+      std::printf("RESULT %s %.17g %.17g %.17g %d %d %d %d %d %d %d", g == &grid ? "insert2d" : "crop2d",
+                  info.resolution, info.max_x, info.max_y, info.num_x_cells, info.num_y_cells,
+                  info.known_empty, info.known_min_x, info.known_min_y, info.known_max_x,
+                  info.known_max_y);
+      for (uint16_t v : cells) std::printf(" %u", v);
+      std::printf("\n");
+    }
+    mapping::scan_matching::proto::FastCorrelativeScanMatcherOptions2D fo;
+    fo.set_linear_search_window(3.);
+    fo.set_angular_search_window(0.5);
+    fo.set_branch_and_bound_depth(2);
+    const mapping::scan_matching::FastCorrelativeScanMatcher2D matcher(*cropped, fo);
+    int32_t wx = 0, wy = 0;
+    if (csm_stack2d_read_level(matcher.stack(), 1, nullptr, &wx, &wy) != CSM_OK) return 1;
+    std::vector<uint8_t> level(static_cast<size_t>(wx) * wy);
+    if (csm_stack2d_read_level(matcher.stack(), 1, level.data(), &wx, &wy) != CSM_OK) return 1;
+    std::printf("RESULT stack2d %d %d", wx, wy);
+    for (uint8_t v : level) std::printf(" %u", v);
+    std::printf("\n");
+  }
   return 0;
 }

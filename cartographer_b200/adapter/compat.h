@@ -92,6 +92,19 @@ class RangeDataInserterOptions3D {
   int nfsv_ = 0;
   float threshold_ = 0.f;
 };
+// mapping/proto/probability_grid_range_data_inserter_options_2d.proto
+class ProbabilityGridRangeDataInserterOptions2D {
+ public:
+  double hit_probability() const { return hit_; }
+  double miss_probability() const { return miss_; }
+  bool insert_free_space() const { return insert_free_space_; }
+  void set_hit_probability(double v) { hit_ = v; }
+  void set_miss_probability(double v) { miss_ = v; }
+  void set_insert_free_space(bool v) { insert_free_space_ = v; }
+ private:
+  double hit_ = 0., miss_ = 0.;
+  bool insert_free_space_ = true;
+};
 }  // namespace proto
 }  // namespace mapping
 

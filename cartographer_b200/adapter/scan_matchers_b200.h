@@ -30,6 +30,7 @@
 #include "cartographer/mapping/proto/scan_matching/fast_correlative_scan_matcher_options_2d.pb.h"
 #include "cartographer/mapping/proto/scan_matching/real_time_correlative_scan_matcher_options.pb.h"
 #include "cartographer/mapping/proto/range_data_inserter_options_3d.pb.h"
+#include "cartographer/mapping/proto/probability_grid_range_data_inserter_options_2d.pb.h"
 #include "cartographer/sensor/point_cloud.h"
 #include "cartographer/sensor/range_data.h"
 #include "cartographer/transform/rigid_transform.h"
@@ -66,9 +67,15 @@ inline std::vector<float> Flatten(const sensor::PointCloud& point_cloud) {
 }
 }  // namespace b200_internal
 
+class DeviceGrid2D;
+
 // fast_correlative_scan_matcher_2d.h:112-136
 class FastCorrelativeScanMatcher2D {
  public:
+  // The stack of a submap whose grid lives on the device (a DeviceGrid2D::ComputeCroppedGrid
+  // result, as Submap2D::Finish leaves it): built from the device cells.
+  FastCorrelativeScanMatcher2D(const DeviceGrid2D& grid,
+                               const proto::FastCorrelativeScanMatcherOptions2D& options);
   FastCorrelativeScanMatcher2D(const Grid2D& grid,
                                const proto::FastCorrelativeScanMatcherOptions2D& options,
                                int device = 0)
@@ -242,13 +249,83 @@ class DeviceGrid2D {
         grid.correspondence_cost_cells().data(), l.cell_limits().num_x_cells,
         l.cell_limits().num_y_cells, l.resolution(), l.max().x(), l.max().y(), device, &grid_));
   }
+  // ProbabilityGrid(limits): the all-unknown grid ActiveSubmaps2D::CreateGrid makes, filled
+  // by ProbabilityGridRangeDataInserter2D below.
+  DeviceGrid2D(const MapLimits& limits, int device) {
+    b200_internal::Check(csm_rt_grid2d_create_empty(
+        limits.resolution(), limits.max().x(), limits.max().y(),
+        limits.cell_limits().num_x_cells, limits.cell_limits().num_y_cells, device, &grid_));
+  }
   ~DeviceGrid2D() { csm_rt_grid2d_destroy(grid_); }
   DeviceGrid2D(const DeviceGrid2D&) = delete;
   DeviceGrid2D& operator=(const DeviceGrid2D&) = delete;
   const csm_rt_grid2d* handle() const { return grid_; }
+  csm_rt_grid2d* mutable_handle() { return grid_; }
+
+  // ProbabilityGrid::ComputeCroppedGrid (probability_grid.cc:91-107), device to device.
+  std::unique_ptr<DeviceGrid2D> ComputeCroppedGrid() const {
+    csm_rt_grid2d* cropped = nullptr;
+    b200_internal::Check(csm_rt_grid2d_crop(grid_, &cropped));
+    return std::unique_ptr<DeviceGrid2D>(new DeviceGrid2D(cropped));
+  }
+  // limits(), the known-cells box and, with cells != nullptr, the cells (num_y x num_x):
+  // what Submap2D::ToProto serialises.
+  csm_rt_grid2d_info Read(std::vector<uint16_t>* cells) const {
+    csm_rt_grid2d_info info;
+    b200_internal::Check(csm_rt_grid2d_read(grid_, &info, nullptr, 0));
+    if (cells != nullptr) {
+      cells->resize(static_cast<size_t>(info.num_x_cells) * info.num_y_cells);
+      b200_internal::Check(csm_rt_grid2d_read(grid_, &info, cells->data(),
+                                              static_cast<int64_t>(cells->size())));
+    }
+    return info;
+  }
 
  private:
+  explicit DeviceGrid2D(csm_rt_grid2d* grid) : grid_(grid) {}
   csm_rt_grid2d* grid_ = nullptr;
+};
+
+inline FastCorrelativeScanMatcher2D::FastCorrelativeScanMatcher2D(
+    const DeviceGrid2D& grid, const proto::FastCorrelativeScanMatcherOptions2D& options)
+    : options_(options) {
+  b200_internal::Check(csm_stack2d_create_from_rt_grid2d(
+      grid.handle(), options.branch_and_bound_depth(), &stack_));
+}
+
+// mapping/2d/probability_grid_range_data_inserter_2d.h:33-52 on device grids: Submap2D
+// (submap_2d.cc) keeps its grid as a DeviceGrid2D and inserts every scan in place, so the
+// real-time matcher and CeresScanMatcher2D read the updated submap without a re-upload, and
+// Submap2D::Finish crops it on the device.
+class ProbabilityGridRangeDataInserter2D {
+ public:
+  explicit ProbabilityGridRangeDataInserter2D(
+      const mapping::proto::ProbabilityGridRangeDataInserterOptions2D& options, int device = 0) {
+    csm_range_inserter_options2d o{};
+    o.hit_probability = options.hit_probability();
+    o.miss_probability = options.miss_probability();
+    o.insert_free_space = options.insert_free_space() ? 1 : 0;
+    b200_internal::Check(csm_range_inserter2d_create(&o, device, &inserter_));
+  }
+  ~ProbabilityGridRangeDataInserter2D() { csm_range_inserter2d_destroy(inserter_); }
+  ProbabilityGridRangeDataInserter2D(const ProbabilityGridRangeDataInserter2D&) = delete;
+  ProbabilityGridRangeDataInserter2D& operator=(const ProbabilityGridRangeDataInserter2D&) =
+      delete;
+
+  // probability_grid_range_data_inserter_2d.cc:124-133; range_data in the grid's frame.
+  void Insert(const sensor::RangeData& range_data, DeviceGrid2D* grid) const {
+    if (grid == nullptr) std::abort();  // CHECK(:127)
+    const std::vector<float> returns = b200_internal::Flatten(range_data.returns);
+    const std::vector<float> misses = b200_internal::Flatten(range_data.misses);
+    const float origin[3] = {range_data.origin.x(), range_data.origin.y(), range_data.origin.z()};
+    b200_internal::Check(csm_range_inserter2d_insert(
+        inserter_, origin, returns.data(), static_cast<int32_t>(range_data.returns.size()),
+        misses.data(), static_cast<int32_t>(range_data.misses.size()), grid->mutable_handle(),
+        nullptr));
+  }
+
+ private:
+  csm_range_inserter2d* inserter_ = nullptr;
 };
 
 // ceres_scan_matcher_2d.h:42-64.  Same constructor and Match signature, except that the

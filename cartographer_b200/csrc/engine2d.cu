@@ -9,6 +9,7 @@
 // build has no FMA (cmake/functions.cmake:100-101).  Transcendentals are
 // evaluated on the host with libm, like the reference.
 #include "engine2d.cuh"
+#include "rtgrid.cuh"
 
 #include <algorithm>
 #include <chrono>
@@ -1549,7 +1550,9 @@ int DivUp(long long a, long long b) { return static_cast<int>((a + b - 1) / b); 
 
 // Fills every layout of the stack (levels, decimated copies, child windows) from the
 // grid's cells; caller holds ctx->mu.  Shared by csm_stack2d_create and csm_stack2d_update.
-static csm_status BuildStack2D(csm_stack2d* st, const uint16_t* cells) {
+// `cells` are host memory with row pitch nx, or (device_pitch > 0) a device array with row
+// pitch device_pitch cells (csm_stack2d_create_from_rt_grid2d).
+static csm_status BuildStack2D(csm_stack2d* st, const uint16_t* cells, int device_pitch = 0) {
   Ctx* ctx = st->ctx;
   const StackDev& h = st->h;
   const int nx = h.nx, ny = h.ny, depth = h.depth, top = depth - 1;
@@ -1563,8 +1566,13 @@ static csm_status BuildStack2D(csm_stack2d* st, const uint16_t* cells) {
   const size_t ncell = static_cast<size_t>(nx) * ny;
   CSM_TRY(d_cells.Reserve(ncell * sizeof(uint16_t)));
   CSM_TRY(d_lut.Reserve(65536));
-  CSM_CUDA(cudaMemcpyAsync(d_cells.p, cells, ncell * sizeof(uint16_t), cudaMemcpyHostToDevice,
-                           ctx->stream));
+  if (device_pitch > 0)
+    CSM_CUDA(cudaMemcpy2DAsync(d_cells.p, static_cast<size_t>(nx) * 2, cells,
+                               static_cast<size_t>(device_pitch) * 2, static_cast<size_t>(nx) * 2,
+                               ny, cudaMemcpyDeviceToDevice, ctx->stream));
+  else
+    CSM_CUDA(cudaMemcpyAsync(d_cells.p, cells, ncell * sizeof(uint16_t), cudaMemcpyHostToDevice,
+                             ctx->stream));
   CSM_CUDA(cudaMemcpyAsync(d_lut.p, lut.data(), 65536, cudaMemcpyHostToDevice, ctx->stream));
   k_stack_level0<<<DivUp(ncell, 256), 256, 0, ctx->stream>>>(
       d_cells.as<uint16_t>(), d_lut.as<uint8_t>(), st->d_levels + st->level_off[0],
@@ -1591,11 +1599,12 @@ static csm_status BuildStack2D(csm_stack2d* st, const uint16_t* cells) {
   return CSM_OK;
 }
 
-extern "C" {
-
-csm_status csm_stack2d_create(const uint16_t* cells, int32_t nx, int32_t ny, double resolution,
-                              double max_x, double max_y, float min_cost, float max_cost,
-                              int32_t depth, int32_t device, csm_stack2d** out) {
+// csm_stack2d_create over host cells (device_pitch == 0) or over a device array of row
+// pitch device_pitch cells; `locked` says the caller already holds the device's ctx->mu.
+static csm_status CreateStack2D(const uint16_t* cells, int device_pitch, bool locked, int32_t nx,
+                                int32_t ny, double resolution, double max_x, double max_y,
+                                float min_cost, float max_cost, int32_t depth, int32_t device,
+                                csm_stack2d** out) {
   CSM_REQUIRE(out != nullptr && cells != nullptr, "null pointer");
   CSM_REQUIRE(nx >= 1 && ny >= 1, "cell limits must be >= 1");  // fast...2d.cc:100-102
   CSM_REQUIRE(depth >= 1 && depth <= kMaxDepth, "branch_and_bound_depth out of range");  // :174
@@ -1605,7 +1614,8 @@ csm_status csm_stack2d_create(const uint16_t* cells, int32_t nx, int32_t ny, dou
               static_cast<long long>(ny) + (1 << (depth - 1)) < 32000, "grid too large");
   Ctx* ctx;
   CSM_TRY(GetCtx(device, &ctx));
-  std::lock_guard<std::mutex> lock(ctx->mu);
+  std::unique_lock<std::mutex> lock(ctx->mu, std::defer_lock);
+  if (!locked) lock.lock();
   CSM_CUDA(cudaSetDevice(device));
   std::unique_ptr<csm_stack2d> st(new csm_stack2d);
   st->ctx = ctx;
@@ -1660,12 +1670,36 @@ csm_status csm_stack2d_create(const uint16_t* cells, int32_t nx, int32_t ny, dou
   if (win_total) CSM_CUDA(cudaMalloc(&st->d_win, win_total * sizeof(unsigned)));
   for (int l = 1; l < depth; ++l) h.win[l] = st->d_win + win_off[l];
   for (int l = 1; l < depth; ++l) st->win_off[l] = win_off[l];
-  CSM_TRY(BuildStack2D(st.get(), cells));
+  CSM_TRY(BuildStack2D(st.get(), cells, device_pitch));
   CSM_CUDA(cudaMalloc(&st->d, sizeof(StackDev)));
   CSM_CUDA(cudaMemcpyAsync(st->d, &h, sizeof(StackDev), cudaMemcpyHostToDevice, ctx->stream));
   CSM_CUDA(cudaStreamSynchronize(ctx->stream));
   *out = st.release();
   return CSM_OK;
+}
+
+extern "C" {
+
+csm_status csm_stack2d_create(const uint16_t* cells, int32_t nx, int32_t ny, double resolution,
+                              double max_x, double max_y, float min_cost, float max_cost,
+                              int32_t depth, int32_t device, csm_stack2d** out) {
+  return CreateStack2D(cells, 0, false, nx, ny, resolution, max_x, max_y, min_cost, max_cost,
+                       depth, device, out);
+}
+
+// The PrecomputationGridStack2D constructor over a ProbabilityGrid handle: level 0 is built
+// from the handle's device cells (one device-to-device copy into the stack's scratch), with
+// the ProbabilityGrid's cost bounds (probability_grid.cc:27-31).
+csm_status csm_stack2d_create_from_rt_grid2d(const csm_rt_grid2d* grid, int32_t depth,
+                                             csm_stack2d** out) {
+  CSM_REQUIRE(grid != nullptr && out != nullptr, "null pointer");
+  CSM_REQUIRE(grid->d_wcells == nullptr, "a TSDF2D handle has no precomputation stack");
+  std::lock_guard<std::mutex> lock(grid->ctx->mu);
+  const float kMinCorrespondenceCost = 1.f - (1.f - 0.1f);   // probability_values.h:64-67
+  const float kMaxCorrespondenceCost = 1.f - 0.1f;
+  return CreateStack2D(grid->d_cells, grid->g.pitch, true, grid->g.nx, grid->g.ny,
+                       grid->g.resolution, grid->g.max_x, grid->g.max_y, kMinCorrespondenceCost,
+                       kMaxCorrespondenceCost, depth, grid->ctx->device, out);
 }
 
 csm_status csm_stack2d_destroy(csm_stack2d* stack) {

@@ -418,29 +418,7 @@ csm_status GridCreate(const uint16_t* cells, const uint16_t* wcells, float trunc
   d.cells = g->d_cells;
   d.wcells = g->d_wcells;
   CSM_TRY(UploadCells(g.get(), cells, wcells, ctx->stream));
-  // TMA box: as wide as the (padded) grid up to 256 cells, as many rows as fit the tile
-  d.bw = std::min(d.pitch, 256);
-  d.bh = std::max(1, std::min(std::min(ny, 256), kRtTileBytes / (d.bw * 2)));
-  if (!wcells) {
-    EncodeTiledFn encode = GetEncodeTiled();
-    if (encode) {
-      const cuuint64_t dims[2] = {static_cast<cuuint64_t>(nx), static_cast<cuuint64_t>(ny)};
-      const cuuint64_t strides[1] = {static_cast<cuuint64_t>(d.pitch) * 2};
-      const cuuint32_t box[2] = {static_cast<cuuint32_t>(d.bw), static_cast<cuuint32_t>(d.bh)};
-      const cuuint32_t estr[2] = {1, 1};
-      const CUresult r = encode(&g->tmap, CU_TENSOR_MAP_DATA_TYPE_UINT16, 2, g->d_cells, dims,
-                                strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                                CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-                                CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-      g->has_tmap = r == CUDA_SUCCESS;
-    }
-    if (!g->has_tmap) {
-      SetError("cuTensorMapEncodeTiled is unavailable or failed");
-      return CSM_E_CUDA;
-    }
-  } else {
-    std::memset(&g->tmap, 0, sizeof(g->tmap));
-  }
+  CSM_TRY(RtGridEncodeTmap(g.get()));
   CSM_CUDA(cudaStreamSynchronize(ctx->stream));
   *out = g.release();
   return CSM_OK;
@@ -758,6 +736,39 @@ csm_status RtMatchHostGrid(const uint16_t* cells, const uint16_t* weight_cells, 
 
 }  // namespace
 
+namespace csm {
+
+csm_status RtGridEncodeTmap(csm_rt_grid2d* g) {
+  RtGridDev& d = g->g;
+  // TMA box: as wide as the (padded) grid up to 256 cells, as many rows as fit the tile
+  d.bw = std::min(d.pitch, 256);
+  d.bh = std::max(1, std::min(std::min(d.ny, 256), kRtTileBytes / (d.bw * 2)));
+  g->has_tmap = false;
+  if (g->d_wcells) {
+    std::memset(&g->tmap, 0, sizeof(g->tmap));
+    return CSM_OK;
+  }
+  EncodeTiledFn encode = GetEncodeTiled();
+  if (encode) {
+    const cuuint64_t dims[2] = {static_cast<cuuint64_t>(d.nx), static_cast<cuuint64_t>(d.ny)};
+    const cuuint64_t strides[1] = {static_cast<cuuint64_t>(d.pitch) * 2};
+    const cuuint32_t box[2] = {static_cast<cuuint32_t>(d.bw), static_cast<cuuint32_t>(d.bh)};
+    const cuuint32_t estr[2] = {1, 1};
+    const CUresult r = encode(&g->tmap, CU_TENSOR_MAP_DATA_TYPE_UINT16, 2, g->d_cells, dims,
+                              strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+                              CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
+                              CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    g->has_tmap = r == CUDA_SUCCESS;
+  }
+  if (!g->has_tmap) {
+    SetError("cuTensorMapEncodeTiled is unavailable or failed");
+    return CSM_E_CUDA;
+  }
+  return CSM_OK;
+}
+
+}  // namespace csm
+
 extern "C" {
 
 csm_status csm_rt_grid2d_create(const uint16_t* cells, int32_t nx, int32_t ny, double resolution,
@@ -772,6 +783,7 @@ csm_status csm_rt_grid2d_update(csm_rt_grid2d* grid, const uint16_t* cells) {
   std::lock_guard<std::mutex> lock(grid->ctx->mu);
   CSM_CUDA(cudaSetDevice(grid->ctx->device));
   CSM_TRY(UploadCells(grid, cells, nullptr, grid->ctx->stream));
+  grid->known_stale = true;
   CSM_CUDA(cudaStreamSynchronize(grid->ctx->stream));
   return CSM_OK;
 }

@@ -332,6 +332,28 @@ class CsmRtResult2D(C.Structure):
                 ("candidates_scored", C.c_int64)]
 
 
+class CsmRtGrid2DInfo(C.Structure):
+    _fields_ = [("num_x_cells", C.c_int32), ("num_y_cells", C.c_int32),
+                ("resolution", C.c_double), ("max_x", C.c_double), ("max_y", C.c_double),
+                ("known_min_x", C.c_int32), ("known_min_y", C.c_int32),
+                ("known_max_x", C.c_int32), ("known_max_y", C.c_int32),
+                ("known_empty", C.c_int32), ("is_tsdf", C.c_int32)]
+
+
+@dataclass
+class GridState:
+    """A ProbabilityGrid read back from the device: correspondence-cost cells[y, x], MapLimits
+    and the known-cells box (min_x, min_y, max_x, max_y), None when empty.  Usable wherever a
+    grid record is taken (FastCorrelativeScanMatcher2D, RealTimeGrid2D)."""
+    cells: np.ndarray
+    resolution: float
+    max_x: float
+    max_y: float
+    known_cells_box: object = None
+    min_cost: float = float(np.float32(1.0) - (np.float32(1.0) - np.float32(0.1)))
+    max_cost: float = float(np.float32(1.0) - np.float32(0.1))
+
+
 class RealTimeGrid2D:
     """A ProbabilityGrid or TSDF2D resident on the device (csm_rt_grid2d): what
     LocalTrajectoryBuilder2D's active submap grid is to the real-time matcher
@@ -364,6 +386,48 @@ class RealTimeGrid2D:
             C.c_double(grid.resolution), C.c_double(grid.max_x), C.c_double(grid.max_y),
             C.c_int32(device), C.byref(self._h)))
 
+    @classmethod
+    def empty(cls, resolution, max_x, max_y, num_x=100, num_y=100, device=0):
+        """An all-unknown ProbabilityGrid of the given limits (csm_rt_grid2d_create_empty), to
+        be filled by ProbabilityGridRangeDataInserter2D.Insert.  ActiveSubmaps2D::CreateGrid
+        makes a 100 x 100 grid with max = origin + 50 * resolution on both axes."""
+        self = cls.__new__(cls)
+        self.device, self.is_tsdf = device, False
+        self._h = C.c_void_p()
+        check(lib().csm_rt_grid2d_create_empty(
+            C.c_double(resolution), C.c_double(max_x), C.c_double(max_y), C.c_int32(num_x),
+            C.c_int32(num_y), C.c_int32(device), C.byref(self._h)))
+        self.shape = (num_y, num_x)
+        return self
+
+    def _info(self, cells=None):
+        info = CsmRtGrid2DInfo()
+        check(lib().csm_rt_grid2d_read(self._h, C.byref(info),
+                                       None if cells is None else ptr(cells, C.c_uint16),
+                                       C.c_int64(0 if cells is None else cells.size)))
+        self.shape = (info.num_y_cells, info.num_x_cells)
+        return info
+
+    def read(self):
+        """The grid as it is on the device: a GridState with cells[y, x], the limits and the
+        known-cells box (csm_rt_grid2d_read)."""
+        info = self._info()
+        cells = np.zeros((info.num_y_cells, info.num_x_cells), np.uint16)
+        info = self._info(cells)
+        box = None if info.known_empty else (info.known_min_x, info.known_min_y,
+                                             info.known_max_x, info.known_max_y)
+        return GridState(cells, info.resolution, info.max_x, info.max_y, box)
+
+    def ComputeCroppedGrid(self):
+        """ProbabilityGrid::ComputeCroppedGrid from device to device: a new RealTimeGrid2D over
+        the known-cells box (csm_rt_grid2d_crop)."""
+        out = RealTimeGrid2D.__new__(RealTimeGrid2D)
+        out.device, out.is_tsdf = self.device, False
+        out._h = C.c_void_p()
+        check(lib().csm_rt_grid2d_crop(self._h, C.byref(out._h)))
+        out._info()
+        return out
+
     def update(self, cells, weight_cells=None):
         cells = np.ascontiguousarray(cells, dtype=np.uint16)
         if cells.shape != self.shape:
@@ -387,6 +451,77 @@ class RealTimeGrid2D:
             self._h = None
 
     __del__ = close
+
+
+# ===========================================================================
+# ProbabilityGridRangeDataInserter2D (mapping/2d/probability_grid_range_data_inserter_2d.h)
+# ===========================================================================
+class CsmRangeInserterOptions2D(C.Structure):
+    _fields_ = [("hit_probability", C.c_double), ("miss_probability", C.c_double),
+                ("insert_free_space", C.c_int32), ("reserved", C.c_int32)]
+
+
+@dataclass
+class ProbabilityGridRangeDataInserterOptions2D:
+    """proto ProbabilityGridRangeDataInserterOptions2D; defaults are
+    configuration_files/trajectory_builder_2d.lua's submaps.range_data_inserter."""
+    hit_probability: float = 0.55
+    miss_probability: float = 0.49
+    insert_free_space: bool = True
+
+    def _c(self):
+        return CsmRangeInserterOptions2D(self.hit_probability, self.miss_probability,
+                                         1 if self.insert_free_space else 0, 0)
+
+
+class ProbabilityGridRangeDataInserter2D:
+    """Insert(origin, returns, grid, misses=None) writes one scan into a ProbabilityGrid
+    RealTimeGrid2D in place, as the reference's Insert(range_data, grid) writes a
+    ProbabilityGrid: origin (2 or 3), returns and misses (n x 3) are in the grid's frame.  The
+    grid grows as the reference's does, and its `shape` follows."""
+
+    def __init__(self, options=None, device=0):
+        self.options = options or ProbabilityGridRangeDataInserterOptions2D()
+        self.last_stats = None
+        self._h = C.c_void_p()
+        o = self.options._c()
+        check(lib().csm_range_inserter2d_create(C.byref(o), C.c_int32(device),
+                                                C.byref(self._h)))
+
+    def Insert(self, origin, returns, grid, misses=None):
+        org = np.zeros(3, np.float32)
+        o = np.asarray(origin, np.float32).reshape(-1)
+        org[:len(o)] = o[:3]
+        ret = _f32(np.zeros((0, 3)) if returns is None else returns)
+        mis = _f32(np.zeros((0, 3)) if misses is None else misses)
+        stats = CsmStats()
+        check(lib().csm_range_inserter2d_insert(
+            self._h, ptr(org, C.c_float), ptr(ret, C.c_float), C.c_int32(len(ret)),
+            ptr(mis, C.c_float), C.c_int32(len(mis)), grid._h, C.byref(stats)))
+        self.last_stats = stats.as_dict()
+        grid._info()
+
+    def close(self):
+        if getattr(self, "_h", None):
+            lib().csm_range_inserter2d_destroy(self._h)
+            self._h = None
+
+    __del__ = close
+
+
+def _fast_from_device_grid(cls, grid, options):
+    """FastCorrelativeScanMatcher2D over a ProbabilityGrid RealTimeGrid2D (typically a
+    ComputeCroppedGrid result): the stack is built from the device cells
+    (csm_stack2d_create_from_rt_grid2d)."""
+    self = cls.__new__(cls)
+    self.options, self.device, self.last_stats = options, grid.device, None
+    self._h = C.c_void_p()
+    check(lib().csm_stack2d_create_from_rt_grid2d(
+        grid._h, C.c_int32(options.branch_and_bound_depth), C.byref(self._h)))
+    return self
+
+
+FastCorrelativeScanMatcher2D.from_device_grid = classmethod(_fast_from_device_grid)
 
 
 def _rt_match_batch(self, initial_pose_estimates, point_clouds, rt_grid):

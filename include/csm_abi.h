@@ -700,6 +700,65 @@ csm_status csm_grid3d_read(const csm_grid3d* grid, int32_t lo[3], int32_t dims[3
 csm_status csm_intensity_grid3d_read(const csm_intensity_grid3d* grid, int32_t lo[3],
                                      int32_t dims[3], float* mean, float* sum, int32_t* count);
 
+/* ---- map writing in 2D: ProbabilityGridRangeDataInserter2D on device grids ------------ */
+/* ProbabilityGridRangeDataInserter2D (mapping/2d/probability_grid_range_data_inserter_2d.cc)
+ * applied in place to a ProbabilityGrid csm_rt_grid2d, so that a 2D submap lives on the device
+ * from its first scan to the stack it becomes.  After every insert, every cell, the limits and
+ * the known-cells box are bit-equal to what the reference's Insert + FinishUpdate leaves:
+ * returns apply the hit table, every pixel of each return's and each miss's RayToPixelMask the
+ * miss table (insert_free_space only), each cell at most once per insert and hits first.  The
+ * handle grows as Grid2D::GrowLimits does (doubling, old cells at the doubling offset).  A
+ * handle's cells must carry no kUpdateMarker, as the reference's FinishUpdate leaves them.  No
+ * match may be in flight on a handle being inserted into. */
+typedef struct csm_range_inserter_options2d {   /* proto ProbabilityGridRangeDataInserterOptions2D */
+  double hit_probability;                       /* in (0.5, 1) */
+  double miss_probability;                      /* in [0, 0.5) */
+  int32_t insert_free_space;                    /* bool */
+  int32_t reserved;
+} csm_range_inserter_options2d;
+/* Owns the hit and miss tables (ComputeLookupTableToApplyCorrespondenceCostOdds,
+ * probability_values.cc:89-105) on one device. */
+typedef struct csm_range_inserter2d csm_range_inserter2d;
+csm_status csm_range_inserter2d_create(const csm_range_inserter_options2d* options,
+                                       int32_t device, csm_range_inserter2d** out);
+csm_status csm_range_inserter2d_destroy(csm_range_inserter2d* inserter);
+/* ProbabilityGridRangeDataInserter2D::Insert(range_data, grid).  origin, returns (num_returns x
+ * {x, y, z}) and misses (num_misses x {x, y, z}) are in the grid's frame; z is ignored.
+ * CSM_E_INVALID, with the handle unchanged, for a TSDF2D handle, a null or non-finite input, a
+ * grid on another device, or an insert that would grow the grid to 30000 cells or more per
+ * axis.  One stream synchronisation; stats (may be NULL) gets host_syncs and device_ms. */
+csm_status csm_range_inserter2d_insert(const csm_range_inserter2d* inserter,
+                                       const float origin[3], const float* returns,
+                                       int32_t num_returns, const float* misses,
+                                       int32_t num_misses, csm_rt_grid2d* grid,
+                                       csm_stats* stats /* may be NULL */);
+/* ActiveSubmaps2D::CreateGrid (mapping/2d/submap_2d.cc): an all-unknown ProbabilityGrid of the
+ * given limits with an empty known-cells box. */
+csm_status csm_rt_grid2d_create_empty(double resolution, double max_x, double max_y,
+                                      int32_t num_x_cells, int32_t num_y_cells, int32_t device,
+                                      csm_rt_grid2d** out);
+/* ProbabilityGrid::ComputeCroppedGrid (probability_grid.cc:91-107) from device to device: a
+ * new handle over the known-cells box (1 x 1 if it is empty) whose known cells went through
+ * SetProbability(GetProbability(v)).  ProbabilityGrid handles only. */
+csm_status csm_rt_grid2d_crop(const csm_rt_grid2d* grid, csm_rt_grid2d** out);
+/* The PrecomputationGridStack2D constructor over a ProbabilityGrid handle: as csm_stack2d_create
+ * on the handle's cells and limits, with kMin/kMaxCorrespondenceCost, without a host copy. */
+csm_status csm_stack2d_create_from_rt_grid2d(const csm_rt_grid2d* grid,
+                                             int32_t branch_and_bound_depth, csm_stack2d** out);
+/* A handle's limits, its known-cells box (inclusive cell bounds; known_empty when there is
+ * none) and, with cells != NULL, its cells (num_y x num_x, row-major; capacity in cells).  A
+ * handle made by csm_rt_grid2d_create or refreshed by an update takes the bounding box of its
+ * non-zero cells as its known-cells box. */
+typedef struct csm_rt_grid2d_info {
+  int32_t num_x_cells, num_y_cells;
+  double resolution, max_x, max_y;
+  int32_t known_min_x, known_min_y, known_max_x, known_max_y;
+  int32_t known_empty;
+  int32_t is_tsdf;
+} csm_rt_grid2d_info;
+csm_status csm_rt_grid2d_read(const csm_rt_grid2d* grid, csm_rt_grid2d_info* info,
+                              uint16_t* cells, int64_t capacity);
+
 /* Test hook: as csm_ceres_evaluate3d, in the problem's residual-block order — per cloud its
  * occupied-space residuals, then its intensity residuals if it has a grid; then 3
  * translation and 3 rotation residuals.  Residuals and rows are uncorrected by the loss, as
