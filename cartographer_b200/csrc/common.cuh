@@ -48,6 +48,22 @@ extern std::atomic<int64_t> g_launches;
     if (_s != CSM_OK) return _s;          \
   } while (0)
 
+inline int DivUp(long long a, long long b) { return static_cast<int>((a + b - 1) / b); }
+
+// Host side of the engines' order-preserving float <-> unsigned map (bounds are kept as
+// unsigned so that atomicMax on them orders like the float scores).
+inline unsigned HostFloatToOrdered(float f) {
+  unsigned u;
+  std::memcpy(&u, &f, 4);
+  return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
+}
+inline float HostOrderedToFloat(unsigned u) {
+  u = (u & 0x80000000u) ? (u & 0x7fffffffu) : ~u;
+  float f;
+  std::memcpy(&f, &u, 4);
+  return f;
+}
+
 #define CSM_LAUNCH_CHECK()                                                          \
   do {                                                                              \
     ::csm::g_launches.fetch_add(1, std::memory_order_relaxed);                      \
@@ -116,6 +132,11 @@ struct Ctx {
     DevBuf& b = dev[name];
     b.stream = stream;
     return b;
+  }
+  // Workspace `name` with at least `bytes`, in *out.
+  csm_status Reserve(const char* name, size_t bytes, DevBuf** out) {
+    *out = &D(name);
+    return (*out)->Reserve(bytes);
   }
   PinnedBuf& P(const char* name) { return pin[name]; }
   // Recycled device buffers of destroyed point clouds (guarded by `mu`): node scans

@@ -71,17 +71,6 @@ __device__ __forceinline__ unsigned FloatToOrdered3(float f) {
 __device__ __forceinline__ float OrderedToFloat3(unsigned u) {
   return __uint_as_float((u & 0x80000000u) ? (u & 0x7fffffffu) : ~u);
 }
-static inline unsigned HostOrd(float f) {
-  unsigned u;
-  std::memcpy(&u, &f, 4);
-  return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
-}
-static inline float HostUnord(unsigned u) {
-  u = (u & 0x80000000u) ? (u & 0x7fffffffu) : ~u;
-  float f;
-  std::memcpy(&f, &u, 4);
-  return f;
-}
 
 struct F3 { float x, y, z; };
 __device__ __forceinline__ F3 Cross3(const F3& a, const F3& b) {
@@ -661,8 +650,6 @@ struct csm_matcher3d {
 
 namespace {
 
-int DivUp3(long long a, long long b) { return static_cast<int>((a + b - 1) / b); }
-
 // ---- Eigen semantics on the host (see oracle/oracle_3d.h for the provenance) ----
 struct Qf { float w, x, y, z; };
 struct Vf { float x, y, z; };
@@ -737,32 +724,17 @@ struct ScanPlan {
   int num_angles = 0;
 };
 
-// Test hooks csm_score_candidates3d / csm_score_top3d / csm_branch_step3d: a match that
-// scores a caller-given candidate list after discretisation (kList), stops after its dives
-// (kTop), or runs one level of the branch step over caller-given parents in place of the
-// level loop (kStep).
-struct Probe3D {
-  enum Mode { kList, kTop, kStep } mode = kTop;
-  // kList
-  const List3* list = nullptr;
-  int list_n = 0;
-  std::vector<int> sums;
-  std::vector<float> scores;
-  // kTop
-  int num_scans = 0, nxc = 0, nzc = 0, top_best = 0;
-  std::vector<int> angle, top_sums;
-  std::vector<float> rot;
-  // kStep
-  int level = 0;
-  const Node3* parents = nullptr;
-  int num_parents = 0;
-  float bound = 0.f;
-  std::vector<Node3> children;   // level >= 2
-  std::vector<Leaf3> leaves;     // level 1
-  // kTop and kStep: the bound afterwards, {candidates scored, parents expanded, gate evaluations}
-  float final_bound = 0.f;
-  unsigned long long counters[3] = {0, 0, 0};
-};
+// The level loop (see engine2d.cu): chunks of the queues, their capacity, the leaf lists and
+// the optimal leaves read back with the first (usually only) synchronise.
+constexpr int kChunk = 1 << 16;
+constexpr int kQueueCap = 8 * kChunk;
+constexpr int kLeafCap = 1 << 20;
+constexpr int kInlineBest = 256;
+// read-back area (pinned): control block | counters | first optimal leaves
+constexpr size_t kRbCtr = 4 * kC3Ints;
+constexpr size_t kRbBest = kRbCtr + 8 * 8;
+// Dives start only from scans whose best lowest-resolution sum is within 3 % of the best.
+constexpr float kDiveRatio = 0.97f;
 
 }  // namespace
 
@@ -872,7 +844,7 @@ csm_status csm_matcher3d_create(const int32_t* hi_idx, const uint16_t* hi_val, i
     CSM_TRY(d_val.Reserve(sizeof(uint16_t) * hi_n));
     CSM_CUDA(cudaMemcpyAsync(d_idx.p, hi_idx, sizeof(int) * 3 * hi_n, cudaMemcpyHostToDevice, s));
     CSM_CUDA(cudaMemcpyAsync(d_val.p, hi_val, sizeof(uint16_t) * hi_n, cudaMemcpyHostToDevice, s));
-    k3_scatter_u8<<<DivUp3(hi_n, 256), 256, 0, s>>>(d_idx.as<int>(), d_val.as<uint16_t>(), hi_n,
+    k3_scatter_u8<<<DivUp(hi_n, 256), 256, 0, s>>>(d_idx.as<int>(), d_val.as<uint16_t>(), hi_n,
                                                     d_lut.as<uint8_t>(), hs.level[0],
                                                     m->d_levels + off[0]);
     CSM_LAUNCH_CHECK();
@@ -910,7 +882,7 @@ csm_status csm_matcher3d_create(const int32_t* hi_idx, const uint16_t* hi_val, i
     CSM_TRY(d_val.Reserve(sizeof(uint16_t) * lo_n));
     CSM_CUDA(cudaMemcpyAsync(d_idx.p, lo_idx, sizeof(int) * 3 * lo_n, cudaMemcpyHostToDevice, s));
     CSM_CUDA(cudaMemcpyAsync(d_val.p, lo_val, sizeof(uint16_t) * lo_n, cudaMemcpyHostToDevice, s));
-    k3_scatter_u16<<<DivUp3(lo_n, 256), 256, 0, s>>>(d_idx.as<int>(), d_val.as<uint16_t>(), lo_n,
+    k3_scatter_u16<<<DivUp(lo_n, 256), 256, 0, s>>>(d_idx.as<int>(), d_val.as<uint16_t>(), lo_n,
                                                      hl, m->d_lowvol);
     CSM_LAUNCH_CHECK();
   }
@@ -970,22 +942,19 @@ csm_status csm_rotational_match3d(const float* submap_hist, const float* hist, i
   std::lock_guard<std::mutex> lock(ctx->mu);
   CSM_CUDA(cudaSetDevice(device));
   cudaStream_t s = ctx->stream;
-  DevBuf& a = ctx->D("rot_a");
-  DevBuf& b = ctx->D("rot_b");
-  DevBuf& c = ctx->D("rot_c");
-  DevBuf& d = ctx->D("rot_d");
-  CSM_TRY(a.Reserve(4 * n));
-  CSM_TRY(b.Reserve(4 * n));
-  CSM_TRY(c.Reserve(4 * num_angles));
-  CSM_TRY(d.Reserve(4 * num_angles));
-  CSM_CUDA(cudaMemcpyAsync(a.p, submap_hist, 4 * n, cudaMemcpyHostToDevice, s));
-  CSM_CUDA(cudaMemcpyAsync(b.p, hist, 4 * n, cudaMemcpyHostToDevice, s));
-  CSM_CUDA(cudaMemcpyAsync(c.p, angles, 4 * num_angles, cudaMemcpyHostToDevice, s));
-  k3_rotational<<<DivUp3(num_angles, 128), 128, 0, s>>>(a.as<float>(), b.as<float>(), n,
-                                                        initial_angle, c.as<float>(), num_angles,
-                                                        d.as<float>());
+  DevBuf *a, *b, *c, *d;
+  CSM_TRY(ctx->Reserve("rot_a", 4 * n, &a));
+  CSM_TRY(ctx->Reserve("rot_b", 4 * n, &b));
+  CSM_TRY(ctx->Reserve("rot_c", 4 * num_angles, &c));
+  CSM_TRY(ctx->Reserve("rot_d", 4 * num_angles, &d));
+  CSM_CUDA(cudaMemcpyAsync(a->p, submap_hist, 4 * n, cudaMemcpyHostToDevice, s));
+  CSM_CUDA(cudaMemcpyAsync(b->p, hist, 4 * n, cudaMemcpyHostToDevice, s));
+  CSM_CUDA(cudaMemcpyAsync(c->p, angles, 4 * num_angles, cudaMemcpyHostToDevice, s));
+  k3_rotational<<<DivUp(num_angles, 128), 128, 0, s>>>(a->as<float>(), b->as<float>(), n,
+                                                        initial_angle, c->as<float>(), num_angles,
+                                                        d->as<float>());
   CSM_LAUNCH_CHECK();
-  CSM_CUDA(cudaMemcpyAsync(scores, d.p, 4 * num_angles, cudaMemcpyDeviceToHost, s));
+  CSM_CUDA(cudaMemcpyAsync(scores, d->p, 4 * num_angles, cudaMemcpyDeviceToHost, s));
   CSM_CUDA(cudaStreamSynchronize(s));
   return CSM_OK;
 }
@@ -1086,456 +1055,436 @@ static csm_status MakeSearch3(const csm_matcher3d* m, float max_range, const dou
   return CSM_OK;
 }
 
-// One match = one stream of launches + one synchronisation.  `dev` (optional) carries the
-// node's clouds already on the device.  `probe` (may be null) turns the call into a Probe3D.
-static csm_status Run3D(Ctx* ctx, const csm_matcher3d* m, const csm_node3d* node,
-                        const NodeDev3* dev, const double node_pose[7],
-                        const double submap_pose[7], int full, float min_score,
-                        csm_result3d* result, csm_stats* stats, bool discretize_only,
-                        int32_t* out_num_scans, int32_t* out_cells, float* out_poses,
-                        float* out_rot, Probe3D* probe = nullptr) {
-  CSM_CUDA(cudaSetDevice(ctx->device));
-  cudaStream_t s = ctx->stream;
-  const float max_range = dev ? dev->max_range : MaxRange3(node);
+namespace {
+
+// One 3D match: its search, scan plan, job record, staging layout, control block and
+// read-back area.  Match3D runs the phases below over it in order; the test hooks run the
+// ones they need.
+struct Match3 {
+  Ctx* ctx = nullptr;
+  cudaStream_t s = nullptr;
+  const csm_matcher3d* m = nullptr;
+  const csm_node3d* node = nullptr;
+  const NodeDev3* dev = nullptr;  // the node's clouds already on the device (optional)
+  float min_score = 0.f;
   HostSearch3 sp;
-  CSM_TRY(MakeSearch3(m, max_range, node_pose, submap_pose, full, &sp));
   ScanPlan plan;
   float initial_angle = 0.f;
-  CSM_TRY(PlanScans(m, node, max_range, sp, &plan, &initial_angle));
-  const int A = plan.num_angles;
-  if (result) std::memset(result, 0, sizeof(*result));
-  if (stats) std::memset(stats, 0, sizeof(*stats));
-  const int n_hi = node->num_high, n_lo = node->num_low, hn = node->histogram_size;
-  if (!discretize_only) CSM_REQUIRE(n_lo >= 1, "empty low-resolution point cloud");
-  const int hmax = m->hs.depth - 1;
-  if (!discretize_only && hmax == 0) {
+  int hmax = 0;
+  Job3 jb;
+  long long per_scan = 0, max_top = 0;
+  // uploads through pinned staging: scans | angles | ones | histogram | clouds
+  size_t o_ang = 0, o_hist = 0;
+  const char* dup = nullptr;
+  DevBuf *d_scans = nullptr, *d_sel = nullptr, *d_rot = nullptr, *d_cells = nullptr,
+         *d_top = nullptr, *d_ctr = nullptr;
+  DevBuf *d_qtop = nullptr, *d_q = nullptr, *d_leaves = nullptr, *d_best = nullptr;
+  unsigned long long* ctr = nullptr;
+  int* ictr = nullptr;    // the control block (kC3*)
+  unsigned* lb = nullptr;
+  // read-back area (pinned): control block | counters | first optimal leaves
+  PinnedBuf* pin = nullptr;
+  int* hp = nullptr;
+  const unsigned long long* hctr = nullptr;
+  const BestLeaf3* best_inline = nullptr;
+  int host_syncs = 0;
+
+  Node3* Queue(int h) const {
+    return h == hmax ? d_qtop->as<Node3>() : d_q->as<Node3>() + static_cast<size_t>(kQueueCap) * h;
+  }
+};
+
+// Host plan: the search, the scan poses of every angle and the lowest-resolution lattice.
+csm_status Plan3D(Match3& x, Ctx* ctx, const csm_matcher3d* m, const csm_node3d* node,
+                  const NodeDev3* dev, const double node_pose[7], const double submap_pose[7],
+                  int full, float min_score) {
+  x.ctx = ctx;
+  x.s = ctx->stream;
+  x.m = m;
+  x.node = node;
+  x.dev = dev;
+  x.min_score = min_score;
+  CSM_CUDA(cudaSetDevice(ctx->device));
+  const float max_range = dev ? dev->max_range : MaxRange3(node);
+  CSM_TRY(MakeSearch3(m, max_range, node_pose, submap_pose, full, &x.sp));
+  CSM_TRY(PlanScans(m, node, max_range, x.sp, &x.plan, &x.initial_angle));
+  x.hmax = m->hs.depth - 1;
+  return CSM_OK;
+}
+
+// A match needs a low-resolution cloud and two levels; discretisation alone does not.
+csm_status RequireMatchable3D(const Match3& x) {
+  CSM_REQUIRE(x.node->num_low >= 1, "empty low-resolution point cloud");
+  if (x.hmax == 0) {
     SetError("branch_and_bound_depth == 1 is not supported by the 3D engine");
     return CSM_E_INVALID;
   }
+  return CSM_OK;
+}
 
-  // ---- uploads through pinned staging: scans | angles | ones | histogram | clouds ----
-  const size_t o_ang = (sizeof(Scan3) * A + 255) / 256 * 256;
-  const size_t o_hist = (o_ang + 4 * static_cast<size_t>(A) + 255) / 256 * 256;
-  const size_t o_hi = (o_hist + 4 * static_cast<size_t>(std::max(1, hn)) + 255) / 256 * 256;
-  const size_t o_lo = dev ? o_hi : (o_hi + 12 * static_cast<size_t>(n_hi) + 255) / 256 * 256;
-  const size_t up_bytes = dev ? o_hi : o_lo + 12 * static_cast<size_t>(std::max(1, n_lo));
+// Workspaces, the job record and the upload of scans, angles, histogram and clouds.
+csm_status Upload3D(Match3& x) {
+  Ctx* ctx = x.ctx;
+  const csm_matcher3d* m = x.m;
+  const int A = x.plan.num_angles, n_hi = x.node->num_high, n_lo = x.node->num_low;
+  const int hn = x.node->histogram_size;
+  x.o_ang = (sizeof(Scan3) * A + 255) / 256 * 256;
+  x.o_hist = (x.o_ang + 4 * static_cast<size_t>(A) + 255) / 256 * 256;
+  const size_t o_hi = (x.o_hist + 4 * static_cast<size_t>(std::max(1, hn)) + 255) / 256 * 256;
+  const size_t o_lo = x.dev ? o_hi : (o_hi + 12 * static_cast<size_t>(n_hi) + 255) / 256 * 256;
+  const size_t up_bytes = x.dev ? o_hi : o_lo + 12 * static_cast<size_t>(std::max(1, n_lo));
   PinnedBuf& up = ctx->P("m3_upload");
-  DevBuf& d_up = ctx->D("m3_upload");
+  DevBuf* d_up;
   CSM_TRY(up.Reserve(up_bytes));
-  CSM_TRY(d_up.Reserve(up_bytes));
+  CSM_TRY(ctx->Reserve("m3_upload", up_bytes, &d_up));
   char* hup = up.as<char>();
-  std::memcpy(hup, plan.scans.data(), sizeof(Scan3) * A);
-  std::memcpy(hup + o_ang, plan.angles.data(), 4 * static_cast<size_t>(A));
-  if (hn) std::memcpy(hup + o_hist, node->rotational_scan_matcher_histogram, 4 * static_cast<size_t>(hn));
-  if (!dev) {
-    std::memcpy(hup + o_hi, node->high_resolution_point_cloud, 12 * static_cast<size_t>(n_hi));
-    if (n_lo) std::memcpy(hup + o_lo, node->low_resolution_point_cloud, 12 * static_cast<size_t>(n_lo));
+  std::memcpy(hup, x.plan.scans.data(), sizeof(Scan3) * A);
+  std::memcpy(hup + x.o_ang, x.plan.angles.data(), 4 * static_cast<size_t>(A));
+  if (hn) std::memcpy(hup + x.o_hist, x.node->rotational_scan_matcher_histogram, 4 * static_cast<size_t>(hn));
+  if (!x.dev) {
+    std::memcpy(hup + o_hi, x.node->high_resolution_point_cloud, 12 * static_cast<size_t>(n_hi));
+    if (n_lo) std::memcpy(hup + o_lo, x.node->low_resolution_point_cloud, 12 * static_cast<size_t>(n_lo));
   }
-  DevBuf& d_scans = ctx->D("m3_scans");
-  DevBuf& d_sel = ctx->D("m3_sel");
-  DevBuf& d_rot = ctx->D("m3_rot");
-  DevBuf& d_cells = ctx->D("m3_cells");
-  DevBuf& d_top = ctx->D("m3_top");
-  DevBuf& d_ctr = ctx->D("m3_ctr");
-  CSM_TRY(d_scans.Reserve(sizeof(Scan3) * A));
-  CSM_TRY(d_sel.Reserve(4 * static_cast<size_t>(A)));
-  CSM_TRY(d_rot.Reserve(4 * static_cast<size_t>(A)));
-  CSM_TRY(d_cells.Reserve(sizeof(short4) * static_cast<size_t>(A) * n_hi));
-  CSM_TRY(d_ctr.Reserve(8 * 8 + 4 * kC3Ints));
-  const char* dup = d_up.as<char>();
-  unsigned long long* ctr = d_ctr.as<unsigned long long>();
-  int* ictr = reinterpret_cast<int*>(ctr + 8);   // the control block (kC3*)
-  unsigned* lb = reinterpret_cast<unsigned*>(ictr) + kC3Bound;
+  CSM_TRY(ctx->Reserve("m3_scans", sizeof(Scan3) * A, &x.d_scans));
+  CSM_TRY(ctx->Reserve("m3_sel", 4 * static_cast<size_t>(A), &x.d_sel));
+  CSM_TRY(ctx->Reserve("m3_rot", 4 * static_cast<size_t>(A), &x.d_rot));
+  CSM_TRY(ctx->Reserve("m3_cells", sizeof(short4) * static_cast<size_t>(A) * n_hi, &x.d_cells));
+  CSM_TRY(ctx->Reserve("m3_ctr", 8 * 8 + 4 * kC3Ints, &x.d_ctr));
+  x.dup = d_up->as<char>();
+  x.ctr = x.d_ctr->as<unsigned long long>();
+  x.ictr = reinterpret_cast<int*>(x.ctr + 8);
+  x.lb = reinterpret_cast<unsigned*>(x.ictr) + kC3Bound;
 
-  Job3 jb;
+  Job3& jb = x.jb;
   std::memset(&jb, 0, sizeof(jb));
   jb.stack = m->d_stack;
   jb.low = m->d_low;
-  jb.hi_xyz = dev ? dev->hi : reinterpret_cast<const float*>(dup + o_hi);
-  jb.lo_xyz = dev ? dev->lo : reinterpret_cast<const float*>(dup + o_lo);
-  jb.scans = d_scans.as<Scan3>();
-  jb.ctl = ictr;
-  jb.cells = d_cells.as<short4>();
+  jb.hi_xyz = x.dev ? x.dev->hi : reinterpret_cast<const float*>(x.dup + o_hi);
+  jb.lo_xyz = x.dev ? x.dev->lo : reinterpret_cast<const float*>(x.dup + o_lo);
+  jb.scans = x.d_scans->as<Scan3>();
+  jb.ctl = x.ictr;
+  jb.cells = x.d_cells->as<short4>();
   jb.n_hi = n_hi;
   jb.n_lo = n_lo;
   jb.max_scans = A;
-  jb.wxy = sp.wxy;
-  jb.wz = sp.wz;
-  const int step = 1 << hmax;
-  jb.nxc = (2 * sp.wxy + step) / step;   // :301-306
-  jb.nzc = (2 * sp.wz + step) / step;
-  jb.min_score = min_score;
+  jb.wxy = x.sp.wxy;
+  jb.wz = x.sp.wz;
+  const int step = 1 << x.hmax;
+  jb.nxc = (2 * x.sp.wxy + step) / step;   // :301-306
+  jb.nzc = (2 * x.sp.wz + step) / step;
+  jb.min_score = x.min_score;
   jb.min_low_d = m->opt.min_low_resolution_score;
-  const long long per_scan = static_cast<long long>(jb.nxc) * jb.nxc * jb.nzc;
-  const long long max_top = per_scan * A;
-  CSM_REQUIRE(max_top < (1LL << 30), "too many lowest-resolution candidates");
+  x.per_scan = static_cast<long long>(jb.nxc) * jb.nxc * jb.nzc;
+  x.max_top = x.per_scan * A;
+  CSM_REQUIRE(x.max_top < (1LL << 30), "too many lowest-resolution candidates");
 
-  CSM_CUDA(cudaEventRecord(ctx->ev0, s));
-  CSM_CUDA(cudaMemcpyAsync(d_up.p, hup, up_bytes, cudaMemcpyHostToDevice, s));
-  CSM_CUDA(cudaMemsetAsync(d_ctr.p, 0, 8 * 8 + 4 * kC3Ints, s));
-  // ---- rotational scores (K7) and the filter, on the device ----
-  const float* d_node_hist = dev && dev->hist ? dev->hist : reinterpret_cast<const float*>(dup + o_hist);
+  CSM_CUDA(cudaEventRecord(ctx->ev0, x.s));
+  CSM_CUDA(cudaMemcpyAsync(d_up->p, hup, up_bytes, cudaMemcpyHostToDevice, x.s));
+  CSM_CUDA(cudaMemsetAsync(x.d_ctr->p, 0, 8 * 8 + 4 * kC3Ints, x.s));
+  return CSM_OK;
+}
+
+// Rotational scores (K7), the filter and the discretisation of the kept scans, on the device.
+csm_status Discretize3D(Match3& x) {
+  Ctx* ctx = x.ctx;
+  cudaStream_t s = x.s;
+  const int A = x.plan.num_angles, hn = x.node->histogram_size;
+  const float* d_node_hist = x.dev && x.dev->hist ? x.dev->hist
+                                                  : reinterpret_cast<const float*>(x.dup + x.o_hist);
   if (hn > 0) {
     ProfBegin(ctx);
-    k3_rotational<<<DivUp3(A, 128), 128, 0, s>>>(m->d_hist, d_node_hist, hn, initial_angle,
-                                                 reinterpret_cast<const float*>(dup + o_ang), A,
-                                                 d_rot.as<float>());
+    k3_rotational<<<DivUp(A, 128), 128, 0, s>>>(x.m->d_hist, d_node_hist, hn, x.initial_angle,
+                                                reinterpret_cast<const float*>(x.dup + x.o_ang), A,
+                                                x.d_rot->as<float>());
     CSM_LAUNCH_CHECK();
     ProfEnd(ctx, "k3_rotational", A);
   } else {
-    k3_fill<<<DivUp3(A, 256), 256, 0, s>>>(d_rot.as<float>(), A, 1.f);
+    k3_fill<<<DivUp(A, 256), 256, 0, s>>>(x.d_rot->as<float>(), A, 1.f);
     CSM_LAUNCH_CHECK();
   }
-  k3_select_scans<<<1, 1024, 0, s>>>(reinterpret_cast<const Scan3*>(dup), d_rot.as<float>(), A,
-                                     m->opt.min_rotational_score, d_scans.as<Scan3>(),
-                                     d_sel.as<int>(), ictr, HostOrd(min_score));
+  k3_select_scans<<<1, 1024, 0, s>>>(reinterpret_cast<const Scan3*>(x.dup), x.d_rot->as<float>(),
+                                     A, x.m->opt.min_rotational_score, x.d_scans->as<Scan3>(),
+                                     x.d_sel->as<int>(), x.ictr, HostFloatToOrdered(x.min_score));
   CSM_LAUNCH_CHECK();
   ProfBegin(ctx);
-  k3_discretize<<<dim3(std::min(DivUp3(n_hi, 256), 64), A), 256, 0, s>>>(jb);
+  k3_discretize<<<dim3(std::min(DivUp(x.jb.n_hi, 256), 64), A), 256, 0, s>>>(x.jb);
   CSM_LAUNCH_CHECK();
-  ProfEnd(ctx, "k3_discretize", static_cast<double>(A) * n_hi);
+  ProfEnd(ctx, "k3_discretize", static_cast<double>(A) * x.jb.n_hi);
 
-  PinnedBuf& pin = ctx->P("m3_readback");
-  const int kInlineBest = 256;
-  const size_t rb_ctr = 4 * kC3Ints;
-  const size_t rb_best = rb_ctr + 8 * 8;
-  CSM_TRY(pin.Reserve(rb_best + sizeof(BestLeaf3) * kInlineBest));
-  int* hp = pin.as<int>();
-  const unsigned long long* hctr = reinterpret_cast<const unsigned long long*>(pin.as<char>() + rb_ctr);
-  const BestLeaf3* best_inline = reinterpret_cast<const BestLeaf3*>(pin.as<char>() + rb_best);
+  x.pin = &ctx->P("m3_readback");
+  CSM_TRY(x.pin->Reserve(kRbBest + sizeof(BestLeaf3) * kInlineBest));
+  x.hp = x.pin->as<int>();
+  x.hctr = reinterpret_cast<const unsigned long long*>(x.pin->as<char>() + kRbCtr);
+  x.best_inline = reinterpret_cast<const BestLeaf3*>(x.pin->as<char>() + kRbBest);
+  return CSM_OK;
+}
 
-  if (discretize_only) {
-    CSM_CUDA(cudaMemcpyAsync(hp, ictr, rb_ctr, cudaMemcpyDeviceToHost, s));
-    CSM_CUDA(cudaStreamSynchronize(s));
-    const int S = hp[kC3Scans];
-    if (out_num_scans) *out_num_scans = S;
-    if (stats) stats->num_scans = S;
-    if (S == 0 || !out_cells) return CSM_OK;
-    std::vector<short4> h(static_cast<size_t>(S) * n_hi);
-    std::vector<Scan3> hs(S);
-    CSM_CUDA(cudaMemcpy(h.data(), d_cells.p, sizeof(short4) * h.size(), cudaMemcpyDeviceToHost));
-    CSM_CUDA(cudaMemcpy(hs.data(), d_scans.p, sizeof(Scan3) * S, cudaMemcpyDeviceToHost));
-    for (size_t i = 0; i < h.size(); ++i) {
-      out_cells[3 * i] = h[i].x;
-      out_cells[3 * i + 1] = h[i].y;
-      out_cells[3 * i + 2] = h[i].z;
-    }
-    for (int k = 0; k < S; ++k) {
-      const Scan3& sc = hs[k];
-      const float v[7] = {sc.tx, sc.ty, sc.tz, sc.qw, sc.qx, sc.qy, sc.qz};
-      if (out_poses) std::memcpy(out_poses + 7 * k, v, sizeof(v));
-      if (out_rot) out_rot[k] = sc.rot_score;
-    }
-    return CSM_OK;
-  }
+// Reads the control block back into x.hp after the work queued so far (one synchronise).
+csm_status ReadCtl3D(Match3& x) {
+  CSM_CUDA(cudaMemcpyAsync(x.hp, x.ictr, kRbCtr, cudaMemcpyDeviceToHost, x.s));
+  CSM_CUDA(cudaStreamSynchronize(x.s));
+  return CSM_OK;
+}
 
-  if (probe && probe->mode == Probe3D::kList) {
-    const int n = probe->list_n;
-    CSM_CUDA(cudaMemcpyAsync(hp, ictr, rb_ctr, cudaMemcpyDeviceToHost, s));
-    CSM_CUDA(cudaStreamSynchronize(s));
-    for (int i = 0; i < n; ++i) {
-      const List3& c = probe->list[i];
-      CSM_REQUIRE(c.scan >= 0 && c.scan < hp[kC3Scans], "candidate scan_index");
-      CSM_REQUIRE(c.depth >= 0 && c.depth <= hmax, "candidate depth");
-    }
-    probe->num_scans = hp[kC3Scans];
-    probe->sums.resize(n);
-    probe->scores.resize(n);
-    if (n == 0) return CSM_OK;
-    DevBuf& d_lc = ctx->D("m3_tie_c");
-    DevBuf& d_ls = ctx->D("m3_tie_s");
-    DevBuf& d_li = ctx->D("m3_probe_sums");
-    CSM_TRY(d_lc.Reserve(sizeof(List3) * n));
-    CSM_TRY(d_ls.Reserve(sizeof(float) * n));
-    CSM_TRY(d_li.Reserve(sizeof(int) * n));
-    CSM_CUDA(cudaMemcpyAsync(d_lc.p, probe->list, sizeof(List3) * n, cudaMemcpyHostToDevice, s));
-    ProfBegin(ctx);
-    k3_score_list<<<n, kT3, 0, s>>>(jb, d_lc.as<List3>(), d_ls.as<float>(), d_li.as<int>());
-    CSM_LAUNCH_CHECK();
-    ProfEnd(ctx, "k3_score_list", n);
-    CSM_CUDA(cudaMemcpyAsync(probe->scores.data(), d_ls.p, sizeof(float) * n,
-                             cudaMemcpyDeviceToHost, s));
-    CSM_CUDA(cudaMemcpyAsync(probe->sums.data(), d_li.p, sizeof(int) * n, cudaMemcpyDeviceToHost,
-                             s));
-    CSM_CUDA(cudaStreamSynchronize(s));
-    return CSM_OK;
-  }
-
-  // ---- lowest-resolution pass + dives (grids sized for all angles; filtered-out scans exit) ----
-  CSM_TRY(d_top.Reserve(sizeof(int) * max_top));
+// Lowest-resolution pass and dives (grids sized for all angles; filtered-out scans exit).
+csm_status TopDive3D(Match3& x) {
+  Ctx* ctx = x.ctx;
+  CSM_TRY(ctx->Reserve("m3_top", sizeof(int) * x.max_top, &x.d_top));
   ProfBegin(ctx);
-  k3_score_top<<<static_cast<int>(max_top), kT3, 0, s>>>(jb, d_top.as<int>(), ictr);
+  k3_score_top<<<static_cast<int>(x.max_top), kT3, 0, x.s>>>(x.jb, x.d_top->as<int>(), x.ictr);
   CSM_LAUNCH_CHECK();
-  ProfEnd(ctx, "k3_score_top", static_cast<double>(max_top));
+  ProfEnd(ctx, "k3_score_top", static_cast<double>(x.max_top));
   ProfBegin(ctx);
-  static const float dive_ratio = getenv("CSM_DIVE_RATIO3") ? atof(getenv("CSM_DIVE_RATIO3")) : 0.97f;
-  k3_dive<<<A, kT3, 0, s>>>(jb, d_top.as<int>(), dive_ratio, lb, ctr);
+  k3_dive<<<x.plan.num_angles, kT3, 0, x.s>>>(x.jb, x.d_top->as<int>(), kDiveRatio, x.lb, x.ctr);
   CSM_LAUNCH_CHECK();
-  ProfEnd(ctx, "k3_dive", static_cast<double>(A) * 8 * hmax);
-  if (probe && probe->mode == Probe3D::kTop) {
-    CSM_CUDA(cudaMemcpyAsync(hp, ictr, rb_ctr, cudaMemcpyDeviceToHost, s));
-    unsigned long long c[8];
-    CSM_CUDA(cudaMemcpyAsync(c, ctr, sizeof(c), cudaMemcpyDeviceToHost, s));
-    CSM_CUDA(cudaStreamSynchronize(s));
-    const int S = hp[kC3Scans];
-    probe->num_scans = S;
-    probe->nxc = jb.nxc;
-    probe->nzc = jb.nzc;
-    probe->top_best = hp[kC3TopBest];
-    probe->final_bound = HostUnord(static_cast<unsigned>(hp[kC3Bound]));
-    probe->counters[0] = c[0];
-    probe->counters[1] = c[1];
-    probe->counters[2] = c[2];
-    probe->angle.resize(S);
-    probe->top_sums.resize(per_scan * S);
-    std::vector<Scan3> hs(S);
-    if (S) {
-      CSM_CUDA(cudaMemcpy(probe->angle.data(), d_sel.p, sizeof(int) * S, cudaMemcpyDeviceToHost));
-      CSM_CUDA(cudaMemcpy(hs.data(), d_scans.p, sizeof(Scan3) * S, cudaMemcpyDeviceToHost));
-      CSM_CUDA(cudaMemcpy(probe->top_sums.data(), d_top.p, sizeof(int) * per_scan * S,
-                          cudaMemcpyDeviceToHost));
-    }
-    probe->rot.resize(S);
-    for (int k = 0; k < S; ++k) probe->rot[k] = hs[k].rot_score;
-    return CSM_OK;
-  }
+  ProfEnd(ctx, "k3_dive", static_cast<double>(x.plan.num_angles) * 8 * x.hmax);
+  return CSM_OK;
+}
 
-  // ---- branch and bound: device-driven level loop (see engine2d.cu) ----
-  const int kChunk = 1 << 16;
-  const int kQueueCap = 8 * kChunk;
-  const int kLeafCap = 1 << 20;
-  DevBuf& d_qtop = ctx->D("m3_qtop");
-  DevBuf& d_q = ctx->D("m3_queues");
-  DevBuf& d_leaves = ctx->D("m3_leaves");
-  DevBuf& d_best = ctx->D("m3_best");
-  CSM_TRY(d_qtop.Reserve(sizeof(Node3) * static_cast<size_t>(
-                                               std::max<long long>(max_top, probe ? probe->num_parents : 0))));
-  CSM_TRY(d_q.Reserve(sizeof(Node3) * static_cast<size_t>(kQueueCap) * std::max(1, hmax)));
-  CSM_TRY(d_leaves.Reserve(sizeof(Leaf3) * static_cast<size_t>(kLeafCap)));
-  CSM_TRY(d_best.Reserve(sizeof(BestLeaf3) * static_cast<size_t>(kLeafCap)));
-  auto queue_ptr = [&](int h) -> Node3* {
-    return h == hmax ? d_qtop.as<Node3>() : d_q.as<Node3>() + static_cast<size_t>(kQueueCap) * h;
-  };
-  k3_filter_top<<<DivUp3(max_top, 256), 256, 0, s>>>(jb, d_top.as<int>(), lb, queue_ptr(hmax),
-                                                     ictr + hmax);
+// Queues of the level loop (the top one holds at least `top_queue` nodes) and the
+// lowest-resolution candidates above the bound as its top queue.
+csm_status FilterTop3D(Match3& x, long long top_queue) {
+  Ctx* ctx = x.ctx;
+  CSM_TRY(ctx->Reserve("m3_qtop", sizeof(Node3) * top_queue, &x.d_qtop));
+  CSM_TRY(ctx->Reserve("m3_queues", sizeof(Node3) * kQueueCap * std::max(1, x.hmax), &x.d_q));
+  CSM_TRY(ctx->Reserve("m3_leaves", sizeof(Leaf3) * kLeafCap, &x.d_leaves));
+  CSM_TRY(ctx->Reserve("m3_best", sizeof(BestLeaf3) * kLeafCap, &x.d_best));
+  k3_filter_top<<<DivUp(x.max_top, 256), 256, 0, x.s>>>(x.jb, x.d_top->as<int>(), x.lb,
+                                                        x.Queue(x.hmax), x.ictr + x.hmax);
   CSM_LAUNCH_CHECK();
-  const int expand_grid = ctx->sm_count * 4;
-  auto level_step = [&](int h) -> csm_status {
-    k3_level_begin<<<1, 32, 0, s>>>(ictr, h, kChunk);
-    CSM_LAUNCH_CHECK();
-    ProfBegin(ctx);
-    k3_expand<<<expand_grid, kT3, 0, s>>>(jb, queue_ptr(h), ictr, h,
-                                          h - 1 >= 1 ? queue_ptr(h - 1) : nullptr,
-                                          ictr + (h - 1 >= 1 ? h - 1 : 23), kQueueCap,
-                                          d_leaves.as<Leaf3>(), kLeafCap, ctr);
-    CSM_LAUNCH_CHECK();
-    ProfEnd(ctx, "k3_expand", 0.);
-    return CSM_OK;
-  };
-  if (probe) {
-    // the level loop over the caller's parents only: its state is reset to them
-    const int h = probe->level, n = probe->num_parents;
-    CSM_REQUIRE(h >= 1 && h <= hmax, "level out of range");
-    CSM_REQUIRE(n >= 0 && (h == hmax || n <= kQueueCap), "number of parents");
-    CSM_CUDA(cudaMemcpyAsync(hp, ictr, rb_ctr, cudaMemcpyDeviceToHost, s));
-    CSM_CUDA(cudaStreamSynchronize(s));
-    const int S = hp[kC3Scans];
-    for (int i = 0; i < n; ++i) {
-      const Node3& p = probe->parents[i];
-      CSM_REQUIRE(p.scan >= 0 && p.scan < S, "parent scan_index");
-      const int dx = p.ox + sp.wxy, dy = p.oy + sp.wxy, dz = p.oz + sp.wz;
-      CSM_REQUIRE(dx >= 0 && dy >= 0 && dz >= 0 && ((dx | dy | dz) & ((1 << h) - 1)) == 0 &&
-                      p.ox <= sp.wxy && p.oy <= sp.wxy && p.oz <= sp.wz,
-                  "parent is not a node of its level's lattice");
-    }
-    for (int l = 1; l <= hmax; ++l) hp[l] = 0;
-    hp[h] = n;
-    hp[kC3Leaf] = 0;
-    hp[kC3Overflow] = 0;
-    hp[kC3Bound] = static_cast<int>(HostOrd(probe->bound));
-    CSM_CUDA(cudaMemcpyAsync(ictr, hp, rb_ctr, cudaMemcpyHostToDevice, s));
-    CSM_CUDA(cudaMemsetAsync(ctr, 0, 8 * 8, s));
-    if (n)
-      CSM_CUDA(cudaMemcpyAsync(queue_ptr(h), probe->parents, sizeof(Node3) * n,
-                               cudaMemcpyHostToDevice, s));
-    for (int done = 0; done < n; done += kChunk) CSM_TRY(level_step(h));
-    unsigned long long c[8];
-    CSM_CUDA(cudaMemcpyAsync(hp, ictr, rb_ctr, cudaMemcpyDeviceToHost, s));
-    CSM_CUDA(cudaMemcpyAsync(c, ctr, sizeof(c), cudaMemcpyDeviceToHost, s));
-    CSM_CUDA(cudaStreamSynchronize(s));
-    if (hp[kC3Overflow]) { SetError("3D branch-and-bound capacity exceeded"); return CSM_E_CAPACITY; }
-    if (h >= 2) {
-      probe->children.resize(hp[h - 1]);
-      if (hp[h - 1])
-        CSM_CUDA(cudaMemcpy(probe->children.data(), queue_ptr(h - 1), sizeof(Node3) * hp[h - 1],
-                            cudaMemcpyDeviceToHost));
-    } else {
-      probe->leaves.resize(hp[kC3Leaf]);
-      if (hp[kC3Leaf])
-        CSM_CUDA(cudaMemcpy(probe->leaves.data(), d_leaves.p, sizeof(Leaf3) * hp[kC3Leaf],
-                            cudaMemcpyDeviceToHost));
-    }
-    probe->final_bound = HostUnord(static_cast<unsigned>(hp[kC3Bound]));
-    for (int k = 0; k < 3; ++k) probe->counters[k] = c[k];
-    return CSM_OK;
-  }
-  int host_syncs = 0;
-  auto collect = [&]() -> csm_status {
-    CSM_CUDA(cudaMemsetAsync(ictr + kC3Best, 0, 4, s));
-    k3_collect<<<ctx->sm_count, 256, 0, s>>>(d_leaves.as<Leaf3>(), d_scans.as<Scan3>(),
-                                             d_sel.as<int>(), ictr, kLeafCap,
-                                             d_best.as<BestLeaf3>(), kLeafCap);
-    CSM_LAUNCH_CHECK();
-    CSM_CUDA(cudaEventRecord(ctx->ev1, s));
-    CSM_CUDA(cudaMemcpyAsync(pin.as<char>(), ictr, rb_ctr, cudaMemcpyDeviceToHost, s));
-    CSM_CUDA(cudaMemcpyAsync(pin.as<char>() + rb_ctr, ctr, 8 * 8, cudaMemcpyDeviceToHost, s));
-    CSM_CUDA(cudaMemcpyAsync(pin.as<char>() + rb_best, d_best.p, sizeof(BestLeaf3) * kInlineBest,
-                             cudaMemcpyDeviceToHost, s));
-    CSM_CUDA(cudaStreamSynchronize(s));
-    ++host_syncs;
-    return CSM_OK;
-  };
-  for (int h = hmax; h >= 1; --h) CSM_TRY(level_step(h));
-  CSM_TRY(collect());
-  for (;;) {   // frontiers larger than one chunk: deepest non-empty level first
-    if (hp[kC3Overflow]) { SetError("3D branch-and-bound capacity exceeded"); return CSM_E_CAPACITY; }
+  return CSM_OK;
+}
+
+// One level step of the device-driven level loop (see engine2d.cu).
+csm_status LevelStep3D(Match3& x, int h) {
+  k3_level_begin<<<1, 32, 0, x.s>>>(x.ictr, h, kChunk);
+  CSM_LAUNCH_CHECK();
+  ProfBegin(x.ctx);
+  k3_expand<<<x.ctx->sm_count * 4, kT3, 0, x.s>>>(x.jb, x.Queue(h), x.ictr, h,
+                                                   h - 1 >= 1 ? x.Queue(h - 1) : nullptr,
+                                                   x.ictr + (h - 1 >= 1 ? h - 1 : 23), kQueueCap,
+                                                   x.d_leaves->as<Leaf3>(), kLeafCap, x.ctr);
+  CSM_LAUNCH_CHECK();
+  ProfEnd(x.ctx, "k3_expand", 0.);
+  return CSM_OK;
+}
+
+// Compaction of the gate-passing optimal leaves + read-back of everything the host needs.
+csm_status Collect3D(Match3& x) {
+  cudaStream_t s = x.s;
+  char* pin = x.pin->as<char>();
+  CSM_CUDA(cudaMemsetAsync(x.ictr + kC3Best, 0, 4, s));
+  k3_collect<<<x.ctx->sm_count, 256, 0, s>>>(x.d_leaves->as<Leaf3>(), x.d_scans->as<Scan3>(),
+                                             x.d_sel->as<int>(), x.ictr, kLeafCap,
+                                             x.d_best->as<BestLeaf3>(), kLeafCap);
+  CSM_LAUNCH_CHECK();
+  CSM_CUDA(cudaEventRecord(x.ctx->ev1, s));
+  CSM_CUDA(cudaMemcpyAsync(pin, x.ictr, kRbCtr, cudaMemcpyDeviceToHost, s));
+  CSM_CUDA(cudaMemcpyAsync(pin + kRbCtr, x.ctr, 8 * 8, cudaMemcpyDeviceToHost, s));
+  CSM_CUDA(cudaMemcpyAsync(pin + kRbBest, x.d_best->p, sizeof(BestLeaf3) * kInlineBest,
+                           cudaMemcpyDeviceToHost, s));
+  CSM_CUDA(cudaStreamSynchronize(s));
+  ++x.host_syncs;
+  return CSM_OK;
+}
+
+// The sweep hmax -> 1, then continuation sweeps for frontiers larger than one chunk,
+// deepest non-empty level first.
+csm_status Sweep3D(Match3& x) {
+  for (int h = x.hmax; h >= 1; --h) CSM_TRY(LevelStep3D(x, h));
+  CSM_TRY(Collect3D(x));
+  for (;;) {
+    if (x.hp[kC3Overflow]) { SetError("3D branch-and-bound capacity exceeded"); return CSM_E_CAPACITY; }
     int h = -1;
-    for (int l = 1; l <= hmax; ++l)
-      if (hp[l] > 0) { h = l; break; }
+    for (int l = 1; l <= x.hmax; ++l)
+      if (x.hp[l] > 0) { h = l; break; }
     if (h < 0) break;
-    for (int l = h; l >= 1; --l) CSM_TRY(level_step(l));
-    CSM_TRY(collect());
+    for (int l = h; l >= 1; --l) CSM_TRY(LevelStep3D(x, l));
+    CSM_TRY(Collect3D(x));
   }
-  const int S = hp[kC3Scans];
-  if (out_num_scans) *out_num_scans = S;
-  const long long total_top = per_scan * S;
-  const unsigned lbh = static_cast<unsigned>(hp[kC3Bound]);
-  const float best_score = HostUnord(lbh);
-  const int n_best = hp[kC3Best];
-  std::vector<BestLeaf3> ties(best_inline, best_inline + std::min(n_best, kInlineBest));
-  if (n_best > kInlineBest) {
-    ties.resize(n_best);
-    CSM_CUDA(cudaMemcpy(ties.data(), d_best.p, sizeof(BestLeaf3) * n_best, cudaMemcpyDeviceToHost));
-    ++host_syncs;
-  }
+  return CSM_OK;
+}
 
-  // ---- tie resolution: first optimal, gate-passing leaf in the reference's DFS order ----
-  int host_resolves = 0;
-  if (ties.size() > 1) {
-    const int T = static_cast<int>(ties.size());
-    std::vector<List3> lc;
-    for (const BestLeaf3& t : ties)
-      for (int l = 1; l <= hmax; ++l)
-        lc.push_back(List3{t.scan, -sp.wxy + (((t.ox + sp.wxy) >> l) << l),
-                           -sp.wxy + (((t.oy + sp.wxy) >> l) << l),
-                           -sp.wz + (((t.oz + sp.wz) >> l) << l), l});
-    std::vector<float> anc(lc.size());
-    DevBuf& d_lc = ctx->D("m3_tie_c");
-    DevBuf& d_ls = ctx->D("m3_tie_s");
-    CSM_TRY(d_lc.Reserve(sizeof(List3) * lc.size()));
-    CSM_TRY(d_ls.Reserve(sizeof(float) * lc.size()));
-    CSM_CUDA(cudaMemcpyAsync(d_lc.p, lc.data(), sizeof(List3) * lc.size(),
-                             cudaMemcpyHostToDevice, s));
-    k3_score_list<<<static_cast<int>(lc.size()), kT3, 0, s>>>(jb, d_lc.as<List3>(),
-                                                               d_ls.as<float>(), nullptr);
-    CSM_LAUNCH_CHECK();
-    CSM_CUDA(cudaMemcpyAsync(anc.data(), d_ls.p, sizeof(float) * lc.size(),
-                             cudaMemcpyDeviceToHost, s));
-    CSM_CUDA(cudaStreamSynchronize(s));
-    ++host_syncs;
-    std::vector<int> top_rank;
-    auto ensure_top_rank = [&]() -> csm_status {
-      if (!top_rank.empty()) return CSM_OK;
-      ++host_resolves;
-      std::vector<int> sums(total_top);
-      CSM_CUDA(cudaMemcpy(sums.data(), d_top.p, sizeof(int) * total_top, cudaMemcpyDeviceToHost));
-      struct Item { float score; int gen; };
-      std::vector<Item> items(total_top);
-      const float kMin = 0.1f, kMax = 1.f - kMin;
-      for (long long i = 0; i < total_top; ++i)
-        items[i] = Item{kMin + (static_cast<float>(sums[i]) / static_cast<float>(n_hi)) *
-                                   ((kMax - kMin) / 255.f),
-                        static_cast<int>(i)};
-      std::sort(items.begin(), items.end(),
-                [](const Item& a, const Item& b) { return a.score > b.score; });
-      top_rank.resize(total_top);
-      for (long long r = 0; r < total_top; ++r) top_rank[items[r].gen] = static_cast<int>(r);
-      return CSM_OK;
-    };
-    csm_status err = CSM_OK;
-    auto before = [&](int a, int b) -> bool {
-      const BestLeaf3& A_ = ties[a];
-      const BestLeaf3& B_ = ties[b];
-      for (int l = hmax; l >= 0; --l) {
-        const int ax = (A_.ox + sp.wxy) >> l, ay = (A_.oy + sp.wxy) >> l, az = (A_.oz + sp.wz) >> l;
-        const int bx = (B_.ox + sp.wxy) >> l, by = (B_.oy + sp.wxy) >> l, bz = (B_.oz + sp.wz) >> l;
-        if (A_.scan == B_.scan && ax == bx && ay == by && az == bz) continue;
-        const float fa = l == 0 ? 0.f : anc[static_cast<size_t>(a) * hmax + (l - 1)];
-        const float fb = l == 0 ? 0.f : anc[static_cast<size_t>(b) * hmax + (l - 1)];
-        if (l > 0 && fa != fb) return fa > fb;
-        if (l == hmax) {
-          if (ensure_top_rank() != CSM_OK) { err = CSM_E_CUDA; return false; }
-          const long long ga = ((static_cast<long long>(A_.scan) * jb.nzc + az) * jb.nxc + ay) * jb.nxc + ax;
-          const long long gb = ((static_cast<long long>(B_.scan) * jb.nzc + bz) * jb.nxc + by) * jb.nxc + bx;
-          return top_rank[ga] < top_rank[gb];
-        }
-        // siblings: generation order z outer, y, x inner
-        if ((az & 1) != (bz & 1)) return (az & 1) < (bz & 1);
-        if ((ay & 1) != (by & 1)) return (ay & 1) < (by & 1);
-        return (ax & 1) < (bx & 1);
+// Tie resolution: the first optimal, gate-passing leaf in the reference's DFS order is moved
+// to ties[0].
+csm_status ResolveTies3D(Match3& x, std::vector<BestLeaf3>& ties, int* host_resolves) {
+  cudaStream_t s = x.s;
+  const int hmax = x.hmax;
+  const HostSearch3& sp = x.sp;
+  const Job3& jb = x.jb;
+  const int T = static_cast<int>(ties.size());
+  std::vector<List3> lc;
+  for (const BestLeaf3& t : ties)
+    for (int l = 1; l <= hmax; ++l)
+      lc.push_back(List3{t.scan, -sp.wxy + (((t.ox + sp.wxy) >> l) << l),
+                         -sp.wxy + (((t.oy + sp.wxy) >> l) << l),
+                         -sp.wz + (((t.oz + sp.wz) >> l) << l), l});
+  std::vector<float> anc(lc.size());
+  DevBuf *d_lc, *d_ls;
+  CSM_TRY(x.ctx->Reserve("m3_tie_c", sizeof(List3) * lc.size(), &d_lc));
+  CSM_TRY(x.ctx->Reserve("m3_tie_s", sizeof(float) * lc.size(), &d_ls));
+  CSM_CUDA(cudaMemcpyAsync(d_lc->p, lc.data(), sizeof(List3) * lc.size(),
+                           cudaMemcpyHostToDevice, s));
+  k3_score_list<<<static_cast<int>(lc.size()), kT3, 0, s>>>(jb, d_lc->as<List3>(),
+                                                             d_ls->as<float>(), nullptr);
+  CSM_LAUNCH_CHECK();
+  CSM_CUDA(cudaMemcpyAsync(anc.data(), d_ls->p, sizeof(float) * lc.size(),
+                           cudaMemcpyDeviceToHost, s));
+  CSM_CUDA(cudaStreamSynchronize(s));
+  ++x.host_syncs;
+  const long long total_top = x.per_scan * x.hp[kC3Scans];
+  std::vector<int> top_rank;
+  auto ensure_top_rank = [&]() -> csm_status {
+    if (!top_rank.empty()) return CSM_OK;
+    ++*host_resolves;
+    std::vector<int> sums(total_top);
+    CSM_CUDA(cudaMemcpy(sums.data(), x.d_top->p, sizeof(int) * total_top, cudaMemcpyDeviceToHost));
+    struct Item { float score; int gen; };
+    std::vector<Item> items(total_top);
+    const float kMin = 0.1f, kMax = 1.f - kMin;
+    for (long long i = 0; i < total_top; ++i)
+      items[i] = Item{kMin + (static_cast<float>(sums[i]) / static_cast<float>(x.jb.n_hi)) *
+                                 ((kMax - kMin) / 255.f),
+                      static_cast<int>(i)};
+    std::sort(items.begin(), items.end(),
+              [](const Item& a, const Item& b) { return a.score > b.score; });
+    top_rank.resize(total_top);
+    for (long long r = 0; r < total_top; ++r) top_rank[items[r].gen] = static_cast<int>(r);
+    return CSM_OK;
+  };
+  csm_status err = CSM_OK;
+  auto before = [&](int a, int b) -> bool {
+    const BestLeaf3& A_ = ties[a];
+    const BestLeaf3& B_ = ties[b];
+    for (int l = hmax; l >= 0; --l) {
+      const int ax = (A_.ox + sp.wxy) >> l, ay = (A_.oy + sp.wxy) >> l, az = (A_.oz + sp.wz) >> l;
+      const int bx = (B_.ox + sp.wxy) >> l, by = (B_.oy + sp.wxy) >> l, bz = (B_.oz + sp.wz) >> l;
+      if (A_.scan == B_.scan && ax == bx && ay == by && az == bz) continue;
+      const float fa = l == 0 ? 0.f : anc[static_cast<size_t>(a) * hmax + (l - 1)];
+      const float fb = l == 0 ? 0.f : anc[static_cast<size_t>(b) * hmax + (l - 1)];
+      if (l > 0 && fa != fb) return fa > fb;
+      if (l == hmax) {
+        if (ensure_top_rank() != CSM_OK) { err = CSM_E_CUDA; return false; }
+        const long long ga = ((static_cast<long long>(A_.scan) * jb.nzc + az) * jb.nxc + ay) * jb.nxc + ax;
+        const long long gb = ((static_cast<long long>(B_.scan) * jb.nzc + bz) * jb.nxc + by) * jb.nxc + bx;
+        return top_rank[ga] < top_rank[gb];
       }
-      return false;
-    };
-    int w = 0;
-    for (int t = 1; t < T; ++t)
-      if (before(t, w)) w = t;
-    if (err != CSM_OK) return err;
-    std::swap(ties[0], ties[w]);
-  }
-
-  if (result) {
-    result->leaves_tied = static_cast<int32_t>(ties.size());
-    if (!ties.empty() && best_score > min_score) {
-      const BestLeaf3& t = ties[0];
-      const Scan3& sc = plan.scans[t.angle];
-      const float res = m->hs.resolution;
-      result->found = 1;
-      result->score = best_score;
-      // GetPoseFromCandidate(...).cast<double>() (:369-375)
-      result->pose_estimate[0] = sc.tx + res * static_cast<float>(t.ox);
-      result->pose_estimate[1] = sc.ty + res * static_cast<float>(t.oy);
-      result->pose_estimate[2] = sc.tz + res * static_cast<float>(t.oz);
-      result->pose_estimate[3] = sc.nw;
-      result->pose_estimate[4] = sc.nx;
-      result->pose_estimate[5] = sc.ny;
-      result->pose_estimate[6] = sc.nz;
-      result->rotational_score = t.rot;
-      result->low_resolution_score = t.low;
-      result->best_scan_index = t.scan;
-      result->best_offset[0] = t.ox;
-      result->best_offset[1] = t.oy;
-      result->best_offset[2] = t.oz;
+      // siblings: generation order z outer, y, x inner
+      if ((az & 1) != (bz & 1)) return (az & 1) < (bz & 1);
+      if ((ay & 1) != (by & 1)) return (ay & 1) < (by & 1);
+      return (ax & 1) < (bx & 1);
     }
+    return false;
+  };
+  int w = 0;
+  for (int t = 1; t < T; ++t)
+    if (before(t, w)) w = t;
+  if (err != CSM_OK) return err;
+  std::swap(ties[0], ties[w]);
+  return CSM_OK;
+}
+
+// The result from the first optimal leaf, and the match's statistics.
+void Result3D(const Match3& x, const std::vector<BestLeaf3>& ties, int host_resolves,
+              csm_result3d* result, csm_stats* stats) {
+  const int S = x.hp[kC3Scans];
+  const long long total_top = x.per_scan * S;
+  const float best_score = HostOrderedToFloat(static_cast<unsigned>(x.hp[kC3Bound]));
+  result->leaves_tied = static_cast<int32_t>(ties.size());
+  if (!ties.empty() && best_score > x.min_score) {
+    const BestLeaf3& t = ties[0];
+    const Scan3& sc = x.plan.scans[t.angle];
+    const float res = x.m->hs.resolution;
+    result->found = 1;
+    result->score = best_score;
+    // GetPoseFromCandidate(...).cast<double>() (:369-375)
+    result->pose_estimate[0] = sc.tx + res * static_cast<float>(t.ox);
+    result->pose_estimate[1] = sc.ty + res * static_cast<float>(t.oy);
+    result->pose_estimate[2] = sc.tz + res * static_cast<float>(t.oz);
+    result->pose_estimate[3] = sc.nw;
+    result->pose_estimate[4] = sc.nx;
+    result->pose_estimate[5] = sc.ny;
+    result->pose_estimate[6] = sc.nz;
+    result->rotational_score = t.rot;
+    result->low_resolution_score = t.low;
+    result->best_scan_index = t.scan;
+    result->best_offset[0] = t.ox;
+    result->best_offset[1] = t.oy;
+    result->best_offset[2] = t.oz;
   }
   if (stats) {
     float ms = 0.f;
-    cudaEventElapsedTime(&ms, ctx->ev0, ctx->ev1);
-    stats->candidates_scored = static_cast<int64_t>(total_top + hctr[0]);
+    cudaEventElapsedTime(&ms, x.ctx->ev0, x.ctx->ev1);
+    stats->candidates_scored = static_cast<int64_t>(total_top + x.hctr[0]);
     stats->lowest_resolution_candidates = total_top;
-    stats->nodes_expanded = static_cast<int64_t>(hctr[1]);
+    stats->nodes_expanded = static_cast<int64_t>(x.hctr[1]);
     stats->leaves_tied = static_cast<int64_t>(ties.size());
     stats->num_scans = S;
     stats->host_tie_resolves = host_resolves;
-    stats->host_syncs = host_syncs;
+    stats->host_syncs = x.host_syncs;
     stats->device_ms = ms;
-    if (result && result->found) {
+    if (result->found) {
       stats->best_scan_index = result->best_scan_index;
       stats->best_x_offset = result->best_offset[0];
       stats->best_y_offset = result->best_offset[1];
     }
   }
+}
+
+// One match = one stream of launches + one synchronisation.  `dev` (optional) carries the
+// node's clouds already on the device.
+csm_status Match3D(Ctx* ctx, const csm_matcher3d* m, const csm_node3d* node,
+                   const NodeDev3* dev, const double node_pose[7], const double submap_pose[7],
+                   int full, float min_score, csm_result3d* result, csm_stats* stats) {
+  Match3 x;
+  CSM_TRY(Plan3D(x, ctx, m, node, dev, node_pose, submap_pose, full, min_score));
+  std::memset(result, 0, sizeof(*result));
+  if (stats) std::memset(stats, 0, sizeof(*stats));
+  CSM_TRY(RequireMatchable3D(x));
+  CSM_TRY(Upload3D(x));
+  CSM_TRY(Discretize3D(x));
+  CSM_TRY(TopDive3D(x));
+  CSM_TRY(FilterTop3D(x, x.max_top));
+  CSM_TRY(Sweep3D(x));
+  const int n_best = x.hp[kC3Best];
+  std::vector<BestLeaf3> ties(x.best_inline, x.best_inline + std::min(n_best, kInlineBest));
+  if (n_best > kInlineBest) {
+    ties.resize(n_best);
+    CSM_CUDA(cudaMemcpy(ties.data(), x.d_best->p, sizeof(BestLeaf3) * n_best, cudaMemcpyDeviceToHost));
+    ++x.host_syncs;
+  }
+  int host_resolves = 0;
+  if (ties.size() > 1) CSM_TRY(ResolveTies3D(x, ties, &host_resolves));
+  Result3D(x, ties, host_resolves, result, stats);
   return CSM_OK;
 }
+
+// A test-hook call on a lane.  One that fails after a launch waits for it before the lane
+// goes back, as every call that succeeds does.
+struct Hook3D {
+  LaneGuard guard;
+  Match3 x;
+  ~Hook3D() { if (guard.lane) cudaStreamSynchronize(guard.lane->stream); }
+};
+
+// The start of a test-hook call: the match csm_match3d would run with the same arguments,
+// planned, uploaded and discretised on a lane.
+csm_status StartHook3D(Hook3D& hk, const csm_matcher3d* m,
+                       const csm_node3d* node, const double node_pose[7],
+                       const double submap_pose[7], int32_t full, float min_score) {
+  CSM_REQUIRE(m && node && node_pose && submap_pose, "null pointer");
+  CSM_REQUIRE(node->num_high >= 1 && node->high_resolution_point_cloud, "high-resolution cloud");
+  CSM_REQUIRE(node->num_low >= 0 && (node->num_low == 0 || node->low_resolution_point_cloud),
+              "low-resolution cloud");
+  CSM_TRY(AcquireLane(m->ctx->device, &hk.guard));
+  Match3& x = hk.x;
+  CSM_TRY(Plan3D(x, hk.guard.lane, m, node, nullptr, node_pose, submap_pose, full, min_score));
+  CSM_TRY(RequireMatchable3D(x));
+  CSM_TRY(Upload3D(x));
+  return Discretize3D(x);
+}
+
+}  // namespace
 
 extern "C" {
 
@@ -1548,10 +1497,9 @@ csm_status csm_match3d(const csm_matcher3d* m, const csm_node3d* node, const dou
               "low-resolution cloud");
   LaneGuard guard;
   CSM_TRY(AcquireLane(m->ctx->device, &guard));
-  return Run3D(guard.lane, m, node, nullptr, node_pose, submap_pose, full, min_score, result,
-               stats, false, nullptr, nullptr, nullptr, nullptr);
+  return Match3D(guard.lane, m, node, nullptr, node_pose, submap_pose, full, min_score, result,
+                 stats);
 }
-
 csm_status csm_match3d_batch(const csm_matcher3d* const* matchers, int32_t num_matchers,
                              const csm_node3d* nodes, int32_t num_nodes, const csm_job3d* jobs,
                              int32_t num_jobs, int32_t max_concurrency, csm_result3d* results,
@@ -1633,10 +1581,9 @@ csm_status csm_match3d_batch(const csm_matcher3d* const* matchers, int32_t num_m
         LaneGuard guard;
         rc = AcquireLane(device, &guard);
         if (rc == CSM_OK)
-          rc = Run3D(guard.lane, matchers[jb.matcher_index], &nodes[jb.node_index],
-                     &ndev[jb.node_index], jb.global_node_pose, jb.global_submap_pose,
-                     jb.full_submap, jb.min_score, &results[j], &st, false, nullptr, nullptr,
-                     nullptr, nullptr);
+          rc = Match3D(guard.lane, matchers[jb.matcher_index], &nodes[jb.node_index],
+                       &ndev[jb.node_index], jb.global_node_pose, jb.global_submap_pose,
+                       jb.full_submap, jb.min_score, &results[j], &st);
       }
       std::lock_guard<std::mutex> lock(mu);
       if (rc != CSM_OK) {
@@ -1672,29 +1619,33 @@ csm_status csm_discretize3d(const csm_matcher3d* m, const csm_node3d* node,
                             int32_t* num_scans, int32_t* cells, float* poses, float* rot) {
   CSM_REQUIRE(m && node && node_pose && submap_pose && num_scans, "null pointer");
   CSM_REQUIRE(node->num_high >= 1 && node->high_resolution_point_cloud, "high-resolution cloud");
-  LaneGuard guard;
-  CSM_TRY(AcquireLane(m->ctx->device, &guard));
-  return Run3D(guard.lane, m, node, nullptr, node_pose, submap_pose, full, 0.f, nullptr, nullptr,
-               true, num_scans, cells, poses, rot);
+  Hook3D hk;
+  CSM_TRY(AcquireLane(m->ctx->device, &hk.guard));
+  Match3& x = hk.x;
+  CSM_TRY(Plan3D(x, hk.guard.lane, m, node, nullptr, node_pose, submap_pose, full, 0.f));
+  CSM_TRY(Upload3D(x));
+  CSM_TRY(Discretize3D(x));
+  CSM_TRY(ReadCtl3D(x));
+  const int S = x.hp[kC3Scans];
+  *num_scans = S;
+  if (S == 0 || !cells) return CSM_OK;
+  std::vector<short4> h(static_cast<size_t>(S) * x.jb.n_hi);
+  std::vector<Scan3> hs(S);
+  CSM_CUDA(cudaMemcpy(h.data(), x.d_cells->p, sizeof(short4) * h.size(), cudaMemcpyDeviceToHost));
+  CSM_CUDA(cudaMemcpy(hs.data(), x.d_scans->p, sizeof(Scan3) * S, cudaMemcpyDeviceToHost));
+  for (size_t i = 0; i < h.size(); ++i) {
+    cells[3 * i] = h[i].x;
+    cells[3 * i + 1] = h[i].y;
+    cells[3 * i + 2] = h[i].z;
+  }
+  for (int k = 0; k < S; ++k) {
+    const Scan3& sc = hs[k];
+    const float v[7] = {sc.tx, sc.ty, sc.tz, sc.qw, sc.qx, sc.qy, sc.qz};
+    if (poses) std::memcpy(poses + 7 * k, v, sizeof(v));
+    if (rot) rot[k] = sc.rot_score;
+  }
+  return CSM_OK;
 }
-
-}  // extern "C"
-
-// Runs `probe` on the match csm_match3d would run with these arguments.
-static csm_status RunProbe3D(const csm_matcher3d* m, const csm_node3d* node,
-                             const double node_pose[7], const double submap_pose[7], int32_t full,
-                             float min_score, Probe3D* probe) {
-  CSM_REQUIRE(m && node && node_pose && submap_pose, "null pointer");
-  CSM_REQUIRE(node->num_high >= 1 && node->high_resolution_point_cloud, "high-resolution cloud");
-  CSM_REQUIRE(node->num_low >= 0 && (node->num_low == 0 || node->low_resolution_point_cloud),
-              "low-resolution cloud");
-  LaneGuard guard;
-  CSM_TRY(AcquireLane(m->ctx->device, &guard));
-  return Run3D(guard.lane, m, node, nullptr, node_pose, submap_pose, full, min_score, nullptr,
-               nullptr, false, nullptr, nullptr, nullptr, nullptr, probe);
-}
-
-extern "C" {
 
 csm_status csm_score_candidates3d(const csm_matcher3d* m, const csm_node3d* node,
                                   const double node_pose[7], const double submap_pose[7],
@@ -1703,13 +1654,31 @@ csm_status csm_score_candidates3d(const csm_matcher3d* m, const csm_node3d* node
   static_assert(sizeof(csm_candidate3d) == sizeof(List3), "csm_candidate3d is List3");
   CSM_REQUIRE(sums && scores && (candidates || num_candidates == 0) && num_candidates >= 0,
               "candidates");
-  Probe3D probe;
-  probe.mode = Probe3D::kList;
-  probe.list = reinterpret_cast<const List3*>(candidates);
-  probe.list_n = num_candidates;
-  CSM_TRY(RunProbe3D(m, node, node_pose, submap_pose, full_submap, 0.f, &probe));
-  std::memcpy(sums, probe.sums.data(), sizeof(int) * num_candidates);
-  std::memcpy(scores, probe.scores.data(), sizeof(float) * num_candidates);
+  Hook3D hk;
+  Match3& x = hk.x;
+  CSM_TRY(StartHook3D(hk, m, node, node_pose, submap_pose, full_submap, 0.f));
+  CSM_TRY(ReadCtl3D(x));
+  const int S = x.hp[kC3Scans];
+  const List3* list = reinterpret_cast<const List3*>(candidates);
+  const int n = num_candidates;
+  for (int i = 0; i < n; ++i) {
+    CSM_REQUIRE(list[i].scan >= 0 && list[i].scan < S, "candidate scan_index");
+    CSM_REQUIRE(list[i].depth >= 0 && list[i].depth <= x.hmax, "candidate depth");
+  }
+  if (n == 0) return CSM_OK;
+  cudaStream_t s = x.s;
+  DevBuf *d_lc, *d_ls, *d_li;
+  CSM_TRY(x.ctx->Reserve("m3_tie_c", sizeof(List3) * n, &d_lc));
+  CSM_TRY(x.ctx->Reserve("m3_tie_s", sizeof(float) * n, &d_ls));
+  CSM_TRY(x.ctx->Reserve("m3_probe_sums", sizeof(int) * n, &d_li));
+  CSM_CUDA(cudaMemcpyAsync(d_lc->p, list, sizeof(List3) * n, cudaMemcpyHostToDevice, s));
+  ProfBegin(x.ctx);
+  k3_score_list<<<n, kT3, 0, s>>>(x.jb, d_lc->as<List3>(), d_ls->as<float>(), d_li->as<int>());
+  CSM_LAUNCH_CHECK();
+  ProfEnd(x.ctx, "k3_score_list", n);
+  CSM_CUDA(cudaMemcpyAsync(scores, d_ls->p, sizeof(float) * n, cudaMemcpyDeviceToHost, s));
+  CSM_CUDA(cudaMemcpyAsync(sums, d_li->p, sizeof(int) * n, cudaMemcpyDeviceToHost, s));
+  CSM_CUDA(cudaStreamSynchronize(s));
   return CSM_OK;
 }
 
@@ -1719,21 +1688,31 @@ csm_status csm_score_top3d(const csm_matcher3d* m, const csm_node3d* node,
                            int32_t lattice[2], int32_t* angle_index, float* rotational_scores,
                            int32_t* sums, int32_t* top_best, float* bound, int64_t counters[2]) {
   CSM_REQUIRE(num_scans && lattice, "null pointer");
-  Probe3D probe;
-  probe.mode = Probe3D::kTop;
-  CSM_TRY(RunProbe3D(m, node, node_pose, submap_pose, full_submap, min_score, &probe));
-  const int S = probe.num_scans;
+  Hook3D hk;
+  Match3& x = hk.x;
+  CSM_TRY(StartHook3D(hk, m, node, node_pose, submap_pose, full_submap, min_score));
+  CSM_TRY(TopDive3D(x));
+  unsigned long long c[8];
+  CSM_CUDA(cudaMemcpyAsync(c, x.ctr, sizeof(c), cudaMemcpyDeviceToHost, x.s));
+  CSM_TRY(ReadCtl3D(x));
+  const int S = x.hp[kC3Scans];
   *num_scans = S;
-  lattice[0] = probe.nxc;
-  lattice[1] = probe.nzc;
-  if (angle_index) std::memcpy(angle_index, probe.angle.data(), sizeof(int) * S);
-  if (rotational_scores) std::memcpy(rotational_scores, probe.rot.data(), sizeof(float) * S);
-  if (sums) std::memcpy(sums, probe.top_sums.data(), sizeof(int) * probe.top_sums.size());
-  if (top_best) *top_best = probe.top_best;
-  if (bound) *bound = probe.final_bound;
+  lattice[0] = x.jb.nxc;
+  lattice[1] = x.jb.nzc;
+  if (S && angle_index)
+    CSM_CUDA(cudaMemcpy(angle_index, x.d_sel->p, sizeof(int) * S, cudaMemcpyDeviceToHost));
+  if (S && rotational_scores) {
+    std::vector<Scan3> hs(S);
+    CSM_CUDA(cudaMemcpy(hs.data(), x.d_scans->p, sizeof(Scan3) * S, cudaMemcpyDeviceToHost));
+    for (int k = 0; k < S; ++k) rotational_scores[k] = hs[k].rot_score;
+  }
+  if (S && sums)
+    CSM_CUDA(cudaMemcpy(sums, x.d_top->p, sizeof(int) * x.per_scan * S, cudaMemcpyDeviceToHost));
+  if (top_best) *top_best = x.hp[kC3TopBest];
+  if (bound) *bound = HostOrderedToFloat(static_cast<unsigned>(x.hp[kC3Bound]));
   if (counters) {
-    counters[0] = static_cast<int64_t>(probe.counters[0]);
-    counters[1] = static_cast<int64_t>(probe.counters[2]);
+    counters[0] = static_cast<int64_t>(c[0]);
+    counters[1] = static_cast<int64_t>(c[2]);
   }
   return CSM_OK;
 }
@@ -1749,22 +1728,50 @@ csm_status csm_branch_step3d(const csm_matcher3d* m, const csm_node3d* node,
   CSM_REQUIRE(num_out && final_bound && counters, "null pointer");
   CSM_REQUIRE(num_parents >= 0 && (parents || num_parents == 0), "parents");
   CSM_REQUIRE(level >= 2 ? children != nullptr : leaves != nullptr, "output records");
-  Probe3D probe;
-  probe.mode = Probe3D::kStep;
-  probe.level = level;
-  probe.parents = reinterpret_cast<const Node3*>(parents);
-  probe.num_parents = num_parents;
-  probe.bound = bound;
-  CSM_TRY(RunProbe3D(m, node, node_pose, submap_pose, full_submap, min_score, &probe));
-  if (level >= 2) {
-    *num_out = static_cast<int32_t>(probe.children.size());
-    std::memcpy(children, probe.children.data(), sizeof(Node3) * probe.children.size());
-  } else {
-    *num_out = static_cast<int32_t>(probe.leaves.size());
-    std::memcpy(leaves, probe.leaves.data(), sizeof(Leaf3) * probe.leaves.size());
+  Hook3D hk;
+  Match3& x = hk.x;
+  CSM_TRY(StartHook3D(hk, m, node, node_pose, submap_pose, full_submap, min_score));
+  cudaStream_t s = x.s;
+  CSM_TRY(TopDive3D(x));
+  CSM_TRY(FilterTop3D(x, std::max<long long>(x.max_top, num_parents)));
+  // the level loop over the caller's parents only: its state is reset to them
+  const int h = level, n = num_parents;
+  CSM_REQUIRE(h >= 1 && h <= x.hmax, "level out of range");
+  CSM_REQUIRE(h == x.hmax || n <= kQueueCap, "number of parents");
+  CSM_TRY(ReadCtl3D(x));
+  const int S = x.hp[kC3Scans];
+  const Node3* ps = reinterpret_cast<const Node3*>(parents);
+  const HostSearch3& sp = x.sp;
+  for (int i = 0; i < n; ++i) {
+    const Node3& p = ps[i];
+    CSM_REQUIRE(p.scan >= 0 && p.scan < S, "parent scan_index");
+    const int dx = p.ox + sp.wxy, dy = p.oy + sp.wxy, dz = p.oz + sp.wz;
+    CSM_REQUIRE(dx >= 0 && dy >= 0 && dz >= 0 && ((dx | dy | dz) & ((1 << h) - 1)) == 0 &&
+                    p.ox <= sp.wxy && p.oy <= sp.wxy && p.oz <= sp.wz,
+                "parent is not a node of its level's lattice");
   }
-  *final_bound = probe.final_bound;
-  for (int k = 0; k < 3; ++k) counters[k] = static_cast<int64_t>(probe.counters[k]);
+  int* hp = x.hp;
+  for (int l = 1; l <= x.hmax; ++l) hp[l] = 0;
+  hp[h] = n;
+  hp[kC3Leaf] = 0;
+  hp[kC3Overflow] = 0;
+  hp[kC3Bound] = static_cast<int>(HostFloatToOrdered(bound));
+  CSM_CUDA(cudaMemcpyAsync(x.ictr, hp, kRbCtr, cudaMemcpyHostToDevice, s));
+  CSM_CUDA(cudaMemsetAsync(x.ctr, 0, 8 * 8, s));
+  if (n) CSM_CUDA(cudaMemcpyAsync(x.Queue(h), ps, sizeof(Node3) * n, cudaMemcpyHostToDevice, s));
+  for (int done = 0; done < n; done += kChunk) CSM_TRY(LevelStep3D(x, h));
+  unsigned long long c[8];
+  CSM_CUDA(cudaMemcpyAsync(c, x.ctr, sizeof(c), cudaMemcpyDeviceToHost, s));
+  CSM_TRY(ReadCtl3D(x));
+  if (hp[kC3Overflow]) { SetError("3D branch-and-bound capacity exceeded"); return CSM_E_CAPACITY; }
+  *num_out = h >= 2 ? hp[h - 1] : hp[kC3Leaf];
+  if (*num_out && h >= 2)
+    CSM_CUDA(cudaMemcpy(children, x.Queue(h - 1), sizeof(Node3) * *num_out,
+                        cudaMemcpyDeviceToHost));
+  if (*num_out && h == 1)
+    CSM_CUDA(cudaMemcpy(leaves, x.d_leaves->p, sizeof(Leaf3) * *num_out, cudaMemcpyDeviceToHost));
+  *final_bound = HostOrderedToFloat(static_cast<unsigned>(hp[kC3Bound]));
+  for (int k = 0; k < 3; ++k) counters[k] = static_cast<int64_t>(c[k]);
   return CSM_OK;
 }
 

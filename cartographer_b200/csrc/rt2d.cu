@@ -502,8 +502,6 @@ void PrepareJob(const RtHostJob& job, const RtGridDev& G, const RtParams& P, dou
       jd->y0 = static_cast<int>(ry0);
     }
   }
-  static const bool origin0_only = getenv("CSM_RT_ORIGIN0") != nullptr;   // debug switch
-  if (origin0_only && (jd->x0 != 0 || jd->y0 != 0)) plan->smem = false;
 }
 
 int NumAngular(const RtHostJob& job, double resolution, double angular_window) {
@@ -608,8 +606,7 @@ csm_status RtRun(Ctx* ctx, const csm_rt_grid2d* grid, const RtHostJob* jobs, int
   CSM_CUDA(cudaMemsetAsync(d_best.p, 0, sizeof(unsigned long long) * num, s));
   const char* d = d_up.as<char>();
   const int total_items = static_cast<int>(items);
-  static const bool no_tma = getenv("CSM_RT_NO_TMA") != nullptr;   // debug: global gathers only
-  const int form = grid->d_wcells ? 2 : ((all_smem && !no_tma) ? 0 : 1);
+  const int form = grid->d_wcells ? 2 : (all_smem ? 0 : 1);
   const size_t smem = form == 0 ? static_cast<size_t>(G.bw) * G.bh * 2 : 0;
   int per_sm = 1;
 #define CSM_RT_LAUNCH(F, A)                                                                     \

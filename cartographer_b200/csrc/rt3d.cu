@@ -157,8 +157,6 @@ Qf HAngleAxis(const Vf& aa) {  // transform/transform.h:85-99
   return Qf{w, scale * aa.x, scale * aa.y, scale * aa.z};
 }
 
-int DivUpR(long long a, long long b) { return static_cast<int>((a + b - 1) / b); }
-
 }  // namespace
 
 extern "C" {
@@ -213,7 +211,7 @@ csm_status csm_grid3d_create(const int32_t* idx, const uint16_t* values, int64_t
     CSM_TRY(d_val.Reserve(sizeof(uint16_t) * n));
     CSM_CUDA(cudaMemcpyAsync(d_idx.p, idx, sizeof(int) * 3 * n, cudaMemcpyHostToDevice, s));
     CSM_CUDA(cudaMemcpyAsync(d_val.p, values, sizeof(uint16_t) * n, cudaMemcpyHostToDevice, s));
-    k_rt3_scatter<<<DivUpR(n, 256), 256, 0, s>>>(d_idx.as<int>(), d_val.as<uint16_t>(), n, d,
+    k_rt3_scatter<<<DivUp(n, 256), 256, 0, s>>>(d_idx.as<int>(), d_val.as<uint16_t>(), n, d,
                                                  g->d_vol);
     CSM_LAUNCH_CHECK();
   }
