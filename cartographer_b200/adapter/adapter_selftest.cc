@@ -437,5 +437,39 @@ int main() {
     for (uint8_t v : level) std::printf(" %u", v);
     std::printf("\n");
   }
+  // ---- TSDFRangeDataInserter2D on a device grid: the reference's InsertPoint
+  // (tsdf_range_data_inserter_2d_test.cc:50-57, the 8 x 1 grid that grows), then two returns
+  // with the lua defaults' normal projection and weighting ----
+  {
+    mapping::proto::TSDFRangeDataInserterOptions2D to;
+    to.set_truncation_distance(2.0);
+    to.set_maximum_weight(10.);
+    to.set_update_free_space(false);
+    to.mutable_normal_estimation_options()->set_num_normal_samples(2);
+    to.mutable_normal_estimation_options()->set_sample_radius(10.);
+    to.set_project_sdf_distance_to_scan_normal(false);
+    const mapping::scan_matching::TSDFRangeDataInserter2D plain(to);
+    to.set_project_sdf_distance_to_scan_normal(true);
+    to.set_update_weight_angle_scan_normal_to_ray_kernel_bandwidth(0.5);
+    to.set_update_weight_distance_cell_to_hit_kernel_bandwidth(0.5);
+    const mapping::scan_matching::TSDFRangeDataInserter2D weighted(to);
+    mapping::scan_matching::DeviceGrid2D grid(
+        mapping::MapLimits(1., 1., 7., mapping::CellLimits{8, 1}), 2.f, 10.f, 0);
+    sensor::RangeData range_data;
+    range_data.origin = {{-0.5f, -0.5f, 0.f}};
+    range_data.returns = sensor::PointCloud({{{{-0.5f, 3.5f, 0.f}}}}, {});
+    plain.Insert(range_data, &grid);
+    range_data.returns = sensor::PointCloud({{{{-0.5f, 3.5f, 0.f}}}, {{{5.5f, 3.5f, 0.f}}}}, {});
+    weighted.Insert(range_data, &grid);
+    std::vector<uint16_t> tsd, weights;
+    const csm_rt_grid2d_info info = grid.Read(&tsd);
+    grid.ReadWeights(&weights);
+    std::printf("RESULT insert_tsdf2d %.17g %.17g %.17g %d %d %d %d %d %d %d", info.resolution,
+                info.max_x, info.max_y, info.num_x_cells, info.num_y_cells, info.known_empty,
+                info.known_min_x, info.known_min_y, info.known_max_x, info.known_max_y);
+    for (uint16_t v : tsd) std::printf(" %u", v);
+    for (uint16_t v : weights) std::printf(" %u", v);
+    std::printf("\n");
+  }
   return 0;
 }

@@ -105,6 +105,44 @@ class ProbabilityGridRangeDataInserterOptions2D {
   double hit_ = 0., miss_ = 0.;
   bool insert_free_space_ = true;
 };
+// mapping/proto/normal_estimation_options_2d.proto
+class NormalEstimationOptions2D {
+ public:
+  int32_t num_normal_samples() const { return num_normal_samples_; }
+  double sample_radius() const { return sample_radius_; }
+  void set_num_normal_samples(int32_t v) { num_normal_samples_ = v; }
+  void set_sample_radius(double v) { sample_radius_ = v; }
+ private:
+  int32_t num_normal_samples_ = 0;
+  double sample_radius_ = 0.;
+};
+// mapping/proto/tsdf_range_data_inserter_options_2d.proto
+class TSDFRangeDataInserterOptions2D {
+ public:
+  double truncation_distance() const { return truncation_distance_; }
+  double maximum_weight() const { return maximum_weight_; }
+  bool update_free_space() const { return update_free_space_; }
+  const NormalEstimationOptions2D& normal_estimation_options() const { return normal_; }
+  NormalEstimationOptions2D* mutable_normal_estimation_options() { return &normal_; }
+  bool project_sdf_distance_to_scan_normal() const { return project_; }
+  int32_t update_weight_range_exponent() const { return range_exponent_; }
+  double update_weight_angle_scan_normal_to_ray_kernel_bandwidth() const { return angle_bw_; }
+  double update_weight_distance_cell_to_hit_kernel_bandwidth() const { return distance_bw_; }
+  void set_truncation_distance(double v) { truncation_distance_ = v; }
+  void set_maximum_weight(double v) { maximum_weight_ = v; }
+  void set_update_free_space(bool v) { update_free_space_ = v; }
+  void set_project_sdf_distance_to_scan_normal(bool v) { project_ = v; }
+  void set_update_weight_range_exponent(int32_t v) { range_exponent_ = v; }
+  void set_update_weight_angle_scan_normal_to_ray_kernel_bandwidth(double v) { angle_bw_ = v; }
+  void set_update_weight_distance_cell_to_hit_kernel_bandwidth(double v) { distance_bw_ = v; }
+ private:
+  double truncation_distance_ = 0., maximum_weight_ = 0.;
+  bool update_free_space_ = false;
+  NormalEstimationOptions2D normal_;
+  bool project_ = false;
+  int32_t range_exponent_ = 0;
+  double angle_bw_ = 0., distance_bw_ = 0.;
+};
 }  // namespace proto
 }  // namespace mapping
 
@@ -227,11 +265,18 @@ class TSDF2D : public Grid2D {
       : Grid2D(limits, -truncation_distance, truncation_distance, std::move(tsd_cells)),
         truncation_distance_(truncation_distance), max_weight_(max_weight),
         weight_cells_(std::move(weight_cells)) {}
+  // the all-unknown TSDF2D ActiveSubmaps2D::CreateGrid makes (tsdf_2d.cc:24-33)
+  TSDF2D(const MapLimits& limits, float truncation_distance, float max_weight)
+      : TSDF2D(limits, truncation_distance, max_weight, Unknown(limits), Unknown(limits)) {}
   GridType GetGridType() const override { return GridType::TSDF; }
   float truncation_distance() const { return truncation_distance_; }
   float max_weight() const { return max_weight_; }
   const std::vector<uint16_t>& weight_cells() const { return weight_cells_; }
  private:
+  static std::vector<uint16_t> Unknown(const MapLimits& l) {
+    return std::vector<uint16_t>(
+        static_cast<size_t>(l.cell_limits().num_x_cells) * l.cell_limits().num_y_cells, 0);
+  }
   float truncation_distance_, max_weight_;
   std::vector<uint16_t> weight_cells_;
 };

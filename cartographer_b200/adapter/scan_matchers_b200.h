@@ -256,6 +256,14 @@ class DeviceGrid2D {
         limits.resolution(), limits.max().x(), limits.max().y(),
         limits.cell_limits().num_x_cells, limits.cell_limits().num_y_cells, device, &grid_));
   }
+  // TSDF2D(limits, truncation_distance, max_weight): the all-unknown TSDF2D
+  // ActiveSubmaps2D::CreateGrid makes for GridType::TSDF, filled by TSDFRangeDataInserter2D below.
+  DeviceGrid2D(const MapLimits& limits, float truncation_distance, float max_weight, int device) {
+    b200_internal::Check(csm_rt_grid2d_create_empty_tsdf(
+        limits.resolution(), limits.max().x(), limits.max().y(),
+        limits.cell_limits().num_x_cells, limits.cell_limits().num_y_cells, truncation_distance,
+        max_weight, device, &grid_));
+  }
   ~DeviceGrid2D() { csm_rt_grid2d_destroy(grid_); }
   DeviceGrid2D(const DeviceGrid2D&) = delete;
   DeviceGrid2D& operator=(const DeviceGrid2D&) = delete;
@@ -279,6 +287,13 @@ class DeviceGrid2D {
                                               static_cast<int64_t>(cells->size())));
     }
     return info;
+  }
+  // The weight cells of a TSDF2D (num_y x num_x); Read gives its tsd cells.
+  void ReadWeights(std::vector<uint16_t>* weight_cells) const {
+    const csm_rt_grid2d_info info = Read(nullptr);
+    weight_cells->resize(static_cast<size_t>(info.num_x_cells) * info.num_y_cells);
+    b200_internal::Check(csm_rt_grid2d_read_weights(grid_, weight_cells->data(),
+                                                    static_cast<int64_t>(weight_cells->size())));
   }
 
  private:
@@ -326,6 +341,45 @@ class ProbabilityGridRangeDataInserter2D {
 
  private:
   csm_range_inserter2d* inserter_ = nullptr;
+};
+
+// mapping/internal/2d/tsdf_range_data_inserter_2d.h:29-50 on device grids: Submap2D with
+// GridType::TSDF keeps its grid as a DeviceGrid2D(limits, truncation, max_weight, device) and
+// inserts every scan in place.
+class TSDFRangeDataInserter2D {
+ public:
+  explicit TSDFRangeDataInserter2D(const mapping::proto::TSDFRangeDataInserterOptions2D& options,
+                                   int device = 0) {
+    csm_tsdf_inserter_options2d o{};
+    o.truncation_distance = options.truncation_distance();
+    o.maximum_weight = options.maximum_weight();
+    o.update_free_space = options.update_free_space() ? 1 : 0;
+    o.num_normal_samples = options.normal_estimation_options().num_normal_samples();
+    o.sample_radius = options.normal_estimation_options().sample_radius();
+    o.project_sdf_distance_to_scan_normal = options.project_sdf_distance_to_scan_normal() ? 1 : 0;
+    o.update_weight_range_exponent = options.update_weight_range_exponent();
+    o.update_weight_angle_scan_normal_to_ray_kernel_bandwidth =
+        options.update_weight_angle_scan_normal_to_ray_kernel_bandwidth();
+    o.update_weight_distance_cell_to_hit_kernel_bandwidth =
+        options.update_weight_distance_cell_to_hit_kernel_bandwidth();
+    b200_internal::Check(csm_tsdf_inserter2d_create(&o, device, &inserter_));
+  }
+  ~TSDFRangeDataInserter2D() { csm_tsdf_inserter2d_destroy(inserter_); }
+  TSDFRangeDataInserter2D(const TSDFRangeDataInserter2D&) = delete;
+  TSDFRangeDataInserter2D& operator=(const TSDFRangeDataInserter2D&) = delete;
+
+  // tsdf_range_data_inserter_2d.cc:131-165; range_data in the grid's frame (misses unused).
+  void Insert(const sensor::RangeData& range_data, DeviceGrid2D* grid) const {
+    if (grid == nullptr) std::abort();
+    const std::vector<float> returns = b200_internal::Flatten(range_data.returns);
+    const float origin[3] = {range_data.origin.x(), range_data.origin.y(), range_data.origin.z()};
+    b200_internal::Check(csm_tsdf_inserter2d_insert(
+        inserter_, origin, returns.data(), static_cast<int32_t>(range_data.returns.size()),
+        grid->mutable_handle(), nullptr));
+  }
+
+ private:
+  csm_tsdf_inserter2d* inserter_ = nullptr;
 };
 
 // ceres_scan_matcher_2d.h:42-64.  Same constructor and Match signature, except that the

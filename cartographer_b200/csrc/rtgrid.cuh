@@ -1,6 +1,6 @@
 // The grid-resident ProbabilityGrid / TSDF2D handle shared by the real-time matcher
-// (rt2d.cu), the post-match refinement (refine2d.cu) and the 2D range data inserter
-// (insert2d.cu).
+// (rt2d.cu), the post-match refinement (refine2d.cu) and the 2D range data inserters
+// (insert2d.cu, insert_tsdf2d.cu).
 #ifndef CSM_RTGRID_CUH_
 #define CSM_RTGRID_CUH_
 

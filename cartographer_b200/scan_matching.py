@@ -343,7 +343,8 @@ class CsmRtGrid2DInfo(C.Structure):
 @dataclass
 class GridState:
     """A ProbabilityGrid read back from the device: correspondence-cost cells[y, x], MapLimits
-    and the known-cells box (min_x, min_y, max_x, max_y), None when empty.  Usable wherever a
+    and the known-cells box (min_x, min_y, max_x, max_y), None when empty.  For a TSDF2D,
+    cells are its tsd cells and weight_cells its weight cells.  Usable wherever a
     grid record is taken (FastCorrelativeScanMatcher2D, RealTimeGrid2D)."""
     cells: np.ndarray
     resolution: float
@@ -352,6 +353,7 @@ class GridState:
     known_cells_box: object = None
     min_cost: float = float(np.float32(1.0) - (np.float32(1.0) - np.float32(0.1)))
     max_cost: float = float(np.float32(1.0) - np.float32(0.1))
+    weight_cells: object = None   # a TSDF2D's weight cells[y, x] (cells are its tsd cells)
 
 
 class RealTimeGrid2D:
@@ -400,6 +402,22 @@ class RealTimeGrid2D:
         self.shape = (num_y, num_x)
         return self
 
+    @classmethod
+    def empty_tsdf(cls, resolution, max_x, max_y, truncation_distance, max_weight, num_x=100,
+                   num_y=100, device=0):
+        """An all-unknown TSDF2D of the given limits and converter
+        (csm_rt_grid2d_create_empty_tsdf), to be filled by TSDFRangeDataInserter2D.Insert:
+        ActiveSubmaps2D::CreateGrid for GridType::TSDF."""
+        self = cls.__new__(cls)
+        self.device, self.is_tsdf = device, True
+        self._h = C.c_void_p()
+        check(lib().csm_rt_grid2d_create_empty_tsdf(
+            C.c_double(resolution), C.c_double(max_x), C.c_double(max_y), C.c_int32(num_x),
+            C.c_int32(num_y), C.c_float(truncation_distance), C.c_float(max_weight),
+            C.c_int32(device), C.byref(self._h)))
+        self.shape = (num_y, num_x)
+        return self
+
     def _info(self, cells=None):
         info = CsmRtGrid2DInfo()
         check(lib().csm_rt_grid2d_read(self._h, C.byref(info),
@@ -416,7 +434,13 @@ class RealTimeGrid2D:
         info = self._info(cells)
         box = None if info.known_empty else (info.known_min_x, info.known_min_y,
                                              info.known_max_x, info.known_max_y)
-        return GridState(cells, info.resolution, info.max_x, info.max_y, box)
+        weights = None
+        if info.is_tsdf:
+            weights = np.zeros_like(cells)
+            check(lib().csm_rt_grid2d_read_weights(self._h, ptr(weights, C.c_uint16),
+                                                   C.c_int64(weights.size)))
+        return GridState(cells, info.resolution, info.max_x, info.max_y, box,
+                         weight_cells=weights)
 
     def ComputeCroppedGrid(self):
         """ProbabilityGrid::ComputeCroppedGrid from device to device: a new RealTimeGrid2D over
@@ -504,6 +528,75 @@ class ProbabilityGridRangeDataInserter2D:
     def close(self):
         if getattr(self, "_h", None):
             lib().csm_range_inserter2d_destroy(self._h)
+            self._h = None
+
+    __del__ = close
+
+
+# ===========================================================================
+# TSDFRangeDataInserter2D (mapping/internal/2d/tsdf_range_data_inserter_2d.h)
+# ===========================================================================
+class CsmTsdfInserterOptions2D(C.Structure):
+    _fields_ = [("truncation_distance", C.c_double), ("maximum_weight", C.c_double),
+                ("update_free_space", C.c_int32), ("num_normal_samples", C.c_int32),
+                ("sample_radius", C.c_double),
+                ("project_sdf_distance_to_scan_normal", C.c_int32),
+                ("update_weight_range_exponent", C.c_int32),
+                ("update_weight_angle_scan_normal_to_ray_kernel_bandwidth", C.c_double),
+                ("update_weight_distance_cell_to_hit_kernel_bandwidth", C.c_double)]
+
+
+@dataclass
+class TSDFRangeDataInserterOptions2D:
+    """proto TSDFRangeDataInserterOptions2D with NormalEstimationOptions2D flattened in; defaults
+    are configuration_files/trajectory_builder_2d.lua's submaps.tsdf_range_data_inserter."""
+    truncation_distance: float = 0.3
+    maximum_weight: float = 10.0
+    update_free_space: bool = False
+    num_normal_samples: int = 4
+    sample_radius: float = 0.5
+    project_sdf_distance_to_scan_normal: bool = True
+    update_weight_range_exponent: int = 0
+    update_weight_angle_scan_normal_to_ray_kernel_bandwidth: float = 0.5
+    update_weight_distance_cell_to_hit_kernel_bandwidth: float = 0.5
+
+    def _c(self):
+        return CsmTsdfInserterOptions2D(
+            self.truncation_distance, self.maximum_weight, 1 if self.update_free_space else 0,
+            self.num_normal_samples, self.sample_radius,
+            1 if self.project_sdf_distance_to_scan_normal else 0,
+            self.update_weight_range_exponent,
+            self.update_weight_angle_scan_normal_to_ray_kernel_bandwidth,
+            self.update_weight_distance_cell_to_hit_kernel_bandwidth)
+
+
+class TSDFRangeDataInserter2D:
+    """Insert(origin, returns, grid) writes one scan into a TSDF2D RealTimeGrid2D in place, as
+    the reference's Insert(range_data, grid) writes a TSDF2D: origin (2 or 3) and returns (n x 3)
+    are in the grid's frame.  The grid grows as the reference's does, and its `shape` follows."""
+
+    def __init__(self, options=None, device=0):
+        self.options = options or TSDFRangeDataInserterOptions2D()
+        self.last_stats = None
+        self._h = C.c_void_p()
+        o = self.options._c()
+        check(lib().csm_tsdf_inserter2d_create(C.byref(o), C.c_int32(device), C.byref(self._h)))
+
+    def Insert(self, origin, returns, grid):
+        org = np.zeros(3, np.float32)
+        o = np.asarray(origin, np.float32).reshape(-1)
+        org[:len(o)] = o[:3]
+        ret = _f32(np.zeros((0, 3)) if returns is None else returns)
+        stats = CsmStats()
+        check(lib().csm_tsdf_inserter2d_insert(
+            self._h, ptr(org, C.c_float), ptr(ret, C.c_float), C.c_int32(len(ret)), grid._h,
+            C.byref(stats)))
+        self.last_stats = stats.as_dict()
+        grid._info()
+
+    def close(self):
+        if getattr(self, "_h", None):
+            lib().csm_tsdf_inserter2d_destroy(self._h)
             self._h = None
 
     __del__ = close

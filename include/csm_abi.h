@@ -759,6 +759,53 @@ typedef struct csm_rt_grid2d_info {
 csm_status csm_rt_grid2d_read(const csm_rt_grid2d* grid, csm_rt_grid2d_info* info,
                               uint16_t* cells, int64_t capacity);
 
+/* ---- map writing in 2D: TSDFRangeDataInserter2D on device grids ----------------------- */
+/* TSDFRangeDataInserter2D (mapping/internal/2d/tsdf_range_data_inserter_2d.cc) applied in place
+ * to a TSDF2D csm_rt_grid2d, so that a TSDF submap lives on the device as a ProbabilityGrid
+ * submap does.  After every insert, every tsd and weight cell, the limits and the known-cells box
+ * are bit-equal to what the reference's Insert + FinishUpdate leaves.  Each cell is written at
+ * most once per insert, from its value before the insert, by the first ray in sorted order that
+ * reaches it with a non-zero weight (DESIGN §9).  The handle grows as Grid2D::GrowLimits does,
+ * both arrays alike.  The inserter's truncation distance and maximum weight drive the update; the
+ * handle's own ones encode and decode its cells.  No match may be in flight on a handle being
+ * inserted into. */
+typedef struct csm_tsdf_inserter_options2d {   /* proto TSDFRangeDataInserterOptions2D */
+  double truncation_distance;                  /* > 0 */
+  double maximum_weight;                       /* > 0 */
+  int32_t update_free_space;                   /* bool */
+  int32_t num_normal_samples;                  /* normal_estimation_options, > 0 */
+  double sample_radius;                        /* normal_estimation_options, > 0 */
+  int32_t project_sdf_distance_to_scan_normal; /* bool */
+  int32_t update_weight_range_exponent;
+  double update_weight_angle_scan_normal_to_ray_kernel_bandwidth;
+  double update_weight_distance_cell_to_hit_kernel_bandwidth;
+} csm_tsdf_inserter_options2d;
+typedef struct csm_tsdf_inserter2d csm_tsdf_inserter2d;
+csm_status csm_tsdf_inserter2d_create(const csm_tsdf_inserter_options2d* options, int32_t device,
+                                      csm_tsdf_inserter2d** out);
+csm_status csm_tsdf_inserter2d_destroy(csm_tsdf_inserter2d* inserter);
+/* TSDFRangeDataInserter2D::Insert(range_data, grid) + FinishUpdate.  origin and returns
+ * (num_returns x {x, y, z}) are in the grid's frame; z enters only the growth and the normals, as
+ * in the reference.  CSM_E_INVALID, with the handle unchanged (cells, weights, limits and box),
+ * for a ProbabilityGrid handle, a null or non-finite input, a grid on another device, an insert
+ * that would grow the grid to 30000 cells or more per axis, a tsd cell on a ray that carries
+ * kUpdateMarker, or a ray whose pixel mask leaves the grown grid (a return whose z differs from
+ * the origin's can reach past the growth the reference computes).  One stream synchronisation;
+ * stats (may be NULL) gets host_syncs and device_ms. */
+csm_status csm_tsdf_inserter2d_insert(const csm_tsdf_inserter2d* inserter, const float origin[3],
+                                      const float* returns, int32_t num_returns,
+                                      csm_rt_grid2d* grid, csm_stats* stats /* may be NULL */);
+/* ActiveSubmaps2D::CreateGrid for GridType::TSDF: an all-unknown TSDF2D (tsd 0, weight 0) of the
+ * given limits and converter, with an empty known-cells box. */
+csm_status csm_rt_grid2d_create_empty_tsdf(double resolution, double max_x, double max_y,
+                                           int32_t num_x_cells, int32_t num_y_cells,
+                                           float truncation_distance, float max_weight,
+                                           int32_t device, csm_rt_grid2d** out);
+/* The weight cells of a TSDF2D handle (num_y x num_x, row-major; capacity in cells).
+ * csm_rt_grid2d_read gives its tsd cells, limits and known-cells box. */
+csm_status csm_rt_grid2d_read_weights(const csm_rt_grid2d* grid, uint16_t* weight_cells,
+                                      int64_t capacity);
+
 /* Test hook: as csm_ceres_evaluate3d, in the problem's residual-block order — per cloud its
  * occupied-space residuals, then its intensity residuals if it has a grid; then 3
  * translation and 3 rotation residuals.  Residuals and rows are uncorrected by the loss, as
