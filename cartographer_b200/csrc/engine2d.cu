@@ -1489,12 +1489,12 @@ void BuildLut(float min_cost, float max_cost, uint8_t* lut, float* min_score, fl
   const float hi = 1.f - min_cost;  // max_score_
   *min_score = lo;
   *max_score = hi;
-  const float kScale = (max_cost - min_cost) / 32766.f;
+  const ValueConversion value_to_cost = MakeValueConversion(min_cost, max_cost);
   for (int v = 0; v < 65536; ++v) {
-    const uint16_t value = static_cast<uint16_t>(v) & static_cast<uint16_t>(~(1u << 15));
+    const uint16_t value = static_cast<uint16_t>(v) & static_cast<uint16_t>(~kUpdateMarker);
     float cost;
     if (value == 0) cost = max_cost;  // unknown -> max_correspondence_cost (grid_2d.cc:69-71)
-    else cost = value * kScale + (min_cost - kScale);
+    else cost = value_to_cost(value);
     const float probability = 1.f - std::abs(cost);
     const long q = std::lround((probability - lo) * (255.f / (hi - lo)));
     lut[v] = static_cast<uint8_t>(q < 0 ? 0 : (q > 255 ? 255 : q));
@@ -1650,8 +1650,6 @@ csm_status csm_stack2d_create_from_rt_grid2d(const csm_rt_grid2d* grid, int32_t 
   CSM_REQUIRE(grid != nullptr && out != nullptr, "null pointer");
   CSM_REQUIRE(grid->d_wcells == nullptr, "a TSDF2D handle has no precomputation stack");
   std::lock_guard<std::mutex> lock(grid->ctx->mu);
-  const float kMinCorrespondenceCost = 1.f - (1.f - 0.1f);   // probability_values.h:64-67
-  const float kMaxCorrespondenceCost = 1.f - 0.1f;
   return CreateStack2D(grid->d_cells, grid->g.pitch, true, grid->g.nx, grid->g.ny,
                        grid->g.resolution, grid->g.max_x, grid->g.max_y, kMinCorrespondenceCost,
                        kMaxCorrespondenceCost, depth, grid->ctx->device, out);

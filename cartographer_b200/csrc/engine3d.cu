@@ -15,6 +15,7 @@
 #include <functional>
 
 #include "common.cuh"
+#include "value_conversion.h"
 
 #include <atomic>
 #include <mutex>
@@ -96,7 +97,7 @@ __device__ __forceinline__ int CellOf(float p, float resolution) {
 }
 // PrecomputationGrid3D::ToProbability(sum / float(N))  (precomputation_grid_3d.h:32-35)
 __device__ __forceinline__ float ToScore3(int sum, int n) {
-  const float kMin = 0.1f;
+  const float kMin = kMinProbability;
   const float kMax = __fsub_rn(1.f, kMin);
   const float k = __fdiv_rn(__fsub_rn(kMax, kMin), 255.f);
   return __fadd_rn(kMin, __fmul_rn(__fdiv_rn(__int2float_rn(sum), __int2float_rn(n)), k));
@@ -825,12 +826,12 @@ csm_status csm_matcher3d_create(const int32_t* hi_idx, const uint16_t* hi_val, i
   // ---- depth 0: ConvertToPrecomputationGrid (precomputation_grid_3d.cc:49-61) ----
   std::vector<uint8_t> lut(65536);
   {
-    const float kMin = 0.1f, kMax = 1.f - kMin;
-    const float kScale = (kMax - kMin) / 32766.f;
+    const ValueConversion probability = MakeValueConversion(kMinProbability, kMaxProbability);
     for (int v = 0; v < 65536; ++v) {
       const uint16_t value = static_cast<uint16_t>(v) & 0x7fff;
-      const float p = value == 0 ? kMin : value * kScale + (kMin - kScale);
-      const long q = std::lround((p - kMin) * (255.f / (kMax - kMin)));
+      const float p = value == 0 ? kMinProbability : probability(value);
+      const long q =
+          std::lround((p - kMinProbability) * (255.f / (kMaxProbability - kMinProbability)));
       lut[v] = static_cast<uint8_t>(q < 0 ? 0 : (q > 255 ? 255 : q));
     }
   }
@@ -872,10 +873,10 @@ csm_status csm_matcher3d_create(const int32_t* hi_idx, const uint16_t* hi_val, i
   hl.p = m->d_lowvol;
   hl.resolution = lo_res;
   {
-    const float kMin = 0.1f, kMax = 1.f - kMin;
-    hl.k_scale = (kMax - kMin) / 32766.f;
-    hl.bias = kMin - hl.k_scale;
-    hl.min_probability = kMin;
+    const ValueConversion probability = MakeValueConversion(kMinProbability, kMaxProbability);
+    hl.k_scale = probability.scale;
+    hl.bias = probability.bias;
+    hl.min_probability = kMinProbability;
   }
   if (lo_n > 0) {
     CSM_TRY(d_idx.Reserve(sizeof(int) * 3 * lo_n));
@@ -1341,10 +1342,10 @@ csm_status ResolveTies3D(Match3& x, std::vector<BestLeaf3>& ties, int* host_reso
     CSM_CUDA(cudaMemcpy(sums.data(), x.d_top->p, sizeof(int) * total_top, cudaMemcpyDeviceToHost));
     struct Item { float score; int gen; };
     std::vector<Item> items(total_top);
-    const float kMin = 0.1f, kMax = 1.f - kMin;
     for (long long i = 0; i < total_top; ++i)
-      items[i] = Item{kMin + (static_cast<float>(sums[i]) / static_cast<float>(x.jb.n_hi)) *
-                                 ((kMax - kMin) / 255.f),
+      items[i] = Item{kMinProbability +
+                          (static_cast<float>(sums[i]) / static_cast<float>(x.jb.n_hi)) *
+                              ((kMaxProbability - kMinProbability) / 255.f),
                       static_cast<int>(i)};
     std::sort(items.begin(), items.end(),
               [](const Item& a, const Item& b) { return a.score > b.score; });

@@ -14,6 +14,7 @@
 #include <string>
 
 #include "engine2d.cuh"
+#include "value_conversion.h"
 
 namespace {
 
@@ -135,10 +136,9 @@ bool ParseGrid2D(Reader r, Grid2DProto* g, std::string* err) {
   if (!r.ok) { *err = "malformed proto::Grid2D"; return false; }
   // MinCorrespondenceCostFromProto / Max... (grid_2d.cc:27-52): legacy grids without the
   // two fields are probability grids with the default bounds
-  const float kMinP = 0.1f, kMaxP = 1.f - kMinP;
   if (g->min_cost == 0.f && g->max_cost == 0.f) {
-    g->min_cost = 1.f - kMaxP;
-    g->max_cost = 1.f - kMinP;
+    g->min_cost = kMinCorrespondenceCost;
+    g->max_cost = kMaxCorrespondenceCost;
   }
   if (g->nx < 1 || g->ny < 1 || static_cast<size_t>(g->nx) * g->ny != g->cells.size()) {
     *err = "cell count does not match the cell limits";

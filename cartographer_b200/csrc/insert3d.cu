@@ -26,6 +26,7 @@
 
 #include "common.cuh"
 #include "grid3d.cuh"
+#include "value_conversion.h"
 
 struct csm_range_inserter3d {
   csm::Ctx* ctx = nullptr;
@@ -36,9 +37,6 @@ struct csm_range_inserter3d {
 
 namespace csm {
 
-constexpr int kValueCount = 32768;          // probability_values.cc:25
-constexpr uint16_t kUpdateMarker = 1u << 15;
-
 struct Box3 {
   int lo[3];
   int n[3];
@@ -47,19 +45,6 @@ struct Box3 {
 __device__ __forceinline__ unsigned long long BoxIndex(const Box3& b, int x, int y, int z) {
   return (static_cast<unsigned long long>(z - b.lo[2]) * b.n[1] + (y - b.lo[1])) * b.n[0] +
          (x - b.lo[0]);
-}
-
-// HybridGrid::ApplyLookupTable: applies `table` unless the cell carries the update marker;
-// returns whether this call applied it.
-__device__ __forceinline__ bool ApplyTable(uint16_t* cell, const uint16_t* __restrict__ table) {
-  unsigned short* c = reinterpret_cast<unsigned short*>(cell);
-  unsigned short old = *c;
-  while (!(old & kUpdateMarker)) {
-    const unsigned short prev = atomicCAS(c, old, table[old]);
-    if (prev == old) return true;
-    old = prev;
-  }
-  return false;
 }
 
 __device__ __forceinline__ void Touched(unsigned long long idx, unsigned long long* list,
@@ -104,9 +89,7 @@ __global__ void k_ins3_finish(const unsigned long long* __restrict__ list,
   const unsigned long long m = *count;
   for (unsigned long long i = blockIdx.x * static_cast<unsigned long long>(blockDim.x) + threadIdx.x;
        i < m; i += static_cast<unsigned long long>(gridDim.x) * blockDim.x) {
-    const unsigned long long idx = list[i];
-    unsigned* word = reinterpret_cast<unsigned*>(vol + (idx & ~1ull));
-    atomicAnd(word, ~(static_cast<unsigned>(kUpdateMarker) << (16 * (idx & 1))));
+    ClearUpdateMarker(vol, list[i]);
   }
 }
 
@@ -167,28 +150,6 @@ __global__ void k_ins3_scatter_made(const int* __restrict__ idx, const float* __
 using namespace csm;
 
 namespace {
-
-// ---- probability_values.{h,cc} in float, as the reference evaluates them ----
-constexpr float kMinProbability = 0.1f;
-constexpr float kMaxProbability = 1.f - kMinProbability;
-
-float Odds(float p) { return p / (1.f - p); }
-float ProbabilityFromOdds(float odds) { return odds / (odds + 1.f); }
-uint16_t ProbabilityToValue(float p) {   // BoundedFloatToValue (probability_values.h:32-44)
-  const float c = p > kMaxProbability ? kMaxProbability : (p < kMinProbability ? kMinProbability : p);
-  return static_cast<uint16_t>(
-      std::lround((c - kMinProbability) * (32766.f / (kMaxProbability - kMinProbability))) + 1);
-}
-// ComputeLookupTableToApplyOdds (probability_values.cc:76-87) over kValueToProbability
-// (SlowValueToBoundedFloat, :29-37)
-void OddsTable(float odds, uint16_t* table) {
-  const float kScale = (kMaxProbability - kMinProbability) / (kValueCount - 2.f);
-  table[0] = ProbabilityToValue(ProbabilityFromOdds(odds)) + kUpdateMarker;
-  for (int cell = 1; cell != kValueCount; ++cell) {
-    const float p = cell * kScale + (kMinProbability - kScale);
-    table[cell] = ProbabilityToValue(ProbabilityFromOdds(odds * Odds(p))) + kUpdateMarker;
-  }
-}
 
 // HybridGridBase::GetCellIndex (hybrid_grid.h:428-433); false outside the 2^14 cube
 // (hybrid_grid.h:387) or for a non-finite point.
@@ -272,8 +233,9 @@ csm_status csm_range_inserter3d_create(const csm_range_inserter_options3d* optio
   ins->options = *options;
   // Odds(options_.hit_probability()): the double option enters Odds(float)
   std::vector<uint16_t> tables(2 * kValueCount);
-  OddsTable(Odds(static_cast<float>(options->hit_probability)), tables.data());
-  OddsTable(Odds(static_cast<float>(options->miss_probability)), tables.data() + kValueCount);
+  ComputeLookupTableToApplyOdds(Odds(static_cast<float>(options->hit_probability)), tables.data());
+  ComputeLookupTableToApplyOdds(Odds(static_cast<float>(options->miss_probability)),
+                                tables.data() + kValueCount);
   CSM_CUDA(cudaMalloc(&ins->d_tables, tables.size() * sizeof(uint16_t)));
   CSM_CUDA(cudaMemcpy(ins->d_tables, tables.data(), tables.size() * sizeof(uint16_t),
                       cudaMemcpyHostToDevice));

@@ -36,7 +36,6 @@ struct csm_tsdf_inserter2d {
 
 namespace csm {
 
-constexpr uint16_t kTsdfUpdateMarker = 1u << 15;   // tsd_value_converter.h:95
 constexpr int kErrMaskOutside = 1, kErrMarked = 2;
 
 // One ray of the insert, in the sorted order.
@@ -125,7 +124,7 @@ __global__ void k_tsdf2_pairs(const TsdfRay2* __restrict__ rays, const int* __re
     t = t > P.truncation ? P.truncation : (t < -P.truncation ? -P.truncation : t);   // Clamp
     float w = R.weight;
     if (P.sigma != 0.f) w = w * TsdfGaussian(t, P.sigma, P.sqrt_two_pi);
-    if (tsd_cells[flat] & kTsdfUpdateMarker) atomicOr(err, kErrMarked);
+    if (tsd_cells[flat] & kUpdateMarker) atomicOr(err, kErrMarked);
     if (w != 0.f) key = static_cast<unsigned>(flat);   // UpdateCell's early return claims nothing
     update_tsd[i] = t;
     update_weight[i] = w;
@@ -296,44 +295,6 @@ csm_status csm_tsdf_inserter2d_destroy(csm_tsdf_inserter2d* inserter) {
   return CSM_OK;
 }
 
-csm_status csm_rt_grid2d_create_empty_tsdf(double resolution, double max_x, double max_y,
-                                           int32_t num_x_cells, int32_t num_y_cells,
-                                           float truncation_distance, float max_weight,
-                                           int32_t device, csm_rt_grid2d** out) {
-  CSM_REQUIRE(out != nullptr, "null pointer");
-  CSM_REQUIRE(resolution > 0. && std::isfinite(resolution) && std::isfinite(max_x) &&
-                  std::isfinite(max_y), "limits");
-  CSM_REQUIRE(num_x_cells >= 1 && num_y_cells >= 1, "sizes");
-  CSM_REQUIRE(num_x_cells < kMaxCells && num_y_cells < kMaxCells, "grid too large");
-  CSM_REQUIRE(truncation_distance > 0.f && max_weight > 0.f && std::isfinite(truncation_distance) &&
-                  std::isfinite(max_weight), "TSDF parameters");
-  Ctx* ctx;
-  CSM_TRY(GetCtx(device, &ctx));
-  std::lock_guard<std::mutex> lock(ctx->mu);
-  CSM_CUDA(cudaSetDevice(device));
-  std::unique_ptr<csm_rt_grid2d> g;
-  CSM_TRY(NewGrid(ctx, num_x_cells, num_y_cells, resolution, max_x, max_y, &g,
-                  truncation_distance, max_weight));
-  CSM_CUDA(cudaStreamSynchronize(ctx->stream));
-  *out = g.release();
-  return CSM_OK;
-}
-
-csm_status csm_rt_grid2d_read_weights(const csm_rt_grid2d* grid, uint16_t* weight_cells,
-                                      int64_t capacity) {
-  CSM_REQUIRE(grid != nullptr && weight_cells != nullptr, "null pointer");
-  CSM_REQUIRE(grid->d_wcells != nullptr, "the grid is not a TSDF2D");
-  std::lock_guard<std::mutex> lock(grid->ctx->mu);
-  const RtGridDev& d = grid->g;
-  CSM_REQUIRE(capacity >= static_cast<int64_t>(d.nx) * d.ny, "capacity");
-  CSM_CUDA(cudaSetDevice(grid->ctx->device));
-  CSM_CUDA(cudaMemcpy2DAsync(weight_cells, static_cast<size_t>(d.nx) * 2, grid->d_wcells,
-                             static_cast<size_t>(d.pitch) * 2, static_cast<size_t>(d.nx) * 2,
-                             d.ny, cudaMemcpyDeviceToHost, grid->ctx->stream));
-  CSM_CUDA(cudaStreamSynchronize(grid->ctx->stream));
-  return CSM_OK;
-}
-
 csm_status csm_tsdf_inserter2d_insert(const csm_tsdf_inserter2d* inserter, const float origin[3],
                                       const float* returns, int32_t num_returns,
                                       csm_rt_grid2d* grid, csm_stats* stats) {
@@ -367,13 +328,9 @@ csm_status csm_tsdf_inserter2d_insert(const csm_tsdf_inserter2d* inserter, const
     hi_x = std::max(hi_x, ex);
     hi_y = std::max(hi_y, ey);
   }
-  constexpr float kPadding = 1e-6f;
-  Limits2 L{grid->g.resolution, grid->g.max_x, grid->g.max_y, grid->g.nx, grid->g.ny};
-  int grow_x = 0, grow_y = 0;
-  CSM_REQUIRE(GrowLimits(lo_x - kPadding, lo_y - kPadding, &L, &grow_x, &grow_y) &&
-                  GrowLimits(hi_x + kPadding, hi_y + kPadding, &L, &grow_x, &grow_y),
-              "the grid would grow past 30000 cells");
-  const bool grow = L.nx != grid->g.nx;
+  GridInsert2 tx(grid);
+  CSM_REQUIRE(tx.Grow(lo_x, lo_y, hi_x, hi_y), "the grid would grow past 30000 cells");
+  const Limits2& L = tx.L;
 
   // ---- sort and normals (:139-152) ----
   const bool angle_weight = opt.update_weight_angle_scan_normal_to_ray_kernel_bandwidth != 0.f;
@@ -458,33 +415,17 @@ csm_status csm_tsdf_inserter2d_insert(const csm_tsdf_inserter2d* inserter, const
   P.project = project ? 1 : 0;
   P.nx = L.nx;
   P.ny = L.ny;
-  P.pitch = grow ? (L.nx + 7) / 8 * 8 : grid->g.pitch;
+  P.pitch = tx.arrays.pitch;
   P.no_claim = static_cast<unsigned>(P.pitch) * static_cast<unsigned>(L.ny);
   P.conv = MakeTsdfConversion(grid->truncation, grid->max_weight);
   P.max_tsd = grid->truncation;   // TSDValueConverter(max_tsd, max_weight)
-  P.tsd_resolution = 32766.f / (grid->truncation - (-grid->truncation));
+  P.tsd_resolution = ValueResolution(-grid->truncation, grid->truncation);
   P.max_w = grid->max_weight;
-  P.weight_resolution = 32766.f / (grid->max_weight - 0.f);
+  P.weight_resolution = ValueResolution(0.f, grid->max_weight);
 
-  CSM_CUDA(cudaSetDevice(ctx->device));
+  CSM_TRY(tx.Begin());
   cudaStream_t s = ctx->stream;
-  CSM_CUDA(cudaEventRecord(ctx->ev0, s));
-  // ---- the known box of a handle made from cells, before its cells move ----
-  const bool box_stale = grid->known_stale;
-  DevBuf& d_box = ctx->D("ins2_box");
-  if (box_stale) {
-    CSM_TRY(d_box.Reserve(4 * sizeof(int)));
-    CSM_TRY(LaunchKnownBox(grid, d_box.as<int>()));
-  }
-  // ---- growth into new arrays, installed only if the insert is not refused ----
-  CellArrays2 work{grid->d_cells, grid->d_wcells, grid->g.pitch};
-  if (grow) CSM_TRY(GrowCellArrays2(grid, L, grow_x, grow_y, s, &work));
-  auto drop_grown = [&]() {
-    if (!grow) return;
-    cudaStreamSynchronize(s);
-    cudaFree(work.cells);
-    cudaFree(work.wcells);
-  };
+  const CellArrays2& work = tx.arrays;
 
   // ---- upload: flags + box | ray records | slot offsets; workspace for slots and pairs ----
   auto align = [](size_t b) { return (b + 255) / 256 * 256; };
@@ -505,24 +446,16 @@ csm_status csm_tsdf_inserter2d_insert(const csm_tsdf_inserter2d* inserter, const
   while (end_bit < 32 && (P.no_claim >> end_bit) != 0) ++end_bit;
   size_t temp_bytes = 0;
   if (num_slots > 0) {
-    const cudaError_t e = cub::DeviceRadixSort::SortPairs(
+    CSM_CUDA(cub::DeviceRadixSort::SortPairs(
         nullptr, temp_bytes, static_cast<unsigned*>(nullptr), static_cast<unsigned*>(nullptr),
-        static_cast<int*>(nullptr), static_cast<int*>(nullptr), num_slots, 0, end_bit, s);
-    if (e != cudaSuccess) {
-      drop_grown();
-      CSM_CUDA(e);
-    }
+        static_cast<int*>(nullptr), static_cast<int*>(nullptr), num_slots, 0, end_bit, s));
   }
   PinnedBuf& up = ctx->P("tsdf2_upload");
   PinnedBuf& h_back = ctx->P("tsdf2_back");
   DevBuf& d_work = ctx->D("tsdf2_work");
-  csm_status st = up.Reserve(up_bytes);
-  if (st == CSM_OK) st = h_back.Reserve(9 * sizeof(int));
-  if (st == CSM_OK) st = d_work.Reserve(o_temp + temp_bytes);
-  if (st != CSM_OK) {
-    drop_grown();
-    return st;
-  }
+  CSM_TRY(up.Reserve(up_bytes));
+  CSM_TRY(h_back.Reserve(5 * sizeof(int)));
+  CSM_TRY(d_work.Reserve(o_temp + temp_bytes));
   char* h = up.as<char>();
   const int init[5] = {0, INT_MAX, INT_MAX, INT_MIN, INT_MIN};
   std::memcpy(h, init, sizeof(init));
@@ -530,77 +463,43 @@ csm_status csm_tsdf_inserter2d_insert(const csm_tsdf_inserter2d* inserter, const
   std::memcpy(h + o_off, off.data(), sizeof(int) * (num_rays + 1));
   char* d = d_work.as<char>();
   int* d_flags = reinterpret_cast<int*>(d);
-  auto launch = [&]() -> csm_status {
-    CSM_CUDA(cudaMemcpyAsync(d, h, up_bytes, cudaMemcpyHostToDevice, s));
-    if (num_rays > 0) {
-      const TsdfRay2* d_rays = reinterpret_cast<const TsdfRay2*>(d + o_rays);
-      int* d_slots = reinterpret_cast<int*>(d + o_slots);
-      int* d_slot_ray = reinterpret_cast<int*>(d + o_slot_ray);
-      unsigned* d_keys = reinterpret_cast<unsigned*>(d + o_keys);
-      unsigned* d_keys_out = reinterpret_cast<unsigned*>(d + o_keys_out);
-      int* d_vals = reinterpret_cast<int*>(d + o_vals);
-      int* d_vals_out = reinterpret_cast<int*>(d + o_vals_out);
-      float* d_utsd = reinterpret_cast<float*>(d + o_utsd);
-      float* d_uw = reinterpret_cast<float*>(d + o_uw);
-      k_tsdf2_rays<<<Blocks(num_rays, 1LL << 30), 256, 0, s>>>(
-          d_rays, reinterpret_cast<const int*>(d + o_off), num_rays, L.nx, L.ny, P.pitch, d_slots,
-          d_slot_ray, d_flags);
-      CSM_LAUNCH_CHECK();
-      k_tsdf2_pairs<<<Blocks(num_slots, 1LL << 30), 256, 0, s>>>(
-          d_rays, d_slots, d_slot_ray, num_slots, P, work.cells, d_keys, d_vals, d_utsd, d_uw,
-          d_flags);
-      CSM_LAUNCH_CHECK();
-      CSM_CUDA(cub::DeviceRadixSort::SortPairs(d + o_temp, temp_bytes, d_keys, d_keys_out, d_vals,
-                                               d_vals_out, num_slots, 0, end_bit, s));
-      g_launches.fetch_add(1, std::memory_order_relaxed);
-      k_tsdf2_apply<<<Blocks(num_slots, 1LL << 30), 256, 0, s>>>(
-          d_keys_out, d_vals_out, num_slots, d_utsd, d_uw, P, work.cells, work.wcells, d_flags);
-      CSM_LAUNCH_CHECK();
-    }
-    int* hb = h_back.as<int>();
-    CSM_CUDA(cudaMemcpyAsync(hb, d_flags, 5 * sizeof(int), cudaMemcpyDeviceToHost, s));
-    if (box_stale)
-      CSM_CUDA(cudaMemcpyAsync(hb + 5, d_box.p, 4 * sizeof(int), cudaMemcpyDeviceToHost, s));
-    CSM_CUDA(cudaEventRecord(ctx->ev1, s));
-    CSM_CUDA(cudaStreamSynchronize(s));
-    return CSM_OK;
-  };
-  st = launch();
-  if (st != CSM_OK) {
-    drop_grown();
-    return st;
+  CSM_CUDA(cudaMemcpyAsync(d, h, up_bytes, cudaMemcpyHostToDevice, s));
+  if (num_rays > 0) {
+    const TsdfRay2* d_rays = reinterpret_cast<const TsdfRay2*>(d + o_rays);
+    int* d_slots = reinterpret_cast<int*>(d + o_slots);
+    int* d_slot_ray = reinterpret_cast<int*>(d + o_slot_ray);
+    unsigned* d_keys = reinterpret_cast<unsigned*>(d + o_keys);
+    unsigned* d_keys_out = reinterpret_cast<unsigned*>(d + o_keys_out);
+    int* d_vals = reinterpret_cast<int*>(d + o_vals);
+    int* d_vals_out = reinterpret_cast<int*>(d + o_vals_out);
+    float* d_utsd = reinterpret_cast<float*>(d + o_utsd);
+    float* d_uw = reinterpret_cast<float*>(d + o_uw);
+    k_tsdf2_rays<<<Blocks(num_rays, 1LL << 30), 256, 0, s>>>(
+        d_rays, reinterpret_cast<const int*>(d + o_off), num_rays, L.nx, L.ny, P.pitch, d_slots,
+        d_slot_ray, d_flags);
+    CSM_LAUNCH_CHECK();
+    k_tsdf2_pairs<<<Blocks(num_slots, 1LL << 30), 256, 0, s>>>(
+        d_rays, d_slots, d_slot_ray, num_slots, P, work.cells, d_keys, d_vals, d_utsd, d_uw,
+        d_flags);
+    CSM_LAUNCH_CHECK();
+    CSM_CUDA(cub::DeviceRadixSort::SortPairs(d + o_temp, temp_bytes, d_keys, d_keys_out, d_vals,
+                                             d_vals_out, num_slots, 0, end_bit, s));
+    g_launches.fetch_add(1, std::memory_order_relaxed);
+    k_tsdf2_apply<<<Blocks(num_slots, 1LL << 30), 256, 0, s>>>(
+        d_keys_out, d_vals_out, num_slots, d_utsd, d_uw, P, work.cells, work.wcells, d_flags);
+    CSM_LAUNCH_CHECK();
   }
+  CSM_CUDA(cudaMemcpyAsync(h_back.p, d_flags, 5 * sizeof(int), cudaMemcpyDeviceToHost, s));
+  CSM_CUDA(cudaEventRecord(ctx->ev1, s));
+  CSM_CUDA(cudaStreamSynchronize(s));
   const int* hb = h_back.as<int>();
   if (hb[0] != 0) {
-    drop_grown();
     SetError("%s:%d: invalid argument: %s", __FILE__, __LINE__,
              (hb[0] & kErrMarked) ? "a tsd cell on a ray carries the update marker"
                                   : "a ray mask leaves the grown grid");
     return CSM_E_INVALID;
   }
-  if (grow) {
-    st = InstallCellArrays2(grid, L, &work);   // work now holds the old arrays
-    cudaFree(work.cells);
-    cudaFree(work.wcells);
-    if (st != CSM_OK) return st;
-  }
-  // ---- the known-cells box: the old one moved by the growth, plus what this insert set ----
-  KnownBox2 known = box_stale ? BoxFrom(hb + 5) : grid->known;
-  if (!known.empty()) {
-    known.lo[0] += grow_x;
-    known.hi[0] += grow_x;
-    known.lo[1] += grow_y;
-    known.hi[1] += grow_y;
-  }
-  known.Extend(BoxFrom(hb + 1));
-  grid->known = known;
-  grid->known_stale = false;
-  if (stats) {
-    std::memset(stats, 0, sizeof(*stats));
-    stats->host_syncs = 1;
-    cudaEventElapsedTime(&stats->device_ms, ctx->ev0, ctx->ev1);
-  }
-  return CSM_OK;
+  return tx.Commit(BoxFrom(hb + 1), stats);
 }
 
 }  // extern "C"

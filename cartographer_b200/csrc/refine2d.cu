@@ -519,14 +519,10 @@ csm_status FillOpts(const csm_ceres_options2d* o, RefOpts* P) {
   P->rotation_weight = o->rotation_weight;
   P->use_nonmonotonic_steps = o->use_nonmonotonic_steps != 0;
   P->max_num_iterations = o->max_num_iterations;
-  // probability_values.h:64-67 and value_conversion_tables.cc:29-37 evaluated in float
-  const float kMinProbability = 0.1f;
-  const float kMaxProbability = 1.f - kMinProbability;
-  const float kMinCost = 1.f - kMaxProbability;
-  const float kMaxCost = 1.f - kMinProbability;
-  P->k_scale = (kMaxCost - kMinCost) / 32766.f;
-  P->cost_bias = kMinCost - P->k_scale;
-  P->max_cost = kMaxCost;
+  const ValueConversion cost = MakeValueConversion(kMinCorrespondenceCost, kMaxCorrespondenceCost);
+  P->k_scale = cost.scale;
+  P->cost_bias = cost.bias;
+  P->max_cost = kMaxCorrespondenceCost;
   return CSM_OK;
 }
 

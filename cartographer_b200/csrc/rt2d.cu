@@ -42,7 +42,6 @@ constexpr int kRtWarps = kRtThreads / 32;
 // has 25), 4 for larger ones — a template parameter, so the common case carries no
 // predicated-off accumulator code (executing all four costs several times the instructions
 // per warp and point)
-constexpr int kRtTileBytes = 100 * 1024;     // staged box (2 CTAs in an H100 SM's 228 KB)
 
 struct RtParams {
   int lin, width, per_scan, npair;
@@ -331,37 +330,16 @@ inline HV3 HRotate(float qw, const HV3& qv, const HV3& v) {
   return r;
 }
 
-typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*,
-                                  const cuuint64_t*, const cuuint64_t*, const cuuint32_t*,
-                                  const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
-                                  CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-
-EncodeTiledFn GetEncodeTiled() {
-  static EncodeTiledFn fn = []() -> EncodeTiledFn {
-    void* p = nullptr;
-    cudaDriverEntryPointQueryResult q;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &q) != cudaSuccess ||
-        q != cudaDriverEntryPointSuccess)
-      return nullptr;
-    return reinterpret_cast<EncodeTiledFn>(p);
-  }();
-  return fn;
-}
-
 void FillParams(RtParams* P, int lin, float truncation, float max_weight) {
   std::memset(P, 0, sizeof(*P));
   P->lin = lin;
   P->width = 2 * lin + 1;
   P->per_scan = P->width * P->width;
   P->npair = (lin + 1) * (lin + 2) / 2;
-  // probability_values.h:64-67 and .cc:29-37 evaluated in float
-  const float kMinProbability = 0.1f;
-  const float kMaxProbability = 1.f - kMinProbability;
-  const float kMinCost = 1.f - kMaxProbability;
-  const float kMaxCost = 1.f - kMinProbability;
-  P->k_scale = (kMaxCost - kMinCost) / 32766.f;
-  P->cost_bias = kMinCost - P->k_scale;
-  P->max_cost = kMaxCost;
+  const ValueConversion cost = MakeValueConversion(kMinCorrespondenceCost, kMaxCorrespondenceCost);
+  P->k_scale = cost.scale;
+  P->cost_bias = cost.bias;
+  P->max_cost = kMaxCorrespondenceCost;
   P->min_probability = kMinProbability;
   if (truncation > 0.f) {
     const TsdfConversion c = MakeTsdfConversion(truncation, max_weight);
@@ -372,56 +350,6 @@ void FillParams(RtParams* P, int lin, float truncation, float max_weight) {
     P->w_bias = c.w_bias;
     P->truncation = truncation;
   }
-}
-
-// Uploads `cells` (host pitch nx) into the handle's padded device array.
-csm_status UploadCells(csm_rt_grid2d* g, const uint16_t* cells, const uint16_t* wcells,
-                       cudaStream_t s) {
-  CSM_CUDA(cudaMemcpy2DAsync(g->d_cells, static_cast<size_t>(g->g.pitch) * 2, cells,
-                             static_cast<size_t>(g->g.nx) * 2, static_cast<size_t>(g->g.nx) * 2,
-                             g->g.ny, cudaMemcpyHostToDevice, s));
-  if (wcells)
-    CSM_CUDA(cudaMemcpy2DAsync(g->d_wcells, static_cast<size_t>(g->g.pitch) * 2, wcells,
-                               static_cast<size_t>(g->g.nx) * 2, static_cast<size_t>(g->g.nx) * 2,
-                               g->g.ny, cudaMemcpyHostToDevice, s));
-  return CSM_OK;
-}
-
-csm_status GridCreate(const uint16_t* cells, const uint16_t* wcells, float truncation,
-                      float max_weight, int32_t nx, int32_t ny, double resolution, double max_x,
-                      double max_y, int32_t device, csm_rt_grid2d** out) {
-  CSM_REQUIRE(out != nullptr && cells != nullptr, "null pointer");
-  CSM_REQUIRE(nx >= 1 && ny >= 1 && resolution > 0., "sizes");
-  CSM_REQUIRE(nx < 30000 && ny < 30000, "grid too large");
-  Ctx* ctx;
-  CSM_TRY(GetCtx(device, &ctx));
-  std::lock_guard<std::mutex> lock(ctx->mu);
-  CSM_CUDA(cudaSetDevice(device));
-  std::unique_ptr<csm_rt_grid2d> g(new csm_rt_grid2d);
-  g->ctx = ctx;
-  g->truncation = truncation;
-  g->max_weight = max_weight;
-  RtGridDev& d = g->g;
-  d.nx = nx;
-  d.ny = ny;
-  d.pitch = (nx + 7) / 8 * 8;  // rows are multiples of 16 bytes (TMA global strides)
-  d.resolution = resolution;
-  d.max_x = max_x;
-  d.max_y = max_y;
-  const size_t bytes = static_cast<size_t>(d.pitch) * ny * 2;
-  CSM_CUDA(cudaMalloc(&g->d_cells, bytes));
-  CSM_CUDA(cudaMemsetAsync(g->d_cells, 0, bytes, ctx->stream));
-  if (wcells) {
-    CSM_CUDA(cudaMalloc(&g->d_wcells, bytes));
-    CSM_CUDA(cudaMemsetAsync(g->d_wcells, 0, bytes, ctx->stream));
-  }
-  d.cells = g->d_cells;
-  d.wcells = g->d_wcells;
-  CSM_TRY(UploadCells(g.get(), cells, wcells, ctx->stream));
-  CSM_TRY(RtGridEncodeTmap(g.get()));
-  CSM_CUDA(cudaStreamSynchronize(ctx->stream));
-  *out = g.release();
-  return CSM_OK;
 }
 
 struct RtHostJob {
@@ -715,7 +643,7 @@ csm_status RtMatchHostGrid(const uint16_t* cells, const uint16_t* weight_cells, 
         slot.reset();
       }
       csm_rt_grid2d* fresh = nullptr;
-      CSM_TRY(GridCreate(cells, weight_cells, truncation, max_weight, nx, ny, resolution, max_x,
+      CSM_TRY(RtGridCreate(cells, weight_cells, truncation, max_weight, nx, ny, resolution, max_x,
                          max_y, device, &fresh));
       slot.reset(fresh);
     }
@@ -733,87 +661,7 @@ csm_status RtMatchHostGrid(const uint16_t* cells, const uint16_t* weight_cells, 
 
 }  // namespace
 
-namespace csm {
-
-csm_status RtGridEncodeTmap(csm_rt_grid2d* g) {
-  RtGridDev& d = g->g;
-  // TMA box: as wide as the (padded) grid up to 256 cells, as many rows as fit the tile
-  d.bw = std::min(d.pitch, 256);
-  d.bh = std::max(1, std::min(std::min(d.ny, 256), kRtTileBytes / (d.bw * 2)));
-  g->has_tmap = false;
-  if (g->d_wcells) {
-    std::memset(&g->tmap, 0, sizeof(g->tmap));
-    return CSM_OK;
-  }
-  EncodeTiledFn encode = GetEncodeTiled();
-  if (encode) {
-    const cuuint64_t dims[2] = {static_cast<cuuint64_t>(d.nx), static_cast<cuuint64_t>(d.ny)};
-    const cuuint64_t strides[1] = {static_cast<cuuint64_t>(d.pitch) * 2};
-    const cuuint32_t box[2] = {static_cast<cuuint32_t>(d.bw), static_cast<cuuint32_t>(d.bh)};
-    const cuuint32_t estr[2] = {1, 1};
-    const CUresult r = encode(&g->tmap, CU_TENSOR_MAP_DATA_TYPE_UINT16, 2, g->d_cells, dims,
-                              strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                              CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-                              CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    g->has_tmap = r == CUDA_SUCCESS;
-  }
-  if (!g->has_tmap) {
-    SetError("cuTensorMapEncodeTiled is unavailable or failed");
-    return CSM_E_CUDA;
-  }
-  return CSM_OK;
-}
-
-}  // namespace csm
-
 extern "C" {
-
-csm_status csm_rt_grid2d_create(const uint16_t* cells, int32_t nx, int32_t ny, double resolution,
-                                double max_x, double max_y, int32_t device, csm_rt_grid2d** out) {
-  return GridCreate(cells, nullptr, 0.f, 0.f, nx, ny, resolution, max_x, max_y, device, out);
-}
-
-csm_status csm_rt_grid2d_update(csm_rt_grid2d* grid, const uint16_t* cells) {
-  CSM_REQUIRE(grid && cells, "null pointer");
-  // the weight cells would go stale
-  CSM_REQUIRE(grid->d_wcells == nullptr, "a TSDF2D handle is updated by csm_rt_grid2d_update_tsdf");
-  std::lock_guard<std::mutex> lock(grid->ctx->mu);
-  CSM_CUDA(cudaSetDevice(grid->ctx->device));
-  CSM_TRY(UploadCells(grid, cells, nullptr, grid->ctx->stream));
-  grid->known_stale = true;
-  CSM_CUDA(cudaStreamSynchronize(grid->ctx->stream));
-  return CSM_OK;
-}
-
-csm_status csm_rt_grid2d_create_tsdf(const uint16_t* tsd_cells, const uint16_t* weight_cells,
-                                     int32_t nx, int32_t ny, double resolution, double max_x,
-                                     double max_y, float truncation_distance, float max_weight,
-                                     int32_t device, csm_rt_grid2d** out) {
-  CSM_REQUIRE(weight_cells != nullptr, "null weight cells");
-  CSM_REQUIRE(truncation_distance > 0.f && max_weight > 0.f, "TSDF parameters");
-  return GridCreate(tsd_cells, weight_cells, truncation_distance, max_weight, nx, ny, resolution,
-                    max_x, max_y, device, out);
-}
-
-csm_status csm_rt_grid2d_update_tsdf(csm_rt_grid2d* grid, const uint16_t* tsd_cells,
-                                     const uint16_t* weight_cells) {
-  CSM_REQUIRE(grid && tsd_cells && weight_cells, "null pointer");
-  CSM_REQUIRE(grid->d_wcells != nullptr, "the grid is not a TSDF2D");
-  std::lock_guard<std::mutex> lock(grid->ctx->mu);
-  CSM_CUDA(cudaSetDevice(grid->ctx->device));
-  CSM_TRY(UploadCells(grid, tsd_cells, weight_cells, grid->ctx->stream));
-  CSM_CUDA(cudaStreamSynchronize(grid->ctx->stream));
-  return CSM_OK;
-}
-
-csm_status csm_rt_grid2d_destroy(csm_rt_grid2d* grid) {
-  if (!grid) return CSM_OK;
-  std::lock_guard<std::mutex> lock(grid->ctx->mu);
-  cudaSetDevice(grid->ctx->device);
-  cudaStreamSynchronize(grid->ctx->stream);
-  delete grid;
-  return CSM_OK;
-}
 
 csm_status csm_rt_match2d_batch(const csm_rt_grid2d* grid, const csm_rt_job2d* jobs,
                                 int32_t num_jobs, double linear_window, double angular_window,
@@ -876,7 +724,7 @@ csm_status csm_rt_score_candidates2d(const uint16_t* cells, int32_t nx, int32_t 
   CSM_REQUIRE(num_scans >= 1 && n >= 1 && num_candidates >= 0, "sizes");
   if (num_candidates == 0) return CSM_OK;
   csm_rt_grid2d* grid = nullptr;
-  CSM_TRY(GridCreate(cells, nullptr, 0.f, 0.f, nx, ny, resolution, max_x, max_y, device, &grid));
+  CSM_TRY(RtGridCreate(cells, nullptr, 0.f, 0.f, nx, ny, resolution, max_x, max_y, device, &grid));
   std::unique_ptr<csm_rt_grid2d> owner(grid);
   LaneGuard guard;
   CSM_TRY(AcquireLane(device, &guard));

@@ -21,6 +21,7 @@
 
 #include "common.cuh"
 #include "grid3d.cuh"
+#include "value_conversion.h"
 
 namespace csm {
 
@@ -199,10 +200,10 @@ csm_status csm_grid3d_create(const int32_t* idx, const uint16_t* values, int64_t
   d.p = g->d_vol;
   d.resolution = resolution;
   {
-    const float kMin = 0.1f, kMax = 1.f - kMin;
-    d.k_scale = (kMax - kMin) / 32766.f;
-    d.bias = kMin - d.k_scale;
-    d.min_probability = kMin;
+    const ValueConversion probability = MakeValueConversion(kMinProbability, kMaxProbability);
+    d.k_scale = probability.scale;
+    d.bias = probability.bias;
+    d.min_probability = kMinProbability;
   }
   if (n > 0) {
     DevBuf& d_idx = ctx->D("g3_idx");

@@ -49,6 +49,7 @@ using std::isfinite;
 }  // namespace
 
 #include "../../cartographer_b200/csrc/refine2d.cu"
+#include "../../cartographer_b200/csrc/value_conversion.h"
 
 extern "C" {
 
@@ -78,13 +79,11 @@ void emu_ceres_match2d(const uint16_t* cells, int nx, int ny, double resolution,
   P.rotation_weight = opts[2];
   P.use_nonmonotonic_steps = opts[3] != 0.;
   P.max_num_iterations = static_cast<int>(opts[4]);
-  const float kMinProbability = 0.1f;
-  const float kMaxProbability = 1.f - kMinProbability;
-  const float kMinCost = 1.f - kMaxProbability;
-  const float kMaxCost = 1.f - kMinProbability;
-  P.k_scale = (kMaxCost - kMinCost) / 32766.f;
-  P.cost_bias = kMinCost - P.k_scale;
-  P.max_cost = kMaxCost;
+  const csm::ValueConversion cost =
+      csm::MakeValueConversion(csm::kMinCorrespondenceCost, csm::kMaxCorrespondenceCost);
+  P.k_scale = cost.scale;
+  P.cost_bias = cost.bias;
+  P.max_cost = csm::kMaxCorrespondenceCost;
   csm::RefResultDev result;
   std::memset(&result, 0, sizeof(result));
   pthread_barrier_init(&g_block_barrier, nullptr, kEmuThreads);

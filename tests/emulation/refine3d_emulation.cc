@@ -46,6 +46,7 @@ using std::isfinite;
 }  // namespace
 
 #include "../../cartographer_b200/csrc/refine3d.cu"
+#include "../../cartographer_b200/csrc/value_conversion.h"
 
 namespace {
 void FillEmuJob(int num_clouds, const uint16_t* const* vol, const int32_t* lo, const int32_t* n,
@@ -62,11 +63,12 @@ void FillEmuJob(int num_clouds, const uint16_t* const* vol, const int32_t* lo, c
       c.n[a] = n[3 * b + a];
     }
     c.resolution = resolution[b];
-    // probability_values.h / value_conversion_tables.cc:29-37 in float, as rt3d.cu fills them
-    const float kMinProbability = 0.1f, kMaxProbability = 1.f - kMinProbability;
-    c.k_scale = (kMaxProbability - kMinProbability) / 32766.f;
-    c.bias = kMinProbability - c.k_scale;
-    c.min_probability = kMinProbability;
+    // as rt3d.cu fills them
+    const csm::ValueConversion probability =
+        csm::MakeValueConversion(csm::kMinProbability, csm::kMaxProbability);
+    c.k_scale = probability.scale;
+    c.bias = probability.bias;
+    c.min_probability = csm::kMinProbability;
     c.npts = npts[b];
     c.xyz_off = static_cast<long long>(cloud->size());
     cloud->insert(cloud->end(), xyz[b], xyz[b] + 3 * static_cast<size_t>(npts[b]));

@@ -19,7 +19,8 @@ SO = os.path.join(HERE, "_build", "librefine3d_emulation.so")
 def emu():
     src = os.path.join(HERE, "refine3d_emulation.cc")
     csrc = os.path.join(HERE, "..", "..", "cartographer_b200", "csrc")
-    deps = [src] + [os.path.join(csrc, f) for f in ("refine3d.cu", "trust_region.cuh")]
+    deps = [src] + [os.path.join(csrc, f) for f in ("refine3d.cu", "trust_region.cuh",
+                                                       "value_conversion.h")]
     if not os.path.exists(SO) or os.path.getmtime(SO) < max(map(os.path.getmtime, deps)):
         os.makedirs(os.path.dirname(SO), exist_ok=True)
         subprocess.check_call(["g++", "-std=c++17", "-O2", "-ffp-contract=off", "-fPIC", "-shared",

@@ -143,7 +143,8 @@ def test_match_recovers_a_perturbed_pose(nonmonotonic):
 def emu():
     src = os.path.join(HERE, "refine2d_tsdf_emulation.cc")
     csrc = os.path.join(HERE, "..", "..", "cartographer_b200", "csrc")
-    deps = [src] + [os.path.join(csrc, f) for f in ("refine2d.cu", "trust_region.cuh")]
+    deps = [src] + [os.path.join(csrc, f) for f in ("refine2d.cu", "trust_region.cuh",
+                                                       "tsdf_conversion.h", "value_conversion.h")]
     if not os.path.exists(SO) or os.path.getmtime(SO) < max(map(os.path.getmtime, deps)):
         os.makedirs(os.path.dirname(SO), exist_ok=True)
         subprocess.check_call(["g++", "-std=c++17", "-O2", "-ffp-contract=off", "-fPIC", "-shared",
