@@ -50,18 +50,26 @@ extern std::atomic<int64_t> g_launches;
 
 inline int DivUp(long long a, long long b) { return static_cast<int>((a + b - 1) / b); }
 
-// Host side of the engines' order-preserving float <-> unsigned map (bounds are kept as
-// unsigned so that atomicMax on them orders like the float scores).
-inline unsigned HostFloatToOrdered(float f) {
+// The engines' order-preserving float <-> unsigned map (bounds are kept as unsigned so that
+// atomicMax on them orders like the float scores).
+__host__ __device__ __forceinline__ unsigned FloatToOrdered(float f) {
+#ifdef __CUDA_ARCH__
+  const unsigned u = __float_as_uint(f);
+#else
   unsigned u;
   std::memcpy(&u, &f, 4);
+#endif
   return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
 }
-inline float HostOrderedToFloat(unsigned u) {
+__host__ __device__ __forceinline__ float OrderedToFloat(unsigned u) {
   u = (u & 0x80000000u) ? (u & 0x7fffffffu) : ~u;
+#ifdef __CUDA_ARCH__
+  return __uint_as_float(u);
+#else
   float f;
   std::memcpy(&f, &u, 4);
   return f;
+#endif
 }
 
 #define CSM_LAUNCH_CHECK()                                                          \

@@ -23,14 +23,6 @@ namespace csm {
 // ---------------------------------------------------------------------------
 // Small device helpers
 // ---------------------------------------------------------------------------
-__device__ __forceinline__ unsigned FloatToOrdered(float f) {
-  unsigned u = __float_as_uint(f);
-  return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
-}
-__device__ __forceinline__ float OrderedToFloat(unsigned u) {
-  return __uint_as_float((u & 0x80000000u) ? (u & 0x7fffffffu) : ~u);
-}
-
 // PrecomputationGrid2D::ToScore(sum / float(N))   (fast...2d.h:74-76, .cc:328-329)
 __device__ __forceinline__ float ToScore(const StackDev& st, int sum, int n) {
   const float mean = __fdiv_rn(__int2float_rn(sum), __int2float_rn(n));
@@ -145,29 +137,6 @@ __global__ void k_stack_window(const uint8_t* __restrict__ lvl, int wx, int wy, 
 // ---------------------------------------------------------------------------
 // K2: GenerateRotatedScans + DiscretizeScans + ShrinkToFit
 // ---------------------------------------------------------------------------
-struct V3 { float x, y, z; };
-__device__ __forceinline__ V3 CrossRn(const V3& a, const V3& b) {
-  return V3{__fsub_rn(__fmul_rn(a.y, b.z), __fmul_rn(a.z, b.y)),
-            __fsub_rn(__fmul_rn(a.z, b.x), __fmul_rn(a.x, b.z)),
-            __fsub_rn(__fmul_rn(a.x, b.y), __fmul_rn(a.y, b.x))};
-}
-// Eigen QuaternionBase::_transformVector followed by "+ translation(0)"
-// (transform/rigid_transform.h:192-196, sensor/point_cloud.cc:56-64).
-__device__ __forceinline__ V3 RotateRn(float qw, const V3& qv, const V3& v) {
-  V3 uv = CrossRn(qv, v);
-  uv.x = __fadd_rn(uv.x, uv.x);
-  uv.y = __fadd_rn(uv.y, uv.y);
-  uv.z = __fadd_rn(uv.z, uv.z);
-  const V3 c = CrossRn(qv, uv);
-  V3 r{__fadd_rn(__fadd_rn(v.x, __fmul_rn(qw, uv.x)), c.x),
-       __fadd_rn(__fadd_rn(v.y, __fmul_rn(qw, uv.y)), c.y),
-       __fadd_rn(__fadd_rn(v.z, __fmul_rn(qw, uv.z)), c.z)};
-  r.x = __fadd_rn(r.x, 0.f);
-  r.y = __fadd_rn(r.y, 0.f);
-  r.z = __fadd_rn(r.z, 0.f);
-  return r;
-}
-
 // One CTA per (job, scan) of the scans from scan0 on.  Writes the scan's cell indices and
 // its LinearBounds after ShrinkToFit (correlative_scan_matcher_2d.cc:73-127), plus the
 // number of lowest-resolution candidates per axis (fast...2d.cc:281-292).
@@ -181,15 +150,13 @@ k_discretize(const JobDev* __restrict__ jobs, const int* __restrict__ scan_job,
   const StackDev& st = *jb.stack;
   const int k = sg - jb.scan_base;
   const float2 cs = jb.trig[k];
-  // Quaternionf(AngleAxisf(a, UnitZ)): w = cos(ha), vec = sin(ha) * (0, 0, 1)
-  const V3 qk{__fmul_rn(cs.y, 0.f), __fmul_rn(cs.y, 0.f), __fmul_rn(cs.y, 1.f)};
-  const V3 q0{jb.q0x, jb.q0y, jb.q0z};
+  const Quatf qk = QuatFromCosSinZ(cs.x, cs.y);
   short2* out = dscan + jb.dscan_off + static_cast<long long>(k) * jb.n;
   int min_ix = INT_MAX, max_ix = INT_MIN, min_iy = INT_MAX, max_iy = INT_MIN;
   for (int p = threadIdx.x; p < jb.n; p += blockDim.x) {
-    const V3 v{jb.xyz[3 * p], jb.xyz[3 * p + 1], jb.xyz[3 * p + 2]};
-    const V3 r0 = RotateRn(jb.q0w, q0, v);   // rotated_point_cloud   (fast...2d.cc:236-239)
-    const V3 r1 = RotateRn(cs.x, qk, r0);    // GenerateRotatedScans  (corr...2d.cc:93-109)
+    const Vec3f v{jb.xyz[3 * p], jb.xyz[3 * p + 1], jb.xyz[3 * p + 2]};
+    const Vec3f r0 = RotateAsRigid3f(jb.q0, v);  // rotated_point_cloud   (fast...2d.cc:236-239)
+    const Vec3f r1 = RotateAsRigid3f(qk, r0);    // GenerateRotatedScans  (corr...2d.cc:93-109)
     // Affine2f(Translation2f) * v = (1*x + 0*y) + t                    (corr...2d.cc:120-121)
     const float px = __fadd_rn(__fadd_rn(__fmul_rn(1.f, r1.x), __fmul_rn(0.f, r1.y)), jb.tx);
     const float py = __fadd_rn(__fadd_rn(__fmul_rn(0.f, r1.x), __fmul_rn(1.f, r1.y)), jb.ty);
@@ -262,14 +229,6 @@ k_discretize(const JobDev* __restrict__ jobs, const int* __restrict__ scan_job,
     atomicAdd(&counters[0], slots);  // every lowest-resolution candidate gets scored
     atomicAdd(&counters[3], slots);
   }
-}
-
-csm_status LaunchDiscretize2D(cudaStream_t stream, const JobDev* jobs, const int* scan_job,
-                              int total_scans, short2* dscan, ScanInfo* info, int shrink,
-                              unsigned long long* counters) {
-  k_discretize<<<total_scans, 128, 0, stream>>>(jobs, scan_job, dscan, info, shrink, counters, 0);
-  CSM_LAUNCH_CHECK();
-  return CSM_OK;
 }
 
 // ---------------------------------------------------------------------------
@@ -1758,35 +1717,18 @@ csm_status csm_cloud_destroy(csm_cloud* cloud) {
 // ---------------------------------------------------------------------------
 namespace {
 
-// SearchParameters(linear, angular, cloud, resolution)   (corr...2d.cc:27-55)
-struct HostSearch {
-  int num_angular;
-  int num_scans;
-  int lin;
-  double step;
-  double angular;  // the angular window it was made for (rotation tables are shared by it)
+// The search of one job, and the angular window it was made for (rotation tables are shared
+// by it).  MatchFullSubmap searches the whole submap (fast...2d.cc:210-225).
+struct HostSearch : SearchParameters2D {
+  double angular;
 };
-HostSearch MakeSearch(double linear_window, double angular_window, float cloud_max_norm,
-                      double resolution) {
-  float max_scan_range = 3.f * resolution;
-  max_scan_range = std::max(cloud_max_norm, max_scan_range);
-  const double kSafetyMargin = 1. - 1e-3;
-  HostSearch s;
-  s.step = kSafetyMargin *
-           std::acos(1. - (resolution * resolution) / (2. * (max_scan_range * max_scan_range)));
-  s.num_angular = static_cast<int>(std::ceil(angular_window / s.step));
-  s.num_scans = 2 * s.num_angular + 1;
-  s.lin = static_cast<int>(std::ceil(linear_window / resolution));
-  s.angular = angular_window;
-  return s;
-}
-
-// The search of one job: MatchFullSubmap searches the whole submap (fast...2d.cc:210-225).
 HostSearch JobSearch(const csm_stack2d* st, const csm_cloud* cl, const csm_job2d& jb,
                      double linear_window, double angular_window) {
   const double res = st->h.resolution;
-  return jb.full_submap ? MakeSearch(1e6 * res, M_PI, cl->max_norm, res)
-                        : MakeSearch(linear_window, angular_window, cl->max_norm, res);
+  const float max_scan_range = std::max(cl->max_norm, static_cast<float>(3.f * res));
+  const double linear = jb.full_submap ? 1e6 * res : linear_window;
+  const double angular = jb.full_submap ? M_PI : angular_window;
+  return HostSearch{MakeSearchParameters2D(linear, angular, max_scan_range, res), angular};
 }
 
 struct TrigKey {
@@ -1806,19 +1748,9 @@ struct TrigTable {
   HostSearch sp;
 };
 
-// Tables [t0, t1) into out (pairs).  GenerateRotatedScans: delta_theta accumulates in
-// double, is cast to float for AngleAxisf, Quaternionf takes cos/sin of the float half angle.
+// Tables [t0, t1) into out (pairs).
 void FillTrigTables(const std::vector<TrigTable>& tables, size_t t0, size_t t1, float* out) {
-  for (size_t t = t0; t < t1; ++t) {
-    const HostSearch& sp = tables[t].sp;
-    float* o = out + 2 * tables[t].off;
-    double delta_theta = -sp.num_angular * sp.step;
-    for (int k = 0; k < sp.num_scans; ++k, delta_theta += sp.step) {
-      const float ha = 0.5f * static_cast<float>(delta_theta);
-      o[2 * k] = std::cos(ha);
-      o[2 * k + 1] = std::sin(ha);
-    }
-  }
+  for (size_t t = t0; t < t1; ++t) FillRotationTable(tables[t].sp, out + 2 * tables[t].off);
 }
 
 struct BatchPlan {
@@ -1982,14 +1914,7 @@ csm_status Plan2D(Batch2D& b, const HostSearch* search) {
     d.num_scans = sp.num_scans;
     d.scan_base = static_cast<int>(plan.total_scans);
     d.lin = sp.lin;
-    {
-      const float ha = 0.5f * static_cast<float>(ith);
-      const float sn = std::sin(ha);
-      d.q0w = std::cos(ha);
-      d.q0x = sn * 0.f;
-      d.q0y = sn * 0.f;
-      d.q0z = sn * 1.f;
-    }
+    d.q0 = QuatFromAngleAxisZ(static_cast<float>(ith));
     d.tx = static_cast<float>(ix);
     d.ty = static_cast<float>(iy);
     d.min_score = jb.min_score;
@@ -2530,7 +2455,7 @@ void Results2D(const Batch2D& b, const std::vector<std::vector<TieLeaf>>& per_jo
                int host_resolves, csm_result2d* results, csm_stats* total) {
   for (int j = 0; j < b.num_jobs; ++j) {
     csm_result2d& r = results[j];
-    const float best_score = HostOrderedToFloat(b.lbh[j]);
+    const float best_score = OrderedToFloat(b.lbh[j]);
     r.found = 0;
     r.leaves_tied = static_cast<int32_t>(per_job[j].size());
     if (!per_job[j].empty() && best_score > b.jobs[j].min_score) {
@@ -2876,7 +2801,7 @@ csm_status csm_branch_step2d(const csm_stack2d* stack, const float* xyz, int32_t
                 p.x_index_offset <= si.max_x && p.y_index_offset <= si.max_y,
                 "parent is not a node of its scan's level lattice");
   }
-  const unsigned lb_in = HostFloatToOrdered(bound);
+  const unsigned lb_in = FloatToOrdered(bound);
   CSM_CUDA(cudaMemsetAsync(b.ictr, 0, sizeof(int) * kCtlInts, s));
   CSM_CUDA(cudaMemsetAsync(b.ctr, 0, sizeof(unsigned long long) * 2, s));
   CSM_CUDA(cudaMemcpyAsync(b.ictr + h, &num_parents, sizeof(int), cudaMemcpyHostToDevice, s));
@@ -2905,7 +2830,7 @@ csm_status csm_branch_step2d(const csm_stack2d* stack, const float* xyz, int32_t
     CSM_CUDA(cudaMemcpy(children, h >= 2 ? b.Queue(h - 1) : b.d_leaves->as<Node>(),
                         sizeof(Node) * cnt, cudaMemcpyDeviceToHost));
   *num_children = cnt;
-  *final_bound = HostOrderedToFloat(lb_out);
+  *final_bound = OrderedToFloat(lb_out);
   counters[0] = static_cast<int64_t>(c[0]);
   counters[1] = static_cast<int64_t>(c[1]);
   return CSM_OK;

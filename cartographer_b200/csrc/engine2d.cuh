@@ -2,7 +2,10 @@
 #ifndef CSM_ENGINE2D_CUH_
 #define CSM_ENGINE2D_CUH_
 
+#include <cmath>
+
 #include "common.cuh"
+#include "rigid3f.h"
 
 namespace csm {
 
@@ -54,7 +57,7 @@ struct JobDev {
   int lin;               // num_linear_perturbations (pre-shrink window)
   int cap;               // top-level slots reserved per scan
   int cap_y;             // max candidates along y (slot = i * nyc + j uses the scan's own nyc)
-  float q0w, q0x, q0y, q0z;  // initial rotation as Quaternionf(AngleAxisf(yaw, UnitZ))
+  Quatf q0;              // initial rotation as Quaternionf(AngleAxisf(yaw, UnitZ))
   float tx, ty;          // initial translation (float casts)
   float min_score;
   long long dscan_off;   // first int2 of this job in the discrete-scan buffer
@@ -74,11 +77,39 @@ struct Node {  // 16 B
   float score;
 };
 
-// Launches K2 (rotate + discretise + optional ShrinkToFit) for `total_scans`
-// scans on `stream`; defined in engine2d.cu, shared with the real-time matcher.
-csm_status LaunchDiscretize2D(cudaStream_t stream, const JobDev* jobs, const int* scan_job,
-                              int total_scans, short2* dscan, ScanInfo* info, int shrink,
-                              unsigned long long* counters);
+// SearchParameters(linear, angular, point cloud, resolution) of both 2D matchers
+// (correlative_scan_matcher_2d.cc:27-55).  `max_scan_range` is the caller's fold over its
+// points, which starts from 3 * resolution.
+struct SearchParameters2D {
+  int num_angular;
+  int num_scans;
+  int lin;
+  double step;
+};
+
+inline SearchParameters2D MakeSearchParameters2D(double linear_window, double angular_window,
+                                                 float max_scan_range, double resolution) {
+  const double kSafetyMargin = 1. - 1e-3;
+  SearchParameters2D s;
+  s.step = kSafetyMargin *
+           std::acos(1. - (resolution * resolution) / (2. * (max_scan_range * max_scan_range)));
+  s.num_angular = static_cast<int>(std::ceil(angular_window / s.step));
+  s.num_scans = 2 * s.num_angular + 1;
+  s.lin = static_cast<int>(std::ceil(linear_window / resolution));
+  return s;
+}
+
+// The rotations of GenerateRotatedScans (correlative_scan_matcher_2d.cc:93-109) as num_scans
+// (cos, sin) pairs into `out`: delta_theta accumulates in double and is cast to float for
+// AngleAxisf, and Quaternionf takes cos / sin of the float half angle (QuatFromCosSinZ).
+inline void FillRotationTable(const SearchParameters2D& sp, float* out) {
+  double delta_theta = -sp.num_angular * sp.step;
+  for (int k = 0; k < sp.num_scans; ++k, delta_theta += sp.step) {
+    const float ha = 0.5f * static_cast<float>(delta_theta);
+    out[2 * k] = std::cos(ha);
+    out[2 * k + 1] = std::sin(ha);
+  }
+}
 
 }  // namespace csm
 

@@ -15,6 +15,7 @@
 #include <functional>
 
 #include "common.cuh"
+#include "rigid3f.h"
 #include "value_conversion.h"
 
 #include <atomic>
@@ -65,32 +66,6 @@ struct Job3 {
 struct Node3 { int scan, ox, oy, oz; float score; };
 struct Leaf3 { int scan, ox, oy, oz; float score, low; };
 
-__device__ __forceinline__ unsigned FloatToOrdered3(float f) {
-  unsigned u = __float_as_uint(f);
-  return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
-}
-__device__ __forceinline__ float OrderedToFloat3(unsigned u) {
-  return __uint_as_float((u & 0x80000000u) ? (u & 0x7fffffffu) : ~u);
-}
-
-struct F3 { float x, y, z; };
-__device__ __forceinline__ F3 Cross3(const F3& a, const F3& b) {
-  return F3{__fsub_rn(__fmul_rn(a.y, b.z), __fmul_rn(a.z, b.y)),
-            __fsub_rn(__fmul_rn(a.z, b.x), __fmul_rn(a.x, b.z)),
-            __fsub_rn(__fmul_rn(a.x, b.y), __fmul_rn(a.y, b.x))};
-}
-// Rigid3f * point: Eigen quaternion rotate, then + translation
-// (transform/rigid_transform.h:192-196).
-__device__ __forceinline__ F3 Apply3(float qw, const F3& qv, const F3& t, const F3& v) {
-  F3 uv = Cross3(qv, v);
-  uv.x = __fadd_rn(uv.x, uv.x);
-  uv.y = __fadd_rn(uv.y, uv.y);
-  uv.z = __fadd_rn(uv.z, uv.z);
-  const F3 c = Cross3(qv, uv);
-  return F3{__fadd_rn(__fadd_rn(__fadd_rn(v.x, __fmul_rn(qw, uv.x)), c.x), t.x),
-            __fadd_rn(__fadd_rn(__fadd_rn(v.y, __fmul_rn(qw, uv.y)), c.y), t.y),
-            __fadd_rn(__fadd_rn(__fadd_rn(v.z, __fmul_rn(qw, uv.z)), c.z), t.z)};
-}
 // HybridGridBase::GetCellIndex (hybrid_grid.h:428-433): lround(p / resolution) in float.
 __device__ __forceinline__ int CellOf(float p, float resolution) {
   return static_cast<int>(lroundf(__fdiv_rn(p, resolution)));
@@ -268,11 +243,11 @@ __global__ void k3_discretize(Job3 jb) {
   const int s = blockIdx.y;
   if (s >= jb.ctl[kC3Scans]) return;
   const Scan3 sc = jb.scans[s];
-  const F3 qv{sc.qx, sc.qy, sc.qz}, t{sc.tx, sc.ty, sc.tz};
+  const Rigid3f pose{Vec3f{sc.tx, sc.ty, sc.tz}, Quatf{sc.qw, sc.qx, sc.qy, sc.qz}};
   const float res = jb.stack->resolution;
   for (int p = blockIdx.x * blockDim.x + threadIdx.x; p < jb.n_hi; p += gridDim.x * blockDim.x) {
-    const F3 v{jb.hi_xyz[3 * p], jb.hi_xyz[3 * p + 1], jb.hi_xyz[3 * p + 2]};
-    const F3 w = Apply3(sc.qw, qv, t, v);
+    const Vec3f v{jb.hi_xyz[3 * p], jb.hi_xyz[3 * p + 1], jb.hi_xyz[3 * p + 2]};
+    const Vec3f w = Rigid3Apply(pose, v);
     const int cx = max(-30000, min(30000, CellOf(w.x, res)));
     const int cy = max(-30000, min(30000, CellOf(w.y, res)));
     const int cz = max(-30000, min(30000, CellOf(w.z, res)));
@@ -358,10 +333,10 @@ __device__ float LowResScore(const Job3& jb, int scan, int ox, int oy, int oz, f
   const Scan3 sc = jb.scans[scan];
   const float res = jb.stack->resolution;
   // GetPoseFromCandidate (:369-375): Translation(res * offset) * scan.pose
-  const F3 t{__fadd_rn(sc.tx, __fmul_rn(res, __int2float_rn(ox))),
-             __fadd_rn(sc.ty, __fmul_rn(res, __int2float_rn(oy))),
-             __fadd_rn(sc.tz, __fmul_rn(res, __int2float_rn(oz)))};
-  const F3 qv{sc.nx, sc.ny, sc.nz};
+  const Rigid3f pose{Vec3f{__fadd_rn(sc.tx, __fmul_rn(res, __int2float_rn(ox))),
+                           __fadd_rn(sc.ty, __fmul_rn(res, __int2float_rn(oy))),
+                           __fadd_rn(sc.tz, __fmul_rn(res, __int2float_rn(oz)))},
+                     Quatf{sc.nw, sc.nx, sc.ny, sc.nz}};
   const Low3Dev& lg = *jb.low;
   __shared__ float s_sum;
   __syncthreads();  // a previous call's readers of s_sum are done
@@ -369,8 +344,8 @@ __device__ float LowResScore(const Job3& jb, int scan, int ox, int oy, int oz, f
   for (int p0 = 0; p0 < jb.n_lo; p0 += kT3) {
     const int p = p0 + threadIdx.x;
     if (p < jb.n_lo) {
-      const F3 v{jb.lo_xyz[3 * p], jb.lo_xyz[3 * p + 1], jb.lo_xyz[3 * p + 2]};
-      const F3 w = Apply3(sc.nw, qv, t, v);
+      const Vec3f v{jb.lo_xyz[3 * p], jb.lo_xyz[3 * p + 1], jb.lo_xyz[3 * p + 2]};
+      const Vec3f w = Rigid3Apply(pose, v);
       const int x = CellOf(w.x, lg.resolution) - lg.lo[0];
       const int y = CellOf(w.y, lg.resolution) - lg.lo[1];
       const int z = CellOf(w.z, lg.resolution) - lg.lo[2];
@@ -480,7 +455,7 @@ k3_dive(Job3 jb, const int* __restrict__ top_sum, float dive_ratio, unsigned* __
     const float low = LowResScore(jb, scan, ox, oy, oz, s_buf);
     if (threadIdx.x == 0) {
       atomicAdd(&counters[2], 1ull);
-      if (static_cast<double>(low) >= jb.min_low_d) atomicMax(lb, FloatToOrdered3(score));
+      if (static_cast<double>(low) >= jb.min_low_d) atomicMax(lb, FloatToOrdered(score));
     }
   }
   if (threadIdx.x == 0) atomicAdd(&counters[0], scored);
@@ -493,7 +468,7 @@ __global__ void k3_filter_top(Job3 jb, const int* __restrict__ top_sum,
   const int per_scan = jb.nxc * jb.nxc * jb.nzc;
   if (c >= jb.ctl[kC3Scans] * per_scan) return;
   const float score = ToScore3(top_sum[c], jb.n_hi);
-  if (!(score > jb.min_score && score >= OrderedToFloat3(*lb))) return;
+  if (!(score > jb.min_score && score >= OrderedToFloat(*lb))) return;
   const int scan = c / per_scan;
   int r = c - scan * per_scan;
   const int kz = r / (jb.nxc * jb.nxc);
@@ -526,7 +501,7 @@ k3_expand(Job3 jb, const Node3* __restrict__ queue, int* __restrict__ ctl, int h
     const Node3 nd = parents[pi];
     // the bound moves while the kernel runs: one thread samples it, all threads agree
     __syncthreads();
-    if (threadIdx.x == 0) s_bound = OrderedToFloat3(*lb);
+    if (threadIdx.x == 0) s_bound = OrderedToFloat(*lb);
     __syncthreads();
     if (!(nd.score >= s_bound)) continue;
     const int half = 1 << (h - 1);
@@ -545,7 +520,7 @@ k3_expand(Job3 jb, const Node3* __restrict__ queue, int* __restrict__ ctl, int h
         const float sc = ToScore3(s_sums[t], jb.n_hi);
         // leaf candidates that cannot beat (or tie) the bound need no gate evaluation
         __syncthreads();
-        if (threadIdx.x == 0) s_go = (sc > jb.min_score && sc >= OrderedToFloat3(*lb)) ? 1 : 0;
+        if (threadIdx.x == 0) s_go = (sc > jb.min_score && sc >= OrderedToFloat(*lb)) ? 1 : 0;
         __syncthreads();
         if (!s_go) continue;
         const int ox = nd.ox + (t & 1) * half, oy = nd.oy + ((t >> 1) & 1) * half,
@@ -554,7 +529,7 @@ k3_expand(Job3 jb, const Node3* __restrict__ queue, int* __restrict__ ctl, int h
         if (threadIdx.x == 0) {
           atomicAdd(&counters[2], 1ull);
           if (static_cast<double>(low) >= jb.min_low_d) {
-            const unsigned o = FloatToOrdered3(sc);
+            const unsigned o = FloatToOrdered(sc);
             const unsigned old = atomicMax(lb, o);
             if (o >= old) {
               const int idx = atomicAdd(leaf_count, 1);
@@ -566,7 +541,7 @@ k3_expand(Job3 jb, const Node3* __restrict__ queue, int* __restrict__ ctl, int h
         __syncthreads();
       }
     } else if (threadIdx.x == 0) {
-      const float bound = OrderedToFloat3(*lb);
+      const float bound = OrderedToFloat(*lb);
       for (int t = 0; t < 8; ++t) {
         if (!((mask >> t) & 1u)) continue;
         const float sc = ToScore3(s_sums[t], jb.n_hi);
@@ -594,7 +569,7 @@ k3_collect(const Leaf3* __restrict__ leaves, const Scan3* __restrict__ scans,
   const int count = min(ctl[kC3Leaf], leaf_cap);
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < count; i += gridDim.x * blockDim.x) {
     const Leaf3 l = leaves[i];
-    if (FloatToOrdered3(l.score) != bound) continue;
+    if (FloatToOrdered(l.score) != bound) continue;
     const int idx = atomicAdd(&ctl[kC3Best], 1);
     if (idx < out_cap)
       out[idx] = BestLeaf3{l.scan, sel[l.scan], l.ox, l.oy, l.oz, l.score, l.low,
@@ -651,71 +626,10 @@ struct csm_matcher3d {
 
 namespace {
 
-// ---- Eigen semantics on the host (see oracle/oracle_3d.h for the provenance) ----
-struct Qf { float w, x, y, z; };
-struct Vf { float x, y, z; };
-Vf HCross(const Vf& a, const Vf& b) {
-  return Vf{a.y * b.z - a.z * b.y, a.z * b.x - a.x * b.z, a.x * b.y - a.y * b.x};
-}
-Vf HRot(const Qf& q, const Vf& v) {  // QuaternionBase::_transformVector
-  const Vf qv{q.x, q.y, q.z};
-  Vf uv = HCross(qv, v);
-  uv.x += uv.x; uv.y += uv.y; uv.z += uv.z;
-  const Vf c = HCross(qv, uv);
-  return Vf{(v.x + q.w * uv.x) + c.x, (v.y + q.w * uv.y) + c.y, (v.z + q.w * uv.z) + c.z};
-}
-Qf HMul(const Qf& a, const Qf& b) {  // Geometry_SSE.h quat_product<float>
-  Qf r;
-  r.x = (a.x * b.w - a.z * b.y) + (a.y * b.z + a.w * b.x);
-  r.y = (a.y * b.w - a.x * b.z) + (a.z * b.x + a.w * b.y);
-  r.z = (a.z * b.w - a.y * b.x) + (a.x * b.y + a.w * b.z);
-  r.w = (a.w * b.w - a.x * b.x) + (-(a.z * b.z + a.y * b.y));
-  return r;
-}
-float HSq(const Qf& q) { return (q.x * q.x + q.z * q.z) + (q.y * q.y + q.w * q.w); }
-Qf HNormalized(const Qf& q) {
-  const float z = HSq(q);
-  if (z > 0.f) {
-    const float n = std::sqrt(z);
-    return Qf{q.w / n, q.x / n, q.y / n, q.z / n};
-  }
-  return q;
-}
-Qf HConj(const Qf& q) { return Qf{q.w, -q.x, -q.y, -q.z}; }
-Qf HInverse(const Qf& q) {
-  const float n2 = HSq(q);
-  if (n2 > 0.f) return Qf{q.w / n2, -q.x / n2, -q.y / n2, -q.z / n2};
-  return Qf{0.f, 0.f, 0.f, 0.f};
-}
-struct Rf { Vf t; Qf q; };
-Rf RInverse(const Rf& r) {  // rigid_transform.h:148-152
-  const Qf rot = HConj(r.q);
-  const Vf v = HRot(rot, r.t);
-  return Rf{Vf{-v.x, -v.y, -v.z}, rot};
-}
-Rf RMul(const Rf& a, const Rf& b) {  // rigid_transform.h:181-189
-  const Vf v = HRot(a.q, b.t);
-  return Rf{Vf{v.x + a.t.x, v.y + a.t.y, v.z + a.t.z}, HNormalized(HMul(a.q, b.q))};
-}
-float HYaw(const Qf& q) {  // transform/transform.h:42-47
-  const Vf d = HRot(q, Vf{1.f, 0.f, 0.f});
-  return std::atan2(d.y, d.x);
-}
-Qf HAngleAxisZ(float angle) {  // transform/transform.h:85-99 with (0, 0, angle)
-  float scale = 0.5f, w = 1.f;
-  const float sq = 0.f * 0.f + 0.f * 0.f + angle * angle;
-  if (sq > 1e-8) {
-    const float norm = std::sqrt(sq);
-    scale = static_cast<float>(std::sin(norm / 2.) / norm);
-    w = static_cast<float>(std::cos(norm / 2.));
-  }
-  return Qf{w, scale * 0.f, scale * 0.f, scale * angle};
-}
-
 struct HostSearch3 {
   int wxy, wz;
   double angular;
-  Rf node, submap;
+  Rigid3f node, submap;
 };
 
 struct ScanPlan {
@@ -999,23 +913,21 @@ static csm_status PlanScans(const csm_matcher3d* m, const csm_node3d* node, floa
   for (int rz = -angular_window_size; rz <= angular_window_size; ++rz)
     plan->angles.push_back(rz * angular_step_size);
   plan->num_angles = static_cast<int>(plan->angles.size());
-  const Rf node_to_submap = RMul(RInverse(sp.submap), sp.node);
+  const Rigid3f node_to_submap = Rigid3Mul(Rigid3Inverse(sp.submap), sp.node);
   // gravity_alignment.inverse().cast<float>()
   const double* g = node->gravity_alignment;
-  const double n2 = (g[1] * g[1] + g[3] * g[3]) + (g[2] * g[2] + g[0] * g[0]);
-  Qf ginv{0.f, 0.f, 0.f, 0.f};
-  if (n2 > 0.)
-    ginv = Qf{static_cast<float>(g[0] / n2), static_cast<float>(-g[1] / n2),
-              static_cast<float>(-g[2] / n2), static_cast<float>(-g[3] / n2)};
-  *initial_angle = HYaw(HMul(node_to_submap.q, ginv));
+  const Quatf ginv = QuatCastInverseD(Quatd{g[0], g[1], g[2], g[3]});
+  *initial_angle = GetYaw(QuatMul(node_to_submap.q, ginv));
   CSM_REQUIRE(node->histogram_size == static_cast<int>(m->hist.size()), "histogram sizes differ");
   plan->scans.clear();
   plan->scans.reserve(plan->num_angles);
-  const Qf sub_inv = HInverse(sp.submap.q);
+  const Quatf sub_inv = QuatInverse(sp.submap.q);
   for (int i = 0; i < plan->num_angles; ++i) {
-    const Qf q = HMul(HMul(sub_inv, HAngleAxisZ(plan->angles[i])), sp.node.q);
+    const Quatf q = QuatMul(
+        QuatMul(sub_inv, AngleAxisVectorToRotationQuaternion(Vec3f{0.f, 0.f, plan->angles[i]})),
+        sp.node.q);
     // GetPoseFromCandidate's rotation: (identity * q).normalized()
-    const Qf nq = HNormalized(HMul(Qf{1.f, 0.f, 0.f, 0.f}, q));
+    const Quatf nq = QuatNormalized(QuatMul(Quatf{1.f, 0.f, 0.f, 0.f}, q));
     Scan3 sc;
     sc.tx = node_to_submap.t.x; sc.ty = node_to_submap.t.y; sc.tz = node_to_submap.t.z;
     sc.qw = q.w; sc.qx = q.x; sc.qy = q.y; sc.qz = q.z;
@@ -1029,12 +941,12 @@ static csm_status PlanScans(const csm_matcher3d* m, const csm_node3d* node, floa
 static csm_status MakeSearch3(const csm_matcher3d* m, float max_range, const double node_pose[7],
                               const double submap_pose[7], int full, HostSearch3* sp) {
   auto cast = [](const double p[7], bool rotation_only) {
-    Rf r;
-    r.t = rotation_only ? Vf{0.f, 0.f, 0.f}
-                        : Vf{static_cast<float>(p[0]), static_cast<float>(p[1]),
-                             static_cast<float>(p[2])};
-    r.q = Qf{static_cast<float>(p[3]), static_cast<float>(p[4]), static_cast<float>(p[5]),
-             static_cast<float>(p[6])};
+    Rigid3f r;
+    r.t = rotation_only ? Vec3f{0.f, 0.f, 0.f}
+                        : Vec3f{static_cast<float>(p[0]), static_cast<float>(p[1]),
+                                static_cast<float>(p[2])};
+    r.q = Quatf{static_cast<float>(p[3]), static_cast<float>(p[4]), static_cast<float>(p[5]),
+                static_cast<float>(p[6])};
     return r;
   };
   const float resolution = m->hs.resolution;
@@ -1205,7 +1117,7 @@ csm_status Discretize3D(Match3& x) {
   }
   k3_select_scans<<<1, 1024, 0, s>>>(reinterpret_cast<const Scan3*>(x.dup), x.d_rot->as<float>(),
                                      A, x.m->opt.min_rotational_score, x.d_scans->as<Scan3>(),
-                                     x.d_sel->as<int>(), x.ictr, HostFloatToOrdered(x.min_score));
+                                     x.d_sel->as<int>(), x.ictr, FloatToOrdered(x.min_score));
   CSM_LAUNCH_CHECK();
   ProfBegin(ctx);
   k3_discretize<<<dim3(std::min(DivUp(x.jb.n_hi, 256), 64), A), 256, 0, s>>>(x.jb);
@@ -1390,7 +1302,7 @@ void Result3D(const Match3& x, const std::vector<BestLeaf3>& ties, int host_reso
               csm_result3d* result, csm_stats* stats) {
   const int S = x.hp[kC3Scans];
   const long long total_top = x.per_scan * S;
-  const float best_score = HostOrderedToFloat(static_cast<unsigned>(x.hp[kC3Bound]));
+  const float best_score = OrderedToFloat(static_cast<unsigned>(x.hp[kC3Bound]));
   result->leaves_tied = static_cast<int32_t>(ties.size());
   if (!ties.empty() && best_score > x.min_score) {
     const BestLeaf3& t = ties[0];
@@ -1710,7 +1622,7 @@ csm_status csm_score_top3d(const csm_matcher3d* m, const csm_node3d* node,
   if (S && sums)
     CSM_CUDA(cudaMemcpy(sums, x.d_top->p, sizeof(int) * x.per_scan * S, cudaMemcpyDeviceToHost));
   if (top_best) *top_best = x.hp[kC3TopBest];
-  if (bound) *bound = HostOrderedToFloat(static_cast<unsigned>(x.hp[kC3Bound]));
+  if (bound) *bound = OrderedToFloat(static_cast<unsigned>(x.hp[kC3Bound]));
   if (counters) {
     counters[0] = static_cast<int64_t>(c[0]);
     counters[1] = static_cast<int64_t>(c[2]);
@@ -1756,7 +1668,7 @@ csm_status csm_branch_step3d(const csm_matcher3d* m, const csm_node3d* node,
   hp[h] = n;
   hp[kC3Leaf] = 0;
   hp[kC3Overflow] = 0;
-  hp[kC3Bound] = static_cast<int>(HostFloatToOrdered(bound));
+  hp[kC3Bound] = static_cast<int>(FloatToOrdered(bound));
   CSM_CUDA(cudaMemcpyAsync(x.ictr, hp, kRbCtr, cudaMemcpyHostToDevice, s));
   CSM_CUDA(cudaMemsetAsync(x.ctr, 0, 8 * 8, s));
   if (n) CSM_CUDA(cudaMemcpyAsync(x.Queue(h), ps, sizeof(Node3) * n, cudaMemcpyHostToDevice, s));
@@ -1771,7 +1683,7 @@ csm_status csm_branch_step3d(const csm_matcher3d* m, const csm_node3d* node,
                         cudaMemcpyDeviceToHost));
   if (*num_out && h == 1)
     CSM_CUDA(cudaMemcpy(leaves, x.d_leaves->p, sizeof(Leaf3) * *num_out, cudaMemcpyDeviceToHost));
-  *final_bound = HostOrderedToFloat(static_cast<unsigned>(hp[kC3Bound]));
+  *final_bound = OrderedToFloat(static_cast<unsigned>(hp[kC3Bound]));
   for (int k = 0; k < 3; ++k) counters[k] = static_cast<int64_t>(c[k]);
   return CSM_OK;
 }

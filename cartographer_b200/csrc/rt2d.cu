@@ -94,23 +94,6 @@ __device__ __forceinline__ void TmaLoad2D(void* dst, const CUtensorMap* map, int
       : "memory");
 }
 
-// Eigen quaternion * vector for a rotation about z (transform/rigid_transform.h:192-196):
-// q = (w, 0, 0, s).  Same operation order as engine2d.cu's RotateRn.
-__device__ __forceinline__ void RotateZ(float w, float s, float vx, float vy, float vz, float& ox,
-                                        float& oy) {
-  const float qx = __fmul_rn(s, 0.f), qy = __fmul_rn(s, 0.f), qz = __fmul_rn(s, 1.f);
-  float ux = __fsub_rn(__fmul_rn(qy, vz), __fmul_rn(qz, vy));
-  float uy = __fsub_rn(__fmul_rn(qz, vx), __fmul_rn(qx, vz));
-  float uz = __fsub_rn(__fmul_rn(qx, vy), __fmul_rn(qy, vx));
-  ux = __fadd_rn(ux, ux);
-  uy = __fadd_rn(uy, uy);
-  uz = __fadd_rn(uz, uz);
-  const float cx = __fsub_rn(__fmul_rn(qy, uz), __fmul_rn(qz, uy));
-  const float cy = __fsub_rn(__fmul_rn(qz, ux), __fmul_rn(qx, uz));
-  ox = __fadd_rn(__fadd_rn(__fadd_rn(vx, __fmul_rn(w, ux)), cx), 0.f);
-  oy = __fadd_rn(__fadd_rn(__fadd_rn(vy, __fmul_rn(w, uy)), cy), 0.f);
-}
-
 // kForm: 0 = ProbabilityGrid staged in shared memory by TMA, 1 = ProbabilityGrid through
 // read-only global gathers, 2 = TSDF2D (two global cell arrays).
 template <int kForm, int kRtAcc>
@@ -187,11 +170,11 @@ k_rt_match(const __grid_constant__ CUtensorMap tmap, const RtGridDev G, const Rt
           if (p0 + lane < jb.n) {
             const float vx = pts[3 * (p0 + lane)], vy = pts[3 * (p0 + lane) + 1],
                         vz = pts[3 * (p0 + lane) + 2];
-            float rx, ry;
-            RotateZ(cs.x, cs.y, vx, vy, vz, rx, ry);   // GenerateRotatedScans (corr...2d.cc:93-109)
+            // GenerateRotatedScans (corr...2d.cc:93-109)
+            const Vec3f r = RotateAsRigid3f(QuatFromCosSinZ(cs.x, cs.y), Vec3f{vx, vy, vz});
             // Affine2f(Translation2f) * v                                    (corr...2d.cc:120-121)
-            const float px = __fadd_rn(__fadd_rn(__fmul_rn(1.f, rx), __fmul_rn(0.f, ry)), jb.tx);
-            const float py = __fadd_rn(__fadd_rn(__fmul_rn(0.f, rx), __fmul_rn(1.f, ry)), jb.ty);
+            const float px = __fadd_rn(__fadd_rn(__fmul_rn(1.f, r.x), __fmul_rn(0.f, r.y)), jb.tx);
+            const float py = __fadd_rn(__fadd_rn(__fmul_rn(0.f, r.x), __fmul_rn(1.f, r.y)), jb.ty);
             // MapLimits::GetCellIndex in double                              (2d/map_limits.h:69-76)
             const double fx = __dsub_rn(__ddiv_rn(__dsub_rn(G.max_y, static_cast<double>(py)),
                                                   G.resolution), 0.5);
@@ -316,20 +299,6 @@ using namespace csm;
 // grid (local_trajectory_builder_2d.cc:77-82); the handle lets many scans share one copy.
 namespace {
 
-struct HV3 { float x, y, z; };
-inline HV3 HCross(const HV3& a, const HV3& b) {
-  return HV3{a.y * b.z - a.z * b.y, a.z * b.x - a.x * b.z, a.x * b.y - a.y * b.x};
-}
-// Same Eigen formula as the device RotateRn (transform/rigid_transform.h:192-196).
-inline HV3 HRotate(float qw, const HV3& qv, const HV3& v) {
-  HV3 uv = HCross(qv, v);
-  uv.x += uv.x; uv.y += uv.y; uv.z += uv.z;
-  const HV3 c = HCross(qv, uv);
-  HV3 r{(v.x + qw * uv.x) + c.x, (v.y + qw * uv.y) + c.y, (v.z + qw * uv.z) + c.z};
-  r.x += 0.f; r.y += 0.f; r.z += 0.f;
-  return r;
-}
-
 void FillParams(RtParams* P, int lin, float truncation, float max_weight) {
   std::memset(P, 0, sizeof(*P));
   P->lin = lin;
@@ -359,45 +328,40 @@ struct RtHostJob {
 };
 
 struct RtPlan {          // per job, host side
-  int num_angular = 0, num_scans = 0;
-  double step = 0.;
+  SearchParameters2D sp;
   bool smem = false;
 };
 
-// Host preparation of one job into the staging buffers: rotated cloud, SearchParameters,
-// rotation table, weight classes (all libm, like the reference).
-void PrepareJob(const RtHostJob& job, const RtGridDev& G, const RtParams& P, double angular_window,
-                double w_t, double w_r, float* xyz_out, float* trig_out, double* w_out,
-                RtPlan* plan, RtJobDev* jd) {
-  // rotated_point_cloud (:123-127): SearchParameters needs its max range.
-  const float yaw = static_cast<float>(job.init[2]);
-  const float ha0 = 0.5f * yaw;
-  const float s0 = std::sin(ha0);
-  const HV3 q0{s0 * 0.f, s0 * 0.f, s0 * 1.f};
-  const float q0w = std::cos(ha0);
-  float max_scan_range = 3.f * G.resolution;  // correlative_scan_matcher_2d.cc:34
+// rotated_point_cloud (:123-127) into xyz_out unless it is null, and its max range as
+// SearchParameters folds it (correlative_scan_matcher_2d.cc:34-38).
+float RotateCloud(const RtHostJob& job, double resolution, float* xyz_out) {
+  const Quatf q0 = QuatFromAngleAxisZ(static_cast<float>(job.init[2]));
+  float max_scan_range = 3.f * resolution;
   for (int i = 0; i < job.n; ++i) {
-    const HV3 r = HRotate(q0w, q0, HV3{job.xyz[3 * i], job.xyz[3 * i + 1], job.xyz[3 * i + 2]});
-    xyz_out[3 * i] = r.x;
-    xyz_out[3 * i + 1] = r.y;
-    xyz_out[3 * i + 2] = r.z;
+    const Vec3f r =
+        RotateAsRigid3f(q0, Vec3f{job.xyz[3 * i], job.xyz[3 * i + 1], job.xyz[3 * i + 2]});
+    if (xyz_out) {
+      xyz_out[3 * i] = r.x;
+      xyz_out[3 * i + 1] = r.y;
+      xyz_out[3 * i + 2] = r.z;
+    }
     const float range = std::sqrt(r.x * r.x + r.y * r.y);
     max_scan_range = std::max(range, max_scan_range);
   }
-  const double kSafetyMargin = 1. - 1e-3;
-  const double step = kSafetyMargin * std::acos(1. - (G.resolution * G.resolution) /
-                                                         (2. * (max_scan_range * max_scan_range)));
-  const int num_angular = plan->num_angular;  // computed by the caller (needed for sizes)
-  plan->step = step;
-  double delta_theta = -num_angular * step;
-  for (int k = 0; k < plan->num_scans; ++k, delta_theta += step) {
-    const float ha = 0.5f * static_cast<float>(delta_theta);
-    trig_out[2 * k] = std::cos(ha);
-    trig_out[2 * k + 1] = std::sin(ha);
-  }
+  return max_scan_range;
+}
+
+// Host preparation of one job into the staging buffers: rotated cloud, rotation table, weight
+// classes (all libm, like the reference).  plan->sp is the job's search (RtRun).
+void PrepareJob(const RtHostJob& job, const RtGridDev& G, const RtParams& P, double w_t,
+                double w_r, float* xyz_out, float* trig_out, double* w_out, RtPlan* plan,
+                RtJobDev* jd) {
+  const float max_scan_range = RotateCloud(job, G.resolution, xyz_out);
+  const SearchParameters2D& sp = plan->sp;
+  FillRotationTable(sp, trig_out);
   // weight classes: |orientation| = a * step (Candidate2D ctor), hypot over {|xo|, |yo|}
-  for (int a = 0; a <= num_angular; ++a) {
-    const double orientation = a * step;
+  for (int a = 0; a <= sp.num_angular; ++a) {
+    const double orientation = a * sp.step;
     for (int jj = 0; jj <= P.lin; ++jj)
       for (int i = 0; i <= jj; ++i) {
         const double cx = -(jj)*G.resolution, cy = -(i)*G.resolution;
@@ -406,8 +370,8 @@ void PrepareJob(const RtHostJob& job, const RtGridDev& G, const RtParams& P, dou
       }
   }
   jd->n = job.n;
-  jd->num_scans = plan->num_scans;
-  jd->num_angular = num_angular;
+  jd->num_scans = sp.num_scans;
+  jd->num_angular = sp.num_angular;
   jd->tx = static_cast<float>(job.init[0]);  // Translation2f(double, double) (:135-137)
   jd->ty = static_cast<float>(job.init[1]);
   // Box the scan can reach: cell of the initial translation +- (max range + window)
@@ -430,25 +394,6 @@ void PrepareJob(const RtHostJob& job, const RtGridDev& G, const RtParams& P, dou
       jd->y0 = static_cast<int>(ry0);
     }
   }
-}
-
-int NumAngular(const RtHostJob& job, double resolution, double angular_window) {
-  // needs the max range of the rotated cloud: identical arithmetic to PrepareJob
-  const float yaw = static_cast<float>(job.init[2]);
-  const float ha0 = 0.5f * yaw;
-  const float s0 = std::sin(ha0);
-  const HV3 q0{s0 * 0.f, s0 * 0.f, s0 * 1.f};
-  const float q0w = std::cos(ha0);
-  float max_scan_range = 3.f * resolution;
-  for (int i = 0; i < job.n; ++i) {
-    const HV3 r = HRotate(q0w, q0, HV3{job.xyz[3 * i], job.xyz[3 * i + 1], job.xyz[3 * i + 2]});
-    const float range = std::sqrt(r.x * r.x + r.y * r.y);
-    max_scan_range = std::max(range, max_scan_range);
-  }
-  const double kSafetyMargin = 1. - 1e-3;
-  const double step = kSafetyMargin * std::acos(1. - (resolution * resolution) /
-                                                         (2. * (max_scan_range * max_scan_range)));
-  return static_cast<int>(std::ceil(angular_window / step));
 }
 
 template <typename F>
@@ -488,22 +433,23 @@ csm_status RtRun(Ctx* ctx, const csm_rt_grid2d* grid, const RtHostJob* jobs, int
   std::vector<RtJobDev> jd(num);
   std::vector<int> bad(1, 0);
   ParallelFor(num, 16, [&](int j) {
-    plan[j].num_angular = NumAngular(jobs[j], G.resolution, angular_window);
-    plan[j].num_scans = 2 * plan[j].num_angular + 1;
+    plan[j].sp = MakeSearchParameters2D(linear_window, angular_window,
+                                        RotateCloud(jobs[j], G.resolution, nullptr), G.resolution);
   });
   long long xyz_f = 0, trig_f = 0, w_d = 0, items = 0, cands = 0;
   for (int j = 0; j < num; ++j) {
-    CSM_REQUIRE(plan[j].num_scans > 0 && plan[j].num_scans < (1 << 20), "angular window / step");
+    const SearchParameters2D& sp = plan[j].sp;
+    CSM_REQUIRE(sp.num_scans > 0 && sp.num_scans < (1 << 20), "angular window / step");
     jd[j].xyz_off = xyz_f;
     jd[j].trig_off = static_cast<int>(trig_f);
     jd[j].w_off = static_cast<int>(w_d);
     jd[j].item_base = static_cast<int>(items);
     xyz_f += 3LL * jobs[j].n;
-    trig_f += plan[j].num_scans;
-    w_d += static_cast<long long>(plan[j].num_angular + 1) * P.npair;
-    items += plan[j].num_scans;
-    cands += static_cast<long long>(plan[j].num_scans) * P.per_scan;
-    CSM_REQUIRE(static_cast<long long>(plan[j].num_scans) * P.per_scan < (1LL << 31),
+    trig_f += sp.num_scans;
+    w_d += static_cast<long long>(sp.num_angular + 1) * P.npair;
+    items += sp.num_scans;
+    cands += static_cast<long long>(sp.num_scans) * P.per_scan;
+    CSM_REQUIRE(static_cast<long long>(sp.num_scans) * P.per_scan < (1LL << 31),
                 "search window too large");
   }
   CSM_REQUIRE(items < (1LL << 30) && trig_f < (1LL << 30) && w_d < (1LL << 30), "batch too large");
@@ -521,7 +467,7 @@ csm_status RtRun(Ctx* ctx, const csm_rt_grid2d* grid, const RtHostJob* jobs, int
   CSM_TRY(rb.Reserve(sizeof(unsigned long long) * num));
   char* h = up.as<char>();
   ParallelFor(num, 16, [&](int j) {
-    PrepareJob(jobs[j], G, P, angular_window, w_t, w_r, reinterpret_cast<float*>(h) + jd[j].xyz_off,
+    PrepareJob(jobs[j], G, P, w_t, w_r, reinterpret_cast<float*>(h) + jd[j].xyz_off,
                reinterpret_cast<float*>(h + off_trig) + 2 * static_cast<size_t>(jd[j].trig_off),
                reinterpret_cast<double*>(h + off_w) + jd[j].w_off, &plan[j], &jd[j]);
   });
@@ -578,12 +524,12 @@ csm_status RtRun(Ctx* ctx, const csm_rt_grid2d* grid, const RtHostJob* jobs, int
     o.score = best_score;
     o.pose_estimate[0] = jobs[j].init[0] + (-yo * G.resolution);
     o.pose_estimate[1] = jobs[j].init[1] + (-xo * G.resolution);
-    o.pose_estimate[2] = jobs[j].init[2] + (scan - plan[j].num_angular) * plan[j].step;
+    o.pose_estimate[2] = jobs[j].init[2] + (scan - plan[j].sp.num_angular) * plan[j].sp.step;
     o.best_scan_index = scan;
     o.best_x_offset = xo;
     o.best_y_offset = yo;
-    o.num_scans = plan[j].num_scans;
-    o.candidates_scored = static_cast<int64_t>(plan[j].num_scans) * P.per_scan;
+    o.num_scans = plan[j].sp.num_scans;
+    o.candidates_scored = static_cast<int64_t>(plan[j].sp.num_scans) * P.per_scan;
   }
   if (stats) {
     float ms = 0.f;

@@ -21,6 +21,7 @@
 
 #include "common.cuh"
 #include "grid3d.cuh"
+#include "rigid3f.h"
 #include "value_conversion.h"
 
 namespace csm {
@@ -59,22 +60,13 @@ k_rt3_match(const Grid3Dev G, const Rt3Params P, const float* __restrict__ xyz,
     float sum = 0.f;
     for (int p0 = 0; p0 < P.n; p0 += kRt3Chunk) {
       __syncthreads();
-      // Rigid3f * point, rotation part: Eigen quaternion * vector
-      // (transform/rigid_transform.h:192-196)
+      // Rigid3f * point, rotation part (transform/rigid_transform.h:192-196)
       for (int i = threadIdx.x; i < kRt3Chunk && p0 + i < P.n; i += blockDim.x) {
-        const float vx = xyz[3 * (p0 + i)], vy = xyz[3 * (p0 + i) + 1], vz = xyz[3 * (p0 + i) + 2];
-        float ux = __fsub_rn(__fmul_rn(q.z, vz), __fmul_rn(q.w, vy));  // qv = (q.y, q.z, q.w)
-        float uy = __fsub_rn(__fmul_rn(q.w, vx), __fmul_rn(q.y, vz));
-        float uz = __fsub_rn(__fmul_rn(q.y, vy), __fmul_rn(q.z, vx));
-        ux = __fadd_rn(ux, ux);
-        uy = __fadd_rn(uy, uy);
-        uz = __fadd_rn(uz, uz);
-        const float cx = __fsub_rn(__fmul_rn(q.z, uz), __fmul_rn(q.w, uy));
-        const float cy = __fsub_rn(__fmul_rn(q.w, ux), __fmul_rn(q.y, uz));
-        const float cz = __fsub_rn(__fmul_rn(q.y, uy), __fmul_rn(q.z, ux));
-        s_x[i] = __fadd_rn(__fadd_rn(vx, __fmul_rn(q.x, ux)), cx);   // q.x holds w
-        s_y[i] = __fadd_rn(__fadd_rn(vy, __fmul_rn(q.x, uy)), cy);
-        s_z[i] = __fadd_rn(__fadd_rn(vz, __fmul_rn(q.x, uz)), cz);
+        const Vec3f v{xyz[3 * (p0 + i)], xyz[3 * (p0 + i) + 1], xyz[3 * (p0 + i) + 2]};
+        const Vec3f w = Rotate(Quatf{q.x, q.y, q.z, q.w}, v);
+        s_x[i] = w.x;
+        s_y[i] = w.y;
+        s_z[i] = w.z;
       }
       __syncthreads();
       if (on) {
@@ -115,50 +107,6 @@ k_rt3_match(const Grid3Dev G, const Rt3Params P, const float* __restrict__ xyz,
 }  // namespace csm
 
 using namespace csm;
-
-namespace {
-
-// ---- Eigen semantics on the host (same restatement as engine3d.cu / oracle_3d.cc) ----
-struct Qf { float w, x, y, z; };
-struct Vf { float x, y, z; };
-Vf HCross(const Vf& a, const Vf& b) {
-  return Vf{a.y * b.z - a.z * b.y, a.z * b.x - a.x * b.z, a.x * b.y - a.y * b.x};
-}
-Vf HRot(const Qf& q, const Vf& v) {  // QuaternionBase::_transformVector
-  const Vf qv{q.x, q.y, q.z};
-  Vf uv = HCross(qv, v);
-  uv.x += uv.x; uv.y += uv.y; uv.z += uv.z;
-  const Vf c = HCross(qv, uv);
-  return Vf{(v.x + q.w * uv.x) + c.x, (v.y + q.w * uv.y) + c.y, (v.z + q.w * uv.z) + c.z};
-}
-Qf HMul(const Qf& a, const Qf& b) {  // Geometry_SSE.h quat_product<float>
-  Qf r;
-  r.x = (a.x * b.w - a.z * b.y) + (a.y * b.z + a.w * b.x);
-  r.y = (a.y * b.w - a.x * b.z) + (a.z * b.x + a.w * b.y);
-  r.z = (a.z * b.w - a.y * b.x) + (a.x * b.y + a.w * b.z);
-  r.w = (a.w * b.w - a.x * b.x) + (-(a.z * b.z + a.y * b.y));
-  return r;
-}
-Qf HNormalized(const Qf& q) {
-  const float z = (q.x * q.x + q.z * q.z) + (q.y * q.y + q.w * q.w);
-  if (z > 0.f) {
-    const float n = std::sqrt(z);
-    return Qf{q.w / n, q.x / n, q.y / n, q.z / n};
-  }
-  return q;
-}
-Qf HAngleAxis(const Vf& aa) {  // transform/transform.h:85-99
-  float scale = 0.5f, w = 1.f;
-  const float sq = aa.x * aa.x + aa.y * aa.y + aa.z * aa.z;
-  if (sq > 1e-8) {
-    const float norm = std::sqrt(sq);
-    scale = static_cast<float>(std::sin(norm / 2.) / norm);
-    w = static_cast<float>(std::cos(norm / 2.));
-  }
-  return Qf{w, scale * aa.x, scale * aa.y, scale * aa.z};
-}
-
-}  // namespace
 
 extern "C" {
 
@@ -260,28 +208,27 @@ csm_status csm_rt_match3d(const csm_grid3d* grid, const float* xyz, int32_t n,
   const long long T = static_cast<long long>(W) * W * W, R = static_cast<long long>(Rw) * Rw * Rw;
   CSM_REQUIRE(T * R < (1LL << 31), "search window too large");
   // initial_pose_estimate.cast<float>()
-  const Vf t_init{static_cast<float>(initial_pose[0]), static_cast<float>(initial_pose[1]),
-                  static_cast<float>(initial_pose[2])};
-  const Qf q_init{static_cast<float>(initial_pose[3]), static_cast<float>(initial_pose[4]),
-                  static_cast<float>(initial_pose[5]), static_cast<float>(initial_pose[6])};
-  // per rotation: transform rotation, candidate rotation = (q_init * q_r).normalized()
-  // (rigid_transform.h:181-189) and GetAngle(transform) (transform.h:34-37)
-  std::vector<Qf> q_r(R), q_c(R);
+  const Rigid3f init{
+      Vec3f{static_cast<float>(initial_pose[0]), static_cast<float>(initial_pose[1]),
+            static_cast<float>(initial_pose[2])},
+      Quatf{static_cast<float>(initial_pose[3]), static_cast<float>(initial_pose[4]),
+            static_cast<float>(initial_pose[5]), static_cast<float>(initial_pose[6])}};
+  // per rotation: candidate rotation = (q_init * q_r).normalized() (rigid_transform.h:181-189)
+  // and GetAngle(transform) (transform.h:34-37)
+  std::vector<Quatf> q_c(R);
   std::vector<float> angle(R);
   {
     long long r = 0;
     for (int rz = -A; rz <= A; ++rz)
       for (int ry = -A; ry <= A; ++ry)
         for (int rx = -A; rx <= A; ++rx, ++r) {
-          const Qf q = HAngleAxis(Vf{rx * angular_step_size, ry * angular_step_size,
-                                     rz * angular_step_size});
-          q_r[r] = q;
-          q_c[r] = HNormalized(HMul(q_init, q));
-          const float vec_norm = std::sqrt(q.x * q.x + q.y * q.y + q.z * q.z);
-          angle[r] = 2.f * std::atan2(vec_norm, std::abs(q.w));
+          const Quatf q = AngleAxisVectorToRotationQuaternion(
+              Vec3f{rx * angular_step_size, ry * angular_step_size, rz * angular_step_size});
+          q_c[r] = QuatNormalized(QuatMul(init.q, q));
+          angle[r] = GetAngle(Rigid3f{Vec3f{0.f, 0.f, 0.f}, q});
         }
   }
-  // per translation: candidate translation = q_init * t + t_init, and its norm class
+  // per translation: candidate translation = initial_pose * t, and its norm class
   std::vector<float4> trans(T);
   std::map<unsigned, int> klass;   // norm bits -> class
   std::vector<float> class_norm;
@@ -290,8 +237,7 @@ csm_status csm_rt_match3d(const csm_grid3d* grid, const float* xyz, int32_t n,
     for (int z = -L; z <= L; ++z)
       for (int y = -L; y <= L; ++y)
         for (int x = -L; x <= L; ++x, ++t) {
-          const Vf tv{x * resolution, y * resolution, z * resolution};
-          const Vf rt = HRot(q_init, tv);
+          const Vec3f tv{x * resolution, y * resolution, z * resolution};
           const float norm = std::sqrt(tv.x * tv.x + tv.y * tv.y + tv.z * tv.z);
           unsigned bits;
           std::memcpy(&bits, &norm, 4);
@@ -302,7 +248,8 @@ csm_status csm_rt_match3d(const csm_grid3d* grid, const float* xyz, int32_t n,
           }
           float cls;
           std::memcpy(&cls, &it->second, 4);
-          trans[t] = make_float4(rt.x + t_init.x, rt.y + t_init.y, rt.z + t_init.z, cls);
+          const Vec3f ct = Rigid3Apply(init, tv);
+          trans[t] = make_float4(ct.x, ct.y, ct.z, cls);
         }
   }
   // weights per (norm class, rotation): exp(-(norm * w_t + angle * w_r)^2) in double (:109-114)
