@@ -95,13 +95,16 @@ __device__ __forceinline__ void TmaLoad2D(void* dst, const CUtensorMap* map, int
 }
 
 // kForm: 0 = ProbabilityGrid staged in shared memory by TMA, 1 = ProbabilityGrid through
-// read-only global gathers, 2 = TSDF2D (two global cell arrays).
-template <int kForm, int kRtAcc>
+// read-only global gathers, 2 = TSDF2D (two global cell arrays).  kScores: also store every
+// candidate's weighted score at scores[item * per_scan + r] (test hook csm_rt_scores2d).
+// TSDF2D only: negz[job] = the smallest generation index whose score is -0.0.
+template <int kForm, int kRtAcc, bool kScores>
 __global__ void __launch_bounds__(kRtThreads, 2)
 k_rt_match(const __grid_constant__ CUtensorMap tmap, const RtGridDev G, const RtParams P,
            const RtJobDev* __restrict__ jobs, int num_jobs, int total_items,
            const float* __restrict__ xyz, const float2* __restrict__ trig,
-           const double* __restrict__ weights, unsigned long long* __restrict__ best) {
+           const double* __restrict__ weights, unsigned long long* __restrict__ best,
+           unsigned* __restrict__ negz, float* __restrict__ scores) {
   extern __shared__ __align__(128) unsigned char s_raw[];
   uint16_t* s_tile = reinterpret_cast<uint16_t*>(s_raw);
   __shared__ __align__(8) uint64_t s_bar;
@@ -158,7 +161,9 @@ k_rt_match(const __grid_constant__ CUtensorMap tmap, const RtGridDev G, const Rt
         float sum[kRtAcc], wsum[kRtAcc];
 #pragma unroll
         for (int a = 0; a < kRtAcc; ++a) {
-          const int r = r0 + lane + 32 * a;    // generation order: x outer, y inner (:98-111)
+          // generation order: x outer, y inner (:98-111).  Idle lanes (r >= per_scan) take the
+          // last candidate's offsets, so that every gather stays within lin of a point's cell
+          const int r = min(r0 + lane + 32 * a, P.per_scan - 1);
           xo[a] = -P.lin + r / P.width;
           yo[a] = -P.lin + r % P.width;
           sum[a] = 0.f;
@@ -181,9 +186,11 @@ k_rt_match(const __grid_constant__ CUtensorMap tmap, const RtGridDev G, const Rt
             const double fy = __dsub_rn(__ddiv_rn(__dsub_rn(G.max_x, static_cast<double>(px)),
                                                   G.resolution), 0.5);
             const long long ix = llround(fx), iy = llround(fy);
-            // far-away points read "outside" for every candidate either way
-            const int cx = static_cast<int>(max(-30000LL, min(30000LL, ix)));
-            const int cy = static_cast<int>(max(-30000LL, min(30000LL, iy)));
+            // offsets are within +-lin, so a cell clamped to [-(lin + 1), n + lin] reads outside
+            // the grid at every offset, as the unclamped cell does; both bounds fit int16
+            // (n < 30000, lin < 2048) for the packing
+            const int cx = static_cast<int>(max(-(P.lin + 1LL), min(G.nx + static_cast<long long>(P.lin), ix)));
+            const int cy = static_cast<int>(max(-(P.lin + 1LL), min(G.ny + static_cast<long long>(P.lin), iy)));
             cell = (cy << 16) | (cx & 0xffff);
           }
           const int cnt = min(32, jb.n - p0);
@@ -216,6 +223,8 @@ k_rt_match(const __grid_constant__ CUtensorMap tmap, const RtGridDev G, const Rt
                 // ProbabilityGrid::GetProbability (2d/probability_grid.cc:78-82)
                 int value;
                 if (kForm == 0) {
+                  // 0 <= idx < bw * bh whenever `in`: x, y lie within lin of a point's cell,
+                  // and the job's box covers every such cell inside the grid (PrepareJob)
                   const int idx = in ? (y - tile_y0) * G.bw + (x - tile_x0) : 0;
                   value = s_tile[idx] & 0x7fff;
                 } else {
@@ -245,11 +254,20 @@ k_rt_match(const __grid_constant__ CUtensorMap tmap, const RtGridDev G, const Rt
           // candidate.score *= exp(...): float *= double                 (:170-174)
           score = __double2float_rn(__dmul_rn(static_cast<double>(score), w));
           const unsigned c_index = static_cast<unsigned>(k * P.per_scan + r);
-          // scores are >= 0, so their bit patterns order like the floats; ties go to the
-          // smaller generation index (std::max_element returns the first maximum)
+          if (kScores) scores[static_cast<size_t>(item) * P.per_scan + r] = score;
+          // ties go to the smaller generation index (std::max_element returns the first
+          // maximum).  ProbabilityGrid scores are > 0, so their bit patterns order like the
+          // floats.  TSDF scores can be negative: order-preserving bits, with -0.0 folded to
+          // +0.0 (the two compare equal); which zero won is kept in negz
+          unsigned bits;
+          if (kForm == 2) {
+            bits = FloatToOrdered(score == 0.f ? 0.f : score);
+            if (__float_as_uint(score) == 0x80000000u) atomicMin(&negz[j], c_index);
+          } else {
+            bits = __float_as_uint(fmaxf(score, 0.f));
+          }
           const unsigned long long kk =
-              (static_cast<unsigned long long>(__float_as_uint(fmaxf(score, 0.f))) << 32) |
-              (0xffffffffu - c_index);
+              (static_cast<unsigned long long>(bits) << 32) | (0xffffffffu - c_index);
           key = max(key, kk);
         }
 #pragma unroll
@@ -417,10 +435,11 @@ void ParallelFor(int n, int max_threads, F f) {
   for (auto& x : th) x.join();
 }
 
-// Runs jobs[0..num) against the grid on `ctx` (a lane).
+// Runs jobs[0..num) against the grid on `ctx` (a lane).  If `scores` (host) is not null it
+// receives every candidate's weighted score, job-major in generation order.
 csm_status RtRun(Ctx* ctx, const csm_rt_grid2d* grid, const RtHostJob* jobs, int num,
                  double linear_window, double angular_window, double w_t, double w_r,
-                 csm_rt_result2d* results, csm_stats* stats) {
+                 csm_rt_result2d* results, csm_stats* stats, float* scores) {
   CSM_CUDA(cudaSetDevice(ctx->device));
   cudaStream_t s = ctx->stream;
   const RtGridDev& G = grid->g;
@@ -461,10 +480,15 @@ csm_status RtRun(Ctx* ctx, const csm_rt_grid2d* grid, const RtHostJob* jobs, int
   DevBuf& d_up = ctx->D("rt_upload");
   DevBuf& d_best = ctx->D("rt_best");
   PinnedBuf& rb = ctx->P("rt_readback");
+  DevBuf& d_scores = ctx->D("rt_scores");
+  const bool tsdf = grid->d_wcells != nullptr;
+  // best keys, then (TSDF2D) the -0.0 indices
+  const size_t best_bytes = (sizeof(unsigned long long) + (tsdf ? sizeof(unsigned) : 0)) * num;
   CSM_TRY(up.Reserve(up_bytes));
   CSM_TRY(d_up.Reserve(up_bytes));
-  CSM_TRY(d_best.Reserve(sizeof(unsigned long long) * num));
-  CSM_TRY(rb.Reserve(sizeof(unsigned long long) * num));
+  CSM_TRY(d_best.Reserve(best_bytes));
+  CSM_TRY(rb.Reserve(best_bytes));
+  if (scores) CSM_TRY(d_scores.Reserve(sizeof(float) * static_cast<size_t>(cands)));
   char* h = up.as<char>();
   ParallelFor(num, 16, [&](int j) {
     PrepareJob(jobs[j], G, P, w_t, w_r, reinterpret_cast<float*>(h) + jd[j].xyz_off,
@@ -478,25 +502,32 @@ csm_status RtRun(Ctx* ctx, const csm_rt_grid2d* grid, const RtHostJob* jobs, int
   CSM_CUDA(cudaEventRecord(ctx->ev0, s));
   CSM_CUDA(cudaMemcpyAsync(d_up.p, h, up_bytes, cudaMemcpyHostToDevice, s));
   CSM_CUDA(cudaMemsetAsync(d_best.p, 0, sizeof(unsigned long long) * num, s));
+  unsigned* d_negz = tsdf ? reinterpret_cast<unsigned*>(d_best.as<unsigned long long>() + num) : nullptr;
+  if (tsdf) CSM_CUDA(cudaMemsetAsync(d_negz, 0xff, sizeof(unsigned) * num, s));
   const char* d = d_up.as<char>();
   const int total_items = static_cast<int>(items);
-  const int form = grid->d_wcells ? 2 : (all_smem ? 0 : 1);
+  const int form = tsdf ? 2 : (all_smem ? 0 : 1);
   const size_t smem = form == 0 ? static_cast<size_t>(G.bw) * G.bh * 2 : 0;
   int per_sm = 1;
-#define CSM_RT_LAUNCH(F, A)                                                                     \
+#define CSM_RT_LAUNCH_K(F, A, S)                                                                \
   do {                                                                                          \
     if (smem > 48 * 1024)                                                                       \
-      CSM_CUDA(cudaFuncSetAttribute(k_rt_match<F, A>,                                           \
+      CSM_CUDA(cudaFuncSetAttribute(k_rt_match<F, A, S>,                                        \
                                     cudaFuncAttributeMaxDynamicSharedMemorySize,                \
                                     static_cast<int>(smem)));                                   \
-    CSM_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_rt_match<F, A>,           \
+    CSM_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_rt_match<F, A, S>,        \
                                                            kRtThreads, smem));                  \
     const int grid_dim = std::max(1, std::min((total_items + kRtWarps - 1) / kRtWarps,          \
                                               ctx->sm_count * std::max(1, per_sm)));            \
-    k_rt_match<F, A><<<grid_dim, kRtThreads, smem, s>>>(                                        \
+    k_rt_match<F, A, S><<<grid_dim, kRtThreads, smem, s>>>(                                     \
         grid->tmap, G, P, reinterpret_cast<const RtJobDev*>(d + off_jobs), num, total_items,    \
         reinterpret_cast<const float*>(d), reinterpret_cast<const float2*>(d + off_trig),       \
-        reinterpret_cast<const double*>(d + off_w), d_best.as<unsigned long long>());           \
+        reinterpret_cast<const double*>(d + off_w), d_best.as<unsigned long long>(), d_negz,    \
+        d_scores.as<float>());                                                                  \
+  } while (0)
+#define CSM_RT_LAUNCH(F, A)                                                                     \
+  do {                                                                                          \
+    if (scores) CSM_RT_LAUNCH_K(F, A, true); else CSM_RT_LAUNCH_K(F, A, false);                 \
   } while (0)
   ProfBegin(ctx);
   const bool one_acc = P.per_scan <= 32;
@@ -504,19 +535,29 @@ csm_status RtRun(Ctx* ctx, const csm_rt_grid2d* grid, const RtHostJob* jobs, int
   else if (form == 1) { if (one_acc) CSM_RT_LAUNCH(1, 1); else CSM_RT_LAUNCH(1, 4); }
   else { if (one_acc) CSM_RT_LAUNCH(2, 1); else CSM_RT_LAUNCH(2, 4); }
 #undef CSM_RT_LAUNCH
+#undef CSM_RT_LAUNCH_K
   CSM_LAUNCH_CHECK();
   ProfEnd(ctx, form == 0 ? "k_rt_match_tma" : (form == 1 ? "k_rt_match_gather" : "k_rt_match_tsdf"),
           static_cast<double>(cands));
   CSM_CUDA(cudaEventRecord(ctx->ev1, s));
-  CSM_CUDA(cudaMemcpyAsync(rb.p, d_best.p, sizeof(unsigned long long) * num,
-                           cudaMemcpyDeviceToHost, s));
+  CSM_CUDA(cudaMemcpyAsync(rb.p, d_best.p, best_bytes, cudaMemcpyDeviceToHost, s));
+  if (scores)
+    CSM_CUDA(cudaMemcpyAsync(scores, d_scores.p, sizeof(float) * static_cast<size_t>(cands),
+                             cudaMemcpyDeviceToHost, s));
   CSM_CUDA(cudaStreamSynchronize(s));
   const unsigned long long* keys = rb.as<unsigned long long>();
+  const unsigned* negz = reinterpret_cast<const unsigned*>(keys + num);
   for (int j = 0; j < num; ++j) {
     const unsigned bits = static_cast<unsigned>(keys[j] >> 32);
     const unsigned best = 0xffffffffu - static_cast<unsigned>(keys[j] & 0xffffffffu);
     float best_score;
-    std::memcpy(&best_score, &bits, 4);
+    if (tsdf) {
+      best_score = OrderedToFloat(bits);
+      // the first of the zero scores won; its sign is not in the key
+      if (best_score == 0.f && negz[j] == best) best_score = -0.f;
+    } else {
+      std::memcpy(&best_score, &bits, 4);
+    }
     const int scan = static_cast<int>(best / P.per_scan);
     const int r = static_cast<int>(best % P.per_scan);
     const int xo = -lin + r / P.width, yo = -lin + r % P.width;
@@ -599,20 +640,17 @@ csm_status RtMatchHostGrid(const uint16_t* cells, const uint16_t* weight_cells, 
   csm_rt_result2d r;
   std::memset(&r, 0, sizeof(r));
   if (stats) std::memset(stats, 0, sizeof(*stats));
-  CSM_TRY(RtRun(lane, grid, &job, 1, linear_window, angular_window, w_t, w_r, &r, stats));
+  CSM_TRY(RtRun(lane, grid, &job, 1, linear_window, angular_window, w_t, w_r, &r, stats,
+                nullptr));
   *score = r.score;
   std::memcpy(pose_estimate, r.pose_estimate, sizeof(double) * 3);
   return CSM_OK;
 }
 
-}  // namespace
-
-extern "C" {
-
-csm_status csm_rt_match2d_batch(const csm_rt_grid2d* grid, const csm_rt_job2d* jobs,
-                                int32_t num_jobs, double linear_window, double angular_window,
-                                double w_t, double w_r, csm_rt_result2d* results,
-                                csm_stats* stats) {
+// csm_rt_match2d_batch; scores (may be null) as in RtRun, over all jobs.
+csm_status RtBatch(const csm_rt_grid2d* grid, const csm_rt_job2d* jobs, int32_t num_jobs,
+                   double linear_window, double angular_window, double w_t, double w_r,
+                   csm_rt_result2d* results, csm_stats* stats, float* scores) {
   CSM_REQUIRE(grid && jobs && results, "null pointer");
   CSM_REQUIRE(num_jobs >= 1, "empty batch");
   for (int j = 0; j < num_jobs; ++j)
@@ -630,9 +668,30 @@ csm_status csm_rt_match2d_batch(const csm_rt_grid2d* grid, const csm_rt_job2d* j
                         {jobs[j0 + j].initial_pose[0], jobs[j0 + j].initial_pose[1],
                          jobs[j0 + j].initial_pose[2]}};
     CSM_TRY(RtRun(guard.lane, grid, hj.data(), cnt, linear_window, angular_window, w_t, w_r,
-                  results + j0, stats));
+                  results + j0, stats, scores));
+    if (scores)
+      for (int j = 0; j < cnt; ++j) scores += results[j0 + j].candidates_scored;
   }
   return CSM_OK;
+}
+
+}  // namespace
+
+extern "C" {
+
+csm_status csm_rt_match2d_batch(const csm_rt_grid2d* grid, const csm_rt_job2d* jobs,
+                                int32_t num_jobs, double linear_window, double angular_window,
+                                double w_t, double w_r, csm_rt_result2d* results,
+                                csm_stats* stats) {
+  return RtBatch(grid, jobs, num_jobs, linear_window, angular_window, w_t, w_r, results, stats,
+                 nullptr);
+}
+
+csm_status csm_rt_scores2d(const csm_rt_grid2d* grid, const csm_rt_job2d* jobs,
+                           int32_t num_jobs, double linear_window, double angular_window,
+                           double w_t, double w_r, csm_rt_result2d* results, float* scores) {
+  return RtBatch(grid, jobs, num_jobs, linear_window, angular_window, w_t, w_r, results, nullptr,
+                 scores);
 }
 
 csm_status csm_rt_match2d(const uint16_t* cells, int32_t nx, int32_t ny, double resolution,

@@ -41,12 +41,15 @@ __global__ void k_rt3_scatter(const int* __restrict__ idx, const uint16_t* __res
 
 constexpr int kRt3Chunk = 256;
 
+// kScores: also store every candidate's weighted score at scores[t * R + r] (test hook
+// csm_rt_scores3d).
+template <bool kScores>
 __global__ void __launch_bounds__(128)
 k_rt3_match(const Grid3Dev G, const Rt3Params P, const float* __restrict__ xyz,
             const float4* __restrict__ rot /* candidate rotation per r: w, x, y, z */,
             const float4* __restrict__ trans /* candidate translation per t: x, y, z, weight class */,
             const double* __restrict__ weights /* [class][r] */,
-            unsigned long long* __restrict__ best) {
+            unsigned long long* __restrict__ best, float* __restrict__ scores) {
   __shared__ float s_x[kRt3Chunk], s_y[kRt3Chunk], s_z[kRt3Chunk];
   __shared__ unsigned long long s_best;
   const int r = blockIdx.x;
@@ -94,6 +97,7 @@ k_rt3_match(const Grid3Dev G, const Rt3Params P, const float* __restrict__ xyz,
       const double w = weights[static_cast<size_t>(__float_as_int(tc.w)) * P.R + r];
       score = __double2float_rn(__dmul_rn(static_cast<double>(score), w));  // float *= double (:109)
       const unsigned c = static_cast<unsigned>(t) * static_cast<unsigned>(P.R) + static_cast<unsigned>(r);
+      if (kScores) scores[c] = score;
       const unsigned long long key =
           (static_cast<unsigned long long>(__float_as_uint(fmaxf(score, 0.f))) << 32) |
           (0xffffffffu - c);
@@ -178,10 +182,16 @@ csm_status csm_grid3d_destroy(csm_grid3d* grid) {
   return CSM_OK;
 }
 
-csm_status csm_rt_match3d(const csm_grid3d* grid, const float* xyz, int32_t n,
-                          const double initial_pose[7], double linear_window,
-                          double angular_window, double w_t, double w_r, float* score,
-                          double pose_estimate[7], csm_stats* stats) {
+}  // extern "C"
+
+namespace {
+
+// csm_rt_match3d.  With num_candidates not null (csm_rt_scores3d) it receives T * R, and if
+// `scores` is not null too, every candidate's weighted score in generation order.
+csm_status Rt3Run(const csm_grid3d* grid, const float* xyz, int32_t n,
+                  const double initial_pose[7], double linear_window, double angular_window,
+                  double w_t, double w_r, float* score, double pose_estimate[7],
+                  csm_stats* stats, float* scores, int64_t* num_candidates) {
   CSM_REQUIRE(grid && xyz && initial_pose && score && pose_estimate, "null pointer");  // :38
   CSM_REQUIRE(n >= 1, "empty point cloud");
   LaneGuard guard;
@@ -207,6 +217,10 @@ csm_status csm_rt_match3d(const csm_grid3d* grid, const float* xyz, int32_t n,
   const int W = 2 * L + 1, Rw = 2 * A + 1;
   const long long T = static_cast<long long>(W) * W * W, R = static_cast<long long>(Rw) * Rw * Rw;
   CSM_REQUIRE(T * R < (1LL << 31), "search window too large");
+  if (num_candidates) {
+    *num_candidates = T * R;
+    if (!scores) return CSM_OK;
+  }
   // initial_pose_estimate.cast<float>()
   const Rigid3f init{
       Vec3f{static_cast<float>(initial_pose[0]), static_cast<float>(initial_pose[1]),
@@ -273,6 +287,8 @@ csm_status csm_rt_match3d(const csm_grid3d* grid, const float* xyz, int32_t n,
   CSM_TRY(d_up.Reserve(bytes));
   CSM_TRY(d_best.Reserve(8));
   CSM_TRY(rb.Reserve(8));
+  DevBuf& d_scores = ctx->D("rt3_scores");
+  if (scores) CSM_TRY(d_scores.Reserve(sizeof(float) * static_cast<size_t>(T * R)));
   char* h = up.as<char>();
   std::memcpy(h, xyz, static_cast<size_t>(n) * 12);
   for (long long r = 0; r < R; ++r)
@@ -288,14 +304,23 @@ csm_status csm_rt_match3d(const csm_grid3d* grid, const float* xyz, int32_t n,
   P.R = static_cast<int>(R);
   const char* d = d_up.as<char>();
   ProfBegin(ctx);
-  k_rt3_match<<<static_cast<int>(R), 128, 0, s>>>(
-      grid->g, P, reinterpret_cast<const float*>(d), reinterpret_cast<const float4*>(d + o_rot),
-      reinterpret_cast<const float4*>(d + o_tr), reinterpret_cast<const double*>(d + o_w),
-      d_best.as<unsigned long long>());
+  if (scores)
+    k_rt3_match<true><<<static_cast<int>(R), 128, 0, s>>>(
+        grid->g, P, reinterpret_cast<const float*>(d), reinterpret_cast<const float4*>(d + o_rot),
+        reinterpret_cast<const float4*>(d + o_tr), reinterpret_cast<const double*>(d + o_w),
+        d_best.as<unsigned long long>(), d_scores.as<float>());
+  else
+    k_rt3_match<false><<<static_cast<int>(R), 128, 0, s>>>(
+        grid->g, P, reinterpret_cast<const float*>(d), reinterpret_cast<const float4*>(d + o_rot),
+        reinterpret_cast<const float4*>(d + o_tr), reinterpret_cast<const double*>(d + o_w),
+        d_best.as<unsigned long long>(), nullptr);
   CSM_LAUNCH_CHECK();
   ProfEnd(ctx, "k_rt3_match", static_cast<double>(T * R));
   CSM_CUDA(cudaEventRecord(ctx->ev1, s));
   CSM_CUDA(cudaMemcpyAsync(rb.p, d_best.p, 8, cudaMemcpyDeviceToHost, s));
+  if (scores)
+    CSM_CUDA(cudaMemcpyAsync(scores, d_scores.p, sizeof(float) * static_cast<size_t>(T * R),
+                             cudaMemcpyDeviceToHost, s));
   CSM_CUDA(cudaStreamSynchronize(s));
   const unsigned long long key = *rb.as<unsigned long long>();
   const unsigned bits = static_cast<unsigned>(key >> 32);
@@ -324,6 +349,29 @@ csm_status csm_rt_match3d(const csm_grid3d* grid, const float* xyz, int32_t n,
     cudaEventElapsedTime(&stats->device_ms, ctx->ev0, ctx->ev1);
   }
   return CSM_OK;
+}
+
+}  // namespace
+
+extern "C" {
+
+csm_status csm_rt_match3d(const csm_grid3d* grid, const float* xyz, int32_t n,
+                          const double initial_pose[7], double linear_window,
+                          double angular_window, double w_t, double w_r, float* score,
+                          double pose_estimate[7], csm_stats* stats) {
+  return Rt3Run(grid, xyz, n, initial_pose, linear_window, angular_window, w_t, w_r, score,
+                pose_estimate, stats, nullptr, nullptr);
+}
+
+csm_status csm_rt_scores3d(const csm_grid3d* grid, const float* xyz, int32_t n,
+                           const double initial_pose[7], double linear_window,
+                           double angular_window, double w_t, double w_r, float* scores,
+                           int64_t* num_candidates) {
+  CSM_REQUIRE(num_candidates, "null pointer");
+  float score = 0.f;
+  double pose[7];
+  return Rt3Run(grid, xyz, n, initial_pose, linear_window, angular_window, w_t, w_r, &score,
+                pose, nullptr, scores, num_candidates);
 }
 
 }  // extern "C"

@@ -643,6 +643,30 @@ def _rt_match_batch(self, initial_pose_estimates, point_clouds, rt_grid):
     return scores, poses, self.last_stats
 
 
+def _rt_scores_batch(self, initial_pose_estimates, point_clouds, rt_grid):
+    """Test hook csm_rt_scores2d: MatchBatch run exactly, plus every candidate's weighted score.
+    Returns (results, scores): results as MatchBatch's last_results, scores[j] job j's float32
+    scores in generation order (scan, x offset, y offset)."""
+    n = len(point_clouds)
+    clouds = [_f32(c) for c in point_clouds]
+    jobs = (CsmRtJob2D * n)()
+    for j in range(n):
+        jobs[j].xyz = ptr(clouds[j], C.c_float)
+        jobs[j].num_points = len(clouds[j])
+        for k in range(3):
+            jobs[j].initial_pose[k] = float(initial_pose_estimates[j][k])
+    res = (CsmRtResult2D * n)()
+    o = self.options
+    args = (rt_grid._h, jobs, C.c_int32(n), C.c_double(o.linear_search_window),
+            C.c_double(o.angular_search_window), C.c_double(o.translation_delta_cost_weight),
+            C.c_double(o.rotation_delta_cost_weight), res)
+    check(lib().csm_rt_scores2d(*args, None))
+    counts = [r.candidates_scored for r in res]
+    flat = np.empty(sum(counts), np.float32)
+    check(lib().csm_rt_scores2d(*args, ptr(flat, C.c_float)))
+    return res, np.split(flat, np.cumsum(counts)[:-1])
+
+
 def _rt_score_candidates(self, grid, discrete_scans, num_angular_perturbations,
                          angular_perturbation_step_size, candidates):
     """RealTimeCorrelativeScanMatcher2D::ScoreCandidates (public in the reference,
@@ -664,6 +688,7 @@ def _rt_score_candidates(self, grid, discrete_scans, num_angular_perturbations,
 
 
 RealTimeCorrelativeScanMatcher2D.MatchBatch = _rt_match_batch
+RealTimeCorrelativeScanMatcher2D.ScoresBatch = _rt_scores_batch
 RealTimeCorrelativeScanMatcher2D.ScoreCandidates = _rt_score_candidates
 
 
@@ -1248,6 +1273,22 @@ class RealTimeCorrelativeScanMatcher3D:
             C.byref(stats)))
         self.last_stats = stats.as_dict()
         return np.float32(score.value), pose
+
+    def Scores(self, initial_pose_estimate, point_cloud, hybrid_grid):
+        """Test hook csm_rt_scores3d: every candidate's weighted score of Match, float32 in
+        generation order (translations z, y, x, then rotations rz, ry, rx)."""
+        xyz = _f32(point_cloud)
+        ip = np.ascontiguousarray(initial_pose_estimate, dtype=np.float64)
+        o = self.options
+        count = C.c_int64(0)
+        args = (hybrid_grid._h, ptr(xyz, C.c_float), C.c_int32(len(xyz)), ptr(ip, C.c_double),
+                C.c_double(o.linear_search_window), C.c_double(o.angular_search_window),
+                C.c_double(o.translation_delta_cost_weight),
+                C.c_double(o.rotation_delta_cost_weight))
+        check(lib().csm_rt_scores3d(*args, None, C.byref(count)))
+        scores = np.empty(count.value, np.float32)
+        check(lib().csm_rt_scores3d(*args, ptr(scores, C.c_float), C.byref(count)))
+        return scores
 
 
 # ===========================================================================

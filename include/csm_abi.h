@@ -301,6 +301,16 @@ csm_status csm_rt_match2d_batch(const csm_rt_grid2d* grid, const csm_rt_job2d* j
                                 double rotation_delta_cost_weight, csm_rt_result2d* results,
                                 csm_stats* stats /* may be NULL */);
 
+/* Test hook: csm_rt_match2d_batch run exactly (same planning, kernel form and launches), and
+ * every candidate's final weighted score: job-major, then scan, x offset, y offset
+ * (generation order, real_time_correlative_scan_matcher_2d.cc:83-115); job j has
+ * results[j].candidates_scored of them.  Call with scores == NULL to get the sizes first. */
+csm_status csm_rt_scores2d(const csm_rt_grid2d* grid, const csm_rt_job2d* jobs, int32_t num_jobs,
+                           double linear_search_window, double angular_search_window,
+                           double translation_delta_cost_weight,
+                           double rotation_delta_cost_weight, csm_rt_result2d* results,
+                           float* scores);
+
 /* RealTimeCorrelativeScanMatcher2D::ScoreCandidates — public in the reference
  * (real_time_correlative_scan_matcher_2d.h:75, .cc:151-176): scores caller-supplied
  * candidates {scan_index, x_index_offset, y_index_offset} against caller-supplied
@@ -571,6 +581,14 @@ csm_status csm_rt_match3d(const csm_grid3d* grid, const float* xyz, int32_t num_
                           double angular_search_window, double translation_delta_cost_weight,
                           double rotation_delta_cost_weight, float* score,
                           double pose_estimate[7], csm_stats* stats /* may be NULL */);
+/* Test hook: the same match run by its own launch code; *num_candidates = T * R, and unless
+ * scores is NULL (sizes only) scores receives every candidate's weighted score in generation
+ * order (translations z, y, x outermost, then rotations rz, ry, rx; :55-98). */
+csm_status csm_rt_scores3d(const csm_grid3d* grid, const float* xyz, int32_t num_points,
+                           const double initial_pose[7], double linear_search_window,
+                           double angular_search_window, double translation_delta_cost_weight,
+                           double rotation_delta_cost_weight, float* scores,
+                           int64_t* num_candidates);
 
 /* ---- post-match refinement in 3D: CeresScanMatcher3D --------------------------- */
 /* ConstraintBuilder3D refines every found match with CeresScanMatcher3D::Match

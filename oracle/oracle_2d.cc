@@ -412,7 +412,8 @@ double RealTimeCorrelativeScanMatcher2D::Match(const Rigid2d& initial_pose_estim
                                                const PointCloud& point_cloud,
                                                const ProbabilityGrid& grid,
                                                Rigid2d* pose_estimate,
-                                               MatchStats* stats) const {
+                                               MatchStats* stats,
+                                               std::vector<float>* scores) const {
   const double initial_rotation = initial_pose_estimate.theta;
   const PointCloud rotated_point_cloud =
       TransformPointCloudRotZ(point_cloud, static_cast<float>(initial_rotation));
@@ -427,6 +428,8 @@ double RealTimeCorrelativeScanMatcher2D::Match(const Rigid2d& initial_pose_estim
                       static_cast<float>(initial_pose_estimate.y));
   std::vector<Candidate2D> candidates = GenerateExhaustiveSearchCandidates(search_parameters);
   ScoreCandidates(grid, discrete_scans, search_parameters, &candidates);
+  if (scores)
+    for (const Candidate2D& c : candidates) scores->push_back(c.score);
   const Candidate2D& best_candidate =
       *std::max_element(candidates.begin(), candidates.end());
   *pose_estimate = Rigid2d{initial_pose_estimate.x + best_candidate.x,
@@ -511,7 +514,8 @@ void RealTimeCorrelativeScanMatcher2D::ScoreCandidates(
 
 double RealTimeCorrelativeScanMatcher2D::Match(const Rigid2d& initial_pose_estimate,
                                                const PointCloud& point_cloud, const TSDF2D& grid,
-                                               Rigid2d* pose_estimate, MatchStats* stats) const {
+                                               Rigid2d* pose_estimate, MatchStats* stats,
+                                               std::vector<float>* scores) const {
   const double initial_rotation = initial_pose_estimate.theta;
   const PointCloud rotated_point_cloud =
       TransformPointCloudRotZ(point_cloud, static_cast<float>(initial_rotation));
@@ -525,6 +529,8 @@ double RealTimeCorrelativeScanMatcher2D::Match(const Rigid2d& initial_pose_estim
                       static_cast<float>(initial_pose_estimate.y));
   std::vector<Candidate2D> candidates = GenerateExhaustiveSearchCandidates(search_parameters);
   ScoreCandidates(grid, discrete_scans, search_parameters, &candidates);
+  if (scores)
+    for (const Candidate2D& c : candidates) scores->push_back(c.score);
   const Candidate2D& best_candidate = *std::max_element(candidates.begin(), candidates.end());
   *pose_estimate = Rigid2d{initial_pose_estimate.x + best_candidate.x,
                            initial_pose_estimate.y + best_candidate.y,

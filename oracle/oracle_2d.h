@@ -258,16 +258,19 @@ class RealTimeCorrelativeScanMatcher2D {  // real_time...2d.h:53-85, .cc:77-176
  public:
   explicit RealTimeCorrelativeScanMatcher2D(const RealTimeOptions& options)
       : options_(options) {}
+  // `scores` (for the tests) receives every candidate's score in generation order, as
+  // max_element sees them
   double Match(const Rigid2d& initial_pose_estimate, const PointCloud& point_cloud,
                const ProbabilityGrid& grid, Rigid2d* pose_estimate,
-               MatchStats* stats = nullptr) const;
+               MatchStats* stats = nullptr, std::vector<float>* scores = nullptr) const;
   void ScoreCandidates(const ProbabilityGrid& grid,
                        const std::vector<DiscreteScan2D>& discrete_scans,
                        const SearchParameters& search_parameters,
                        std::vector<Candidate2D>* candidates) const;
   // TSDF grid type (real_time_correlative_scan_matcher_2d.cc:38-59, 160-166)
   double Match(const Rigid2d& initial_pose_estimate, const PointCloud& point_cloud,
-               const TSDF2D& grid, Rigid2d* pose_estimate, MatchStats* stats = nullptr) const;
+               const TSDF2D& grid, Rigid2d* pose_estimate, MatchStats* stats = nullptr,
+               std::vector<float>* scores = nullptr) const;
   void ScoreCandidates(const TSDF2D& grid, const std::vector<DiscreteScan2D>& discrete_scans,
                        const SearchParameters& search_parameters,
                        std::vector<Candidate2D>* candidates) const;

@@ -679,7 +679,8 @@ float RealTimeCorrelativeScanMatcher3D::Match(const Rigid3d& initial_pose_estima
                                               const PointCloud& point_cloud,
                                               const HybridGrid& hybrid_grid,
                                               Rigid3d* pose_estimate, int64_t* num_candidates,
-                                              int64_t* best_index) const {
+                                              int64_t* best_index,
+                                              std::vector<float>* scores) const {
   float best_score = -1.f;
   // initial_pose_estimate.cast<float>()
   const Rigid3f initial{
@@ -699,6 +700,7 @@ float RealTimeCorrelativeScanMatcher3D::Match(const Rigid3d& initial_pose_estima
     for (size_t i = 0; i < point_cloud.size(); ++i)   // sensor::TransformPointCloud
       transformed[i] = Rigid3Apply(candidate, point_cloud[i]);
     const float score = ScoreCandidate(hybrid_grid, transformed, transform);
+    if (scores) scores->push_back(score);
     if (score > best_score) {
       best_score = score;
       *pose_estimate = Rigid3d{Vec3d{candidate.t.x, candidate.t.y, candidate.t.z},

@@ -240,10 +240,12 @@ class RealTimeCorrelativeScanMatcher3D {  // real_time_correlative_scan_matcher_
  public:
   explicit RealTimeCorrelativeScanMatcher3D(const RealTimeOptions3D& options)
       : options_(options) {}
-  // .cc:34-53; num_candidates / best_index (generation order) are reported for the tests
+  // .cc:34-53; num_candidates / best_index (generation order) and every candidate's score in
+  // generation order are reported for the tests
   float Match(const Rigid3d& initial_pose_estimate, const PointCloud& point_cloud,
               const HybridGrid& hybrid_grid, Rigid3d* pose_estimate,
-              int64_t* num_candidates = nullptr, int64_t* best_index = nullptr) const;
+              int64_t* num_candidates = nullptr, int64_t* best_index = nullptr,
+              std::vector<float>* scores = nullptr) const;
   std::vector<Rigid3f> GenerateExhaustiveSearchTransforms(float resolution,
                                                           const PointCloud& point_cloud) const;
   float ScoreCandidate(const HybridGrid& hybrid_grid, const PointCloud& transformed_point_cloud,

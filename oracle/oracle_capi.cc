@@ -288,6 +288,42 @@ double orc_rt2d_match_tsdf(const uint16_t* tsd, const uint16_t* weight, int nx, 
   FillStats(stats, stats_out);
   return score;
 }
+// Every candidate's score of the same matches, in generation order, as max_element sees them:
+// the first min(cap, count) are written to `scores`; returns the count.
+int64_t orc_rt2d_scores(const uint16_t* cells, int nx, int ny, double res, double max_x,
+                        double max_y, const float* xyz, int n, const double* init_pose,
+                        double lin, double ang, double w_t, double w_r, float* scores,
+                        int64_t cap) {
+  const ProbabilityGrid grid =
+      MakeGrid(cells, nx, ny, res, max_x, max_y, kMinCorrespondenceCost, kMaxCorrespondenceCost);
+  const RealTimeCorrelativeScanMatcher2D matcher(RealTimeOptions{lin, ang, w_t, w_r});
+  Rigid2d pose{0, 0, 0};
+  std::vector<float> all;
+  matcher.Match(Rigid2d{init_pose[0], init_pose[1], init_pose[2]}, MakeCloud(xyz, n), grid,
+                &pose, nullptr, &all);
+  const int64_t count = static_cast<int64_t>(all.size());
+  if (scores) std::memcpy(scores, all.data(), sizeof(float) * std::min(cap, count));
+  return count;
+}
+
+int64_t orc_rt2d_scores_tsdf(const uint16_t* tsd, const uint16_t* weight, int nx, int ny,
+                             double res, double max_x, double max_y, float truncation,
+                             float max_weight, const float* xyz, int n, const double* init_pose,
+                             double lin, double ang, double w_t, double w_r, float* scores,
+                             int64_t cap) {
+  TSDF2D grid(MapLimits{res, max_x, max_y, CellLimits{nx, ny}}, truncation, max_weight);
+  std::memcpy(grid.tsd_cells.data(), tsd, sizeof(uint16_t) * size_t(nx) * ny);
+  std::memcpy(grid.weight_cells.data(), weight, sizeof(uint16_t) * size_t(nx) * ny);
+  const RealTimeCorrelativeScanMatcher2D matcher(RealTimeOptions{lin, ang, w_t, w_r});
+  Rigid2d pose{0, 0, 0};
+  std::vector<float> all;
+  matcher.Match(Rigid2d{init_pose[0], init_pose[1], init_pose[2]}, MakeCloud(xyz, n), grid,
+                &pose, nullptr, &all);
+  const int64_t count = static_cast<int64_t>(all.size());
+  if (scores) std::memcpy(scores, all.data(), sizeof(float) * std::min(cap, count));
+  return count;
+}
+
 void orc_tsdf_values(float truncation, float max_weight, float tsd, float w, uint16_t* out2) {
   const TSDF2D g(MapLimits{1., 0., 0., CellLimits{1, 1}}, truncation, max_weight);
   out2[0] = g.TSDToValue(tsd);
@@ -407,6 +443,21 @@ float orc_rt3d_match(void* hybrid, const float* xyz, int n, const double* initia
   pose_out[3] = pose.q.w; pose_out[4] = pose.q.x; pose_out[5] = pose.q.y; pose_out[6] = pose.q.z;
   if (stats_out) { stats_out[0] = num; stats_out[1] = best; }
   return score;
+}
+
+// Every candidate's score of the same match in generation order (translations z, y, x, then
+// rotations rz, ry, rx): the first min(cap, count) are written to `scores`; returns the count.
+int64_t orc_rt3d_scores(void* hybrid, const float* xyz, int n, const double* initial_pose,
+                        double lin, double ang, double w_t, double w_r, float* scores,
+                        int64_t cap) {
+  const HybridGrid* g = static_cast<HybridGrid*>(hybrid);
+  const RealTimeCorrelativeScanMatcher3D matcher(RealTimeOptions3D{lin, ang, w_t, w_r});
+  Rigid3d pose{Vec3d{0., 0., 0.}, Quatd{1., 0., 0., 0.}};
+  std::vector<float> all;
+  matcher.Match(MakeRigid3d(initial_pose), MakeCloud(xyz, n), *g, &pose, nullptr, nullptr, &all);
+  const int64_t count = static_cast<int64_t>(all.size());
+  if (scores) std::memcpy(scores, all.data(), sizeof(float) * std::min(cap, count));
+  return count;
 }
 
 void* orc_fast3d_create(void* hi, void* lo, const float* hist, int hist_n, int bb_depth,

@@ -47,6 +47,9 @@ def lib():
         _lib.orc_hybrid_create.restype = C.c_void_p
         _lib.orc_hybrid_get_probability.restype = C.c_float
         _lib.orc_rt3d_match.restype = C.c_float
+        _lib.orc_rt2d_scores.restype = C.c_int64
+        _lib.orc_rt2d_scores_tsdf.restype = C.c_int64
+        _lib.orc_rt3d_scores.restype = C.c_int64
     return _lib
 
 
@@ -271,6 +274,40 @@ def rt2d_match_tsdf(tsd_cells, weight_cells, resolution, max_x, max_y, truncatio
                 **{k: int(stats[i]) for i, k in enumerate(STAT_KEYS)})
 
 
+def _sized(call):
+    """call(scores_ptr, cap) -> count: count first, then the scores (float32)."""
+    n = call(None, C.c_int64(0))
+    out = np.empty(n, np.float32)
+    call(_p(out, C.c_float), C.c_int64(n))
+    return out
+
+
+def rt2d_scores(grid, xyz, init_pose, lin, ang, w_t, w_r):
+    """Every candidate's score of rt2d_match's Match, in generation order (scan, x offset,
+    y offset), as std::max_element sees them."""
+    xyz = _f32(xyz)
+    ip = np.ascontiguousarray(init_pose, dtype=np.float64)
+    return _sized(lambda out, cap: lib().orc_rt2d_scores(
+        _p(grid.cells, C.c_uint16), C.c_int(grid.num_x), C.c_int(grid.num_y),
+        C.c_double(grid.resolution), C.c_double(grid.max_x), C.c_double(grid.max_y),
+        _p(xyz, C.c_float), C.c_int(len(xyz)), _p(ip, C.c_double), C.c_double(lin),
+        C.c_double(ang), C.c_double(w_t), C.c_double(w_r), out, cap))
+
+
+def rt2d_scores_tsdf(tsd_cells, weight_cells, resolution, max_x, max_y, truncation, max_weight,
+                     xyz, init_pose, lin, ang, w_t, w_r):
+    """As rt2d_scores, for rt2d_match_tsdf's Match."""
+    tsd, wgt = _u16(tsd_cells), _u16(weight_cells)
+    ny, nx = tsd.shape
+    xyz = _f32(xyz)
+    ip = np.ascontiguousarray(init_pose, dtype=np.float64)
+    return _sized(lambda out, cap: lib().orc_rt2d_scores_tsdf(
+        _p(tsd, C.c_uint16), _p(wgt, C.c_uint16), C.c_int(nx), C.c_int(ny), C.c_double(resolution),
+        C.c_double(max_x), C.c_double(max_y), C.c_float(truncation), C.c_float(max_weight),
+        _p(xyz, C.c_float), C.c_int(len(xyz)), _p(ip, C.c_double), C.c_double(lin),
+        C.c_double(ang), C.c_double(w_t), C.c_double(w_r), out, cap))
+
+
 def rt2d_score_candidates(grid, discrete_scans, num_lin, num_ang, step, w_t, w_r, cand):
     ds = _i32(discrete_scans)
     cand = _i32(cand)
@@ -475,6 +512,16 @@ def rt3d_match(hybrid_grid, xyz, initial_pose, lin, ang, w_t, w_r):
                                  _p(stats, C.c_int64))
     return dict(score=np.float32(score), pose=pose, candidates_scored=int(stats[0]),
                 best_index=int(stats[1]))
+
+
+def rt3d_scores(hybrid_grid, xyz, initial_pose, lin, ang, w_t, w_r):
+    """Every candidate's score of rt3d_match's Match, in generation order (translations z, y,
+    x, then rotations rz, ry, rx), as its `score > best_score` loop sees them."""
+    xyz = _f32(xyz)
+    ip = np.ascontiguousarray(initial_pose, dtype=np.float64)
+    return _sized(lambda out, cap: lib().orc_rt3d_scores(
+        hybrid_grid._h, _p(xyz, C.c_float), C.c_int(len(xyz)), _p(ip, C.c_double),
+        C.c_double(lin), C.c_double(ang), C.c_double(w_t), C.c_double(w_r), out, cap))
 
 
 # ---- CeresScanMatcher2D restatement (oracle_ceres2d.h; parity unpinned against Ceres) ----
