@@ -6,6 +6,7 @@
 #include <cuda_runtime.h>
 
 #include <atomic>
+#include <cmath>
 #include <cstdarg>
 #include <cstdint>
 #include <cstdio>
@@ -177,6 +178,15 @@ void ProfCommit(Ctx* ctx, const char* name, double units);  // waits for it and 
 inline void ProfEnd(Ctx* ctx, const char* name, double units) {
   ProfStop(ctx);
   ProfCommit(ctx, name, units);
+}
+
+// Whether p[0 .. n) holds no NaN and no infinity: the check every entry point makes on
+// coordinates that come from outside before they reach a float -> int conversion.
+template <typename T>
+inline bool Finite(const T* p, size_t n) {
+  for (size_t i = 0; i < n; ++i)
+    if (!std::isfinite(p[i])) return false;
+  return true;
 }
 
 }  // namespace csm

@@ -80,15 +80,6 @@ __global__ void k_ins2_finish(const int* __restrict__ hit_flat, int n,
 
 using namespace csm;
 
-namespace {
-
-bool Finite(const float* p, size_t n) {
-  for (size_t i = 0; i < n; ++i)
-    if (!std::isfinite(p[i])) return false;
-  return true;
-}
-
-}  // namespace
 
 extern "C" {
 

@@ -169,12 +169,6 @@ namespace {
 
 struct P3 { float x, y, z; };
 
-bool Finite(const float* p, size_t n) {
-  for (size_t i = 0; i < n; ++i)
-    if (!std::isfinite(p[i])) return false;
-  return true;
-}
-
 // Eigen's norm() / normalized() of float vectors: the squares summed in index order, one sqrt,
 // a division per component.
 float Norm2(float x, float y) { return std::sqrt(x * x + y * y); }

@@ -571,6 +571,10 @@ csm_status csm_ceres_match2d_batch(const csm_ceres_job2d* jobs, int32_t num_jobs
     CSM_REQUIRE(jobs[j].grid != nullptr && jobs[j].xyz != nullptr, "null pointer");
     CSM_REQUIRE(jobs[j].num_points >= 1, "empty point cloud");
     CSM_REQUIRE(jobs[j].grid->ctx->device == device, "grids of one batch share a device");
+    // a NaN would reach static_cast<int>(floor(r)) and lround: refused, as the inserters do
+    CSM_REQUIRE(Finite(jobs[j].xyz, 3 * static_cast<size_t>(jobs[j].num_points)) &&
+                    Finite(jobs[j].target_translation, 2) && Finite(jobs[j].initial_pose, 3),
+                "non-finite point, target or pose");
     floats += 3LL * jobs[j].num_points;
   }
   CSM_REQUIRE(floats < (1LL << 31), "batch too large");
@@ -639,6 +643,9 @@ csm_status csm_ceres_evaluate2d(const csm_rt_grid2d* grid, const float* xyz, int
   CSM_REQUIRE(grid && xyz && target_translation && pose && residuals, "null pointer");
   CSM_REQUIRE(num_points >= 1, "empty point cloud");
   CSM_REQUIRE(grid->d_wcells == nullptr, "the grid must be a ProbabilityGrid");
+  CSM_REQUIRE(Finite(xyz, 3 * static_cast<size_t>(num_points)) && Finite(target_translation, 2) &&
+                  Finite(pose, 3) && std::isfinite(target_angle),
+              "non-finite point, target or pose");
   RefOpts P;
   CSM_TRY(FillOpts(options, &P));
   LaneGuard guard;
@@ -684,6 +691,9 @@ csm_status csm_ceres_evaluate2d_checked(const csm_rt_grid2d* grid, const float* 
     *valid = 1;
     return CSM_OK;
   }
+  CSM_REQUIRE(Finite(xyz, 3 * static_cast<size_t>(num_points)) && Finite(target_translation, 2) &&
+                  Finite(pose, 3) && std::isfinite(target_angle),
+              "non-finite point, target or pose");
   RefOpts P;
   CSM_TRY(FillOpts(options, &P));
   LaneGuard guard;

@@ -620,7 +620,11 @@ csm_status CheckJob(const csm_ceres_job3d& j, int device) {
     CSM_REQUIRE(j.grid[b] != nullptr && j.xyz[b] != nullptr, "null pointer");
     CSM_REQUIRE(j.num_points[b] >= 1, "empty point cloud");
     CSM_REQUIRE(j.grid[b]->ctx->device == device, "grids of one batch share a device");
+    // a NaN would reach lroundf in CellOf: refused, as the inserters do
+    CSM_REQUIRE(Finite(j.xyz[b], 3 * static_cast<size_t>(j.num_points[b])), "non-finite point");
   }
+  CSM_REQUIRE(Finite(j.target_translation, 3) && Finite(j.initial_pose, 7),
+              "non-finite target or pose");
   return CSM_OK;
 }
 
@@ -659,6 +663,8 @@ csm_status CheckIntensityJob(const csm_ceres_job3d& j, const csm_ceres_intensity
     if (ij.intensity_grid[b] == nullptr) continue;
     CSM_REQUIRE(ij.intensities[b] != nullptr, "an intensity grid needs the cloud's intensities");
     CSM_REQUIRE(ij.intensity_grid[b]->ctx->device == device, "grids of one batch share a device");
+    CSM_REQUIRE(Finite(ij.intensities[b], static_cast<size_t>(j.num_points[b])),
+                "non-finite intensity");
   }
   return CSM_OK;
 }
@@ -834,6 +840,7 @@ csm_status Evaluate3(const csm_ceres_job3d* job, const csm_ceres_intensity_job3d
                      const csm_ceres_intensity_options3d* intensity_options, const double pose[7],
                      double* residuals, double* jacobian) {
   CSM_REQUIRE(job && pose && residuals, "null pointer");
+  CSM_REQUIRE(Finite(pose, 7), "non-finite pose");
   int device;
   long long floats;
   Ref3Opts P;

@@ -370,7 +370,13 @@ typedef struct csm_ceres_job2d {
  * failed at the initial estimate initial_cost = final_cost = -1 and iterations = 0.  A trial
  * step where the cost function fails counts as a step of infinite cost and is rejected.  Like
  * Ceres, 1 and 3 stop BEFORE taking the step that triggered them, and the lowest-cost iterate
- * visited is what is returned. */
+ * visited is what is returned.
+ *
+ * Every csm_ceres_* entry point (2D and 3D, the batches and the test hooks) returns
+ * CSM_E_INVALID, with the results untouched and nothing launched, when a cloud coordinate, an
+ * intensity, a pose, a target translation or a target angle is NaN or infinite: such a value
+ * would reach a float -> int conversion (floor, lround) whose result the reference leaves
+ * undefined.  One such job refuses its whole batch. */
 typedef struct csm_ceres_result2d {
   double pose_estimate[3];
   double initial_cost, final_cost; /* Solver::Summary::initial_cost / final_cost */

@@ -630,6 +630,27 @@ void orc_ceres2d_match(const uint16_t* cells, int nx, int ny, double res, double
   summary_out[4] = sum.termination;
 }
 
+// orc_ceres2d_match with the per-iteration trace: returns the number of records and writes
+// at most `cap` of them (kCeresTraceDoubles doubles each, PackCeresTrace's order) to `trace`.
+int orc_ceres2d_match_traced(const uint16_t* cells, int nx, int ny, double res, double max_x,
+                             double max_y, const float* xyz, int n, const double* opts,
+                             const double* target_xy, const double* init_pose, double* pose_out,
+                             double* summary_out, double* trace, int cap) {
+  const ProbabilityGrid grid =
+      MakeGrid(cells, nx, ny, res, max_x, max_y, kMinCorrespondenceCost, kMaxCorrespondenceCost);
+  CeresSummary2D sum;
+  std::vector<CeresIterationTrace> records;
+  CeresMatch2D(grid, MakeCloud(xyz, n), CeresOpts(opts), target_xy, init_pose, pose_out, &sum,
+               &records);
+  summary_out[0] = sum.initial_cost;
+  summary_out[1] = sum.final_cost;
+  summary_out[2] = sum.iterations;
+  summary_out[3] = sum.num_successful_steps;
+  summary_out[4] = sum.termination;
+  if (static_cast<int>(records.size()) <= cap) PackCeresTrace(records, trace);
+  return static_cast<int>(records.size());
+}
+
 // ---- CeresScanMatcher3D restatement (oracle_ceres3d.h) ---------------------------
 // opts = {translation_weight, rotation_weight, use_nonmonotonic_steps, max_num_iterations,
 //         occupied_space_weight_0, occupied_space_weight_1, ...}
@@ -684,6 +705,25 @@ void orc_ceres3d_match(void** hybrids, const float* const* xyz, const int32_t* n
   summary_out[2] = sum.iterations;
   summary_out[3] = sum.num_successful_steps;
   summary_out[4] = sum.termination;
+}
+
+// as orc_ceres2d_match_traced
+int orc_ceres3d_match_traced(void** hybrids, const float* const* xyz, const int32_t* n,
+                             int num_clouds, const double* opts, const double* target_t,
+                             const double* init_pose, double* pose_out, double* summary_out,
+                             double* trace, int cap) {
+  const Clouds3 c(hybrids, xyz, n, num_clouds);
+  CeresSummary2D sum;
+  std::vector<CeresIterationTrace> records;
+  CeresMatch3D(c.pairs, CeresOpts3(opts, num_clouds), target_t, init_pose, pose_out, &sum,
+               &records);
+  summary_out[0] = sum.initial_cost;
+  summary_out[1] = sum.final_cost;
+  summary_out[2] = sum.iterations;
+  summary_out[3] = sum.num_successful_steps;
+  summary_out[4] = sum.termination;
+  if (static_cast<int>(records.size()) <= cap) PackCeresTrace(records, trace);
+  return static_cast<int>(records.size());
 }
 
 }  // extern "C"

@@ -175,10 +175,29 @@ double Norm3(const double v[3]) { return std::sqrt(v[0] * v[0] + v[1] * v[1] + v
 
 }  // namespace
 
+CeresIterationTrace::CeresIterationTrace() {
+  const double nan = std::numeric_limits<double>::quiet_NaN();
+  x_cost = gradient_max_norm = radius_before = radius_after = nan;
+  candidate_cost = model_cost_change = step_quality = nan;
+  step_norm = step_norm_threshold = cost_change = cost_change_threshold = nan;
+  evaluator_minimum_cost = evaluator_candidate_cost = nan;
+}
+
+void PackCeresTrace(const std::vector<CeresIterationTrace>& trace, double* out) {
+  for (const CeresIterationTrace& t : trace) {
+    const double rec[kCeresTraceDoubles] = {
+        static_cast<double>(t.outcome), t.reused_diagonal ? 1. : 0., t.reference_switched ? 1. : 0.,
+        t.x_cost, t.gradient_max_norm, t.radius_before, t.radius_after, t.candidate_cost,
+        t.model_cost_change, t.step_quality, t.step_norm, t.step_norm_threshold, t.cost_change,
+        t.cost_change_threshold, t.evaluator_minimum_cost, t.evaluator_candidate_cost};
+    out = std::copy(rec, rec + kCeresTraceDoubles, out);
+  }
+}
+
 void CeresMatch2D(const ProbabilityGrid& grid, const PointCloud& cloud,
                   const CeresScanMatcherOptions2D& options, const double target_translation[2],
                   const double initial_pose[3], double pose_estimate[3],
-                  CeresSummary2D* summary) {
+                  CeresSummary2D* summary, std::vector<CeresIterationTrace>* trace) {
   // Solver::Options defaults the reference leaves untouched
   const double kInitialRadius = 1e4, kMaxRadius = 1e16, kMinRadius = 1e-32;
   const double kMinRelativeDecrease = 1e-3;
@@ -227,17 +246,30 @@ void CeresMatch2D(const ProbabilityGrid& grid, const PointCloud& cloud,
         best[2] = x[2];
       }
     }
+    const double gmax = std::max(std::abs(at_x.g[0]), std::max(std::abs(at_x.g[1]), std::abs(at_x.g[2])));
+    CeresIterationTrace rec;
+    rec.x_cost = x_cost;
+    rec.gradient_max_norm = gmax;
+    rec.radius_before = rec.radius_after = radius;
+    rec.reused_diagonal = reuse_diagonal;
+    auto record = [&](int outcome) {
+      rec.outcome = outcome;
+      rec.radius_after = radius;
+      if (trace != nullptr) trace->push_back(rec);
+    };
     if (iteration >= options.max_num_iterations) {
       sum.termination = kCeresNoConvergence;
+      record(kStepLoopExit);
       break;
     }
-    const double gmax = std::max(std::abs(at_x.g[0]), std::max(std::abs(at_x.g[1]), std::abs(at_x.g[2])));
     if (gmax <= kGradientTolerance) {
       sum.termination = kCeresGradientTolerance;
+      record(kStepLoopExit);
       break;
     }
     if (radius <= kMinRadius) {
       sum.termination = kCeresMinTrustRegionRadius;
+      record(kStepLoopExit);
       break;
     }
     ++iteration;
@@ -276,12 +308,14 @@ void CeresMatch2D(const ProbabilityGrid& grid, const PointCloud& cloud,
     if (!valid) {
       if (++num_invalid >= kMaxConsecutiveInvalidSteps) {
         sum.termination = kCeresInvalidSteps;
+        record(kStepInvalid);
         break;
       }
       // treated as a rejected step whose diagonal is recomputed
       radius = radius / decrease_factor;
       decrease_factor *= 2.0;
       reuse_diagonal = false;
+      record(kStepInvalid);
       continue;
     }
     num_invalid = 0;
@@ -292,12 +326,20 @@ void CeresMatch2D(const ProbabilityGrid& grid, const PointCloud& cloud,
         Evaluate(grid, cloud, options, target_translation, target_angle, cand, false).cost;
 
     const double diff[3] = {x[0] - cand[0], x[1] - cand[1], x[2] - cand[2]};
+    rec.candidate_cost = candidate_cost;
+    rec.model_cost_change = model_cost_change;
+    rec.step_norm = Norm3(diff);
+    rec.step_norm_threshold = kParameterTolerance * (x_norm + kParameterTolerance);
     if (Norm3(diff) <= kParameterTolerance * (x_norm + kParameterTolerance)) {
       sum.termination = kCeresParameterTolerance;   // the step is not taken
+      record(kStepParameterTolerance);
       break;
     }
+    rec.cost_change = std::abs(x_cost - candidate_cost);
+    rec.cost_change_threshold = kFunctionTolerance * x_cost;
     if (std::abs(x_cost - candidate_cost) <= kFunctionTolerance * x_cost) {
       sum.termination = kCeresFunctionTolerance;    // the step is not taken
+      record(kStepFunctionTolerance);
       break;
     }
 
@@ -305,6 +347,7 @@ void CeresMatch2D(const ProbabilityGrid& grid, const PointCloud& cloud,
     const double historical_decrease =
         (reference_cost - candidate_cost) / (acc_reference + model_cost_change);
     const double step_quality = std::max(relative_decrease, historical_decrease);
+    rec.step_quality = step_quality;
 
     if (step_quality > kMinRelativeDecrease) {
       x[0] = cand[0];
@@ -321,6 +364,8 @@ void CeresMatch2D(const ProbabilityGrid& grid, const PointCloud& cloud,
       reuse_diagonal = false;
       // step evaluator: accepted
       current_cost = candidate_cost;
+      rec.evaluator_minimum_cost = ev_minimum_cost;
+      rec.evaluator_candidate_cost = candidate_cost_ev;
       acc_candidate += model_cost_change;
       acc_reference += model_cost_change;
       if (current_cost < ev_minimum_cost) {
@@ -338,12 +383,15 @@ void CeresMatch2D(const ProbabilityGrid& grid, const PointCloud& cloud,
       if (num_nonmonotonic == max_nonmonotonic) {
         reference_cost = candidate_cost_ev;
         acc_reference = acc_candidate;
+        rec.reference_switched = true;
       }
+      record(kStepAccepted);
     } else {
       // LevenbergMarquardtStrategy::StepRejected
       radius = radius / decrease_factor;
       decrease_factor *= 2.0;
       reuse_diagonal = true;
+      record(kStepRejected);
     }
   }
   sum.iterations = iteration;

@@ -57,6 +57,37 @@ struct CeresSummary2D {
   int termination = kCeresNoConvergence;
 };
 
+// One record per pass of the trust-region loop, for tests that must show which branch of the
+// minimiser a case took.  Every deciding quantity is beside its threshold: step_quality
+// against min_relative_decrease (1e-3), step_norm against step_norm_threshold (parameter
+// tolerance), cost_change against cost_change_threshold (function tolerance),
+// gradient_max_norm against 1e-10, and for an accepted step candidate_cost against the step
+// evaluator's evaluator_minimum_cost (a lower cost resets the non-monotonic count) and, when
+// it is not lower, against evaluator_candidate_cost (both as they were before the step).
+// Fields a pass did not reach are NaN.
+enum CeresStepOutcome {
+  kStepAccepted = 0,
+  kStepRejected = 1,
+  kStepInvalid = 2,              // no valid trial step; the radius shrinks and the pass repeats
+  kStepParameterTolerance = 3,   // stopped, the step is not taken
+  kStepFunctionTolerance = 4,    // stopped, the step is not taken
+  kStepLoopExit = 5,             // stopped before a trial step (see the summary's termination)
+};
+
+struct CeresIterationTrace {
+  int outcome = kStepLoopExit;
+  bool reused_diagonal = false;      // the damping diagonal was kept from the rejected pass before
+  bool reference_switched = false;   // the step evaluator's reference cost was replaced
+  double x_cost, gradient_max_norm, radius_before, radius_after;
+  double candidate_cost, model_cost_change, step_quality;
+  double step_norm, step_norm_threshold, cost_change, cost_change_threshold;
+  double evaluator_minimum_cost, evaluator_candidate_cost;
+  CeresIterationTrace();
+};
+constexpr int kCeresTraceDoubles = 16;
+// {outcome, reused_diagonal, reference_switched, x_cost, ... cost_change_threshold}
+void PackCeresTrace(const std::vector<CeresIterationTrace>& trace, double* out);
+
 // residuals (n + 3) and the row-major (n + 3) x 3 Jacobian of the three residual blocks at
 // `pose` = {x, y, theta}; `jacobian` may be null (then the plain-double evaluation path).
 void EvaluateCeresResiduals2D(const ProbabilityGrid& grid, const PointCloud& cloud,
@@ -69,7 +100,7 @@ void EvaluateCeresResiduals2D(const ProbabilityGrid& grid, const PointCloud& clo
 void CeresMatch2D(const ProbabilityGrid& grid, const PointCloud& cloud,
                   const CeresScanMatcherOptions2D& options, const double target_translation[2],
                   const double initial_pose[3], double pose_estimate[3],
-                  CeresSummary2D* summary);
+                  CeresSummary2D* summary, std::vector<CeresIterationTrace>* trace = nullptr);
 
 }  // namespace oracle
 

@@ -307,7 +307,7 @@ double Norm(const double* v, int n) {
 void CeresMatch3D(const std::vector<PointCloudAndHybridGrid>& clouds,
                   const CeresScanMatcherOptions3D& options, const double target_translation[3],
                   const double initial_pose[7], double pose_estimate[7],
-                  CeresSummary2D* summary) {
+                  CeresSummary2D* summary, std::vector<CeresIterationTrace>* trace) {
   const double kInitialRadius = 1e4, kMaxRadius = 1e16, kMinRadius = 1e-32;
   const double kMinRelativeDecrease = 1e-3;
   const double kMinLmDiagonal = 1e-6, kMaxLmDiagonal = 1e32;
@@ -343,23 +343,37 @@ void CeresMatch3D(const std::vector<PointCloudAndHybridGrid>& clouds,
         for (int k = 0; k < 7; ++k) best[k] = x[k];
       }
     }
-    if (iteration >= options.max_num_iterations) {
-      sum.termination = kCeresNoConvergence;
-      break;
-    }
+    // |x - (x (+) -g)|_inf
+    double gmax = 0.;
     {
-      // |x - (x (+) -g)|_inf
-      double neg[kN], moved[7], gmax = 0.;
+      double neg[kN], moved[7];
       for (int a = 0; a < kN; ++a) neg[a] = -at_x.g[a];
       Plus(x, neg, moved);
       for (int k = 0; k < 7; ++k) gmax = std::max(gmax, std::abs(x[k] - moved[k]));
-      if (gmax <= kGradientTolerance) {
-        sum.termination = kCeresGradientTolerance;
-        break;
-      }
+    }
+    CeresIterationTrace rec;
+    rec.x_cost = x_cost;
+    rec.gradient_max_norm = gmax;
+    rec.radius_before = rec.radius_after = radius;
+    rec.reused_diagonal = reuse_diagonal;
+    auto record = [&](int outcome) {
+      rec.outcome = outcome;
+      rec.radius_after = radius;
+      if (trace != nullptr) trace->push_back(rec);
+    };
+    if (iteration >= options.max_num_iterations) {
+      sum.termination = kCeresNoConvergence;
+      record(kStepLoopExit);
+      break;
+    }
+    if (gmax <= kGradientTolerance) {
+      sum.termination = kCeresGradientTolerance;
+      record(kStepLoopExit);
+      break;
     }
     if (radius <= kMinRadius) {
       sum.termination = kCeresMinTrustRegionRadius;
+      record(kStepLoopExit);
       break;
     }
     ++iteration;
@@ -395,11 +409,13 @@ void CeresMatch3D(const std::vector<PointCloudAndHybridGrid>& clouds,
     if (!valid) {
       if (++num_invalid >= kMaxConsecutiveInvalidSteps) {
         sum.termination = kCeresInvalidSteps;
+        record(kStepInvalid);
         break;
       }
       radius = radius / decrease_factor;
       decrease_factor *= 2.0;
       reuse_diagonal = false;
+      record(kStepInvalid);
       continue;
     }
     num_invalid = 0;
@@ -411,18 +427,27 @@ void CeresMatch3D(const std::vector<PointCloudAndHybridGrid>& clouds,
         Evaluate(clouds, options, target_translation, target_rotation, cand, false).cost;
     double diff[7];
     for (int k = 0; k < 7; ++k) diff[k] = x[k] - cand[k];
+    rec.candidate_cost = candidate_cost;
+    rec.model_cost_change = model_cost_change;
+    rec.step_norm = Norm(diff, 7);
+    rec.step_norm_threshold = kParameterTolerance * (x_norm + kParameterTolerance);
     if (Norm(diff, 7) <= kParameterTolerance * (x_norm + kParameterTolerance)) {
       sum.termination = kCeresParameterTolerance;
+      record(kStepParameterTolerance);
       break;
     }
+    rec.cost_change = std::abs(x_cost - candidate_cost);
+    rec.cost_change_threshold = kFunctionTolerance * x_cost;
     if (std::abs(x_cost - candidate_cost) <= kFunctionTolerance * x_cost) {
       sum.termination = kCeresFunctionTolerance;
+      record(kStepFunctionTolerance);
       break;
     }
     const double relative_decrease = (current_cost - candidate_cost) / model_cost_change;
     const double historical_decrease =
         (reference_cost - candidate_cost) / (acc_reference + model_cost_change);
     const double step_quality = std::max(relative_decrease, historical_decrease);
+    rec.step_quality = step_quality;
     if (step_quality > kMinRelativeDecrease) {
       for (int k = 0; k < 7; ++k) x[k] = cand[k];
       x_norm = Norm(x, 7);
@@ -435,6 +460,8 @@ void CeresMatch3D(const std::vector<PointCloudAndHybridGrid>& clouds,
       decrease_factor = 2.0;
       reuse_diagonal = false;
       current_cost = candidate_cost;
+      rec.evaluator_minimum_cost = ev_minimum_cost;
+      rec.evaluator_candidate_cost = candidate_cost_ev;
       acc_candidate += model_cost_change;
       acc_reference += model_cost_change;
       if (current_cost < ev_minimum_cost) {
@@ -452,11 +479,14 @@ void CeresMatch3D(const std::vector<PointCloudAndHybridGrid>& clouds,
       if (num_nonmonotonic == max_nonmonotonic) {
         reference_cost = candidate_cost_ev;
         acc_reference = acc_candidate;
+        rec.reference_switched = true;
       }
+      record(kStepAccepted);
     } else {
       radius = radius / decrease_factor;
       decrease_factor *= 2.0;
       reuse_diagonal = true;
+      record(kStepRejected);
     }
   }
   sum.iterations = iteration;

@@ -58,7 +58,7 @@ void EvaluateCeresResiduals3D(const std::vector<PointCloudAndHybridGrid>& clouds
 void CeresMatch3D(const std::vector<PointCloudAndHybridGrid>& clouds,
                   const CeresScanMatcherOptions3D& options, const double target_translation[3],
                   const double initial_pose[7], double pose_estimate[7],
-                  CeresSummary2D* summary);
+                  CeresSummary2D* summary, std::vector<CeresIterationTrace>* trace = nullptr);
 
 }  // namespace oracle
 

@@ -529,6 +529,34 @@ CERES_TERMINATION = ("NO_CONVERGENCE", "FUNCTION_TOLERANCE", "GRADIENT_TOLERANCE
                      "PARAMETER_TOLERANCE", "MIN_TRUST_REGION_RADIUS", "INVALID_STEPS")
 
 
+# One record per pass of the trust-region loop (oracle_ceres2d.h, CeresIterationTrace); the
+# Python restatements in tests/ append the same dicts.
+CERES_STEP_OUTCOME = ("ACCEPTED", "REJECTED", "INVALID", "PARAMETER_TOLERANCE",
+                      "FUNCTION_TOLERANCE", "LOOP_EXIT")
+CERES_TRACE_KEYS = ("outcome", "reused_diagonal", "reference_switched", "x_cost",
+                    "gradient_max_norm", "radius_before", "radius_after", "candidate_cost",
+                    "model_cost_change", "step_quality", "step_norm", "step_norm_threshold",
+                    "cost_change", "cost_change_threshold", "evaluator_minimum_cost",
+                    "evaluator_candidate_cost")
+
+
+def ceres_trace_record(outcome, **values):
+    """A trace record with every key; what the pass did not reach is NaN."""
+    rec = dict.fromkeys(CERES_TRACE_KEYS, float("nan"))
+    rec.update(outcome=outcome, reused_diagonal=False, reference_switched=False)
+    rec.update(values)
+    return rec
+
+
+def _traced(call):
+    """call(trace_ptr, cap) -> count: the records as dicts."""
+    buf = np.zeros((256, len(CERES_TRACE_KEYS)), np.float64)
+    count = call(_p(buf, C.c_double), C.c_int(len(buf)))
+    assert count <= len(buf)
+    return [dict(zip(CERES_TRACE_KEYS, (CERES_STEP_OUTCOME[int(r[0])], bool(r[1]), bool(r[2]))
+                     + tuple(float(v) for v in r[3:]))) for r in buf[:count]]
+
+
 def _ceres_opts(occupied_space_weight, translation_weight, rotation_weight,
                 use_nonmonotonic_steps, max_num_iterations):
     return np.array([occupied_space_weight, translation_weight, rotation_weight,
@@ -556,8 +584,9 @@ def ceres2d_evaluate(grid, xyz, pose, target_xy, target_angle, occupied_space_we
 
 def ceres2d_match(grid, xyz, target_xy, initial_pose, occupied_space_weight=20.0,
                   translation_weight=10.0, rotation_weight=1.0, use_nonmonotonic_steps=True,
-                  max_num_iterations=10):
-    """CeresScanMatcher2D::Match -> dict(pose, initial_cost, final_cost, iterations, ...)."""
+                  max_num_iterations=10, trace=False):
+    """CeresScanMatcher2D::Match -> dict(pose, initial_cost, final_cost, iterations, ...);
+    with trace also "trace", the per-iteration records."""
     xyz = _f32(xyz)
     o = _ceres_opts(occupied_space_weight, translation_weight, rotation_weight,
                     use_nonmonotonic_steps, max_num_iterations)
@@ -565,14 +594,18 @@ def ceres2d_match(grid, xyz, target_xy, initial_pose, occupied_space_weight=20.0
     ip = np.ascontiguousarray(initial_pose, np.float64)
     pose = np.zeros(3, np.float64)
     sm = np.zeros(5, np.float64)
-    lib().orc_ceres2d_match(_p(grid.cells, C.c_uint16), C.c_int(grid.num_x), C.c_int(grid.num_y),
-                            C.c_double(grid.resolution), C.c_double(grid.max_x),
-                            C.c_double(grid.max_y), _p(xyz, C.c_float), C.c_int(len(xyz)),
-                            _p(o, C.c_double), _p(t, C.c_double), _p(ip, C.c_double),
-                            _p(pose, C.c_double), _p(sm, C.c_double))
+    args = (_p(grid.cells, C.c_uint16), C.c_int(grid.num_x), C.c_int(grid.num_y),
+            C.c_double(grid.resolution), C.c_double(grid.max_x), C.c_double(grid.max_y),
+            _p(xyz, C.c_float), C.c_int(len(xyz)), _p(o, C.c_double), _p(t, C.c_double),
+            _p(ip, C.c_double), _p(pose, C.c_double), _p(sm, C.c_double))
+    extra = {}
+    if trace:
+        extra["trace"] = _traced(lambda buf, cap: lib().orc_ceres2d_match_traced(*args, buf, cap))
+    else:
+        lib().orc_ceres2d_match(*args)
     return dict(pose=pose, initial_cost=float(sm[0]), final_cost=float(sm[1]),
                 iterations=int(sm[2]), num_successful_steps=int(sm[3]),
-                termination=CERES_TERMINATION[int(sm[4])])
+                termination=CERES_TERMINATION[int(sm[4])], **extra)
 
 
 # ---- CeresScanMatcher3D restatement (oracle_ceres3d.h; parity unpinned against Ceres) ----
@@ -618,8 +651,10 @@ def ceres3d_evaluate(clouds_and_grids, pose, target_translation, target_rotation
 
 def ceres3d_match(clouds_and_grids, target_translation, initial_pose,
                   occupied_space_weights=(5.0, 30.0), translation_weight=10.0,
-                  rotation_weight=1.0, use_nonmonotonic_steps=False, max_num_iterations=10):
-    """CeresScanMatcher3D::Match (no intensity grids, only_optimize_yaw = false)."""
+                  rotation_weight=1.0, use_nonmonotonic_steps=False, max_num_iterations=10,
+                  trace=False):
+    """CeresScanMatcher3D::Match (no intensity grids, only_optimize_yaw = false); with trace
+    also "trace", the per-iteration records."""
     num, clouds, hy, xs, ns, o = _ceres3d_args(clouds_and_grids, occupied_space_weights,
                                                translation_weight, rotation_weight,
                                                use_nonmonotonic_steps, max_num_iterations)
@@ -627,9 +662,13 @@ def ceres3d_match(clouds_and_grids, target_translation, initial_pose,
     ip = np.ascontiguousarray(initial_pose, np.float64)
     pose = np.zeros(7, np.float64)
     sm = np.zeros(5, np.float64)
-    lib().orc_ceres3d_match(hy, xs, _p(ns, C.c_int32), C.c_int(num), _p(o, C.c_double),
-                            _p(tt, C.c_double), _p(ip, C.c_double), _p(pose, C.c_double),
-                            _p(sm, C.c_double))
+    args = (hy, xs, _p(ns, C.c_int32), C.c_int(num), _p(o, C.c_double), _p(tt, C.c_double),
+            _p(ip, C.c_double), _p(pose, C.c_double), _p(sm, C.c_double))
+    extra = {}
+    if trace:
+        extra["trace"] = _traced(lambda buf, cap: lib().orc_ceres3d_match_traced(*args, buf, cap))
+    else:
+        lib().orc_ceres3d_match(*args)
     return dict(pose=pose, initial_cost=float(sm[0]), final_cost=float(sm[1]),
                 iterations=int(sm[2]), num_successful_steps=int(sm[3]),
-                termination=CERES_TERMINATION[int(sm[4])])
+                termination=CERES_TERMINATION[int(sm[4])], **extra)

@@ -51,20 +51,18 @@ using std::isfinite;
 #include "../../cartographer_b200/csrc/refine2d.cu"
 #include "../../cartographer_b200/csrc/value_conversion.h"
 
-extern "C" {
+namespace {
 
-// One CTA of k_ceres_match2d for one job.  opts = {occupied, translation, rotation,
-// use_nonmonotonic_steps, max_num_iterations}; out = {pose[3], initial_cost, final_cost,
-// iterations, num_successful_steps, termination}.
-void emu_ceres_match2d(const uint16_t* cells, int nx, int ny, double resolution, double max_x,
-                       double max_y, const float* xyz, int n, const double* opts,
-                       const double* target_xy, const double* init_pose, double* out) {
+// One CTA of k_ceres_match2d for one job whose rows are `pitch` cells apart.
+void RunMatch2D(const uint16_t* cells, int nx, int ny, int pitch, double resolution, double max_x,
+                double max_y, const float* xyz, int n, const double* opts,
+                const double* target_xy, const double* init_pose, double* out) {
   csm::RefJobDev job;
   std::memset(&job, 0, sizeof(job));
   job.cells = cells;
   job.nx = nx;
   job.ny = ny;
-  job.pitch = nx;
+  job.pitch = pitch;
   job.n = n;
   job.xyz_off = 0;
   job.resolution = resolution;
@@ -106,6 +104,27 @@ void emu_ceres_match2d(const uint16_t* cells, int nx, int ny, double resolution,
   out[5] = result.iterations;
   out[6] = result.num_successful_steps;
   out[7] = result.termination;
+}
+
+}  // namespace
+
+extern "C" {
+
+// opts = {occupied, translation, rotation, use_nonmonotonic_steps, max_num_iterations};
+// out = {pose[3], initial_cost, final_cost, iterations, num_successful_steps, termination}.
+void emu_ceres_match2d(const uint16_t* cells, int nx, int ny, double resolution, double max_x,
+                       double max_y, const float* xyz, int n, const double* opts,
+                       const double* target_xy, const double* init_pose, double* out) {
+  RunMatch2D(cells, nx, ny, nx, resolution, max_x, max_y, xyz, n, opts, target_xy, init_pose, out);
+}
+
+// As emu_ceres_match2d with the cells in rows of `pitch` >= nx, as a device handle keeps them.
+void emu_ceres_match2d_pitched(const uint16_t* cells, int nx, int ny, int pitch,
+                               double resolution, double max_x, double max_y, const float* xyz,
+                               int n, const double* opts, const double* target_xy,
+                               const double* init_pose, double* out) {
+  RunMatch2D(cells, nx, ny, pitch, resolution, max_x, max_y, xyz, n, opts, target_xy, init_pose,
+             out);
 }
 
 }  // extern "C"

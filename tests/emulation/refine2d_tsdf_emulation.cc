@@ -49,22 +49,18 @@ using std::isfinite;
 #include "../../cartographer_b200/csrc/refine2d.cu"
 #include "../../cartographer_b200/csrc/tsdf_conversion.h"
 
-extern "C" {
+namespace {
 
-// One CTA of k_ceres_match2d for one TSDF2D job.  grid = {resolution, max_x, max_y,
-// truncation, max_weight}; opts = {occupied, translation, rotation, use_nonmonotonic_steps,
-// max_num_iterations}; out = {pose[3], initial_cost, final_cost, iterations,
-// num_successful_steps, termination}.
-void emu_ceres_match2d_tsdf(const uint16_t* tsd_cells, const uint16_t* weight_cells, int nx,
-                            int ny, const double* grid, const float* xyz, int n,
-                            const double* opts, const double* target_xy,
-                            const double* init_pose, double* out) {
+// One CTA of k_ceres_match2d for one TSDF2D job whose rows are `pitch` cells apart.
+void RunMatchTsdf(const uint16_t* tsd_cells, const uint16_t* weight_cells, int nx, int ny,
+                  int pitch, const double* grid, const float* xyz, int n, const double* opts,
+                  const double* target_xy, const double* init_pose, double* out) {
   csm::RefJobDev job;
   std::memset(&job, 0, sizeof(job));
   job.cells = tsd_cells;
   job.nx = nx;
   job.ny = ny;
-  job.pitch = nx;
+  job.pitch = pitch;
   job.n = n;
   job.resolution = grid[0];
   job.max_x = grid[1];
@@ -109,6 +105,30 @@ void emu_ceres_match2d_tsdf(const uint16_t* tsd_cells, const uint16_t* weight_ce
   out[5] = result.iterations;
   out[6] = result.num_successful_steps;
   out[7] = result.termination;
+}
+
+}  // namespace
+
+extern "C" {
+
+// grid = {resolution, max_x, max_y, truncation, max_weight}; opts = {occupied, translation,
+// rotation, use_nonmonotonic_steps, max_num_iterations}; out = {pose[3], initial_cost,
+// final_cost, iterations, num_successful_steps, termination}.
+void emu_ceres_match2d_tsdf(const uint16_t* tsd_cells, const uint16_t* weight_cells, int nx,
+                            int ny, const double* grid, const float* xyz, int n,
+                            const double* opts, const double* target_xy,
+                            const double* init_pose, double* out) {
+  RunMatchTsdf(tsd_cells, weight_cells, nx, ny, nx, grid, xyz, n, opts, target_xy, init_pose, out);
+}
+
+// As emu_ceres_match2d_tsdf with both cell arrays in rows of `pitch` >= nx.
+void emu_ceres_match2d_tsdf_pitched(const uint16_t* tsd_cells, const uint16_t* weight_cells,
+                                    int nx, int ny, int pitch, const double* grid,
+                                    const float* xyz, int n, const double* opts,
+                                    const double* target_xy, const double* init_pose,
+                                    double* out) {
+  RunMatchTsdf(tsd_cells, weight_cells, nx, ny, pitch, grid, xyz, n, opts, target_xy, init_pose,
+               out);
 }
 
 }  // extern "C"

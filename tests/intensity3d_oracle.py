@@ -347,9 +347,10 @@ def _norm(v):
 
 def match(entries, target_translation, initial_pose, intensity_options,
           occupied_space_weights=(5.0, 30.0), translation_weight=10.0, rotation_weight=1.0,
-          use_nonmonotonic_steps=False, max_num_iterations=10):
+          use_nonmonotonic_steps=False, max_num_iterations=10, trace=None):
     """CeresScanMatcher3D::Match with intensity blocks: oracle_ceres3d.cc's CeresMatch3D on the
-    Huber-corrected normal equations -> dict(pose, initial_cost, final_cost, iterations, ...)."""
+    Huber-corrected normal equations -> dict(pose, initial_cost, final_cost, iterations, ...).
+    `trace`: a list that receives one pyoracle.ceres_trace_record per pass of the loop."""
     k_initial_radius, k_max_radius, k_min_radius = 1e4, 1e16, 1e-32
     k_min_relative_decrease, k_min_diag, k_max_diag = 1e-3, 1e-6, 1e32
     k_max_invalid, k_ftol, k_gtol, k_ptol = 5, 1e-6, 1e-10, 1e-8
@@ -378,15 +379,26 @@ def match(entries, target_translation, initial_pose, intensity_options,
             successful += 1
             if x_cost < minimum_cost:
                 minimum_cost, best = x_cost, list(x)
+        moved = plus(x, [-v for v in gx])
+        gmax = max(abs(x[k] - moved[k]) for k in range(7))
+        rec = dict(x_cost=x_cost, gradient_max_norm=gmax, radius_before=radius,
+                   reused_diagonal=reuse_diagonal)
+
+        def record(outcome, **more):
+            if trace is not None:
+                trace.append(pyoracle.ceres_trace_record(outcome, radius_after=radius, **rec,
+                                                         **more))
         if iteration >= max_num_iterations:
             termination = 0
+            record("LOOP_EXIT")
             break
-        moved = plus(x, [-v for v in gx])
-        if max(abs(x[k] - moved[k]) for k in range(7)) <= k_gtol:
+        if gmax <= k_gtol:
             termination = 2
+            record("LOOP_EXIT")
             break
         if radius <= k_min_radius:
             termination = 4
+            record("LOOP_EXIT")
             break
         iteration += 1
         last_step_successful = False
@@ -418,24 +430,33 @@ def match(entries, target_translation, initial_pose, intensity_options,
             num_invalid += 1
             if num_invalid >= k_max_invalid:
                 termination = 5
+                record("INVALID")
                 break
             radius /= decrease_factor
             decrease_factor *= 2.0
             reuse_diagonal = False
+            record("INVALID")
             continue
         num_invalid = 0
         cand = plus(x, [step[a] * scale[a] for a in range(6)])
         candidate_cost = ev(cand, False)[0]
+        rec.update(candidate_cost=candidate_cost, model_cost_change=model_cost_change,
+                   step_norm=_norm([x[k] - cand[k] for k in range(7)]),
+                   step_norm_threshold=k_ptol * (x_norm + k_ptol))
         if _norm([x[k] - cand[k] for k in range(7)]) <= k_ptol * (x_norm + k_ptol):
             termination = 3
+            record("PARAMETER_TOLERANCE")
             break
+        rec.update(cost_change=abs(x_cost - candidate_cost), cost_change_threshold=k_ftol * x_cost)
         if abs(x_cost - candidate_cost) <= k_ftol * x_cost:
             termination = 1
+            record("FUNCTION_TOLERANCE")
             break
         relative_decrease = (current_cost - candidate_cost) / model_cost_change
         historical_decrease = (reference_cost - candidate_cost) / (acc_reference +
                                                                    model_cost_change)
         step_quality = max(relative_decrease, historical_decrease)
+        rec.update(step_quality=step_quality)
         if step_quality > k_min_relative_decrease:
             x = cand
             x_norm = _norm(x)
@@ -445,6 +466,8 @@ def match(entries, target_translation, initial_pose, intensity_options,
             radius = min(k_max_radius, radius / max(1.0 / 3.0, 1.0 - t * t * t))
             decrease_factor, reuse_diagonal = 2.0, False
             current_cost = candidate_cost
+            rec.update(evaluator_minimum_cost=ev_minimum_cost,
+                       evaluator_candidate_cost=candidate_cost_ev)
             acc_candidate += model_cost_change
             acc_reference += model_cost_change
             if current_cost < ev_minimum_cost:
@@ -456,10 +479,13 @@ def match(entries, target_translation, initial_pose, intensity_options,
                     candidate_cost_ev, acc_candidate = current_cost, 0.0
             if num_nonmonotonic == max_nonmonotonic:
                 reference_cost, acc_reference = candidate_cost_ev, acc_candidate
+                rec.update(reference_switched=True)
+            record("ACCEPTED")
         else:
             radius /= decrease_factor
             decrease_factor *= 2.0
             reuse_diagonal = True
+            record("REJECTED")
     return dict(pose=np.array(best), initial_cost=initial_cost, final_cost=minimum_cost,
                 iterations=iteration, num_successful_steps=successful,
                 termination=CERES_TERMINATION[termination])

@@ -25,6 +25,8 @@ import sys
 
 import numpy as np
 
+from oracle.pyoracle import ceres_trace_record
+
 F = np.float32
 UPDATE_MARKER = 1 << 15
 DBL_MAX = sys.float_info.max
@@ -278,8 +280,9 @@ def _norm3(v):
 
 def match(g, xyz, target_xy, initial_pose, occupied_space_weight=20.0, translation_weight=10.0,
           rotation_weight=1.0, use_nonmonotonic_steps=True, max_num_iterations=10,
-          evaluator=None):
+          evaluator=None, trace=None):
     """CeresScanMatcher2D::Match on a TSDF2D; the summary dict of pyoracle.ceres2d_match.
+    `trace`: a list that receives one pyoracle.ceres_trace_record per pass of the loop.
     `evaluator` replaces the cost (same signature and return as evaluate()): the tests run
     this loop on the ProbabilityGrid cost of oracle/ to keep it equal to the C++ loop there."""
     opts = (occupied_space_weight, translation_weight, rotation_weight)
@@ -322,14 +325,24 @@ def match(g, xyz, target_xy, initial_pose, occupied_space_weight=20.0, translati
                 minimum_cost = x_cost
                 best = list(x)
             last_step_successful = False
+        gmax = max(abs(gr[0]), max(abs(gr[1]), abs(gr[2])))
+        rec = dict(x_cost=x_cost, gradient_max_norm=gmax, radius_before=radius,
+                   reused_diagonal=reuse_diagonal)
+
+        def record(outcome, **more):
+            if trace is not None:
+                trace.append(ceres_trace_record(outcome, radius_after=radius, **rec, **more))
         if iteration >= max_num_iterations:
             termination = 0
+            record("LOOP_EXIT")
             break
-        if max(abs(gr[0]), max(abs(gr[1]), abs(gr[2]))) <= 1e-10:
+        if gmax <= 1e-10:
             termination = 2
+            record("LOOP_EXIT")
             break
         if radius <= k_min_radius:
             termination = 4
+            record("LOOP_EXIT")
             break
         iteration += 1
         hs = [h[0] * scale[0] * scale[0], h[1] * scale[0] * scale[1], h[2] * scale[0] * scale[2],
@@ -356,10 +369,12 @@ def match(g, xyz, target_xy, initial_pose, occupied_space_weight=20.0, translati
             num_invalid += 1
             if num_invalid >= 5:
                 termination = 5
+                record("INVALID")
                 break
             radius = radius / decrease_factor
             decrease_factor *= 2.0
             reuse_diagonal = False
+            record("INVALID")
             continue
         num_invalid = 0
         cand = [x[0] + step[0] * scale[0], x[1] + step[1] * scale[1], x[2] + step[2] * scale[2]]
@@ -367,15 +382,21 @@ def match(g, xyz, target_xy, initial_pose, occupied_space_weight=20.0, translati
         candidate_cost = DBL_MAX if at_cand is None else at_cand[0]
         trial_failures[0] += at_cand is None
         diff = [x[0] - cand[0], x[1] - cand[1], x[2] - cand[2]]
+        rec.update(candidate_cost=candidate_cost, model_cost_change=model_cost_change,
+                   step_norm=_norm3(diff), step_norm_threshold=1e-8 * (x_norm + 1e-8))
         if _norm3(diff) <= 1e-8 * (x_norm + 1e-8):
             termination = 3
+            record("PARAMETER_TOLERANCE")
             break
+        rec.update(cost_change=abs(x_cost - candidate_cost), cost_change_threshold=1e-6 * x_cost)
         if abs(x_cost - candidate_cost) <= 1e-6 * x_cost:
             termination = 1
+            record("FUNCTION_TOLERANCE")
             break
         relative_decrease = (current_cost - candidate_cost) / model_cost_change
         historical_decrease = (reference_cost - candidate_cost) / (acc_reference + model_cost_change)
         step_quality = max(relative_decrease, historical_decrease)
+        rec.update(step_quality=step_quality)
         if step_quality > 1e-3:
             x = cand
             x_norm = _norm3(x)
@@ -384,6 +405,8 @@ def match(g, xyz, target_xy, initial_pose, occupied_space_weight=20.0, translati
             decrease_factor = 2.0
             reuse_diagonal = False
             current_cost = candidate_cost
+            rec.update(evaluator_minimum_cost=ev_minimum_cost,
+                       evaluator_candidate_cost=candidate_cost_ev)
             acc_candidate += model_cost_change
             acc_reference += model_cost_change
             if current_cost < ev_minimum_cost:
@@ -399,6 +422,8 @@ def match(g, xyz, target_xy, initial_pose, occupied_space_weight=20.0, translati
             if num_nonmonotonic == max_nonmonotonic:
                 reference_cost = candidate_cost_ev
                 acc_reference = acc_candidate
+                rec.update(reference_switched=True)
+            record("ACCEPTED")
             at_x = _normal(g, xyz, x, target, target_angle, opts, True, evaluator)
             if at_x is None:   # FAILURE: the parameters keep the initial estimate
                 return done(init, initial_cost, initial_cost, iteration, successful, 6)
@@ -408,4 +433,5 @@ def match(g, xyz, target_xy, initial_pose, occupied_space_weight=20.0, translati
             radius = radius / decrease_factor
             decrease_factor *= 2.0
             reuse_diagonal = True
+            record("REJECTED")
     return done(best, initial_cost, minimum_cost, iteration, successful, termination)
