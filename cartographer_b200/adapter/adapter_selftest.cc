@@ -390,6 +390,103 @@ int main() {
       std::printf(" %08x:%08x:%d", Bits(mean[i]), Bits(sum[i]), count[i]);
     std::printf("\n");
   }
+  // ---- FastCorrelativeScanMatcher3D and ConstraintBuilder3D on inserted device grids: the
+  // axis cloud inserted twice from its sensor position into empty grids; the same built from
+  // host HybridGrids of the grids' non-zero voxels prints the *_host lines, which
+  // tests/test_gpu_adapter_matcher3d_from_grid.py holds equal to the *_dev lines ----
+  {
+    mapping::proto::RangeDataInserterOptions3D io;
+    io.set_hit_probability(0.7);
+    io.set_miss_probability(0.4);
+    io.set_num_free_space_voxels(2);
+    io.set_intensity_threshold(100.f);
+    const mapping::scan_matching::RangeDataInserter3D inserter(io);
+    mapping::scan_matching::DeviceHybridGrid dhi(0.05f, 0), dlo(0.1f, 0);
+    sensor::RangeData range_data;
+    range_data.origin = {{tx, ty, tz}};
+    for (const auto& p : cloud3.points())
+      range_data.returns.push_back({{{p.position.x() + tx, p.position.y() + ty,
+                                      p.position.z() + tz}}});
+    for (int i = 0; i < 2; ++i) {
+      inserter.Insert(range_data, &dhi, nullptr);
+      inserter.Insert(range_data, &dlo, nullptr);
+    }
+    mapping::HybridGrid hhi(0.05f), hlo(0.1f);
+    for (auto gp : {std::make_pair(&dhi, &hhi), std::make_pair(&dlo, &hlo)}) {
+      int32_t lo[3], dims[3];
+      if (csm_grid3d_read(gp.first->handle(), lo, dims, nullptr) != CSM_OK) return 1;
+      std::vector<uint16_t> values(static_cast<size_t>(dims[0]) * dims[1] * dims[2]);
+      if (csm_grid3d_read(gp.first->handle(), lo, dims, values.data()) != CSM_OK) return 1;
+      for (int z = 0; z < dims[2]; ++z)
+        for (int y = 0; y < dims[1]; ++y)
+          for (int x = 0; x < dims[0]; ++x) {
+            const uint16_t v = values[(static_cast<size_t>(z) * dims[1] + y) * dims[0] + x];
+            if (v != 0) gp.second->Set(x + lo[0], y + lo[1], z + lo[2], v);
+          }
+    }
+    using Matcher3D = mapping::scan_matching::FastCorrelativeScanMatcher3D;
+    auto print = [](const char* name, const std::unique_ptr<Matcher3D::Result>& r) {
+      std::printf("RESULT %s %d", name, r ? 1 : 0);
+      if (r)
+        std::printf(" %08x %.17g %.17g %.17g %.17g %.17g %.17g %.17g %08x %08x", Bits(r->score),
+                    r->pose_estimate.translation().x(), r->pose_estimate.translation().y(),
+                    r->pose_estimate.translation().z(), r->pose_estimate.rotation().w(),
+                    r->pose_estimate.rotation().x(), r->pose_estimate.rotation().y(),
+                    r->pose_estimate.rotation().z(), Bits(r->rotational_score),
+                    Bits(r->low_resolution_score));
+      std::printf("\n");
+    };
+    const Matcher3D mdev(dhi, &dlo, &histogram, o3);
+    const Matcher3D mhost(hhi, &hlo, &histogram, o3);
+    const transform::Quaterniond q{1., 0., 0., 0.};
+    for (const Matcher3D* m : {&mdev, &mhost}) {
+      const char* side = m == &mdev ? "dev" : "host";
+      char name[64];
+      std::snprintf(name, sizeof(name), "fast3d_grid_%s", side);
+      const auto r = m->Match(transform::Rigid3d(), transform::Rigid3d(), data, 0.1f);
+      if (!r) return 1;
+      print(name, r);
+      std::snprintf(name, sizeof(name), "fast3d_grid_full_%s", side);
+      print(name, m->MatchFullSubmap(q, q, data, 0.1f));
+    }
+    using mapping::constraints::ConstraintBuilder3D;
+    mapping::constraints::proto::ConstraintBuilderOptions bo;
+    bo.sampling_ratio_ = 1.0;
+    bo.min_score_ = 0.1;
+    bo.global_localization_min_score_ = 0.1;
+    bo.fast3d_ = o3;
+    common::InlineThreadPool pool;
+    const mapping::constraints::DeviceSubmap3D dsub{&dhi, &dlo, &histogram};
+    const mapping::Submap3D hsub(&hhi, &hlo, &histogram);
+    for (int side = 0; side < 2; ++side) {
+      for (int refine = 0; refine < 2; ++refine) {
+        ConstraintBuilder3D builder(bo, &pool);
+        builder.set_device_refinement(refine == 1);
+        const mapping::SubmapId sid{0, 0};
+        if (side == 0) {
+          builder.MaybeAddConstraint(sid, &dsub, mapping::NodeId{0, 0}, &data,
+                                     transform::Rigid3d(), transform::Rigid3d());
+          builder.MaybeAddGlobalConstraint(sid, &dsub, mapping::NodeId{0, 1}, &data, q, q);
+        } else {
+          builder.MaybeAddConstraint(sid, &hsub, mapping::NodeId{0, 0}, &data,
+                                     transform::Rigid3d(), transform::Rigid3d());
+          builder.MaybeAddGlobalConstraint(sid, &hsub, mapping::NodeId{0, 1}, &data, q, q);
+        }
+        builder.NotifyEndOfNode();
+        ConstraintBuilder3D::Result got;
+        builder.WhenDone([&](const ConstraintBuilder3D::Result& r) { got = r; });
+        if (got.size() != 2) return 1;
+        for (const auto& c : got) {
+          const transform::Rigid3d& z = c.pose.zbar_ij;
+          std::printf("RESULT cb3d_grid%s_%s %d %.17g %.17g %.17g %.17g %.17g %.17g %.17g\n",
+                      refine ? "_refined" : "", side == 0 ? "dev" : "host", c.node_id.node_index,
+                      z.translation().x(), z.translation().y(), z.translation().z(),
+                      z.rotation().w(), z.rotation().x(), z.rotation().y(), z.rotation().z());
+        }
+        builder.DeleteScanMatcher(sid);
+      }
+    }
+  }
   // ---- ProbabilityGridRangeDataInserter2D on a device grid: the reference's InsertPointCloud
   // (range_data_inserter_2d_test.cc:47-58) with one miss, then a return that makes the grid
   // grow; the cropped grid and a stack built from it ----

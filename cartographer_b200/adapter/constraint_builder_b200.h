@@ -330,6 +330,17 @@ class ConstraintBuilder2D {
 };
 
 #ifndef CSM_ADAPTER_REAL_CARTOGRAPHER
+// A Submap3D whose grids live on the device, as Submap3D::InsertData leaves them when it
+// inserts through scan_matching::RangeDataInserter3D: what ConstraintBuilder3D reads of it.
+// The builder keeps the pointers, so the grids and the histogram must stay alive (and
+// unchanged) until the WhenDone callback has run (constraint_builder_2d.h:76-77).
+struct DeviceSubmap3D {
+  const scan_matching::DeviceHybridGrid* high_resolution_hybrid_grid;
+  const scan_matching::DeviceHybridGrid* low_resolution_hybrid_grid;
+  const std::vector<float>* rotational_scan_matcher_histogram;
+  int grid_size_in_voxels = 0;   // HybridGrid::grid_size(); 0 derives it from the grid
+};
+
 class ConstraintBuilder3D {
  public:
   using Constraint = PoseGraphInterface::Constraint;
@@ -358,21 +369,17 @@ class ConstraintBuilder3D {
                           const NodeId& node_id, const TrajectoryNodeData* constant_data,
                           const transform::Rigid3d& global_node_pose,
                           const transform::Rigid3d& global_submap_pose) {
-    // |(global_submap_pose^-1 * global_node_pose).translation()| = |t_node - t_submap|
-    const double dx = global_node_pose.translation().x() - global_submap_pose.translation().x();
-    const double dy = global_node_pose.translation().y() - global_submap_pose.translation().y();
-    const double dz = global_node_pose.translation().z() - global_submap_pose.translation().z();
-    if (std::sqrt(dx * dx + dy * dy + dz * dz) > options_.max_constraint_distance()) return;
-    if (!per_submap_sampler_
-             .emplace(std::piecewise_construct, std::forward_as_tuple(submap_id),
-                      std::forward_as_tuple(options_.sampling_ratio()))
-             .first->second.Pulse()) {
-      return;
-    }
-    std::lock_guard<std::mutex> lock(mutex_);
-    pending_.push_back(Pending{submap_id, submap, node_id, constant_data, global_node_pose,
-                               global_submap_pose, false,
-                               static_cast<float>(options_.min_score())});
+    AddLocal(submap_id, submap, nullptr, node_id, constant_data, global_node_pose,
+             global_submap_pose);
+  }
+  // The same for a submap kept on the device: its matcher is built from its grids without a
+  // host copy, and the refinement reads them directly.
+  void MaybeAddConstraint(const SubmapId& submap_id, const DeviceSubmap3D* submap,
+                          const NodeId& node_id, const TrajectoryNodeData* constant_data,
+                          const transform::Rigid3d& global_node_pose,
+                          const transform::Rigid3d& global_submap_pose) {
+    AddLocal(submap_id, nullptr, submap, node_id, constant_data, global_node_pose,
+             global_submap_pose);
   }
 
   // constraint_builder_3d.cc:116-142
@@ -380,11 +387,15 @@ class ConstraintBuilder3D {
                                 const NodeId& node_id, const TrajectoryNodeData* constant_data,
                                 const transform::Quaterniond& global_node_rotation,
                                 const transform::Quaterniond& global_submap_rotation) {
-    std::lock_guard<std::mutex> lock(mutex_);
-    pending_.push_back(Pending{submap_id, submap, node_id, constant_data,
-                               transform::Rigid3d({{0., 0., 0.}}, global_node_rotation),
-                               transform::Rigid3d({{0., 0., 0.}}, global_submap_rotation), true,
-                               static_cast<float>(options_.global_localization_min_score())});
+    AddGlobal(submap_id, submap, nullptr, node_id, constant_data, global_node_rotation,
+              global_submap_rotation);
+  }
+  void MaybeAddGlobalConstraint(const SubmapId& submap_id, const DeviceSubmap3D* submap,
+                                const NodeId& node_id, const TrajectoryNodeData* constant_data,
+                                const transform::Quaterniond& global_node_rotation,
+                                const transform::Quaterniond& global_submap_rotation) {
+    AddGlobal(submap_id, nullptr, submap, node_id, constant_data, global_node_rotation,
+              global_submap_rotation);
   }
 
   void NotifyEndOfNode() {
@@ -422,13 +433,48 @@ class ConstraintBuilder3D {
  private:
   struct Pending {
     SubmapId submap_id;
-    const Submap3D* submap;
+    const Submap3D* submap;                 // one of the two is set
+    const DeviceSubmap3D* device_submap;
     NodeId node_id;
     const TrajectoryNodeData* constant_data;
     transform::Rigid3d global_node_pose, global_submap_pose;
     bool full;
     float min_score;
   };
+
+  void AddLocal(const SubmapId& submap_id, const Submap3D* submap,
+                const DeviceSubmap3D* device_submap, const NodeId& node_id,
+                const TrajectoryNodeData* constant_data,
+                const transform::Rigid3d& global_node_pose,
+                const transform::Rigid3d& global_submap_pose) {
+    // |(global_submap_pose^-1 * global_node_pose).translation()| = |t_node - t_submap|
+    const double dx = global_node_pose.translation().x() - global_submap_pose.translation().x();
+    const double dy = global_node_pose.translation().y() - global_submap_pose.translation().y();
+    const double dz = global_node_pose.translation().z() - global_submap_pose.translation().z();
+    if (std::sqrt(dx * dx + dy * dy + dz * dz) > options_.max_constraint_distance()) return;
+    if (!per_submap_sampler_
+             .emplace(std::piecewise_construct, std::forward_as_tuple(submap_id),
+                      std::forward_as_tuple(options_.sampling_ratio()))
+             .first->second.Pulse()) {
+      return;
+    }
+    std::lock_guard<std::mutex> lock(mutex_);
+    pending_.push_back(Pending{submap_id, submap, device_submap, node_id, constant_data,
+                               global_node_pose, global_submap_pose, false,
+                               static_cast<float>(options_.min_score())});
+  }
+
+  void AddGlobal(const SubmapId& submap_id, const Submap3D* submap,
+                 const DeviceSubmap3D* device_submap, const NodeId& node_id,
+                 const TrajectoryNodeData* constant_data,
+                 const transform::Quaterniond& global_node_rotation,
+                 const transform::Quaterniond& global_submap_rotation) {
+    std::lock_guard<std::mutex> lock(mutex_);
+    pending_.push_back(Pending{submap_id, submap, device_submap, node_id, constant_data,
+                               transform::Rigid3d({{0., 0., 0.}}, global_node_rotation),
+                               transform::Rigid3d({{0., 0., 0.}}, global_submap_rotation), true,
+                               static_cast<float>(options_.global_localization_min_score())});
+  }
 
   static void Flatten(const HybridGrid& grid, std::vector<int32_t>* idx,
                       std::vector<uint16_t>* val) {
@@ -446,22 +492,24 @@ class ConstraintBuilder3D {
   }
 
   // DispatchScanMatcherConstruction (constraint_builder_3d.cc:172-198)
-  csm_matcher3d* MatcherFor(const SubmapId& submap_id, const Submap3D* submap) {
-    csm_matcher3d*& m = matchers_[submap_id];
-    if (m == nullptr) {
-      const auto& o3 = options_.fast_correlative_scan_matcher_options_3d();
+  csm_matcher3d* MatcherFor(const Pending& p) {
+    csm_matcher3d*& m = matchers_[p.submap_id];
+    if (m == nullptr && p.device_submap != nullptr) {
+      const DeviceSubmap3D& d = *p.device_submap;
+      const csm_options3d o = scan_matching::b200_internal::Options3D(
+          options_.fast_correlative_scan_matcher_options_3d());
+      scan_matching::b200_internal::Check(csm_matcher3d_create_from_grid3d(
+          d.high_resolution_hybrid_grid->handle(), d.grid_size_in_voxels,
+          d.low_resolution_hybrid_grid->handle(), d.rotational_scan_matcher_histogram->data(),
+          static_cast<int32_t>(d.rotational_scan_matcher_histogram->size()), &o, &m));
+    } else if (m == nullptr) {
+      const Submap3D* submap = p.submap;
       std::vector<int32_t> hi_idx, lo_idx;
       std::vector<uint16_t> hi_val, lo_val;
       Flatten(submap->high_resolution_hybrid_grid(), &hi_idx, &hi_val);
       Flatten(submap->low_resolution_hybrid_grid(), &lo_idx, &lo_val);
-      csm_options3d o;
-      o.branch_and_bound_depth = o3.branch_and_bound_depth();
-      o.full_resolution_depth = o3.full_resolution_depth();
-      o.min_rotational_score = o3.min_rotational_score();
-      o.min_low_resolution_score = o3.min_low_resolution_score();
-      o.linear_xy_search_window = o3.linear_xy_search_window();
-      o.linear_z_search_window = o3.linear_z_search_window();
-      o.angular_search_window = o3.angular_search_window();
+      const csm_options3d o = scan_matching::b200_internal::Options3D(
+          options_.fast_correlative_scan_matcher_options_3d());
       const std::vector<float>& hist = submap->rotational_scan_matcher_histogram();
       scan_matching::b200_internal::Check(csm_matcher3d_create(
           hi_idx.data(), hi_val.data(), static_cast<int64_t>(hi_val.size()),
@@ -490,7 +538,7 @@ class ConstraintBuilder3D {
         auto mi = matcher_index.find(p.submap_id);
         if (mi == matcher_index.end()) {
           mi = matcher_index.emplace(p.submap_id, static_cast<int>(matchers.size())).first;
-          matchers.push_back(MatcherFor(p.submap_id, p.submap));
+          matchers.push_back(MatcherFor(p));
         }
         auto ni = node_index.find(p.constant_data);
         if (ni == node_index.end()) {
@@ -538,12 +586,21 @@ class ConstraintBuilder3D {
         for (size_t i = 0; i < pending_.size(); ++i) {
           if (!results[i].found) continue;
           const Pending& p = pending_[i];
-          auto& grids = device_grids_[p.submap_id];
-          if (grids.first == nullptr) {
-            grids.first.reset(new scan_matching::DeviceHybridGrid(
-                p.submap->high_resolution_hybrid_grid(), device_));
-            grids.second.reset(new scan_matching::DeviceHybridGrid(
-                p.submap->low_resolution_hybrid_grid(), device_));
+          const scan_matching::DeviceHybridGrid* high;
+          const scan_matching::DeviceHybridGrid* low;
+          if (p.device_submap != nullptr) {   // the submap's own grids
+            high = p.device_submap->high_resolution_hybrid_grid;
+            low = p.device_submap->low_resolution_hybrid_grid;
+          } else {
+            auto& grids = device_grids_[p.submap_id];
+            if (grids.first == nullptr) {
+              grids.first.reset(new scan_matching::DeviceHybridGrid(
+                  p.submap->high_resolution_hybrid_grid(), device_));
+              grids.second.reset(new scan_matching::DeviceHybridGrid(
+                  p.submap->low_resolution_hybrid_grid(), device_));
+            }
+            high = grids.first.get();
+            low = grids.second.get();
           }
           const csm_result3d& r = results[i];
           scan_matching::CeresScanMatcher3D::Job job;
@@ -553,8 +610,8 @@ class ConstraintBuilder3D {
               transform::Quaterniond{r.pose_estimate[3], r.pose_estimate[4], r.pose_estimate[5],
                                      r.pose_estimate[6]});
           job.point_clouds_and_hybrid_grids = {
-              {&p.constant_data->high_resolution_point_cloud, grids.first.get()},
-              {&p.constant_data->low_resolution_point_cloud, grids.second.get()}};
+              {&p.constant_data->high_resolution_point_cloud, high},
+              {&p.constant_data->low_resolution_point_cloud, low}};
           refined_of[i] = rjobs.size();
           rjobs.push_back(job);
         }

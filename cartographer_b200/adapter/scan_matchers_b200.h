@@ -466,6 +466,22 @@ class CeresScanMatcher2D {
 };
 
 #ifndef CSM_ADAPTER_REAL_CARTOGRAPHER
+namespace b200_internal {
+inline csm_options3d Options3D(const proto::FastCorrelativeScanMatcherOptions3D& options) {
+  csm_options3d o;
+  o.branch_and_bound_depth = options.branch_and_bound_depth();
+  o.full_resolution_depth = options.full_resolution_depth();
+  o.min_rotational_score = options.min_rotational_score();
+  o.min_low_resolution_score = options.min_low_resolution_score();
+  o.linear_xy_search_window = options.linear_xy_search_window();
+  o.linear_z_search_window = options.linear_z_search_window();
+  o.angular_search_window = options.angular_search_window();
+  return o;
+}
+}  // namespace b200_internal
+
+class DeviceHybridGrid;
+
 // fast_correlative_scan_matcher_3d.h:66-101.  (Inside a Cartographer checkout the
 // same body is used with HybridGrid::Iterator for the voxel walk, Eigen::VectorXf
 // for the histograms and TrajectoryNode::Data — see INTEGRATION.md §3.)
@@ -478,6 +494,15 @@ class FastCorrelativeScanMatcher3D {
     float low_resolution_score;
   };
 
+  // The matcher of a submap whose grids live on the device (Submap3D::InsertData on
+  // DeviceHybridGrids): built from the grids' non-zero voxels device to device, on their
+  // device.  It owns its copies; grid_size_in_voxels as HybridGrid::grid_size() (0 = derive it
+  // from the high-resolution grid's non-zero voxels).
+  FastCorrelativeScanMatcher3D(const DeviceHybridGrid& hybrid_grid,
+                               const DeviceHybridGrid* low_resolution_hybrid_grid,
+                               const std::vector<float>* rotational_scan_matcher_histogram,
+                               const proto::FastCorrelativeScanMatcherOptions3D& options,
+                               int grid_size_in_voxels = 0);
   FastCorrelativeScanMatcher3D(const HybridGrid& hybrid_grid,
                                const HybridGrid* low_resolution_hybrid_grid,
                                const std::vector<float>* rotational_scan_matcher_histogram,
@@ -487,14 +512,7 @@ class FastCorrelativeScanMatcher3D {
     std::vector<uint16_t> hi_val, lo_val;
     Flatten(hybrid_grid, &hi_idx, &hi_val);
     Flatten(*low_resolution_hybrid_grid, &lo_idx, &lo_val);
-    csm_options3d o;
-    o.branch_and_bound_depth = options.branch_and_bound_depth();
-    o.full_resolution_depth = options.full_resolution_depth();
-    o.min_rotational_score = options.min_rotational_score();
-    o.min_low_resolution_score = options.min_low_resolution_score();
-    o.linear_xy_search_window = options.linear_xy_search_window();
-    o.linear_z_search_window = options.linear_z_search_window();
-    o.angular_search_window = options.angular_search_window();
+    const csm_options3d o = b200_internal::Options3D(options);
     b200_internal::Check(csm_matcher3d_create(
         hi_idx.data(), hi_val.data(), static_cast<int64_t>(hi_val.size()),
         hybrid_grid.resolution(), hybrid_grid.grid_size(), lo_idx.data(), lo_val.data(),
@@ -601,6 +619,17 @@ class DeviceHybridGrid {
  private:
   csm_grid3d* grid_ = nullptr;
 };
+
+inline FastCorrelativeScanMatcher3D::FastCorrelativeScanMatcher3D(
+    const DeviceHybridGrid& hybrid_grid, const DeviceHybridGrid* low_resolution_hybrid_grid,
+    const std::vector<float>* rotational_scan_matcher_histogram,
+    const proto::FastCorrelativeScanMatcherOptions3D& options, int grid_size_in_voxels) {
+  const csm_options3d o = b200_internal::Options3D(options);
+  b200_internal::Check(csm_matcher3d_create_from_grid3d(
+      hybrid_grid.handle(), grid_size_in_voxels, low_resolution_hybrid_grid->handle(),
+      rotational_scan_matcher_histogram->data(),
+      static_cast<int32_t>(rotational_scan_matcher_histogram->size()), &o, &matcher_));
+}
 
 // An IntensityHybridGrid resident on the device (csm_intensity_grid3d), for the intensity
 // residual blocks of CeresScanMatcher3D (LocalTrajectoryBuilder3D passes the active submap's

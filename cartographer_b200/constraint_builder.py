@@ -392,11 +392,27 @@ class ConstraintBuilderOptions3D:
 @dataclass
 class Submap3D:
     """What the builder needs of a Submap3D (constraint_builder_3d.cc:172-198):
-    high / low resolution hybrid grids and the rotational scan matcher histogram."""
+    high / low resolution hybrid grids and the rotational scan matcher histogram.
+
+    The two grids are either host records (.resolution, .indices, .values) or, for a submap
+    kept on the device as RangeDataInserter3D fills it, two scan_matching.DeviceHybridGrids.
+    A device submap's matcher and refinement read its grids where they are; the caller keeps
+    them alive until WhenDone has run its callback."""
     high_resolution_hybrid_grid: object
     low_resolution_hybrid_grid: object
     rotational_scan_matcher_histogram: object
     grid_size_in_voxels: int = 0
+
+
+def _is_device_submap(submap):
+    """True for a Submap3D whose two grids are DeviceHybridGrids, False for host grids;
+    ValueError for one of each."""
+    from .scan_matching import DeviceHybridGrid
+    on_device = [isinstance(g, DeviceHybridGrid)
+                 for g in (submap.high_resolution_hybrid_grid, submap.low_resolution_hybrid_grid)]
+    if on_device[0] != on_device[1]:
+        raise ValueError("Submap3D: both grids must be DeviceHybridGrids, or neither")
+    return on_device[0]
 
 
 @dataclass
@@ -412,7 +428,9 @@ class _Job3:
 
 class CudaExecutor3D:
     """One csm_matcher3d per submap (DispatchScanMatcherConstruction,
-    constraint_builder_3d.cc:172-198); jobs run through csm_match3d_batch."""
+    constraint_builder_3d.cc:172-198); jobs run through csm_match3d_batch.  A device
+    submap's matcher is built from its DeviceHybridGrids without a host copy, and its
+    refinement reads them directly."""
 
     def __init__(self, options, device=0, threads=8):
         from . import scan_matching as sm
@@ -421,7 +439,8 @@ class CudaExecutor3D:
         self.device = device
         self.threads = threads
         self.matchers = {}
-        self.grids = {}    # submap id -> (high, low) DeviceHybridGrid, for the refinement
+        # submap id -> (high, low) DeviceHybridGrid uploaded for the refinement (host submaps)
+        self.grids = {}
         self.stats = {"candidates_scored": 0, "device_ms": 0.0, "searched": 0, "refined": 0,
                       "refine_device_ms": 0.0}
 
@@ -441,12 +460,16 @@ class CudaExecutor3D:
         pairs = []
         for i in idx:
             sid = jobs[i].submap_id
-            if sid not in self.grids:
-                sub = submaps[sid]
-                self.grids[sid] = (sm.DeviceHybridGrid(sub.high_resolution_hybrid_grid, self.device),
-                                   sm.DeviceHybridGrid(sub.low_resolution_hybrid_grid, self.device))
+            sub = submaps[sid]
+            if _is_device_submap(sub):
+                hi, lo = sub.high_resolution_hybrid_grid, sub.low_resolution_hybrid_grid
+            else:
+                if sid not in self.grids:
+                    self.grids[sid] = (
+                        sm.DeviceHybridGrid(sub.high_resolution_hybrid_grid, self.device),
+                        sm.DeviceHybridGrid(sub.low_resolution_hybrid_grid, self.device))
+                hi, lo = self.grids[sid]
             node = nodes[jobs[i].node_key]
-            hi, lo = self.grids[sid]
             pairs.append([(node.high_resolution_point_cloud, hi),
                           (node.low_resolution_point_cloud, lo)])
         matcher = sm.CeresScanMatcher3D(self.options.ceres_scan_matcher_options_3d)
@@ -466,15 +489,21 @@ class CudaExecutor3D:
         for j in jobs:
             if j.submap_id not in self.matchers:
                 sub = submaps[j.submap_id]
-                self.matchers[j.submap_id] = sm.FastCorrelativeScanMatcher3D(
-                    sub.high_resolution_hybrid_grid, sub.low_resolution_hybrid_grid,
-                    sub.rotational_scan_matcher_histogram,
-                    sm.FastCorrelativeScanMatcherOptions3D(
-                        o.branch_and_bound_depth, o.full_resolution_depth,
-                        o.min_rotational_score, o.min_low_resolution_score,
-                        o.linear_xy_search_window, o.linear_z_search_window,
-                        o.angular_search_window),
-                    device=self.device, grid_size_in_voxels=sub.grid_size_in_voxels)
+                fo = sm.FastCorrelativeScanMatcherOptions3D(
+                    o.branch_and_bound_depth, o.full_resolution_depth, o.min_rotational_score,
+                    o.min_low_resolution_score, o.linear_xy_search_window,
+                    o.linear_z_search_window, o.angular_search_window)
+                if _is_device_submap(sub):
+                    m = sm.FastCorrelativeScanMatcher3D.from_device_grids(
+                        sub.high_resolution_hybrid_grid, sub.low_resolution_hybrid_grid,
+                        sub.rotational_scan_matcher_histogram, fo,
+                        grid_size_in_voxels=sub.grid_size_in_voxels)
+                else:
+                    m = sm.FastCorrelativeScanMatcher3D(
+                        sub.high_resolution_hybrid_grid, sub.low_resolution_hybrid_grid,
+                        sub.rotational_scan_matcher_histogram, fo, device=self.device,
+                        grid_size_in_voxels=sub.grid_size_in_voxels)
+                self.matchers[j.submap_id] = m
 
         # one csm_match3d_batch call: the library keeps `threads` matches in flight on
         # separate CUDA streams (the reference's pool threads call Match concurrently
@@ -516,6 +545,12 @@ class ConstraintBuilder3D:
         self.last_records = None
 
     def _register(self, submap_id, submap, constant_data):
+        if self.pg is not None and _is_device_submap(submap):
+            import torch.distributed as dist
+            if dist.get_world_size(self.pg) > 1:
+                # the queue is sharded submap-major, but a device submap stays on the GPU that
+                # inserted it
+                raise ValueError("device-resident submaps are not sharded over several ranks")
         self._submaps[submap_id] = submap
         self._submap_order.setdefault(submap_id, len(self._submap_order))
         key = id(constant_data)

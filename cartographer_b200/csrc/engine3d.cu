@@ -15,6 +15,7 @@
 #include <functional>
 
 #include "common.cuh"
+#include "grid3d.cuh"
 #include "rigid3f.h"
 #include "value_conversion.h"
 
@@ -104,6 +105,99 @@ __global__ void k3_scatter_u16(const int* __restrict__ idx, const uint16_t* __re
   const int x = idx[3 * i] - v.lo[0], y = idx[3 * i + 1] - v.lo[1], z = idx[3 * i + 2] - v.lo[2];
   out[(static_cast<size_t>(z) * v.n[1] + y) * v.n[0] + x] = values[i];
 }
+
+// ---- the same from a csm_grid3d's dense box (csm_matcher3d_create_from_grid3d) ----
+// Launch shape of the three kernels below: x along a row of the box they walk (coalesced),
+// blockIdx.y strides over the rows (y + n1 * z).
+struct Box16 {
+  const uint16_t* p;
+  int lo[3];
+  int n[3];
+};
+
+// The bounding box of the non-zero cells of `b`, as offsets from b.lo: mn[0..2] receives the
+// min (atomicMin; the caller sets them to 0xffffffff), mx[0..2] the max + 1 (atomicMax; the
+// caller zeroes them), so mx[0] != 0 is the "any non-zero cell" flag.  Per thread, then per
+// block (warp reductions + shared memory), then six atomics per block that saw a cell.
+__global__ void __launch_bounds__(256)
+k3_nonzero_box(Box16 b, unsigned* __restrict__ mn_out, unsigned* __restrict__ mx_out) {
+  __shared__ unsigned s[6][8];
+  unsigned mn[3] = {0xffffffffu, 0xffffffffu, 0xffffffffu}, mx[3] = {0u, 0u, 0u};
+  const int x = blockIdx.x * blockDim.x + threadIdx.x;
+  const long long rows = static_cast<long long>(b.n[1]) * b.n[2];
+  if (x < b.n[0]) {
+    for (long long r = blockIdx.y; r < rows; r += gridDim.y) {
+      if (__ldg(b.p + r * b.n[0] + x) == 0) continue;
+      const unsigned y = static_cast<unsigned>(r % b.n[1]), z = static_cast<unsigned>(r / b.n[1]);
+      const unsigned c[3] = {static_cast<unsigned>(x), y, z};
+#pragma unroll
+      for (int a = 0; a < 3; ++a) {
+        mn[a] = min(mn[a], c[a]);
+        mx[a] = max(mx[a], c[a] + 1u);
+      }
+    }
+  }
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+#pragma unroll
+  for (int a = 0; a < 3; ++a) {
+    mn[a] = __reduce_min_sync(0xffffffffu, mn[a]);
+    mx[a] = __reduce_max_sync(0xffffffffu, mx[a]);
+    if (lane == 0) {
+      s[a][warp] = mn[a];
+      s[3 + a][warp] = mx[a];
+    }
+  }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    unsigned v[6];
+    for (int a = 0; a < 6; ++a) {
+      v[a] = s[a][0];
+      for (int w = 1; w < static_cast<int>(blockDim.x >> 5); ++w)
+        v[a] = a < 3 ? min(v[a], s[a][w]) : max(v[a], s[a][w]);
+    }
+    if (v[3] != 0u)
+      for (int a = 0; a < 3; ++a) {
+        atomicMin(&mn_out[a], v[a]);
+        atomicMax(&mx_out[a], v[3 + a]);
+      }
+  }
+}
+
+// The value of cell (x, y, z) of the source box, 0 outside it.
+__device__ __forceinline__ uint16_t Val16(const Box16& b, int x, int y, int z) {
+  const int lx = x - b.lo[0], ly = y - b.lo[1], lz = z - b.lo[2];
+  if (static_cast<unsigned>(lx) >= static_cast<unsigned>(b.n[0]) ||
+      static_cast<unsigned>(ly) >= static_cast<unsigned>(b.n[1]) ||
+      static_cast<unsigned>(lz) >= static_cast<unsigned>(b.n[2]))
+    return 0;
+  return __ldg(b.p + (static_cast<size_t>(lz) * b.n[1] + ly) * b.n[0] + lx);
+}
+
+// Depth 0 (ConvertToPrecomputationGrid) in gather form: one thread per level-0 cell.  A cell
+// outside the source box reads 0, which the LUT maps to 0 as the scatter form's memset leaves it.
+__global__ void __launch_bounds__(256)
+k3_gather_u8(Box16 src, const uint8_t* __restrict__ lut, Vol8 v, uint8_t* __restrict__ out) {
+  const int x = blockIdx.x * blockDim.x + threadIdx.x;
+  if (x >= v.n[0]) return;
+  const long long rows = static_cast<long long>(v.n[1]) * v.n[2];
+  for (long long r = blockIdx.y; r < rows; r += gridDim.y) {
+    const int y = static_cast<int>(r % v.n[1]), z = static_cast<int>(r / v.n[1]);
+    out[r * v.n[0] + x] = __ldg(lut + Val16(src, x + v.lo[0], y + v.lo[1], z + v.lo[2]));
+  }
+}
+
+// The low-resolution volume: the cells of the source box inside `v`, copied as they are.
+__global__ void __launch_bounds__(256)
+k3_gather_u16(Box16 src, Low3Dev v, uint16_t* __restrict__ out) {
+  const int x = blockIdx.x * blockDim.x + threadIdx.x;
+  if (x >= v.n[0]) return;
+  const long long rows = static_cast<long long>(v.n[1]) * v.n[2];
+  for (long long r = blockIdx.y; r < rows; r += gridDim.y) {
+    const int y = static_cast<int>(r % v.n[1]), z = static_cast<int>(r / v.n[1]);
+    out[r * v.n[0] + x] = Val16(src, x + v.lo[0], y + v.lo[1], z + v.lo[2]);
+  }
+}
+
 // PrecomputeGrid (precomputation_grid_3d.cc:63-81) in gather form: the reference
 // scatters every source voxel to the 8 cells idx - shift*octant (then floor-halves
 // the index if half_resolution); the cell c therefore receives the max over
@@ -651,48 +745,45 @@ constexpr size_t kRbBest = kRbCtr + 8 * 8;
 // Dives start only from scans whose best lowest-resolution sum is within 3 % of the best.
 constexpr float kDiveRatio = 0.97f;
 
-}  // namespace
-
-extern "C" {
-
-csm_status csm_matcher3d_create(const int32_t* hi_idx, const uint16_t* hi_val, int64_t hi_n,
-                                float hi_res, int32_t hi_grid_size, const int32_t* lo_idx,
-                                const uint16_t* lo_val, int64_t lo_n, float lo_res,
-                                const float* submap_hist, int32_t hist_n,
-                                const csm_options3d* options, int32_t device,
-                                csm_matcher3d** out) {
-  CSM_REQUIRE(out && options, "null pointer");
-  CSM_REQUIRE(hi_n >= 0 && lo_n >= 0 && (hi_n == 0 || (hi_idx && hi_val)) &&
-              (lo_n == 0 || (lo_idx && lo_val)), "voxel lists");
-  CSM_REQUIRE(hi_res > 0.f && lo_res > 0.f, "resolution");
+// The options csm_matcher3d_create accepts (fast_correlative_scan_matcher_3d.cc:60-61).
+csm_status CheckOptions3D(const csm_options3d* options) {
   CSM_REQUIRE(options->branch_and_bound_depth >= 1 &&
               options->branch_and_bound_depth <= kMaxDepth3, "branch_and_bound_depth");  // :60
   CSM_REQUIRE(options->full_resolution_depth >= 1, "full_resolution_depth");            // :61
-  CSM_REQUIRE(hist_n >= 0 && (hist_n == 0 || submap_hist), "histogram");
-  Ctx* ctx;
-  CSM_TRY(GetCtx(device, &ctx));
-  std::lock_guard<std::mutex> lock(ctx->mu);
-  CSM_CUDA(cudaSetDevice(device));
+  return CSM_OK;
+}
+
+// The inclusive bounding box of a set of voxels; {0, 0, 0} for an empty set.
+struct VoxelBox3 {
+  int lo[3] = {0, 0, 0};
+  int hi[3] = {0, 0, 0};
+};
+
+// What the two ways to build a csm_matcher3d differ in: how depth 0 and the low-resolution
+// volume are filled, on the context's stream, into volumes already zeroed.  Each gets the
+// box it fills and its destination; FillDepth0 also gets the device LUT of
+// ConvertToPrecomputationGrid (precomputation_grid_3d.cc:49-61).
+using FillDepth0 = std::function<csm_status(const Vol8& level0, uint8_t* dst, const uint8_t* lut)>;
+using FillLow = std::function<csm_status(const Low3Dev& low, uint16_t* dst)>;
+
+// FastCorrelativeScanMatcher3D's ctor over voxel boxes that are already known: level
+// geometry, the 24 GB guard, the allocations, the precomputation chain, the low-resolution
+// volume and the upload of the records and histogram; one stream synchronisation at the end.
+// The caller holds ctx->mu, has made the context's device current and checked `options`.
+csm_status BuildMatcher3D(Ctx* ctx, const VoxelBox3& hi_box, float hi_res, int32_t hi_grid_size,
+                          const VoxelBox3& lo_box, float lo_res, const float* submap_hist,
+                          int32_t hist_n, const csm_options3d* options,
+                          const FillDepth0& fill_depth0, const FillLow& fill_low,
+                          csm_matcher3d** out) {
+  const int* lo0 = hi_box.lo;
+  const int* hi0 = hi_box.hi;
+  for (int a = 0; a < 3; ++a)
+    CSM_REQUIRE(lo0[a] >= -8192 && hi0[a] < 8192, "voxel index outside the 2^14 cube");  // :387
   cudaStream_t s = ctx->stream;
   std::unique_ptr<csm_matcher3d> m(new csm_matcher3d);
   m->ctx = ctx;
   m->opt = *options;
   m->hist.assign(submap_hist, submap_hist + hist_n);
-
-  auto bbox = [](const int32_t* idx, int64_t n, int lo[3], int hi[3]) {
-    for (int a = 0; a < 3; ++a) { lo[a] = INT_MAX; hi[a] = INT_MIN; }
-    for (int64_t i = 0; i < n; ++i)
-      for (int a = 0; a < 3; ++a) {
-        lo[a] = std::min(lo[a], idx[3 * i + a]);
-        hi[a] = std::max(hi[a], idx[3 * i + a]);
-      }
-    if (n == 0)
-      for (int a = 0; a < 3; ++a) { lo[a] = 0; hi[a] = 0; }
-  };
-  int lo0[3], hi0[3];
-  bbox(hi_idx, hi_n, lo0, hi0);
-  for (int a = 0; a < 3; ++a)
-    CSM_REQUIRE(lo0[a] >= -8192 && hi0[a] < 8192, "voxel index outside the 2^14 cube");  // :387
   // HybridGrid::grid_size(): 64 << bits, bits >= 1, grown until every index fits
   int gs = 128;
   for (int a = 0; a < 3; ++a)
@@ -749,36 +840,22 @@ csm_status csm_matcher3d_create(const int32_t* hi_idx, const uint16_t* hi_val, i
       lut[v] = static_cast<uint8_t>(q < 0 ? 0 : (q > 255 ? 255 : q));
     }
   }
-  DevBuf& d_idx = ctx->D("m3_idx");
-  DevBuf& d_val = ctx->D("m3_val");
   DevBuf& d_lut = ctx->D("m3_lut");
   CSM_TRY(d_lut.Reserve(65536));
   CSM_CUDA(cudaMemcpyAsync(d_lut.p, lut.data(), 65536, cudaMemcpyHostToDevice, s));
-  if (hi_n > 0) {
-    CSM_TRY(d_idx.Reserve(sizeof(int) * 3 * hi_n));
-    CSM_TRY(d_val.Reserve(sizeof(uint16_t) * hi_n));
-    CSM_CUDA(cudaMemcpyAsync(d_idx.p, hi_idx, sizeof(int) * 3 * hi_n, cudaMemcpyHostToDevice, s));
-    CSM_CUDA(cudaMemcpyAsync(d_val.p, hi_val, sizeof(uint16_t) * hi_n, cudaMemcpyHostToDevice, s));
-    k3_scatter_u8<<<DivUp(hi_n, 256), 256, 0, s>>>(d_idx.as<int>(), d_val.as<uint16_t>(), hi_n,
-                                                    d_lut.as<uint8_t>(), hs.level[0],
-                                                    m->d_levels + off[0]);
-    CSM_LAUNCH_CHECK();
-  }
+  CSM_TRY(fill_depth0(hs.level[0], m->d_levels + off[0], d_lut.as<uint8_t>()));
   for (int d = 1; d < hs.depth; ++d) {
     k3_precompute<<<ctx->sm_count * 16, 256, 0, s>>>(hs.level[d - 1], hs.level[d],
                                                      m->d_levels + off[d], shifts[d], halfs[d]);
     CSM_LAUNCH_CHECK();
   }
-  CSM_CUDA(cudaStreamSynchronize(s));  // d_idx / d_val are reused below
 
   // ---- low-resolution grid ----
   Low3Dev& hl = m->hl;
   std::memset(&hl, 0, sizeof(hl));
-  int llo[3], lhi[3];
-  bbox(lo_idx, lo_n, llo, lhi);
   for (int a = 0; a < 3; ++a) {
-    hl.lo[a] = llo[a];
-    hl.n[a] = lhi[a] - llo[a] + 1;
+    hl.lo[a] = lo_box.lo[a];
+    hl.n[a] = lo_box.hi[a] - lo_box.lo[a] + 1;
   }
   const size_t lvox = static_cast<size_t>(hl.n[0]) * hl.n[1] * hl.n[2];
   CSM_REQUIRE(lvox < (size_t(4) << 30), "dense low-resolution volume too large");
@@ -792,15 +869,7 @@ csm_status csm_matcher3d_create(const int32_t* hi_idx, const uint16_t* hi_val, i
     hl.bias = probability.bias;
     hl.min_probability = kMinProbability;
   }
-  if (lo_n > 0) {
-    CSM_TRY(d_idx.Reserve(sizeof(int) * 3 * lo_n));
-    CSM_TRY(d_val.Reserve(sizeof(uint16_t) * lo_n));
-    CSM_CUDA(cudaMemcpyAsync(d_idx.p, lo_idx, sizeof(int) * 3 * lo_n, cudaMemcpyHostToDevice, s));
-    CSM_CUDA(cudaMemcpyAsync(d_val.p, lo_val, sizeof(uint16_t) * lo_n, cudaMemcpyHostToDevice, s));
-    k3_scatter_u16<<<DivUp(lo_n, 256), 256, 0, s>>>(d_idx.as<int>(), d_val.as<uint16_t>(), lo_n,
-                                                     hl, m->d_lowvol);
-    CSM_LAUNCH_CHECK();
-  }
+  CSM_TRY(fill_low(hl, m->d_lowvol));
   CSM_CUDA(cudaMalloc(&m->d_stack, sizeof(Stack3Dev)));
   CSM_CUDA(cudaMalloc(&m->d_low, sizeof(Low3Dev)));
   CSM_CUDA(cudaMalloc(&m->d_hist, sizeof(float) * std::max(1, hist_n)));
@@ -811,6 +880,155 @@ csm_status csm_matcher3d_create(const int32_t* hi_idx, const uint16_t* hi_val, i
                              cudaMemcpyHostToDevice, s));
   CSM_CUDA(cudaStreamSynchronize(s));
   *out = m.release();
+  return CSM_OK;
+}
+
+VoxelBox3 ListBox3(const int32_t* idx, int64_t n) {
+  VoxelBox3 b;
+  if (n == 0) return b;
+  for (int a = 0; a < 3; ++a) { b.lo[a] = INT_MAX; b.hi[a] = INT_MIN; }
+  for (int64_t i = 0; i < n; ++i)
+    for (int a = 0; a < 3; ++a) {
+      b.lo[a] = std::min(b.lo[a], idx[3 * i + a]);
+      b.hi[a] = std::max(b.hi[a], idx[3 * i + a]);
+    }
+  return b;
+}
+
+Box16 HandleBox(const csm_grid3d* g) {
+  Box16 b;
+  b.p = g->g.p;
+  for (int a = 0; a < 3; ++a) {
+    b.lo[a] = g->g.lo[a];
+    b.n[a] = g->g.n[a];
+  }
+  return b;
+}
+
+// Launch shape of k3_nonzero_box / k3_gather_*: x along the rows of a box of n[0] x rows
+// cells, blockIdx.y over the rows, at most `max_blocks` blocks in all.
+dim3 RowGrid(int nx, long long rows, int max_blocks) {
+  const int bx = DivUp(nx, 256);
+  const long long by = std::max<long long>(1, std::min<long long>(rows, max_blocks / bx));
+  return dim3(bx, static_cast<unsigned>(std::min<long long>(by, 65535)));
+}
+
+}  // namespace
+
+extern "C" {
+
+csm_status csm_matcher3d_create(const int32_t* hi_idx, const uint16_t* hi_val, int64_t hi_n,
+                                float hi_res, int32_t hi_grid_size, const int32_t* lo_idx,
+                                const uint16_t* lo_val, int64_t lo_n, float lo_res,
+                                const float* submap_hist, int32_t hist_n,
+                                const csm_options3d* options, int32_t device,
+                                csm_matcher3d** out) {
+  CSM_REQUIRE(out && options, "null pointer");
+  CSM_REQUIRE(hi_n >= 0 && lo_n >= 0 && (hi_n == 0 || (hi_idx && hi_val)) &&
+              (lo_n == 0 || (lo_idx && lo_val)), "voxel lists");
+  CSM_REQUIRE(hi_res > 0.f && lo_res > 0.f, "resolution");
+  CSM_TRY(CheckOptions3D(options));
+  CSM_REQUIRE(hist_n >= 0 && (hist_n == 0 || submap_hist), "histogram");
+  Ctx* ctx;
+  CSM_TRY(GetCtx(device, &ctx));
+  std::lock_guard<std::mutex> lock(ctx->mu);
+  CSM_CUDA(cudaSetDevice(device));
+  cudaStream_t s = ctx->stream;
+  DevBuf& d_idx = ctx->D("m3_idx");
+  DevBuf& d_val = ctx->D("m3_val");
+  // depth 0 and the low-resolution volume scattered from the lists; both lists go through
+  // the same staging, so the second waits until the first has been read
+  auto fill_depth0 = [&](const Vol8& level0, uint8_t* dst, const uint8_t* lut) -> csm_status {
+    if (hi_n == 0) return CSM_OK;
+    CSM_TRY(d_idx.Reserve(sizeof(int) * 3 * hi_n));
+    CSM_TRY(d_val.Reserve(sizeof(uint16_t) * hi_n));
+    CSM_CUDA(cudaMemcpyAsync(d_idx.p, hi_idx, sizeof(int) * 3 * hi_n, cudaMemcpyHostToDevice, s));
+    CSM_CUDA(cudaMemcpyAsync(d_val.p, hi_val, sizeof(uint16_t) * hi_n, cudaMemcpyHostToDevice, s));
+    k3_scatter_u8<<<DivUp(hi_n, 256), 256, 0, s>>>(d_idx.as<int>(), d_val.as<uint16_t>(), hi_n,
+                                                    lut, level0, dst);
+    CSM_LAUNCH_CHECK();
+    return CSM_OK;
+  };
+  auto fill_low = [&](const Low3Dev& low, uint16_t* dst) -> csm_status {
+    CSM_CUDA(cudaStreamSynchronize(s));
+    if (lo_n == 0) return CSM_OK;
+    CSM_TRY(d_idx.Reserve(sizeof(int) * 3 * lo_n));
+    CSM_TRY(d_val.Reserve(sizeof(uint16_t) * lo_n));
+    CSM_CUDA(cudaMemcpyAsync(d_idx.p, lo_idx, sizeof(int) * 3 * lo_n, cudaMemcpyHostToDevice, s));
+    CSM_CUDA(cudaMemcpyAsync(d_val.p, lo_val, sizeof(uint16_t) * lo_n, cudaMemcpyHostToDevice, s));
+    k3_scatter_u16<<<DivUp(lo_n, 256), 256, 0, s>>>(d_idx.as<int>(), d_val.as<uint16_t>(), lo_n,
+                                                     low, dst);
+    CSM_LAUNCH_CHECK();
+    return CSM_OK;
+  };
+  return BuildMatcher3D(ctx, ListBox3(hi_idx, hi_n), hi_res, hi_grid_size, ListBox3(lo_idx, lo_n),
+                        lo_res, submap_hist, hist_n, options, fill_depth0, fill_low, out);
+}
+
+csm_status csm_matcher3d_create_from_grid3d(const csm_grid3d* hybrid_grid,
+                                            int32_t grid_size_in_voxels,
+                                            const csm_grid3d* low_resolution_hybrid_grid,
+                                            const float* submap_hist, int32_t hist_n,
+                                            const csm_options3d* options, csm_matcher3d** out) {
+  CSM_REQUIRE(hybrid_grid && low_resolution_hybrid_grid && options && out, "null pointer");
+  CSM_REQUIRE(hybrid_grid->ctx == low_resolution_hybrid_grid->ctx,
+              "the two grids are on different devices");
+  CSM_TRY(CheckOptions3D(options));
+  CSM_REQUIRE(hist_n >= 0 && (hist_n == 0 || submap_hist), "histogram");
+  Ctx* ctx = hybrid_grid->ctx;
+  std::lock_guard<std::mutex> lock(ctx->mu);
+  CSM_CUDA(cudaSetDevice(ctx->device));
+  cudaStream_t s = ctx->stream;
+  const Box16 src[2] = {HandleBox(hybrid_grid), HandleBox(low_resolution_hybrid_grid)};
+  // ---- the non-zero boxes: [min x y z of both handles | max + 1 of both handles] ----
+  DevBuf* d_box;
+  CSM_TRY(ctx->Reserve("m3g_box", 12 * sizeof(unsigned), &d_box));
+  unsigned* box = d_box->as<unsigned>();
+  // with csm_profile_enable, the device spans of this call are recorded as "m3g_nonzero_box"
+  // (the two passes) and "m3g_build" (everything after the read-back)
+  ProfBegin(ctx);
+  CSM_CUDA(cudaMemsetAsync(box, 0xff, 6 * sizeof(unsigned), s));
+  CSM_CUDA(cudaMemsetAsync(box + 6, 0, 6 * sizeof(unsigned), s));
+  double cells = 0.;
+  for (int k = 0; k < 2; ++k) {
+    const long long rows = static_cast<long long>(src[k].n[1]) * src[k].n[2];
+    k3_nonzero_box<<<RowGrid(src[k].n[0], rows, ctx->sm_count * 8), 256, 0, s>>>(
+        src[k], box + 3 * k, box + 6 + 3 * k);
+    CSM_LAUNCH_CHECK();
+    cells += static_cast<double>(rows) * src[k].n[0];
+  }
+  ProfEnd(ctx, "m3g_nonzero_box", cells);
+  PinnedBuf& pin = ctx->P("m3g_box");
+  CSM_TRY(pin.Reserve(12 * sizeof(unsigned)));
+  unsigned* h = pin.as<unsigned>();
+  CSM_CUDA(cudaMemcpyAsync(h, box, 12 * sizeof(unsigned), cudaMemcpyDeviceToHost, s));
+  CSM_CUDA(cudaStreamSynchronize(s));
+  VoxelBox3 vb[2];
+  for (int k = 0; k < 2; ++k) {
+    if (h[6 + 3 * k] == 0u) continue;   // no non-zero cell: the empty list's box
+    for (int a = 0; a < 3; ++a) {
+      vb[k].lo[a] = src[k].lo[a] + static_cast<int>(h[3 * k + a]);
+      vb[k].hi[a] = src[k].lo[a] + static_cast<int>(h[6 + 3 * k + a]) - 1;
+    }
+  }
+  // ---- depth 0 and the low-resolution volume gathered from the handles ----
+  auto fill_depth0 = [&](const Vol8& level0, uint8_t* dst, const uint8_t* lut) -> csm_status {
+    const long long rows = static_cast<long long>(level0.n[1]) * level0.n[2];
+    k3_gather_u8<<<RowGrid(level0.n[0], rows, 1 << 16), 256, 0, s>>>(src[0], lut, level0, dst);
+    CSM_LAUNCH_CHECK();
+    return CSM_OK;
+  };
+  auto fill_low = [&](const Low3Dev& low, uint16_t* dst) -> csm_status {
+    const long long rows = static_cast<long long>(low.n[1]) * low.n[2];
+    k3_gather_u16<<<RowGrid(low.n[0], rows, 1 << 16), 256, 0, s>>>(src[1], low, dst);
+    CSM_LAUNCH_CHECK();
+    return CSM_OK;
+  };
+  ProfBegin(ctx);
+  CSM_TRY(BuildMatcher3D(ctx, vb[0], hybrid_grid->g.resolution, grid_size_in_voxels, vb[1],
+                         low_resolution_hybrid_grid->g.resolution, submap_hist, hist_n, options,
+                         fill_depth0, fill_low, out));
+  ProfEnd(ctx, "m3g_build", 0.);
   return CSM_OK;
 }
 

@@ -891,6 +891,26 @@ class FastCorrelativeScanMatcher3D:
                                                     C.byref(self._h)))
         return self
 
+    @classmethod
+    def from_device_grids(cls, hybrid_grid, low_resolution_hybrid_grid,
+                          rotational_scan_matcher_histogram, options, grid_size_in_voxels=0):
+        """From two DeviceHybridGrids (typically filled by RangeDataInserter3D), device to
+        device (csm_matcher3d_create_from_grid3d): the matcher the constructor builds from the
+        grids' non-zero voxels, on the grids' device.  It owns its copies, so later inserts
+        into the grids do not change it."""
+        self = cls.__new__(cls)
+        self.options, self.last_stats = options, None
+        hist = np.ascontiguousarray(rotational_scan_matcher_histogram, np.float32).reshape(-1)
+        o = CsmOptions3D(options.branch_and_bound_depth, options.full_resolution_depth,
+                         options.min_rotational_score, options.min_low_resolution_score,
+                         options.linear_xy_search_window, options.linear_z_search_window,
+                         options.angular_search_window)
+        self._h = C.c_void_p()
+        check(lib().csm_matcher3d_create_from_grid3d(
+            hybrid_grid._h, C.c_int32(grid_size_in_voxels), low_resolution_hybrid_grid._h,
+            ptr(hist, C.c_float), C.c_int32(len(hist)), C.byref(o), C.byref(self._h)))
+        return self
+
     def close(self):
         if getattr(self, "_h", None):
             lib().csm_matcher3d_destroy(self._h)

@@ -721,6 +721,21 @@ csm_status csm_range_inserter3d_insert(const csm_range_inserter3d* inserter,
  * (x - lo.x)).  For an intensity grid, sum and count (each may be NULL) are every voxel's
  * AverageIntensityData and mean its GetIntensity. */
 csm_status csm_grid3d_read(const csm_grid3d* grid, int32_t lo[3], int32_t dims[3], uint16_t* out);
+/* FastCorrelativeScanMatcher3D's ctor over device-resident grids: what csm_matcher3d_create
+ * builds from the NON-ZERO voxels of `hybrid_grid` and `low_resolution_hybrid_grid` (HybridGrid's
+ * iterator skips value 0, hybrid_grid.h:57) and their resolutions, device to device, without a
+ * host copy: every level, the low-resolution box, the derived grid size and every match result
+ * are the same.  The matcher lives on the handles' device and owns its copies: later inserts
+ * into, or destruction of, the handles do not change it.  No insert may be in flight on either
+ * handle during the call.  grid_size_in_voxels as in csm_matcher3d_create (0 = derive it from
+ * the high-resolution grid's non-zero voxels).  CSM_E_INVALID, with *out unwritten and nothing
+ * allocated, for a null handle, options or out, handles on different devices, or options
+ * csm_matcher3d_create refuses.  Two stream synchronisations. */
+csm_status csm_matcher3d_create_from_grid3d(const csm_grid3d* hybrid_grid,
+                                            int32_t grid_size_in_voxels,
+                                            const csm_grid3d* low_resolution_hybrid_grid,
+                                            const float* submap_histogram, int32_t histogram_size,
+                                            const csm_options3d* options, csm_matcher3d** out);
 csm_status csm_intensity_grid3d_read(const csm_intensity_grid3d* grid, int32_t lo[3],
                                      int32_t dims[3], float* mean, float* sum, int32_t* count);
 
