@@ -137,12 +137,13 @@ __global__ void k_stack_window(const uint8_t* __restrict__ lvl, int wx, int wy, 
 // ---------------------------------------------------------------------------
 // K2: GenerateRotatedScans + DiscretizeScans + ShrinkToFit
 // ---------------------------------------------------------------------------
-// One CTA per (job, scan) of the scans from scan0 on.  Writes the scan's cell indices and
-// its LinearBounds after ShrinkToFit (correlative_scan_matcher_2d.cc:73-127), plus the
+// One CTA per (job, scan) of the scans from scan0 on.  Writes the scan's cell indices (and,
+// with `merge`, its entries: JobDev::ent) and its LinearBounds after ShrinkToFit
+// (correlative_scan_matcher_2d.cc:73-127), plus the
 // number of lowest-resolution candidates per axis (fast...2d.cc:281-292).
 __global__ void __launch_bounds__(128)
 k_discretize(const JobDev* __restrict__ jobs, const int* __restrict__ scan_job,
-             short2* __restrict__ dscan, ScanInfo* __restrict__ info, int shrink,
+             short2* __restrict__ dscan, ScanInfo* __restrict__ info, int shrink, int merge,
              unsigned long long* __restrict__ counters, int scan0) {
   const int sg = scan0 + blockIdx.x;
   const int j = scan_job[sg];
@@ -151,7 +152,8 @@ k_discretize(const JobDev* __restrict__ jobs, const int* __restrict__ scan_job,
   const int k = sg - jb.scan_base;
   const float2 cs = jb.trig[k];
   const Quatf qk = QuatFromCosSinZ(cs.x, cs.y);
-  short2* out = dscan + jb.dscan_off + static_cast<long long>(k) * jb.n;
+  const long long base = jb.dscan_off + static_cast<long long>(k) * jb.n;
+  short2* out = dscan + base;
   int min_ix = INT_MAX, max_ix = INT_MIN, min_iy = INT_MAX, max_iy = INT_MIN;
   for (int p = threadIdx.x; p < jb.n; p += blockDim.x) {
     const Vec3f v{jb.xyz[3 * p], jb.xyz[3 * p + 1], jb.xyz[3 * p + 2]};
@@ -185,14 +187,86 @@ k_discretize(const JobDev* __restrict__ jobs, const int* __restrict__ scan_job,
     min_iy = min(min_iy, __shfl_xor_sync(0xffffffffu, min_iy, o));
     max_iy = max(max_iy, __shfl_xor_sync(0xffffffffu, max_iy, o));
   }
-  const int warp = threadIdx.x >> 5;
-  if ((threadIdx.x & 31) == 0) {
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  if (lane == 0) {
     red[warp][0] = min_ix;
     red[warp][1] = max_ix;
     red[warp][2] = min_iy;
     red[warp][3] = max_iy;
   }
-  __syncthreads();
+  __syncthreads();  // also: every cell of the scan is in `out`
+  // Merge the cells into entries (JobDev::ent / wt): a point whose cell differs from its
+  // predecessor's starts a run, and a run is cut every kMaxWeight points.  Each thread takes
+  // 4 consecutive points, so a round of the CTA covers 512 points with two barriers.
+  static_assert(kMaxWeight > 0 && (kMaxWeight & (kMaxWeight - 1)) == 0, "power of two");
+  constexpr int kPer = 4;
+  __shared__ int s_run[4], s_ent[4];
+  const int* __restrict__ cell = reinterpret_cast<const int*>(out);
+  int* __restrict__ ent = reinterpret_cast<int*>(jb.ent + base);
+  uint8_t* __restrict__ wt = jb.wt + base;
+  int run_c = -1, ent_c = 0;  // last run start before the round, entries before the round
+  for (int p0 = 0; merge && p0 < jb.n; p0 += kPer * 128) {
+    const int q0 = p0 + kPer * threadIdx.x;
+    int c[kPer + 2];          // c[0] = point q0 - 1, c[1 + u] = point q0 + u, c[5] = q0 + 4
+#pragma unroll
+    for (int u = 0; u < kPer + 2; ++u) {
+      const int q = q0 - 1 + u;
+      c[u] = q >= 0 && q < jb.n ? cell[q] : 0;
+    }
+    int lh = -1;              // last run start among the thread's points
+#pragma unroll
+    for (int u = 0; u < kPer; ++u) {
+      const int q = q0 + u;
+      if (q < jb.n && (q == 0 || c[u + 1] != c[u])) lh = q;
+    }
+    // run start before the thread's points: max over earlier threads and rounds
+    int incl = lh;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+      const int v = __shfl_up_sync(0xffffffffu, incl, o);
+      if (lane >= o) incl = max(incl, v);
+    }
+    int rs = __shfl_up_sync(0xffffffffu, incl, 1);
+    if (lane == 0) rs = -1;
+    if (lane == 31) s_run[warp] = incl;
+    __syncthreads();
+    rs = max(rs, run_c);
+    for (int w = 0; w < 4; ++w) {
+      if (w < warp) rs = max(rs, s_run[w]);
+      run_c = max(run_c, s_run[w]);
+    }
+    int off[kPer], cnt = 0;
+#pragma unroll
+    for (int u = 0; u < kPer; ++u) {
+      const int q = q0 + u;
+      if (q < jb.n && (q == 0 || c[u + 1] != c[u])) rs = q;
+      off[u] = q - rs;
+      if (q < jb.n && (off[u] & (kMaxWeight - 1)) == 0) ++cnt;
+    }
+    int ce = cnt;             // inclusive count of entry starts
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+      const int v = __shfl_up_sync(0xffffffffu, ce, o);
+      if (lane >= o) ce += v;
+    }
+    if (lane == 31) s_ent[warp] = ce;
+    __syncthreads();
+    int e = ent_c + ce - cnt - 1;  // entry of the point before the thread's first
+    for (int w = 0; w < 4; ++w) {
+      if (w < warp) e += s_ent[w];
+      ent_c += s_ent[w];
+    }
+#pragma unroll
+    for (int u = 0; u < kPer; ++u) {
+      const int q = q0 + u;
+      if (q >= jb.n) break;
+      if ((off[u] & (kMaxWeight - 1)) == 0) ++e;
+      if (q + 1 >= jb.n || c[u + 2] != c[u + 1] || ((off[u] + 1) & (kMaxWeight - 1)) == 0) {
+        ent[e] = c[u + 1];   // the entry's last point writes it
+        wt[e] = static_cast<uint8_t>((off[u] & (kMaxWeight - 1)) + 1);
+      }
+    }
+  }
   if (threadIdx.x == 0) {
     for (int w = 1; w < 4; ++w) {
       red[0][0] = min(red[0][0], red[w][0]);
@@ -218,7 +292,7 @@ k_discretize(const JobDev* __restrict__ jobs, const int* __restrict__ scan_job,
     const int step = 1 << (st.depth - 1);
     si.nxc = (si.max_x - si.min_x + step) / step;
     si.nyc = (si.max_y - si.min_y + step) / step;
-    si.pad = 0;
+    si.entries = ent_c;
     if (shrink && (si.nyc > jb.cap_y || static_cast<long long>(si.nxc) * jb.cap_y > jb.cap)) {
       // the host's a-priori slot bound must cover the lattice (reported as an error)
       counters[6] = 1ull;
@@ -480,14 +554,14 @@ k_score_top_dense(const JobDev* __restrict__ jobs, const ScanInfo* __restrict__ 
 // read exactly one tile of the decimated level: jd rows of ids bytes, contiguous in
 // memory (phase (ax, ay) of StackDev::dec4).  MatchFullSubmap lattices are wider than
 // that tile (most candidate/point pairs lie outside the grid), so instead of every
-// candidate walking all points, ONE WARP walks the points of a scan and adds each
-// point's tile into the lattice:
+// candidate walking all points, ONE WARP walks the entries of a scan and adds each
+// entry's tile, times its weight, into the lattice:
 //   * lane l owns the tile words f = l - 1 + 32*it (fully coalesced 128 B loads);
 //   * the word offset between tile and lattice, (qx, qy), only changes when the point
 //     moves to another coarse cell; consecutive beams mostly stay in one, so the
-//     lanes accumulate in REGISTERS (packed u16 pairs) across a run of points and add
+//     lanes accumulate in REGISTERS (packed u16 pairs) across a run of entries and add
 //     the run into the 32-bit lattice in shared memory when (qx, qy) changes (or
-//     after 256 points, before the u16 lanes can overflow);
+//     once the run's weight would pass 256, before the u16 lanes can overflow);
 //   * copy k = qx & 3 of dec4 aligns tile words with lattice quads.
 // Integer sums are order independent, so the result equals k_score_top_dense's.
 #ifndef CSM_TILE_THREADS
@@ -502,12 +576,14 @@ k_score_top_tile(const JobDev* __restrict__ jobs, const ScanInfo* __restrict__ i
                  const long long* __restrict__ scan_slot_base, int scan0, int scan_end,
                  int lat_ints) {
   extern __shared__ __align__(16) int s_lat_all[];
-  __shared__ __align__(16) int s_key_all[kTileWarps][32], s_off_all[kTileWarps][32];
+  __shared__ __align__(16) int s_key_all[kTileWarps][32], s_off_all[kTileWarps][32],
+      s_wt_all[kTileWarps][32];
   constexpr int kNoKey = 0x7fff7fff;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   int* __restrict__ s_lat = s_lat_all + warp * lat_ints;  // [nyc][qr] quads of 4 ints
   int* __restrict__ s_key = s_key_all[warp];
   int* __restrict__ s_off = s_off_all[warp];
+  int* __restrict__ s_wt = s_wt_all[warp];
   const int nwarps = gridDim.x * kTileWarps;
   for (int sg = scan0 + blockIdx.x * kTileWarps + warp; sg < scan_end; sg += nwarps) {
     const ScanInfo si = info[sg];
@@ -522,15 +598,17 @@ k_score_top_tile(const JobDev* __restrict__ jobs, const ScanInfo* __restrict__ i
     const int W = jd * rw + 1;       // tile words incl. the one before the tile (f = -1)
     const int qr = (si.nxc + 3) >> 2;
     const int lat_n = qr * 4 * si.nyc;
-    const short2* __restrict__ pts = dscan + jb.dscan_off +
-                                   static_cast<long long>(sg - jb.scan_base) * jb.n;
+    const long long base = jb.dscan_off + static_cast<long long>(sg - jb.scan_base) * jb.n;
+    const short2* __restrict__ pts = jb.ent + base;
+    const uint8_t* __restrict__ wts = jb.wt + base;
+    const int m = si.entries;
     int* __restrict__ out = top_sum + scan_slot_base[sg];
     for (int t = lane; t < lat_n; t += 32) s_lat[t] = 0;
     unsigned a02[kIters], a13[kIters];
 #pragma unroll
     for (int it = 0; it < kIters; ++it) a02[it] = a13[it] = 0u;
     int cur_key = kNoKey;      // (qy << 16) | (qx & 0xffff) of the current run
-    int run = 0;
+    int run = 0;               // weight of the current run
     const uint8_t* cur_base = dec;
     // adds the run's register sums into the lattice
     // tile row and byte column (before the copy shift k) of this lane's words
@@ -566,28 +644,32 @@ k_score_top_tile(const JobDev* __restrict__ jobs, const ScanInfo* __restrict__ i
         a02[it] = a13[it] = 0u;
       }
     };
-    for (int p0 = 0; p0 < jb.n; p0 += 32) {
-      int my_off = 0, my_key = kNoKey;
-      if (p0 + lane < jb.n) {
+    for (int p0 = 0; p0 < m; p0 += 32) {
+      int my_off = 0, my_key = kNoKey, my_wt = 0;
+      if (p0 + lane < m) {
         const short2 c = pts[p0 + lane];
         const int bx = c.x + si.min_x + s1, by = c.y + si.min_y + s1;
         const int qx = bx >> h, qy = by >> h;  // floor division
         if (qx > -32000 && qx < 32000 && qy > -32000 && qy < 32000) {
           my_off = ((((by & s1) << h) | (bx & s1)) * jd) * ids;
           my_key = (qy << 16) | (qx & 0xffff);
+          my_wt = wts[p0 + lane];
         }
       }
       __syncwarp();
       s_key[lane] = my_key;
       s_off[lane] = my_off;
+      s_wt[lane] = my_wt;
       __syncwarp();
-      for (int t = 0; t < 32; t += 4) {   // points past the end carry kNoKey
+      for (int t = 0; t < 32; t += 4) {   // entries past the end carry kNoKey
         const int4 key = *reinterpret_cast<const int4*>(s_key + t);
         const int4 off = *reinterpret_cast<const int4*>(s_off + t);
+        const int4 wt = *reinterpret_cast<const int4*>(s_wt + t);
+        const int w4 = (wt.x + wt.y) + (wt.z + wt.w);
         if (key.x == cur_key && key.y == cur_key && key.z == cur_key && key.w == cur_key &&
-            run <= 252 && cur_key != kNoKey) {
-          // four points of the current run: 4 * kIters independent loads in flight
-          run += 4;
+            run + w4 <= 256 && cur_key != kNoKey) {
+          // four entries of the current run: 4 * kIters independent loads in flight
+          run += w4;
           unsigned w[4][kIters];
 #pragma unroll
           for (int it = 0; it < kIters; ++it) {
@@ -599,31 +681,35 @@ k_score_top_tile(const JobDev* __restrict__ jobs, const ScanInfo* __restrict__ i
           }
 #pragma unroll
           for (int it = 0; it < kIters; ++it) {
-            a02[it] += (__byte_perm(w[0][it], 0u, 0x4240) + __byte_perm(w[1][it], 0u, 0x4240)) +
-                       (__byte_perm(w[2][it], 0u, 0x4240) + __byte_perm(w[3][it], 0u, 0x4240));
-            a13[it] += (__byte_perm(w[0][it], 0u, 0x4341) + __byte_perm(w[1][it], 0u, 0x4341)) +
-                       (__byte_perm(w[2][it], 0u, 0x4341) + __byte_perm(w[3][it], 0u, 0x4341));
+            a02[it] += (__byte_perm(w[0][it], 0u, 0x4240) * wt.x +
+                        __byte_perm(w[1][it], 0u, 0x4240) * wt.y) +
+                       (__byte_perm(w[2][it], 0u, 0x4240) * wt.z +
+                        __byte_perm(w[3][it], 0u, 0x4240) * wt.w);
+            a13[it] += (__byte_perm(w[0][it], 0u, 0x4341) * wt.x +
+                        __byte_perm(w[1][it], 0u, 0x4341) * wt.y) +
+                       (__byte_perm(w[2][it], 0u, 0x4341) * wt.z +
+                        __byte_perm(w[3][it], 0u, 0x4341) * wt.w);
           }
           continue;
         }
 #pragma unroll 1
         for (int u = 0; u < 4; ++u) {
-          const int ku = s_key[t + u], ou = s_off[t + u];
-          if (ku != cur_key || run == 256) {
+          const int ku = s_key[t + u], ou = s_off[t + u], wu = s_wt[t + u];
+          if (ku != cur_key || run + wu > 256) {
             if (run) flush();
             cur_key = ku;
             run = 0;
             cur_base = dec + (cur_key & 3) * lpad - 4 + 4 * lane;
           }
-          if (ku == kNoKey) continue;  // point cannot hit the grid / past the end
-          ++run;
+          if (ku == kNoKey) continue;  // entry cannot hit the grid / past the end
+          run += wu;
           const unsigned* __restrict__ q = reinterpret_cast<const unsigned*>(cur_base + ou);
 #pragma unroll
           for (int it = 0; it < kIters; ++it) {
             if (lane + 32 * it < W) {
               const unsigned w = __ldg(q + 32 * it);
-              a02[it] += __byte_perm(w, 0u, 0x4240);  // bytes 0 and 2 in u16 lanes
-              a13[it] += __byte_perm(w, 0u, 0x4341);  // bytes 1 and 3
+              a02[it] += __byte_perm(w, 0u, 0x4240) * wu;  // bytes 0 and 2 in u16 lanes
+              a13[it] += __byte_perm(w, 0u, 0x4341) * wu;  // bytes 1 and 3
             }
           }
         }
@@ -1811,7 +1897,8 @@ struct Batch2D {
   int total_scans = 0;
   // workspaces
   DevBuf *d_trig = nullptr, *d_jobs = nullptr, *d_scan_job = nullptr, *d_slot_base = nullptr,
-         *d_info = nullptr, *d_dscan = nullptr, *d_top = nullptr, *d_lb = nullptr,
+         *d_info = nullptr, *d_dscan = nullptr, *d_ent = nullptr, *d_wt = nullptr,
+         *d_top = nullptr, *d_lb = nullptr,
          *d_ctr = nullptr, *d_job_best = nullptr;
   DevBuf *d_qtop = nullptr, *d_q = nullptr, *d_leaves = nullptr, *d_best = nullptr,
          *d_scan_cnt = nullptr, *d_scan_off = nullptr, *d_items = nullptr, *d_sorted = nullptr;
@@ -1971,11 +2058,17 @@ csm_status Upload2D(Batch2D& b) {
   CSM_TRY(ctx->Reserve("slot_base", sizeof(long long) * plan.total_scans, &b.d_slot_base));
   CSM_TRY(ctx->Reserve("info", sizeof(ScanInfo) * plan.total_scans, &b.d_info));
   CSM_TRY(ctx->Reserve("dscan", sizeof(short2) * plan.total_points, &b.d_dscan));
+  CSM_TRY(ctx->Reserve("dscan_ent", sizeof(short2) * plan.total_points, &b.d_ent));
+  CSM_TRY(ctx->Reserve("dscan_wt", plan.total_points, &b.d_wt));
   CSM_TRY(ctx->Reserve("lb", sizeof(unsigned) * num_jobs, &b.d_lb));
   CSM_TRY(ctx->Reserve("counters", sizeof(unsigned long long) * 8 + sizeof(int) * kCtlInts,
                        &b.d_ctr));
   CSM_TRY(ctx->Reserve("job_best", sizeof(int) * num_jobs, &b.d_job_best));
-  for (int j = 0; j < num_jobs; ++j) plan.jobs[j].trig = b.d_trig->as<float2>() + b.trig_off[j];
+  for (int j = 0; j < num_jobs; ++j) {
+    plan.jobs[j].trig = b.d_trig->as<float2>() + b.trig_off[j];
+    plan.jobs[j].ent = b.d_ent->as<short2>();
+    plan.jobs[j].wt = b.d_wt->as<uint8_t>();
+  }
 
   // uploads go through pinned staging so that they are truly asynchronous (the
   // previous call on this lane has completed: every call ends with a synchronise)
@@ -1997,8 +2090,8 @@ csm_status Upload2D(Batch2D& b) {
 }
 
 // Jobs [j0, j1): the rotation tables they use first are computed into the staging buffer
-// and uploaded, then their scans are discretised.
-csm_status Discretize2D(Batch2D& b, int j0, int j1) {
+// and uploaded, then their scans are discretised (`merge`: also as entries, for the tile form).
+csm_status Discretize2D(Batch2D& b, int j0, int j1, bool merge) {
   cudaStream_t s = b.s;
   const size_t t0 = b.tables_before[j0], t1 = b.tables_before[j1];
   if (t1 > t0) FillTrigTables(b.trig_tables, t0, t1, b.up_trig);
@@ -2015,7 +2108,7 @@ csm_status Discretize2D(Batch2D& b, int j0, int j1) {
   if (s1 > s0) {
     k_discretize<<<s1 - s0, 128, 0, s>>>(b.d_jobs->as<JobDev>(), b.d_scan_job->as<int>(),
                                          b.d_dscan->as<short2>(), b.d_info->as<ScanInfo>(), 1,
-                                         b.ctr, s0);
+                                         merge ? 1 : 0, b.ctr, s0);
     CSM_LAUNCH_CHECK();
   }
   const long long pt0 = b.plan.jobs[j0].dscan_off;
@@ -2115,7 +2208,7 @@ csm_status TopPass2D(Batch2D& b) {
   }
   for (size_t g = 0, j0 = 0; g < group_end.size(); j0 = group_end[g++]) {
     const int j1 = group_end[g];
-    CSM_TRY(Discretize2D(b, static_cast<int>(j0), j1));
+    CSM_TRY(Discretize2D(b, static_cast<int>(j0), j1, use_tile_top));
     if (use_tile_top) {
       ProfBegin(ctx);
       CSM_TRY(LaunchTile2D(b, plan.jobs[j0].scan_base, b.ScanEnd(j1), tile_words, lat_ints));
@@ -2699,7 +2792,7 @@ csm_status csm_discretize2d(const csm_stack2d* stack, const float* xyz, int32_t 
   CSM_TRY(PlanHook2D(hk, Forms2D()));
   Batch2D& b = hk.b;
   CSM_TRY(Upload2D(b));
-  CSM_TRY(Discretize2D(b, 0, 1));
+  CSM_TRY(Discretize2D(b, 0, 1, false));
   std::vector<short2> h_ds(discrete_scans ? b.plan.total_points : 0);
   if (discrete_scans)
     CSM_CUDA(cudaMemcpyAsync(h_ds.data(), b.d_dscan->p, sizeof(short2) * h_ds.size(),

@@ -60,15 +60,25 @@ struct JobDev {
   Quatf q0;              // initial rotation as Quaternionf(AngleAxisf(yaw, UnitZ))
   float tx, ty;          // initial translation (float casts)
   float min_score;
-  long long dscan_off;   // first int2 of this job in the discrete-scan buffer
+  // Discrete scans: scan k of the job owns n slots from dscan_off + k * n of the point
+  // buffer (short2 cells per point), of `ent` and of `wt`.  When the tile form of the
+  // lowest-resolution pass runs, the first ScanInfo::entries slots of `ent` / `wt` hold the
+  // runs of equal consecutive cells in beam order, one entry per run of at most kMaxWeight
+  // points, with the run length as weight, and the tile pass walks those.
+  short2* ent;
+  uint8_t* wt;
+  long long dscan_off;   // first slot of this job in the discrete-scan buffers
   long long top_off;     // first slot of this job in the top-level sum buffer
 };
+
+// Largest weight of one entry (the tile pass flushes its packed u16 sums by weight).
+constexpr int kMaxWeight = 4;
 
 struct ScanInfo {
   int job;
   int min_x, max_x, min_y, max_y;  // LinearBounds after ShrinkToFit
   int nxc, nyc;                    // lowest-resolution candidates per axis
-  int pad;
+  int entries;                     // entries of the discrete scan (0 unless merged)
 };
 
 struct Node {  // 16 B
