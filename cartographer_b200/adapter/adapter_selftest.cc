@@ -534,6 +534,133 @@ int main() {
     for (uint8_t v : level) std::printf(" %u", v);
     std::printf("\n");
   }
+  // ---- ConstraintBuilder2D on device submaps: two submaps grown by the inserter in a 6 m x 4 m
+  // room with a pillar, cropped, and driven through the reference's call cycle
+  // (constraint_builder_2d_test.cc:58-112) as DeviceSubmap2Ds, unrefined and with the device
+  // refinement.  The same queues on host Submap2Ds made from the cells read back print the
+  // *_host lines, which tests/test_gpu_adapter_cb2d_device_submaps.py holds equal to the
+  // *_dev lines ----
+  {
+    // a 1° scan of the room [-3, 3] x [-2, 2] with the pillar [1, 1.4] x [0.5, 0.9], from (x, y)
+    const auto scan = [](double x, double y) {
+      std::vector<sensor::RangefinderPoint> points;
+      for (int k = 0; k < 360; ++k) {
+        const double a = k * M_PI / 180. + 0.01, c = std::cos(a), s = std::sin(a);
+        double t = 1e9;
+        for (double wall : {3. - x, -3. - x})
+          if (c * wall > 0) t = std::min(t, wall / c);
+        for (double wall : {2. - y, -2. - y})
+          if (s * wall > 0) t = std::min(t, wall / s);
+        for (double px : {1. - x, 1.4 - x}) {   // the pillar's two x faces
+          const double u = px / c;
+          if (u > 0 && y + u * s >= 0.5 && y + u * s <= 0.9) t = std::min(t, u);
+        }
+        for (double py : {0.5 - y, 0.9 - y}) {   // and its two y faces
+          const double u = py / s;
+          if (u > 0 && x + u * c >= 1. && x + u * c <= 1.4) t = std::min(t, u);
+        }
+        points.push_back({{{static_cast<float>(t * c), static_cast<float>(t * s), 0.f}}});
+      }
+      return points;
+    };
+    mapping::proto::ProbabilityGridRangeDataInserterOptions2D io;
+    io.set_hit_probability(0.55);
+    io.set_miss_probability(0.49);
+    io.set_insert_free_space(true);
+    const mapping::scan_matching::ProbabilityGridRangeDataInserter2D inserter(io);
+    const double origins[2][2] = {{-0.4, -0.3}, {0.6, 0.2}};
+    std::vector<std::unique_ptr<mapping::scan_matching::DeviceGrid2D>> cropped;
+    std::vector<std::unique_ptr<mapping::Grid2D>> host_grids;
+    for (const auto& o : origins) {
+      // ActiveSubmaps2D::CreateGrid(origin): 100 x 100 cells, max = origin + 50 * resolution
+      mapping::scan_matching::DeviceGrid2D grid(
+          mapping::MapLimits(0.05, o[0] + 2.5, o[1] + 2.5, mapping::CellLimits{100, 100}), 0);
+      for (int k = 0; k < 4; ++k) {
+        const double x = o[0] + 0.1 * k, y = o[1] - 0.05 * k;
+        sensor::RangeData range_data;
+        range_data.origin = {{static_cast<float>(x), static_cast<float>(y), 0.f}};
+        for (const auto& p : scan(x, y))
+          range_data.returns.push_back({{{p.position.x() + static_cast<float>(x),
+                                          p.position.y() + static_cast<float>(y), 0.f}}});
+        inserter.Insert(range_data, &grid);
+      }
+      cropped.push_back(grid.ComputeCroppedGrid());
+      std::vector<uint16_t> cells;
+      const csm_rt_grid2d_info info = cropped.back()->Read(&cells);
+      if (info.is_tsdf != 0 || cropped.back()->device() != 0) return 1;
+      host_grids.emplace_back(new mapping::Grid2D(
+          mapping::MapLimits(info.resolution, info.max_x, info.max_y,
+                             mapping::CellLimits{info.num_x_cells, info.num_y_cells}),
+          1.f - 0.9f, 1.f - 0.1f, cells));   // kMin / kMaxCorrespondenceCost
+    }
+    const transform::Rigid2d local_poses[2] = {transform::Rigid2d({-0.4, -0.3}, 0.),
+                                               transform::Rigid2d({0.6, 0.2}, 0.)};
+    const mapping::constraints::DeviceSubmap2D dsubs[2] = {{cropped[0].get(), local_poses[0]},
+                                                            {cropped[1].get(), local_poses[1]}};
+    const mapping::Submap2D hsubs[2] = {{host_grids[0].get(), local_poses[0]},
+                                        {host_grids[1].get(), local_poses[1]}};
+    mapping::TrajectoryNodeData nodes[2];
+    const double node_xy[2][2] = {{0.1, 0.3}, {-0.7, -0.5}};
+    for (int n = 0; n < 2; ++n)
+      for (const auto& p : scan(node_xy[n][0], node_xy[n][1]))
+        nodes[n].filtered_gravity_aligned_point_cloud.push_back(p);
+    using mapping::constraints::ConstraintBuilder2D;
+    mapping::constraints::proto::ConstraintBuilderOptions bo;
+    bo.sampling_ratio_ = 1.0;
+    bo.max_constraint_distance_ = 10.0;
+    bo.min_score_ = 0.3;
+    bo.global_localization_min_score_ = 0.3;
+    bo.fast2d_ = options;   // 1 m / 0.3 rad window, depth 4
+    common::InlineThreadPool pool;
+    for (int refine = 0; refine < 2; ++refine) {
+      for (int side = 0; side < 2; ++side) {
+        ConstraintBuilder2D builder(bo, &pool);
+        builder.set_device_refinement(refine == 1);
+        // two rounds, with DeleteScanMatcher in between: the second rebuilds both stacks
+        for (int round = 0; round < 2; ++round) {
+          for (int n = 0; n < 2; ++n) {
+            for (int s = 0; s < 2; ++s) {
+              const mapping::SubmapId sid{0, s};
+              // a start 5 cm and 0.02 rad off the node's true pose
+              const transform::Rigid2d relative =
+                  local_poses[s].inverse() *
+                  transform::Rigid2d({node_xy[n][0] + 0.05, node_xy[n][1] - 0.03}, 0.02);
+              if (side == 0)
+                builder.MaybeAddConstraint(sid, &dsubs[s], mapping::NodeId{0, n}, &nodes[n],
+                                           relative);
+              else
+                builder.MaybeAddConstraint(sid, &hsubs[s], mapping::NodeId{0, n}, &nodes[n],
+                                           relative);
+            }
+            const mapping::SubmapId gid{0, n};
+            if (side == 0)
+              builder.MaybeAddGlobalConstraint(gid, &dsubs[n], mapping::NodeId{0, n}, &nodes[n]);
+            else
+              builder.MaybeAddGlobalConstraint(gid, &hsubs[n], mapping::NodeId{0, n}, &nodes[n]);
+            builder.NotifyEndOfNode();
+          }
+          int calls = 0;
+          ConstraintBuilder2D::Result got;
+          builder.WhenDone([&](const ConstraintBuilder2D::Result& r) { ++calls; got = r; });
+          if (calls != 1 || got.empty() || builder.GetNumFinishedNodes() != 2 * (round + 1))
+            return 1;
+          for (const auto& c : got) {
+            const transform::Rigid3d& z = c.pose.zbar_ij;
+            std::printf("RESULT cb2d_device_submaps%s_%s %d %d %d %.17g %.17g %.17g %.17g %lld\n",
+                        refine ? "_refined" : "", side == 0 ? "dev" : "host", round,
+                        c.submap_id.submap_index, c.node_id.node_index, z.translation().x(),
+                        z.translation().y(), z.rotation().w(), z.rotation().z(),
+                        static_cast<long long>(builder.last_stats().candidates_scored));
+          }
+          for (int s = 0; s < 2; ++s) builder.DeleteScanMatcher(mapping::SubmapId{0, s});
+        }
+      }
+    }
+    // the handles outlive their builders and are still readable
+    std::vector<uint16_t> after;
+    cropped[0]->Read(&after);
+    if (after != host_grids[0]->correspondence_cost_cells()) return 1;
+  }
   // ---- TSDFRangeDataInserter2D on a device grid: the reference's InsertPoint
   // (tsdf_range_data_inserter_2d_test.cc:50-57, the 8 x 1 grid that grows), then two returns
   // with the lua defaults' normal projection and weighting ----

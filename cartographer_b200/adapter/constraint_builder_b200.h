@@ -46,6 +46,19 @@ inline transform::Rigid3d Embed3D(const transform::Rigid2d& t) {
 }
 }  // namespace b200_internal
 
+// A finished Submap2D whose grid lives on the device, as Submap2D::Finish leaves it when the
+// submap was grown by scan_matching::ProbabilityGridRangeDataInserter2D and cropped with
+// DeviceGrid2D::ComputeCroppedGrid: what ConstraintBuilder2D reads of it.  Unlike
+// DeviceSubmap3D it is not limited to the stand-in build, because ConstraintBuilder2D is not.
+// The builder keeps the pointer, so the grid must stay alive (and unchanged) until the
+// WhenDone callback of every drain holding one of its pairs has run
+// (constraint_builder_2d.h:76-77).  The stack is built from the grid and owns its levels:
+// DeleteScanMatcher never touches the grid, and adding the submap again rebuilds the stack.
+struct DeviceSubmap2D {
+  const scan_matching::DeviceGrid2D* grid;   // the cropped ProbabilityGrid handle
+  transform::Rigid2d local_pose_2d;          // ComputeSubmapPose(submap)
+};
+
 class ConstraintBuilder2D {
  public:
   using Constraint = PoseGraphInterface::Constraint;
@@ -89,25 +102,27 @@ class ConstraintBuilder2D {
   void MaybeAddConstraint(const SubmapId& submap_id, const Submap2D* submap,
                           const NodeId& node_id, const TrajectoryNodeData* constant_data,
                           const transform::Rigid2d& initial_relative_pose) {
-    if (initial_relative_pose.translation().norm() > options_.max_constraint_distance()) return;
-    if (!per_submap_sampler_
-             .emplace(std::piecewise_construct, std::forward_as_tuple(submap_id),
-                      std::forward_as_tuple(options_.sampling_ratio()))
-             .first->second.Pulse()) {
-      return;
-    }
-    std::lock_guard<std::mutex> lock(mutex_);
-    // initial_pose = ComputeSubmapPose(*submap) * initial_relative_pose (:196-197)
-    Push(submap_id, submap, node_id, constant_data, submap->local_pose_2d() * initial_relative_pose,
-         false, static_cast<float>(options_.min_score()));
+    AddLocal(submap_id, submap, nullptr, node_id, constant_data, initial_relative_pose);
+  }
+  // The same for a submap kept on the device: its stack is built from the grid without a host
+  // copy, and the refinement reads the grid directly.  The grid must be a ProbabilityGrid on
+  // this builder's device, and the builder a single-GPU one.
+  void MaybeAddConstraint(const SubmapId& submap_id, const DeviceSubmap2D* submap,
+                          const NodeId& node_id, const TrajectoryNodeData* constant_data,
+                          const transform::Rigid2d& initial_relative_pose) {
+    RequireUsable(submap);
+    AddLocal(submap_id, nullptr, submap, node_id, constant_data, initial_relative_pose);
   }
 
   // constraint_builder_2d.cc:114-137
   void MaybeAddGlobalConstraint(const SubmapId& submap_id, const Submap2D* submap,
                                 const NodeId& node_id, const TrajectoryNodeData* constant_data) {
-    std::lock_guard<std::mutex> lock(mutex_);
-    Push(submap_id, submap, node_id, constant_data, transform::Rigid2d::Identity(), true,
-         static_cast<float>(options_.global_localization_min_score()));
+    AddGlobal(submap_id, submap, nullptr, node_id, constant_data);
+  }
+  void MaybeAddGlobalConstraint(const SubmapId& submap_id, const DeviceSubmap2D* submap,
+                                const NodeId& node_id, const TrajectoryNodeData* constant_data) {
+    RequireUsable(submap);
+    AddGlobal(submap_id, nullptr, submap, node_id, constant_data);
   }
 
   void NotifyEndOfNode() {  // :139-151
@@ -148,7 +163,8 @@ class ConstraintBuilder2D {
  private:
   struct Pending {
     SubmapId submap_id;
-    const Submap2D* submap;
+    const Submap2D* submap;                 // one of the two is set
+    const DeviceSubmap2D* device_submap;
     NodeId node_id;
     const TrajectoryNodeData* constant_data;
     transform::Rigid2d initial_pose;
@@ -158,23 +174,76 @@ class ConstraintBuilder2D {
   struct SubmapStack {
     const Grid2D* grid = nullptr;
     csm_stack2d* stack = nullptr;
-    std::unique_ptr<scan_matching::DeviceGrid2D> device_grid;   // for the refinement
+    // the refinement's upload of a host submap's grid; a device submap's is its own
+    std::unique_ptr<scan_matching::DeviceGrid2D> device_grid;
   };
 
-  void Push(const SubmapId& submap_id, const Submap2D* submap, const NodeId& node_id,
-            const TrajectoryNodeData* constant_data, const transform::Rigid2d& initial_pose,
-            bool full, float min_score) {
-    b200_internal::Require(submap != nullptr && submap->grid() != nullptr, "grid");  // :167
-    pending_.push_back(Pending{submap_id, submap, node_id, constant_data, initial_pose, full,
-                               min_score});
+  // Refusals for a device submap, before anything is queued: its handle exists only in this
+  // process and on the device it was made on, and only a ProbabilityGrid has a stack.
+  void RequireUsable(const DeviceSubmap2D* submap) const {
+    b200_internal::Require(submap != nullptr && submap->grid != nullptr, "grid");
+    b200_internal::Require(ctx_ == nullptr, "device submaps need a single-GPU builder");
+    b200_internal::Require(submap->grid->device() == device_,
+                           "the device submap lives on another device than the builder");
+    csm_rt_grid2d_info info;
+    scan_matching::b200_internal::Check(
+        csm_rt_grid2d_read(submap->grid->handle(), &info, nullptr, 0));
+    b200_internal::Require(info.is_tsdf == 0, "device submaps must be ProbabilityGrids");
   }
 
-  // DispatchScanMatcherConstruction (:165-186): one device stack per submap, built once.
-  csm_stack2d* StackFor(const SubmapId& submap_id, const Grid2D* grid) {
-    SubmapStack& entry = stacks_[submap_id];
-    if (entry.stack == nullptr) {
+  static const transform::Rigid2d& LocalPose(const Submap2D* submap,
+                                             const DeviceSubmap2D* device_submap) {
+    return device_submap != nullptr ? device_submap->local_pose_2d : submap->local_pose_2d();
+  }
+
+  void AddLocal(const SubmapId& submap_id, const Submap2D* submap,
+                const DeviceSubmap2D* device_submap, const NodeId& node_id,
+                const TrajectoryNodeData* constant_data,
+                const transform::Rigid2d& initial_relative_pose) {
+    if (initial_relative_pose.translation().norm() > options_.max_constraint_distance()) return;
+    if (!per_submap_sampler_
+             .emplace(std::piecewise_construct, std::forward_as_tuple(submap_id),
+                      std::forward_as_tuple(options_.sampling_ratio()))
+             .first->second.Pulse()) {
+      return;
+    }
+    std::lock_guard<std::mutex> lock(mutex_);
+    // initial_pose = ComputeSubmapPose(*submap) * initial_relative_pose (:196-197)
+    Push(submap_id, submap, device_submap, node_id, constant_data,
+         LocalPose(submap, device_submap) * initial_relative_pose, false,
+         static_cast<float>(options_.min_score()));
+  }
+
+  void AddGlobal(const SubmapId& submap_id, const Submap2D* submap,
+                 const DeviceSubmap2D* device_submap, const NodeId& node_id,
+                 const TrajectoryNodeData* constant_data) {
+    std::lock_guard<std::mutex> lock(mutex_);
+    Push(submap_id, submap, device_submap, node_id, constant_data,
+         transform::Rigid2d::Identity(), true,
+         static_cast<float>(options_.global_localization_min_score()));
+  }
+
+  void Push(const SubmapId& submap_id, const Submap2D* submap,
+            const DeviceSubmap2D* device_submap, const NodeId& node_id,
+            const TrajectoryNodeData* constant_data, const transform::Rigid2d& initial_pose,
+            bool full, float min_score) {
+    if (device_submap == nullptr)
+      b200_internal::Require(submap != nullptr && submap->grid() != nullptr, "grid");  // :167
+    pending_.push_back(Pending{submap_id, submap, device_submap, node_id, constant_data,
+                               initial_pose, full, min_score});
+  }
+
+  // DispatchScanMatcherConstruction (:165-186): one device stack per submap, built once; a
+  // device submap's from its grid, device to device.
+  csm_stack2d* StackFor(const Pending& p) {
+    SubmapStack& entry = stacks_[p.submap_id];
+    const auto& fo = options_.fast_correlative_scan_matcher_options();
+    if (entry.stack == nullptr && p.device_submap != nullptr) {
+      scan_matching::b200_internal::Check(csm_stack2d_create_from_rt_grid2d(
+          p.device_submap->grid->handle(), fo.branch_and_bound_depth(), &entry.stack));
+    } else if (entry.stack == nullptr) {
+      const Grid2D* grid = p.submap->grid();
       const MapLimits& l = grid->limits();
-      const auto& fo = options_.fast_correlative_scan_matcher_options();
       scan_matching::b200_internal::Check(csm_stack2d_create(
           grid->correspondence_cost_cells().data(), l.cell_limits().num_x_cells,
           l.cell_limits().num_y_cells, l.resolution(), l.max().x(), l.max().y(),
@@ -191,6 +260,11 @@ class ConstraintBuilder2D {
     {
       std::lock_guard<std::mutex> lock(mutex_);
       b200_internal::Require(when_done_ != nullptr, "no callback");
+      if (refiner_) {   // Refiner takes a host Grid2D, which a device submap does not have
+        for (const Pending& p : pending_)
+          b200_internal::Require(p.device_submap == nullptr,
+                                 "set_refiner cannot refine on a device submap");
+      }
       const auto& fo = options_.fast_correlative_scan_matcher_options();
       // distinct stacks / clouds of this queue
       std::vector<const csm_stack2d*> stacks;
@@ -206,7 +280,7 @@ class ConstraintBuilder2D {
           si = stack_index.emplace(p.submap_id, static_cast<int>(stacks.size())).first;
           const int owner = OwnerOf(p.submap_id);
           owners.push_back(owner);
-          stacks.push_back(owner == rank_ ? StackFor(p.submap_id, p.submap->grid()) : nullptr);
+          stacks.push_back(owner == rank_ ? StackFor(p) : nullptr);
         }
         auto ci = cloud_index.find(p.constant_data);
         if (ci == cloud_index.end()) {
@@ -264,15 +338,21 @@ class ConstraintBuilder2D {
         for (size_t i = 0; i < pending_.size(); ++i) {
           if (!results[i].found) continue;
           const Pending& p = pending_[i];
-          SubmapStack& entry = stacks_[p.submap_id];
-          if (entry.device_grid == nullptr)
-            entry.device_grid.reset(new scan_matching::DeviceGrid2D(*p.submap->grid(), device_));
+          const scan_matching::DeviceGrid2D* grid = nullptr;
+          if (p.device_submap != nullptr) {   // the submap's own grid
+            grid = p.device_submap->grid;
+          } else {
+            SubmapStack& entry = stacks_[p.submap_id];
+            if (entry.device_grid == nullptr)
+              entry.device_grid.reset(new scan_matching::DeviceGrid2D(*p.submap->grid(), device_));
+            grid = entry.device_grid.get();
+          }
           refined_of[i] = rjobs.size();
           rjobs.push_back(scan_matching::CeresScanMatcher2D::Job{
               {results[i].pose_estimate[0], results[i].pose_estimate[1]},
               transform::Rigid2d({results[i].pose_estimate[0], results[i].pose_estimate[1]},
                                  results[i].pose_estimate[2]),
-              &p.constant_data->filtered_gravity_aligned_point_cloud, entry.device_grid.get()});
+              &p.constant_data->filtered_gravity_aligned_point_cloud, grid});
         }
         scan_matching::CeresScanMatcher2D(options_.ceres_scan_matcher_options(), device_)
             .MatchBatch(rjobs, &refined, nullptr);
@@ -289,7 +369,7 @@ class ConstraintBuilder2D {
                                    *p.submap->grid());
         // constraint_transform = ComputeSubmapPose(*submap).inverse() * pose_estimate (:251-252)
         const transform::Rigid2d constraint_transform =
-            p.submap->local_pose_2d().inverse() * pose_estimate;
+            LocalPose(p.submap, p.device_submap).inverse() * pose_estimate;
         result.push_back(Constraint{p.submap_id,
                                     p.node_id,
                                     {b200_internal::Embed3D(constraint_transform),

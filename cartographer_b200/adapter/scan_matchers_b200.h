@@ -239,7 +239,7 @@ class RealTimeCorrelativeScanMatcher2D {
 // real-time matcher and the refinement below take the submap's grid.
 class DeviceGrid2D {
  public:
-  explicit DeviceGrid2D(const Grid2D& grid, int device = 0) {
+  explicit DeviceGrid2D(const Grid2D& grid, int device = 0) : device_(device) {
     if (grid.GetGridType() != GridType::PROBABILITY_GRID) {
       std::fprintf(stderr, "DeviceGrid2D (b200): only ProbabilityGrid is supported\n");
       std::abort();
@@ -251,14 +251,15 @@ class DeviceGrid2D {
   }
   // ProbabilityGrid(limits): the all-unknown grid ActiveSubmaps2D::CreateGrid makes, filled
   // by ProbabilityGridRangeDataInserter2D below.
-  DeviceGrid2D(const MapLimits& limits, int device) {
+  DeviceGrid2D(const MapLimits& limits, int device) : device_(device) {
     b200_internal::Check(csm_rt_grid2d_create_empty(
         limits.resolution(), limits.max().x(), limits.max().y(),
         limits.cell_limits().num_x_cells, limits.cell_limits().num_y_cells, device, &grid_));
   }
   // TSDF2D(limits, truncation_distance, max_weight): the all-unknown TSDF2D
   // ActiveSubmaps2D::CreateGrid makes for GridType::TSDF, filled by TSDFRangeDataInserter2D below.
-  DeviceGrid2D(const MapLimits& limits, float truncation_distance, float max_weight, int device) {
+  DeviceGrid2D(const MapLimits& limits, float truncation_distance, float max_weight, int device)
+      : device_(device) {
     b200_internal::Check(csm_rt_grid2d_create_empty_tsdf(
         limits.resolution(), limits.max().x(), limits.max().y(),
         limits.cell_limits().num_x_cells, limits.cell_limits().num_y_cells, truncation_distance,
@@ -269,12 +270,13 @@ class DeviceGrid2D {
   DeviceGrid2D& operator=(const DeviceGrid2D&) = delete;
   const csm_rt_grid2d* handle() const { return grid_; }
   csm_rt_grid2d* mutable_handle() { return grid_; }
+  int device() const { return device_; }   // the CUDA device the cells live on
 
   // ProbabilityGrid::ComputeCroppedGrid (probability_grid.cc:91-107), device to device.
   std::unique_ptr<DeviceGrid2D> ComputeCroppedGrid() const {
     csm_rt_grid2d* cropped = nullptr;
     b200_internal::Check(csm_rt_grid2d_crop(grid_, &cropped));
-    return std::unique_ptr<DeviceGrid2D>(new DeviceGrid2D(cropped));
+    return std::unique_ptr<DeviceGrid2D>(new DeviceGrid2D(cropped, device_));
   }
   // limits(), the known-cells box and, with cells != nullptr, the cells (num_y x num_x):
   // what Submap2D::ToProto serialises.
@@ -297,7 +299,8 @@ class DeviceGrid2D {
   }
 
  private:
-  explicit DeviceGrid2D(csm_rt_grid2d* grid) : grid_(grid) {}
+  DeviceGrid2D(csm_rt_grid2d* grid, int device) : device_(device), grid_(grid) {}
+  int device_;
   csm_rt_grid2d* grid_ = nullptr;
 };
 

@@ -50,9 +50,31 @@ class ConstraintBuilderOptions:
 
 @dataclass
 class Submap2D:
-    """What the builder needs of a Submap2D: its grid and local pose (x, y, yaw)."""
+    """What the builder needs of a Submap2D: its grid and local pose (x, y, yaw).
+
+    The grid is either a host record (.cells, .resolution, .max_x, .max_y, .min_cost,
+    .max_cost) or, for a finished submap kept on the device as
+    ProbabilityGridRangeDataInserter2D fills it and RealTimeGrid2D.ComputeCroppedGrid crops it,
+    a ProbabilityGrid scan_matching.RealTimeGrid2D on the builder's device.  A device submap's
+    stack and refinement read its grid where it is; the caller keeps it alive until WhenDone
+    has run its callback, and DeleteScanMatcher never closes it."""
     grid: object
     local_pose: tuple = (0.0, 0.0, 0.0)
+
+
+def _is_device_grid(grid, device):
+    """True for a Submap2D grid that is a RealTimeGrid2D, False for a host record; ValueError
+    for a TSDF handle (it has no precomputation stack) or one on another device than
+    `device`.  Reads only the handle's attributes: nothing reaches the library."""
+    from .scan_matching import RealTimeGrid2D
+    if not isinstance(grid, RealTimeGrid2D):
+        return False
+    if grid.is_tsdf:
+        raise ValueError("Submap2D: a TSDF RealTimeGrid2D cannot close loops")
+    if grid.device != device:
+        raise ValueError("Submap2D: the grid lives on device %d, the builder on device %d"
+                         % (grid.device, device))
+    return True
 
 
 @dataclass
@@ -110,7 +132,9 @@ class _Job:
 class CudaExecutor:
     """Drains a list of jobs through csm_match2d_batch on one device.  Keeps one
     device stack per submap (DispatchScanMatcherConstruction,
-    constraint_builder_2d.cc:165-186) and one device cloud per node scan."""
+    constraint_builder_2d.cc:165-186) and one device cloud per node scan.  A device
+    submap's stack is built from its RealTimeGrid2D without a host copy, and its
+    refinement reads that grid directly."""
 
     def __init__(self, options, device=0):
         from . import scan_matching as sm
@@ -118,7 +142,8 @@ class CudaExecutor:
         self.options = options
         self.device = device
         self.matchers = {}
-        self.grids = {}     # submap id -> RealTimeGrid2D (only with the Ceres refinement on)
+        # submap id -> RealTimeGrid2D uploaded for the Ceres refinement (host submaps only)
+        self.grids = {}
         self.clouds = {}
         self.stats = {"candidates_scored": 0, "device_ms": 0.0, "searched": 0, "refined": 0,
                       "refine_device_ms": 0.0}
@@ -126,10 +151,13 @@ class CudaExecutor:
     def ensure_matcher(self, submap_id, grid):
         if submap_id not in self.matchers:
             o = self.options
-            self.matchers[submap_id] = self.sm.FastCorrelativeScanMatcher2D(
-                grid, self.sm.FastCorrelativeScanMatcherOptions2D(
-                    o.linear_search_window, o.angular_search_window, o.branch_and_bound_depth),
-                device=self.device)
+            fo = self.sm.FastCorrelativeScanMatcherOptions2D(
+                o.linear_search_window, o.angular_search_window, o.branch_and_bound_depth)
+            if _is_device_grid(grid, self.device):
+                m = self.sm.FastCorrelativeScanMatcher2D.from_device_grid(grid, fo)
+            else:
+                m = self.sm.FastCorrelativeScanMatcher2D(grid, fo, device=self.device)
+            self.matchers[submap_id] = m
 
     def delete_matcher(self, submap_id):
         m = self.matchers.pop(submap_id, None)
@@ -145,14 +173,18 @@ class CudaExecutor:
         idx = [i for i, r in enumerate(out) if r[0]]
         if not idx:
             return out
+        grids = []
         for i in idx:
             sid = jobs[i].submap_id
-            if sid not in self.grids:
-                self.grids[sid] = sm.RealTimeGrid2D(submaps[sid].grid, device=self.device)
+            grid = submaps[sid].grid
+            if not _is_device_grid(grid, self.device):
+                if sid not in self.grids:
+                    self.grids[sid] = sm.RealTimeGrid2D(grid, device=self.device)
+                grid = self.grids[sid]
+            grids.append(grid)
         matcher = sm.CeresScanMatcher2D(self.options.ceres_scan_matcher_options)
         poses, _ = matcher.MatchBatch([out[i][2][:2] for i in idx], [out[i][2] for i in idx],
-                                      [clouds[jobs[i].cloud_key] for i in idx],
-                                      [self.grids[jobs[i].submap_id] for i in idx])
+                                      [clouds[jobs[i].cloud_key] for i in idx], grids)
         self.stats["refined"] += len(idx)
         self.stats["refine_device_ms"] += matcher.last_stats["device_ms"]
         out = list(out)
@@ -224,6 +256,14 @@ class ConstraintBuilder2D:
         self.last_records = None
 
     # -- queue --------------------------------------------------------------------
+    def _check_submap(self, submap):
+        """Refuses, before anything is queued, a device submap the builder cannot use: a TSDF
+        handle, a handle on another device, or any device submap when the queue is sharded
+        over several ranks (a device submap stays on the GPU that inserted it)."""
+        device = getattr(self.executor, "device", self.device)
+        if _is_device_grid(submap.grid, device) and self._world()[1] > 1:
+            raise ValueError("device-resident submaps are not sharded over several ranks")
+
     def _register(self, submap_id, submap, constant_data):
         self._submaps[submap_id] = submap
         self._submap_order.setdefault(submap_id, len(self._submap_order))
@@ -235,6 +275,7 @@ class ConstraintBuilder2D:
                            initial_relative_pose):
         """constraint_builder_2d.cc:77-112.  constant_data is the node's
         filtered_gravity_aligned_point_cloud (N x 3 float32)."""
+        self._check_submap(submap)
         if math.hypot(initial_relative_pose[0], initial_relative_pose[1]) > \
                 self.options.max_constraint_distance:
             return
@@ -249,6 +290,7 @@ class ConstraintBuilder2D:
 
     def MaybeAddGlobalConstraint(self, submap_id, submap, node_id, constant_data):
         """constraint_builder_2d.cc:114-137."""
+        self._check_submap(submap)
         key = self._register(submap_id, submap, constant_data)
         self._jobs.append(_Job(submap_id, node_id, key, (0.0, 0.0, 0.0), True,
                                self.options.global_localization_min_score))
