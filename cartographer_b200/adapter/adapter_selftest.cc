@@ -22,6 +22,14 @@ static unsigned Bits(float f) {
 // Host-only part (runs everywhere): the builder's gating and WhenDone cycle when no
 // pair survives the gates — nothing reaches the device — and the sampler's sequence
 // (common/fixed_ratio_sampler_test.cc).
+// A serialised grid (DeviceHybridGrid / DeviceGrid2D::ToProto, the bytes in this stand-in
+// build) as one hex RESULT line.
+static void PrintBytes(const char* name, const std::string& bytes) {
+  std::printf("RESULT %s ", name);
+  for (unsigned char c : bytes) std::printf("%02x", c);
+  std::printf("\n");
+}
+
 static int HostOnlyChecks() {
   using mapping::constraints::ConstraintBuilder2D;
   common::FixedRatioSampler half(0.5);
@@ -389,6 +397,7 @@ int main() {
     for (size_t i = 0; i < vox; ++i)
       std::printf(" %08x:%08x:%d", Bits(mean[i]), Bits(sum[i]), count[i]);
     std::printf("\n");
+    PrintBytes("grid_to_proto_insert3d", grid.ToProto());
   }
   // ---- FastCorrelativeScanMatcher3D and ConstraintBuilder3D on inserted device grids: the
   // axis cloud inserted twice from its sensor position into empty grids; the same built from
@@ -520,6 +529,7 @@ int main() {
                   info.known_max_y);
       for (uint16_t v : cells) std::printf(" %u", v);
       std::printf("\n");
+      PrintBytes(g == &grid ? "grid_to_proto_insert2d" : "grid_to_proto_crop2d", g->ToProto());
     }
     mapping::scan_matching::proto::FastCorrelativeScanMatcherOptions2D fo;
     fo.set_linear_search_window(3.);
@@ -694,6 +704,7 @@ int main() {
     for (uint16_t v : tsd) std::printf(" %u", v);
     for (uint16_t v : weights) std::printf(" %u", v);
     std::printf("\n");
+    PrintBytes("grid_to_proto_insert_tsdf2d", grid.ToProto());
   }
   return 0;
 }

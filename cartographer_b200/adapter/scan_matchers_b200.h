@@ -18,6 +18,7 @@
 #include <cstdio>
 #include <cstdlib>
 #include <memory>
+#include <string>
 #include <vector>
 
 #include "../../include/csm_abi.h"
@@ -29,6 +30,7 @@
 #include "cartographer/mapping/proto/scan_matching/ceres_scan_matcher_options_2d.pb.h"
 #include "cartographer/mapping/proto/scan_matching/fast_correlative_scan_matcher_options_2d.pb.h"
 #include "cartographer/mapping/proto/scan_matching/real_time_correlative_scan_matcher_options.pb.h"
+#include "cartographer/mapping/proto/hybrid_grid.pb.h"
 #include "cartographer/mapping/proto/range_data_inserter_options_3d.pb.h"
 #include "cartographer/mapping/proto/probability_grid_range_data_inserter_options_2d.pb.h"
 #include "cartographer/sensor/point_cloud.h"
@@ -65,6 +67,36 @@ inline std::vector<float> Flatten(const sensor::PointCloud& point_cloud) {
   }
   return xyz;
 }
+// The serialised message of one *_to_proto entry point (sized by a first call).  A message
+// of 2 GiB or more, which protobuf cannot hold, aborts as the reference's serialiser does.
+template <typename Handle>
+std::string Serialize(csm_status (*to_proto)(const Handle*, uint8_t*, int64_t, int64_t*),
+                      const Handle* handle) {
+  int64_t size = 0;
+  if (!Check(to_proto(handle, nullptr, 0, &size))) std::abort();
+  std::string bytes(static_cast<size_t>(size), '\0');
+  if (!Check(to_proto(handle, reinterpret_cast<uint8_t*>(&bytes[0]), size, &size))) std::abort();
+  return bytes;
+}
+// A proto::HybridGrid / proto::Grid2D parsed from those bytes in a Cartographer checkout; the
+// bytes themselves in the stand-in build.
+#ifdef CSM_ADAPTER_REAL_CARTOGRAPHER
+template <typename Message>
+Message Parse(const std::string& bytes) {
+  Message message;
+  if (!message.ParseFromString(bytes)) std::abort();
+  return message;
+}
+using HybridGridProto = ::cartographer::mapping::proto::HybridGrid;
+using Grid2DProto = ::cartographer::mapping::proto::Grid2D;
+#else
+template <typename Message>
+Message Parse(const std::string& bytes) {
+  return bytes;
+}
+using HybridGridProto = std::string;
+using Grid2DProto = std::string;
+#endif
 }  // namespace b200_internal
 
 class DeviceGrid2D;
@@ -289,6 +321,12 @@ class DeviceGrid2D {
                                               static_cast<int64_t>(cells->size())));
     }
     return info;
+  }
+  // ProbabilityGrid::ToProto / TSDF2D::ToProto (csm_rt_grid2d_to_proto): the grid part of
+  // Submap2D::ToProto, byte for byte what the reference serialises.
+  b200_internal::Grid2DProto ToProto() const {
+    return b200_internal::Parse<b200_internal::Grid2DProto>(
+        b200_internal::Serialize(csm_rt_grid2d_to_proto, grid_));
   }
   // The weight cells of a TSDF2D (num_y x num_x); Read gives its tsd cells.
   void ReadWeights(std::vector<uint16_t>* weight_cells) const {
@@ -618,6 +656,12 @@ class DeviceHybridGrid {
   DeviceHybridGrid& operator=(const DeviceHybridGrid&) = delete;
   const csm_grid3d* handle() const { return grid_; }
   csm_grid3d* mutable_handle() { return grid_; }
+  // HybridGrid::ToProto (hybrid_grid.h:528-540, csm_grid3d_to_proto): what Submap3D::ToProto
+  // writes for its high- and low-resolution grids.
+  b200_internal::HybridGridProto ToProto() const {
+    return b200_internal::Parse<b200_internal::HybridGridProto>(
+        b200_internal::Serialize(csm_grid3d_to_proto, grid_));
+  }
 
  private:
   csm_grid3d* grid_ = nullptr;

@@ -14,8 +14,12 @@
 #include <cmath>
 #include <functional>
 
+#include <cub/block/block_scan.cuh>
+#include <cub/device/device_scan.cuh>
+
 #include "common.cuh"
 #include "grid3d.cuh"
+#include "proto_write.h"
 #include "rigid3f.h"
 #include "value_conversion.h"
 
@@ -195,6 +199,92 @@ k3_gather_u16(Box16 src, Low3Dev v, uint16_t* __restrict__ out) {
   for (long long r = blockIdx.y; r < rows; r += gridDim.y) {
     const int y = static_cast<int>(r % v.n[1]), z = static_cast<int>(r / v.n[1]);
     out[r * v.n[0] + x] = Val16(src, x + v.lo[0], y + v.lo[1], z + v.lo[2]);
+  }
+}
+
+// ---- the non-zero voxels of a csm_grid3d in HybridGrid's iteration order (csm_grid3d_voxels) ----
+// HybridGrid is DynamicGrid<NestedGrid<FlatGrid<uint16, 3>, 3>> (hybrid_grid.h), and each level
+// walks its cells in ToFlatIndex order, z outermost (:40-43), skipping null meta cells and value 0
+// (:57, :106-115).  The DynamicGrid shifts an index by grid_size() / 2 = 2^(bits - 1) * 64, a
+// multiple of 64 (:263-264), so its meta cells are the 64^3 blocks floor(index / 64) in z, y, x
+// order, whatever bits_ is and however the grid grew; inside them come the NestedGrid's 8^3 blocks
+// and inside those the cells, both in z, y, x order.  The kernels below enumerate the 64-aligned
+// cover of the non-zero box in that blocked order and compact the non-zero cells stably: tile t is
+// kVoxTile consecutive cells of the enumeration (4 of the 8^3 blocks, 128 tiles per 64^3 block),
+// and thread k of a tile holds the x-row (z & 7, y & 7) = ((k & 63) >> 3, k & 7) of its block
+// k >> 6.  No sort is needed.
+constexpr int kVoxThreads = 256;
+constexpr int kVoxTile = 8 * kVoxThreads;
+
+struct VoxCover {
+  Box16 src;
+  int lo[3];   // multiples of 64
+  int nb[3];   // 64^3 blocks per axis
+};
+
+// The 8 cells x .. x + 7 of this thread's row in tile t, and their values in v.
+__device__ __forceinline__ void VoxRow(const VoxCover& c, long long t, int* x, int* y, int* z,
+                                       uint16_t v[8]) {
+  const long long m = t >> 7;                                          // the 64^3 block
+  const int f = static_cast<int>(t & 127) * 4 + (threadIdx.x >> 6);    // the 8^3 block in it
+  const int r = threadIdx.x & 63;
+  const long long bxy = static_cast<long long>(c.nb[0]) * c.nb[1];
+  const int bz = static_cast<int>(m / bxy);
+  const int by = static_cast<int>((m % bxy) / c.nb[0]);
+  const int bx = static_cast<int>(m % c.nb[0]);
+  *x = c.lo[0] + 64 * bx + 8 * (f & 7);
+  *y = c.lo[1] + 64 * by + 8 * ((f >> 3) & 7) + (r & 7);
+  *z = c.lo[2] + 64 * bz + 8 * (f >> 6) + (r >> 3);
+#pragma unroll
+  for (int i = 0; i < 8; ++i) v[i] = Val16(c.src, *x + i, *y, *z);
+}
+
+// Pass 1: counts[t] = the non-zero cells of tile t.
+__global__ void __launch_bounds__(kVoxThreads)
+k3_voxel_count(VoxCover c, long long* __restrict__ counts) {
+  __shared__ int s[kVoxThreads / 32];
+  int x, y, z;
+  uint16_t v[8];
+  VoxRow(c, blockIdx.x, &x, &y, &z, v);
+  int n = 0;
+#pragma unroll
+  for (int i = 0; i < 8; ++i) n += v[i] != 0;
+  n = __reduce_add_sync(0xffffffffu, n);
+  if ((threadIdx.x & 31) == 0) s[threadIdx.x >> 5] = n;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    int total = 0;
+    for (int w = 0; w < kVoxThreads / 32; ++w) total += s[w];
+    counts[blockIdx.x] = total;
+  }
+}
+
+// Pass 2: the non-zero cells of tile t written from offsets[t] on, in enumeration order:
+// idx as {x, y, z}, val as held.
+__global__ void __launch_bounds__(kVoxThreads)
+k3_voxel_write(VoxCover c, const long long* __restrict__ counts,
+               const long long* __restrict__ offsets, int* __restrict__ idx,
+               uint16_t* __restrict__ val) {
+  typedef cub::BlockScan<int, kVoxThreads> Scan;
+  __shared__ typename Scan::TempStorage scan;
+  if (counts[blockIdx.x] == 0) return;   // uniform over the block
+  int x, y, z;
+  uint16_t v[8];
+  VoxRow(c, blockIdx.x, &x, &y, &z, v);
+  int n = 0;
+#pragma unroll
+  for (int i = 0; i < 8; ++i) n += v[i] != 0;
+  int before;
+  Scan(scan).ExclusiveSum(n, before);
+  long long o = offsets[blockIdx.x] + before;
+#pragma unroll
+  for (int i = 0; i < 8; ++i) {
+    if (v[i] == 0) continue;
+    idx[3 * o] = x + i;
+    idx[3 * o + 1] = y;
+    idx[3 * o + 2] = z;
+    val[o] = v[i];
+    ++o;
   }
 }
 
@@ -913,6 +1003,77 @@ dim3 RowGrid(int nx, long long rows, int max_blocks) {
   return dim3(bx, static_cast<unsigned>(std::min<long long>(by, 65535)));
 }
 
+// The number *n of non-zero voxels of `g` and, when it is at most list_capacity, the voxels in
+// HybridGrid's iteration order (k3_voxel_*) in the device workspaces "g3v_idx" ({x, y, z} each)
+// and "g3v_val" (*d_idx, *d_val), ready on the stream.  Caller holds ctx->mu.  One stream synchronisation for
+// the non-zero box and, if the grid has a non-zero voxel, one for the count.
+csm_status DeviceVoxels3D(const csm_grid3d* g, long long list_capacity, long long* n,
+                          const int** d_idx, const uint16_t** d_val) {
+  Ctx* ctx = g->ctx;
+  cudaStream_t s = ctx->stream;
+  VoxCover c;
+  c.src = HandleBox(g);
+  DevBuf* d_box;
+  CSM_TRY(ctx->Reserve("g3v_box", 6 * sizeof(unsigned), &d_box));
+  unsigned* box = d_box->as<unsigned>();
+  CSM_CUDA(cudaMemsetAsync(box, 0xff, 3 * sizeof(unsigned), s));
+  CSM_CUDA(cudaMemsetAsync(box + 3, 0, 3 * sizeof(unsigned), s));
+  const long long rows = static_cast<long long>(c.src.n[1]) * c.src.n[2];
+  k3_nonzero_box<<<RowGrid(c.src.n[0], rows, ctx->sm_count * 8), 256, 0, s>>>(c.src, box, box + 3);
+  CSM_LAUNCH_CHECK();
+  PinnedBuf& pin = ctx->P("g3v_box");
+  CSM_TRY(pin.Reserve(6 * sizeof(unsigned) + sizeof(long long)));
+  unsigned* h = pin.as<unsigned>();
+  CSM_CUDA(cudaMemcpyAsync(h, box, 6 * sizeof(unsigned), cudaMemcpyDeviceToHost, s));
+  CSM_CUDA(cudaStreamSynchronize(s));
+  *n = 0;
+  if (h[3] == 0u) return CSM_OK;   // no non-zero cell
+  // the 64-aligned cover of the non-zero box (floor division: indices may be negative)
+  long long tiles = static_cast<long long>(262144 / kVoxTile);
+  for (int a = 0; a < 3; ++a) {
+    const int b0 = (c.src.lo[a] + static_cast<int>(h[a]) + 8192) / 64 - 128;
+    const int b1 = (c.src.lo[a] + static_cast<int>(h[3 + a]) - 1 + 8192) / 64 - 128;
+    c.lo[a] = 64 * b0;
+    c.nb[a] = b1 - b0 + 1;
+    tiles *= c.nb[a];
+  }
+  if (tiles >= INT_MAX) {   // one block per tile
+    SetError("the non-zero box of the grid is too large to enumerate");
+    return CSM_E_CAPACITY;
+  }
+  // counts[tiles] stays 0, so that the exclusive scan's last entry is the total
+  size_t scan_bytes = 0;
+  CSM_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, scan_bytes, static_cast<long long*>(nullptr),
+                                         static_cast<long long*>(nullptr), tiles + 1, s));
+  const size_t o_off = (sizeof(long long) * (tiles + 1) + 255) / 256 * 256;
+  const size_t o_temp = 2 * o_off;
+  DevBuf* d_work;
+  CSM_TRY(ctx->Reserve("g3v_scan", o_temp + scan_bytes, &d_work));
+  long long* counts = d_work->as<long long>();
+  long long* offsets = reinterpret_cast<long long*>(d_work->as<char>() + o_off);
+  CSM_CUDA(cudaMemsetAsync(counts + tiles, 0, sizeof(long long), s));
+  k3_voxel_count<<<static_cast<unsigned>(tiles), kVoxThreads, 0, s>>>(c, counts);
+  CSM_LAUNCH_CHECK();
+  CSM_CUDA(cub::DeviceScan::ExclusiveSum(d_work->as<char>() + o_temp, scan_bytes, counts, offsets,
+                                         tiles + 1, s));
+  g_launches.fetch_add(1, std::memory_order_relaxed);
+  long long* h_n = reinterpret_cast<long long*>(h + 6);
+  CSM_CUDA(cudaMemcpyAsync(h_n, offsets + tiles, sizeof(long long), cudaMemcpyDeviceToHost, s));
+  CSM_CUDA(cudaStreamSynchronize(s));
+  *n = *h_n;
+  if (*n > list_capacity) return CSM_OK;
+  DevBuf* out_idx;
+  DevBuf* out_val;
+  CSM_TRY(ctx->Reserve("g3v_idx", sizeof(int) * 3 * *n, &out_idx));
+  CSM_TRY(ctx->Reserve("g3v_val", sizeof(uint16_t) * *n, &out_val));
+  k3_voxel_write<<<static_cast<unsigned>(tiles), kVoxThreads, 0, s>>>(
+      c, counts, offsets, out_idx->as<int>(), out_val->as<uint16_t>());
+  CSM_LAUNCH_CHECK();
+  *d_idx = out_idx->as<int>();
+  *d_val = out_val->as<uint16_t>();
+  return CSM_OK;
+}
+
 }  // namespace
 
 extern "C" {
@@ -1029,6 +1190,88 @@ csm_status csm_matcher3d_create_from_grid3d(const csm_grid3d* hybrid_grid,
                          low_resolution_hybrid_grid->g.resolution, submap_hist, hist_n, options,
                          fill_depth0, fill_low, out));
   ProfEnd(ctx, "m3g_build", 0.);
+  return CSM_OK;
+}
+
+csm_status csm_grid3d_voxels(const csm_grid3d* grid, int32_t* indices, uint16_t* values,
+                             int64_t capacity, int64_t* num_voxels) {
+  CSM_REQUIRE(grid && num_voxels, "null pointer");
+  CSM_REQUIRE((indices == nullptr) == (values == nullptr), "indices and values go together");
+  Ctx* ctx = grid->ctx;
+  std::lock_guard<std::mutex> lock(ctx->mu);
+  CSM_CUDA(cudaSetDevice(ctx->device));
+  long long n = 0;
+  const int* d_idx = nullptr;
+  const uint16_t* d_val = nullptr;
+  CSM_TRY(DeviceVoxels3D(grid, indices ? capacity : -1, &n, &d_idx, &d_val));
+  *num_voxels = n;
+  if (!indices || n == 0) return CSM_OK;
+  if (capacity < n) {
+    SetError("capacity %lld is below the %lld non-zero voxels", static_cast<long long>(capacity), n);
+    return CSM_E_CAPACITY;
+  }
+  cudaStream_t s = ctx->stream;
+  CSM_CUDA(cudaMemcpyAsync(indices, d_idx, sizeof(int) * 3 * n, cudaMemcpyDeviceToHost, s));
+  CSM_CUDA(cudaMemcpyAsync(values, d_val, sizeof(uint16_t) * n, cudaMemcpyDeviceToHost, s));
+  CSM_CUDA(cudaStreamSynchronize(s));
+  return CSM_OK;
+}
+
+csm_status csm_grid3d_to_proto(const csm_grid3d* grid, uint8_t* buf, int64_t capacity,
+                               int64_t* size) {
+  using namespace wire;
+  CSM_REQUIRE(grid && size, "null pointer");
+  Ctx* ctx = grid->ctx;
+  std::lock_guard<std::mutex> lock(ctx->mu);
+  CSM_CUDA(cudaSetDevice(ctx->device));
+  long long n = 0;
+  const int* d_idx = nullptr;
+  const uint16_t* d_val = nullptr;
+  CSM_TRY(DeviceVoxels3D(grid, LLONG_MAX, &n, &d_idx, &d_val));
+  PinnedBuf& h_idx = ctx->P("g3v_idx");
+  PinnedBuf& h_val = ctx->P("g3v_val");
+  if (n > 0) {
+    CSM_TRY(h_idx.Reserve(sizeof(int) * 3 * n));
+    CSM_TRY(h_val.Reserve(sizeof(uint16_t) * n));
+    cudaStream_t s = ctx->stream;
+    CSM_CUDA(cudaMemcpyAsync(h_idx.p, d_idx, sizeof(int) * 3 * n, cudaMemcpyDeviceToHost, s));
+    CSM_CUDA(cudaMemcpyAsync(h_val.p, d_val, sizeof(uint16_t) * n, cudaMemcpyDeviceToHost, s));
+    CSM_CUDA(cudaStreamSynchronize(s));
+  }
+  const int* idx = h_idx.as<int>();
+  const uint16_t* val = h_val.as<uint16_t>();
+  // proto::HybridGrid (hybrid_grid.proto): resolution = 1, packed sint32 x / y / z_indices =
+  // 3 / 4 / 5, packed int32 values = 6; HybridGrid::ToProto adds the voxels in iteration order
+  int64_t len[4] = {0, 0, 0, 0};
+  for (long long i = 0; i < n; ++i) {
+    for (int a = 0; a < 3; ++a) len[a] += VarintSize(ZigZag32(idx[3 * i + a]));
+    len[3] += VarintSize(val[i]);
+  }
+  const float resolution = grid->g.resolution;
+  int64_t total = FloatFieldSize(resolution);
+  if (n > 0)
+    for (int f = 0; f < 4; ++f) total += DelimitedSize(len[f]);
+  *size = total;
+  if (total >= (int64_t(1) << 31)) {
+    SetError("a serialized HybridGrid of %lld bytes exceeds protobuf's 2 GiB limit",
+             static_cast<long long>(total));
+    return CSM_E_CAPACITY;
+  }
+  if (!buf) return CSM_OK;
+  if (capacity < total) {
+    SetError("capacity %lld is below the %lld bytes of the message",
+             static_cast<long long>(capacity), static_cast<long long>(total));
+    return CSM_E_CAPACITY;
+  }
+  uint8_t* p = PutFloatField(buf, 1, resolution);
+  if (n > 0) {
+    for (int a = 0; a < 3; ++a) {
+      p = PutDelimitedHeader(p, 3 + a, len[a]);
+      for (long long i = 0; i < n; ++i) p = PutVarint(p, ZigZag32(idx[3 * i + a]));
+    }
+    p = PutDelimitedHeader(p, 6, len[3]);
+    for (long long i = 0; i < n; ++i) p = PutVarint(p, val[i]);
+  }
   return CSM_OK;
 }
 

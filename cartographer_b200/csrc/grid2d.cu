@@ -11,6 +11,7 @@
 #include <vector>
 
 #include "insert2d.cuh"
+#include "proto_write.h"
 #include "rtgrid.cuh"
 
 namespace csm {
@@ -487,6 +488,98 @@ csm_status csm_rt_grid2d_read_weights(const csm_rt_grid2d* grid, uint16_t* weigh
                              static_cast<size_t>(d.pitch) * 2, static_cast<size_t>(d.nx) * 2,
                              d.ny, cudaMemcpyDeviceToHost, grid->ctx->stream));
   CSM_CUDA(cudaStreamSynchronize(grid->ctx->stream));
+  return CSM_OK;
+}
+
+csm_status csm_rt_grid2d_to_proto(const csm_rt_grid2d* grid, uint8_t* buf, int64_t capacity,
+                                  int64_t* size) {
+  using namespace wire;
+  CSM_REQUIRE(grid != nullptr && size != nullptr, "null pointer");
+  csm_rt_grid2d* g = const_cast<csm_rt_grid2d*>(grid);   // the box is a cache
+  Ctx* ctx = g->ctx;
+  std::lock_guard<std::mutex> lock(ctx->mu);
+  CSM_CUDA(cudaSetDevice(ctx->device));
+  CSM_TRY(KnownBox(g));
+  const RtGridDev& d = g->g;
+  const bool tsdf = g->d_wcells != nullptr;
+  const size_t cells = static_cast<size_t>(d.nx) * d.ny;
+  PinnedBuf& staging = ctx->P("g2p_cells");
+  CSM_TRY(staging.Reserve(sizeof(uint16_t) * cells * (tsdf ? 2 : 1)));
+  uint16_t* h = staging.as<uint16_t>();
+  const uint16_t* arrays[2] = {g->d_cells, g->d_wcells};
+  for (int k = 0; k < (tsdf ? 2 : 1); ++k)
+    CSM_CUDA(cudaMemcpy2DAsync(h + k * cells, static_cast<size_t>(d.nx) * 2, arrays[k],
+                               static_cast<size_t>(d.pitch) * 2, static_cast<size_t>(d.nx) * 2,
+                               d.ny, cudaMemcpyDeviceToHost, ctx->stream));
+  CSM_CUDA(cudaStreamSynchronize(ctx->stream));
+  auto packed_len = [&](const uint16_t* c) {
+    int64_t n = 0;
+    for (size_t i = 0; i < cells; ++i) n += VarintSize(c[i]);
+    return n;
+  };
+  // proto::Grid2D (grid_2d.proto): limits = 1 {resolution = 1, max = 2 {x = 1, y = 2},
+  // cell_limits = 3 {num_x_cells = 1, num_y_cells = 2}}, cells = 2, known_cells_box = 3
+  // {max_x = 1, max_y = 2, min_x = 3, min_y = 4}, probability_grid_2d = 4 {} | tsdf_2d = 5
+  // {truncation_distance = 1, max_weight = 2, weight_cells = 3}, min / max_correspondence_cost =
+  // 6 / 7.  MapLimits' ToProto always sets max and cell_limits (map_limits.h:98-104).
+  const int64_t max_len = DoubleFieldSize(d.max_x) + DoubleFieldSize(d.max_y);
+  const int64_t cell_limits_len = Int32FieldSize(d.nx) + Int32FieldSize(d.ny);
+  const int64_t limits_len = DoubleFieldSize(d.resolution) + DelimitedSize(max_len) +
+                             DelimitedSize(cell_limits_len);
+  const int64_t cells_len = packed_len(h);
+  const KnownBox2& box = g->known;
+  const int32_t box_fields[4] = {box.hi[0], box.hi[1], box.lo[0], box.lo[1]};
+  int64_t box_len = 0;
+  for (int f = 0; f < 4; ++f) box_len += Int32FieldSize(box_fields[f]);
+  int64_t weights_len = 0, tsdf_len = 0;
+  if (tsdf) {
+    weights_len = packed_len(h + cells);
+    tsdf_len = FloatFieldSize(g->truncation) + FloatFieldSize(g->max_weight) +
+               DelimitedSize(weights_len);
+  }
+  const float min_cost = tsdf ? -g->truncation : kMinCorrespondenceCost;
+  const float max_cost = tsdf ? g->truncation : kMaxCorrespondenceCost;
+  const int64_t total = DelimitedSize(limits_len) + DelimitedSize(cells_len) +
+                        (box.empty() ? 0 : DelimitedSize(box_len)) +
+                        DelimitedSize(tsdf ? tsdf_len : 0) + FloatFieldSize(min_cost) +
+                        FloatFieldSize(max_cost);
+  *size = total;
+  if (total >= (int64_t(1) << 31)) {
+    SetError("a serialized Grid2D of %lld bytes exceeds protobuf's 2 GiB limit",
+             static_cast<long long>(total));
+    return CSM_E_CAPACITY;
+  }
+  if (!buf) return CSM_OK;
+  if (capacity < total) {
+    SetError("capacity %lld is below the %lld bytes of the message",
+             static_cast<long long>(capacity), static_cast<long long>(total));
+    return CSM_E_CAPACITY;
+  }
+  uint8_t* p = PutDelimitedHeader(buf, 1, limits_len);
+  p = PutDoubleField(p, 1, d.resolution);
+  p = PutDelimitedHeader(p, 2, max_len);
+  p = PutDoubleField(p, 1, d.max_x);
+  p = PutDoubleField(p, 2, d.max_y);
+  p = PutDelimitedHeader(p, 3, cell_limits_len);
+  p = PutInt32Field(p, 1, d.nx);
+  p = PutInt32Field(p, 2, d.ny);
+  p = PutDelimitedHeader(p, 2, cells_len);
+  for (size_t i = 0; i < cells; ++i) p = PutVarint(p, h[i]);
+  if (!box.empty()) {
+    p = PutDelimitedHeader(p, 3, box_len);
+    for (int f = 0; f < 4; ++f) p = PutInt32Field(p, 1 + f, box_fields[f]);
+  }
+  if (tsdf) {
+    p = PutDelimitedHeader(p, 5, tsdf_len);
+    p = PutFloatField(p, 1, g->truncation);
+    p = PutFloatField(p, 2, g->max_weight);
+    p = PutDelimitedHeader(p, 3, weights_len);
+    for (size_t i = 0; i < cells; ++i) p = PutVarint(p, h[cells + i]);
+  } else {
+    p = PutDelimitedHeader(p, 4, 0);
+  }
+  p = PutFloatField(p, 6, min_cost);
+  PutFloatField(p, 7, max_cost);
   return CSM_OK;
 }
 

@@ -356,6 +356,15 @@ class GridState:
     weight_cells: object = None   # a TSDF2D's weight cells[y, x] (cells are its tsd cells)
 
 
+def _serialize(fn, handle, capacity):
+    """bytes of fn(handle, buf, capacity, &size), a *_to_proto entry point, given a capacity
+    that holds the message."""
+    buf = np.zeros(max(capacity, 1), np.uint8)
+    size = C.c_int64()
+    check(fn(handle, ptr(buf, C.c_uint8), C.c_int64(buf.size), C.byref(size)))
+    return buf[:size.value].tobytes()
+
+
 class RealTimeGrid2D:
     """A ProbabilityGrid or TSDF2D resident on the device (csm_rt_grid2d): what
     LocalTrajectoryBuilder2D's active submap grid is to the real-time matcher
@@ -441,6 +450,15 @@ class RealTimeGrid2D:
                                                    C.c_int64(weights.size)))
         return GridState(cells, info.resolution, info.max_x, info.max_y, box,
                          weight_cells=weights)
+
+    def to_proto(self):
+        """The serialised proto::Grid2D that ProbabilityGrid::ToProto or TSDF2D::ToProto gives
+        for this grid (csm_rt_grid2d_to_proto), as bytes."""
+        info = self._info()
+        cells = info.num_x_cells * info.num_y_cells
+        # at most 3 bytes per cell (values below 2^15) in each packed array, and 128 for the rest
+        return _serialize(lib().csm_rt_grid2d_to_proto, self._h,
+                          128 + 3 * cells * (2 if info.is_tsdf else 1))
 
     def ComputeCroppedGrid(self):
         """ProbabilityGrid::ComputeCroppedGrid from device to device: a new RealTimeGrid2D over
@@ -1139,6 +1157,26 @@ class DeviceHybridGrid:
         check(lib().csm_grid3d_read(self._h, ptr(lo, C.c_int32), ptr(dims, C.c_int32),
                                     ptr(out, C.c_uint16)))
         return lo, out
+
+    def voxels(self):
+        """(indices, values): the non-zero voxels in HybridGrid's iteration order, the order
+        HybridGrid::ToProto writes them (csm_grid3d_voxels) — n x 3 int32 and n uint16."""
+        n = C.c_int64()
+        check(lib().csm_grid3d_voxels(self._h, None, None, C.c_int64(0), C.byref(n)))
+        idx = np.zeros((n.value, 3), np.int32)
+        val = np.zeros(n.value, np.uint16)
+        if n.value:
+            check(lib().csm_grid3d_voxels(self._h, ptr(idx, C.c_int32), ptr(val, C.c_uint16),
+                                          C.c_int64(n.value), C.byref(n)))
+        return idx, val
+
+    def to_proto(self):
+        """The serialised proto::HybridGrid that HybridGrid::ToProto gives for this grid
+        (csm_grid3d_to_proto), as bytes."""
+        n = C.c_int64()
+        check(lib().csm_grid3d_voxels(self._h, None, None, C.c_int64(0), C.byref(n)))
+        # resolution, four packed-field headers, at most 5 bytes per index and 3 per value
+        return _serialize(lib().csm_grid3d_to_proto, self._h, 5 + 4 * 11 + 18 * n.value)
 
     def close(self):
         if getattr(self, "_h", None):

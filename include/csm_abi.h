@@ -739,6 +739,43 @@ csm_status csm_matcher3d_create_from_grid3d(const csm_grid3d* hybrid_grid,
 csm_status csm_intensity_grid3d_read(const csm_intensity_grid3d* grid, int32_t lo[3],
                                      int32_t dims[3], float* mean, float* sum, int32_t* count);
 
+/* ---- saving device grids: HybridGrid::ToProto and Grid2D::ToProto --------------------------- */
+/* What Submap3D::ToProto / Submap2D::ToProto serialise (and MapBuilder::SerializeState saves),
+ * straight from the device handles.  Encoding: fields in field-number order; implicit-presence
+ * scalars omitted when zero, including a MapLimits max.x of 0.0 and a known-cells box coordinate of
+ * 0; a float or double is omitted only when its bit pattern is all zeros, so -0.0 IS written (the
+ * bit-pattern test of protobuf C++'s generated serialisers); repeated scalars packed, and omitted
+ * when empty; a present empty sub-message written with length 0.  No protobuf runtime is involved.
+ * A handle carries no update marker between calls (the inserters finish every update), as
+ * ToProto's CHECK(update_indices_.empty()) requires; no insert may be in flight on it, and the
+ * handle is left unchanged.  With buf == NULL only *size is written; a capacity below *size returns
+ * CSM_E_CAPACITY with *size the needed size and nothing written, and so does a message of 2^31
+ * bytes or more (protobuf's limit), whatever the capacity. */
+
+/* The non-zero voxels of a csm_grid3d in HybridGrid's iteration order, which ToProto writes
+ * (hybrid_grid.h:528-540, iterator :300-340): n x {x, y, z} indices and n values as the handle
+ * holds them, the flat form csm_grid3d_create and csm_matcher3d_create take.  With
+ * indices == values == NULL only *num_voxels is written; a capacity (in voxels) below it returns
+ * CSM_E_CAPACITY with *num_voxels set and nothing written.  Three stream synchronisations (the
+ * non-zero box, the count, the copy; one when the grid has no non-zero voxel, two without a list). */
+csm_status csm_grid3d_voxels(const csm_grid3d* grid, int32_t* indices, uint16_t* values,
+                             int64_t capacity, int64_t* num_voxels);
+/* A serialised cartographer.mapping.proto.HybridGrid (hybrid_grid.proto): resolution, then the
+ * csm_grid3d_voxels list as packed sint32 x / y / z indices and packed int32 values.  A grid with
+ * no non-zero voxel gives the resolution field alone.  The stream synchronisations of
+ * csm_grid3d_voxels; the encoding runs on the host. */
+csm_status csm_grid3d_to_proto(const csm_grid3d* grid, uint8_t* buf, int64_t capacity,
+                               int64_t* size);
+/* A serialised cartographer.mapping.proto.Grid2D, as ProbabilityGrid::ToProto or TSDF2D::ToProto
+ * writes it (grid_2d.cc:166-183, probability_grid.cc:84-89, tsdf_2d.cc:107-116): limits, every
+ * cell (num_y x num_x, row-major), the known-cells box unless it is empty, probability_grid_2d {}
+ * or tsdf_2d {truncation_distance, max_weight, weight_cells} from the handle's own converter, and
+ * the min / max correspondence cost (ProbabilityGrid: kMin/kMaxCorrespondenceCost; TSDF2D:
+ * -/+ truncation_distance).  One or two stream synchronisations (the known-cells box of a handle
+ * made from cells, the cell copy). */
+csm_status csm_rt_grid2d_to_proto(const csm_rt_grid2d* grid, uint8_t* buf, int64_t capacity,
+                                  int64_t* size);
+
 /* ---- map writing in 2D: ProbabilityGridRangeDataInserter2D on device grids ------------ */
 /* ProbabilityGridRangeDataInserter2D (mapping/2d/probability_grid_range_data_inserter_2d.cc)
  * applied in place to a ProbabilityGrid csm_rt_grid2d, so that a 2D submap lives on the device
