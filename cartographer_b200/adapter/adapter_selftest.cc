@@ -8,6 +8,7 @@
 
 #include "constraint_builder_b200.h"
 #include "scan_matchers_b200.h"
+#include "voxel_filter_b200.h"
 
 using namespace cartographer;
 
@@ -705,6 +706,46 @@ int main() {
     for (uint16_t v : weights) std::printf(" %u", v);
     std::printf("\n");
     PrintBytes("grid_to_proto_insert_tsdf2d", grid.ToProto());
+  }
+  {
+    // sensor::VoxelFilter's four overloads and AdaptiveVoxelFilter: every payload carries the
+    // point's input index, so the RESULT lines list the kept indices
+    const int n = 2000;
+    sensor::PointCloud cloud;
+    std::vector<float> intensities;
+    std::vector<sensor::RangefinderPoint> points;
+    sensor::TimedPointCloud timed;
+    std::vector<sensor::TimedPointCloudOriginData::RangeMeasurement> measurements;
+    for (int i = 0; i < n; ++i) {
+      const sensor::RangefinderPoint p{{{float((i * 37) % 101) * 0.05f,
+                                         float((i * 53) % 89) * 0.05f, float(i % 13) * 0.1f}}};
+      cloud.push_back(p);
+      intensities.push_back(float(i));
+      points.push_back(p);
+      timed.push_back({{{p.position.x(), p.position.y(), p.position.z()}}, float(i)});
+      measurements.push_back({timed.back(), 0.f, size_t(i)});
+    }
+    const sensor::PointCloud with_intensities(cloud.points(), intensities);
+    const sensor::PointCloud a = sensor::VoxelFilter(with_intensities, 0.3f);
+    std::printf("RESULT vf_cloud");
+    for (float v : a.intensities()) std::printf(" %d", int(v));
+    std::printf("\n");
+    std::printf("RESULT vf_points %zu\n", sensor::VoxelFilter(points, 0.3f).size());
+    std::printf("RESULT vf_timed");
+    for (const auto& p : sensor::VoxelFilter(timed, 0.2f)) std::printf(" %d", int(p.time));
+    std::printf("\n");
+    std::printf("RESULT vf_range");
+    for (const auto& m : sensor::VoxelFilter(measurements, 0.5f))
+      std::printf(" %zu", m.origin_index);
+    std::printf("\n");
+    sensor::proto::AdaptiveVoxelFilterOptions options;
+    options.set_max_length(2.f);
+    options.set_min_num_points(150.f);
+    options.set_max_range(4.f);
+    const sensor::PointCloud b = sensor::AdaptiveVoxelFilter(with_intensities, options);
+    std::printf("RESULT vf_adaptive");
+    for (float v : b.intensities()) std::printf(" %d", int(v));
+    std::printf("\n");
   }
   return 0;
 }

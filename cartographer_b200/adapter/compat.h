@@ -72,6 +72,34 @@ struct RangeData {
   PointCloud returns;
   PointCloud misses;
 };
+// sensor/rangefinder_point.h:36-40 and sensor/point_cloud.h:95 (TimedPointCloud).
+struct TimedRangefinderPoint {
+  struct { float v[3]; float x() const { return v[0]; } float y() const { return v[1]; } float z() const { return v[2]; } } position;
+  float time;
+};
+using TimedPointCloud = std::vector<TimedRangefinderPoint>;
+// sensor/timed_point_cloud_data.h:36-45.
+struct TimedPointCloudOriginData {
+  struct RangeMeasurement {
+    TimedRangefinderPoint point_time;
+    float intensity;
+    size_t origin_index;
+  };
+};
+namespace proto {
+// sensor/proto/adaptive_voxel_filter_options.proto: three float fields.
+class AdaptiveVoxelFilterOptions {
+ public:
+  float max_length() const { return max_length_; }
+  float min_num_points() const { return min_num_points_; }
+  float max_range() const { return max_range_; }
+  void set_max_length(float v) { max_length_ = v; }
+  void set_min_num_points(float v) { min_num_points_ = v; }
+  void set_max_range(float v) { max_range_ = v; }
+ private:
+  float max_length_ = 0.f, min_num_points_ = 0.f, max_range_ = 0.f;
+};
+}  // namespace proto
 }  // namespace sensor
 
 namespace mapping {

@@ -882,6 +882,40 @@ csm_status csm_rt_grid2d_create_empty_tsdf(double resolution, double max_x, doub
 csm_status csm_rt_grid2d_read_weights(const csm_rt_grid2d* grid, uint16_t* weight_cells,
                                       int64_t capacity);
 
+/* ---- scan filtering: VoxelFilter and AdaptiveVoxelFilter ------------------------------- */
+/* sensor::VoxelFilter (sensor/internal/voxel_filter.cc:88-180) on many clouds at once: per
+ * cloud, the input indices the reference's reservoir sampling keeps (one std::minstd_rand0 of
+ * seed 1 per cloud, libstdc++'s uniform_int_distribution), bit for bit, in input order.
+ * xyz[c] holds num_points[c] x {x, y, z}.  kept_indices (capacity sum of num_points) receives
+ * the clouds' kept indices one cloud after another, each index into its own cloud; num_kept[c]
+ * their count.  The four VoxelFilter overloads differ only in the payload that follows the
+ * kept points.  CSM_E_INVALID, writing no output, for a negative count, a null pointer where
+ * data is required, a non-finite coordinate, a resolution that is not finite and > 0, or more
+ * than 2^30 points in one call.  One stream synchronisation; stats (may be NULL) gets
+ * host_syncs and device_ms. */
+csm_status csm_voxel_filter_batch(const float* const* xyz, const int32_t* num_points,
+                                  const float* resolution, int32_t num_clouds, int32_t device,
+                                  int32_t* kept_indices, int32_t* num_kept,
+                                  csm_stats* stats /* may be NULL */);
+typedef struct csm_adaptive_voxel_filter_options {   /* proto AdaptiveVoxelFilterOptions */
+  float max_length;                                  /* finite, > 0 */
+  float min_num_points;                              /* a float field: compared as float */
+  float max_range;                                   /* not NaN; may be +infinity */
+  int32_t reserved;
+} csm_adaptive_voxel_filter_options;
+/* sensor::AdaptiveVoxelFilter (voxel_filter.cc:31-75, 192-197) per cloud with its own options:
+ * the points within max_range, then, unless there are at most min_num_points of them, the
+ * VoxelFilter of those points at the length the reference's halving and bisection settle on
+ * (the last halving length when none leaves min_num_points).  The search runs on the device;
+ * whatever the number of lengths tried, one stream synchronisation.  Output, refusals and stats
+ * as csm_voxel_filter_batch (indices into the unfiltered input cloud); a NaN min_num_points or
+ * max_range is refused too.  CSM_E_INTERNAL if a bisection does not settle within 8 steps. */
+csm_status csm_adaptive_voxel_filter_batch(const float* const* xyz, const int32_t* num_points,
+                                           const csm_adaptive_voxel_filter_options* options,
+                                           int32_t num_clouds, int32_t device,
+                                           int32_t* kept_indices, int32_t* num_kept,
+                                           csm_stats* stats /* may be NULL */);
+
 /* Test hook: as csm_ceres_evaluate3d, in the problem's residual-block order — per cloud its
  * occupied-space residuals, then its intensity residuals if it has a grid; then 3
  * translation and 3 rotation residuals.  Residuals and rows are uncorrected by the loss, as
