@@ -399,6 +399,19 @@ int main() {
       std::printf(" %08x:%08x:%d", Bits(mean[i]), Bits(sum[i]), count[i]);
     std::printf("\n");
     PrintBytes("grid_to_proto_insert3d", grid.ToProto());
+    // Submap3D::ToResponseProto on device grids: the version, then the high-resolution grid's
+    // texture and the low-resolution grid's (a fresh one here: no voxel, the 2 x 2 texture)
+    {
+      const transform::Rigid3d pose({{0.5, -0.25, 0.125}},
+                                    {0.96592582628906831, 0., 0., 0.25881904510252074});
+      const mapping::scan_matching::DeviceHybridGrid low(2.f, 0);
+      std::string high_texture, low_texture;
+      grid.AddToTextureProto(pose, &high_texture);
+      low.AddToTextureProto(pose, &low_texture);
+      std::printf("RESULT texture_response3d 2\n");
+      PrintBytes("texture_response3d_high", high_texture);
+      PrintBytes("texture_response3d_low", low_texture);
+    }
   }
   // ---- FastCorrelativeScanMatcher3D and ConstraintBuilder3D on inserted device grids: the
   // axis cloud inserted twice from its sensor position into empty grids; the same built from
@@ -531,6 +544,12 @@ int main() {
       for (uint16_t v : cells) std::printf(" %u", v);
       std::printf("\n");
       PrintBytes(g == &grid ? "grid_to_proto_insert2d" : "grid_to_proto_crop2d", g->ToProto());
+      // Submap2D::ToResponseProto: the version, then the grid's texture with the local pose
+      const transform::Rigid3d local_pose({{0.5, -0.25, 0.}},
+                                          {0.96592582628906831, 0., 0., 0.25881904510252074});
+      std::string texture;
+      if (!g->DrawToSubmapTexture(&texture, local_pose)) return 1;
+      PrintBytes(g == &grid ? "texture_response2d_insert" : "texture_response2d_crop", texture);
     }
     mapping::scan_matching::proto::FastCorrelativeScanMatcherOptions2D fo;
     fo.set_linear_search_window(3.);

@@ -32,6 +32,7 @@
 #include "cartographer/mapping/proto/scan_matching/real_time_correlative_scan_matcher_options.pb.h"
 #include "cartographer/mapping/proto/hybrid_grid.pb.h"
 #include "cartographer/mapping/proto/range_data_inserter_options_3d.pb.h"
+#include "cartographer/mapping/proto/submap_visualization.pb.h"
 #include "cartographer/mapping/proto/probability_grid_range_data_inserter_options_2d.pb.h"
 #include "cartographer/sensor/point_cloud.h"
 #include "cartographer/sensor/range_data.h"
@@ -89,6 +90,7 @@ Message Parse(const std::string& bytes) {
 }
 using HybridGridProto = ::cartographer::mapping::proto::HybridGrid;
 using Grid2DProto = ::cartographer::mapping::proto::Grid2D;
+using SubmapTextureProto = ::cartographer::mapping::proto::SubmapQuery::Response::SubmapTexture;
 #else
 template <typename Message>
 Message Parse(const std::string& bytes) {
@@ -96,7 +98,30 @@ Message Parse(const std::string& bytes) {
 }
 using HybridGridProto = std::string;
 using Grid2DProto = std::string;
+using SubmapTextureProto = std::string;
 #endif
+// The serialised texture one *_to_texture entry point draws with `pose`.  Every call does the
+// whole work, so the first goes with a buffer that holds most textures and a second, sized
+// exactly, only when that one was too small.
+template <typename Handle>
+std::string DrawTexture(csm_status (*to_texture)(const Handle*, const double*, uint8_t*, int64_t,
+                                                 int64_t*),
+                        const Handle* handle, const transform::Rigid3d& pose) {
+  const double p[7] = {pose.translation().x(), pose.translation().y(), pose.translation().z(),
+                       pose.rotation().w(),    pose.rotation().x(),    pose.rotation().y(),
+                       pose.rotation().z()};
+  std::string bytes(size_t(1) << 16, '\0');
+  int64_t size = 0;
+  csm_status st = to_texture(handle, p, reinterpret_cast<uint8_t*>(&bytes[0]),
+                             static_cast<int64_t>(bytes.size()), &size);
+  if (st == CSM_E_CAPACITY && size > static_cast<int64_t>(bytes.size())) {
+    bytes.resize(static_cast<size_t>(size));
+    st = to_texture(handle, p, reinterpret_cast<uint8_t*>(&bytes[0]), size, &size);
+  }
+  if (!Check(st)) std::abort();
+  bytes.resize(static_cast<size_t>(size));
+  return bytes;
+}
 }  // namespace b200_internal
 
 class DeviceGrid2D;
@@ -327,6 +352,15 @@ class DeviceGrid2D {
   b200_internal::Grid2DProto ToProto() const {
     return b200_internal::Parse<b200_internal::Grid2DProto>(
         b200_internal::Serialize(csm_rt_grid2d_to_proto, grid_));
+  }
+  // ProbabilityGrid::DrawToSubmapTexture / TSDF2D::DrawToSubmapTexture
+  // (csm_rt_grid2d_to_texture): the texture Submap2D::ToResponseProto adds with the submap's
+  // local pose.
+  bool DrawToSubmapTexture(b200_internal::SubmapTextureProto* texture,
+                           const transform::Rigid3d& local_pose) const {
+    *texture = b200_internal::Parse<b200_internal::SubmapTextureProto>(
+        b200_internal::DrawTexture(csm_rt_grid2d_to_texture, grid_, local_pose));
+    return true;
   }
   // The weight cells of a TSDF2D (num_y x num_x); Read gives its tsd cells.
   void ReadWeights(std::vector<uint16_t>* weight_cells) const {
@@ -661,6 +695,14 @@ class DeviceHybridGrid {
   b200_internal::HybridGridProto ToProto() const {
     return b200_internal::Parse<b200_internal::HybridGridProto>(
         b200_internal::Serialize(csm_grid3d_to_proto, grid_));
+  }
+  // AddToTextureProto (mapping/3d/submap_3d.cc:146-176, csm_grid3d_to_texture): the texture
+  // Submap3D::ToResponseProto adds for this grid with the global submap pose, the
+  // high-resolution grid's first.
+  void AddToTextureProto(const transform::Rigid3d& global_submap_pose,
+                         b200_internal::SubmapTextureProto* texture) const {
+    *texture = b200_internal::Parse<b200_internal::SubmapTextureProto>(
+        b200_internal::DrawTexture(csm_grid3d_to_texture, grid_, global_submap_pose));
   }
 
  private:

@@ -1076,6 +1076,15 @@ csm_status DeviceVoxels3D(const csm_grid3d* g, long long list_capacity, long lon
 
 }  // namespace
 
+namespace csm {
+
+csm_status NonZeroVoxels3D(const csm_grid3d* g, long long list_capacity, long long* n,
+                           const int** d_idx, const uint16_t** d_val) {
+  return DeviceVoxels3D(g, list_capacity, n, d_idx, d_val);
+}
+
+}  // namespace csm
+
 extern "C" {
 
 csm_status csm_matcher3d_create(const int32_t* hi_idx, const uint16_t* hi_val, int64_t hi_n,

@@ -285,6 +285,8 @@ const std::vector<uint16_t>& CropTable() {
 
 namespace csm {
 
+csm_status RefreshKnownBox(csm_rt_grid2d* grid) { return KnownBox(grid); }
+
 csm_status UploadCells(csm_rt_grid2d* g, const uint16_t* cells, const uint16_t* wcells,
                        cudaStream_t s) {
   CSM_CUDA(cudaMemcpy2DAsync(g->d_cells, static_cast<size_t>(g->g.pitch) * 2, cells,

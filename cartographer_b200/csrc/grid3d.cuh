@@ -56,4 +56,14 @@ struct csm_intensity_grid3d {
   }
 };
 
+namespace csm {
+
+// The number *n of non-zero voxels of `g` and, when it is at most list_capacity, the voxels in
+// HybridGrid's iteration order in device workspaces: *d_idx ({x, y, z} each) and *d_val, ready on
+// the context's stream (engine3d.cu, what csm_grid3d_voxels returns).  Caller holds ctx->mu.
+csm_status NonZeroVoxels3D(const csm_grid3d* g, long long list_capacity, long long* n,
+                           const int** d_idx, const uint16_t** d_val);
+
+}  // namespace csm
+
 #endif  // CSM_GRID3D_CUH_

@@ -89,6 +89,10 @@ csm_status RtGridCreate(const uint16_t* cells, const uint16_t* wcells, float tru
                         float max_weight, int32_t nx, int32_t ny, double resolution, double max_x,
                         double max_y, int32_t device, csm_rt_grid2d** out);
 
+// Brings grid->known up to date (one stream synchronisation when it is stale).  Caller holds
+// ctx->mu.
+csm_status RefreshKnownBox(csm_rt_grid2d* grid);
+
 // Uploads `cells` (and `wcells` if not null; host row pitch nx) into the handle's arrays on
 // stream s.  The caller marks the known-cells box stale when the cells change.
 csm_status UploadCells(csm_rt_grid2d* g, const uint16_t* cells, const uint16_t* wcells,

@@ -365,6 +365,22 @@ def _serialize(fn, handle, capacity):
     return buf[:size.value].tobytes()
 
 
+def _texture(fn, handle, pose):
+    """bytes of fn(handle, pose, buf, capacity, &size), a *_to_texture entry point: every call
+    does the whole work, so a first try with a buffer that holds most textures, and a second
+    with the exact size only when it did not."""
+    p = np.ascontiguousarray(pose, np.float64).reshape(7)
+    size = C.c_int64()
+    buf = np.zeros(1 << 20, np.uint8)
+    st = fn(handle, ptr(p, C.c_double), ptr(buf, C.c_uint8), C.c_int64(buf.size), C.byref(size))
+    if st == 3 and size.value > buf.size:   # CSM_E_CAPACITY
+        buf = np.zeros(size.value, np.uint8)
+        st = fn(handle, ptr(p, C.c_double), ptr(buf, C.c_uint8), C.c_int64(buf.size),
+                C.byref(size))
+    check(st)
+    return buf[:size.value].tobytes()
+
+
 class RealTimeGrid2D:
     """A ProbabilityGrid or TSDF2D resident on the device (csm_rt_grid2d): what
     LocalTrajectoryBuilder2D's active submap grid is to the real-time matcher
@@ -459,6 +475,13 @@ class RealTimeGrid2D:
         # at most 3 bytes per cell (values below 2^15) in each packed array, and 128 for the rest
         return _serialize(lib().csm_rt_grid2d_to_proto, self._h,
                           128 + 3 * cells * (2 if info.is_tsdf else 1))
+
+    def to_texture(self, local_pose):
+        """The serialised proto::SubmapQuery::Response::SubmapTexture that
+        ProbabilityGrid::DrawToSubmapTexture or TSDF2D::DrawToSubmapTexture draws for this grid
+        with the submap's local pose (tx, ty, tz, qw, qx, qy, qz), as Submap2D::ToResponseProto
+        adds it (csm_rt_grid2d_to_texture), as bytes."""
+        return _texture(lib().csm_rt_grid2d_to_texture, self._h, local_pose)
 
     def ComputeCroppedGrid(self):
         """ProbabilityGrid::ComputeCroppedGrid from device to device: a new RealTimeGrid2D over
@@ -1177,6 +1200,13 @@ class DeviceHybridGrid:
         check(lib().csm_grid3d_voxels(self._h, None, None, C.c_int64(0), C.byref(n)))
         # resolution, four packed-field headers, at most 5 bytes per index and 3 per value
         return _serialize(lib().csm_grid3d_to_proto, self._h, 5 + 4 * 11 + 18 * n.value)
+
+    def to_texture(self, global_submap_pose):
+        """The serialised proto::SubmapQuery::Response::SubmapTexture that AddToTextureProto
+        draws for this grid under the global submap pose (tx, ty, tz, qw, qx, qy, qz):
+        Submap3D::ToResponseProto adds the high-resolution grid's texture, then the
+        low-resolution grid's (csm_grid3d_to_texture), as bytes."""
+        return _texture(lib().csm_grid3d_to_texture, self._h, global_submap_pose)
 
     def close(self):
         if getattr(self, "_h", None):

@@ -776,6 +776,43 @@ csm_status csm_grid3d_to_proto(const csm_grid3d* grid, uint8_t* buf, int64_t cap
 csm_status csm_rt_grid2d_to_proto(const csm_rt_grid2d* grid, uint8_t* buf, int64_t capacity,
                                   int64_t* size);
 
+/* ---- drawing submaps for display: Submap2D / Submap3D::ToResponseProto ------------------------ */
+/* A serialised cartographer.mapping.proto.SubmapQuery.Response.SubmapTexture, the texture
+ * MapBuilder::SubmapToProto serves and io::FetchSubmapTextures paints, straight from a device
+ * handle: cells = 1 (the value / alpha byte pairs, x fastest, gzip'd as common::FastGzipString
+ * does: boost's gzip header with XFL 4 and OS 255, raw deflate at level 1, window 15, memLevel 8,
+ * then CRC-32 and ISIZE), width = 2, height = 3, resolution = 4 and slice_pose = 5 (Rigid3d
+ * {translation {x, y, z}, rotation {x, y, z, w}}), with the encoding rules of the *_to_proto
+ * entry points above.  Poses are {tx, ty, tz, qw, qx, qy, qz}; a non-finite component returns
+ * CSM_E_INVALID.  The pixel values are bit for bit the reference's; the step function
+ * ProbabilityToLogOddsInteger is a table of its 254 steps, built on the host with the reference's
+ * expression on the host's logf.  Every call, including one with buf == NULL, does the whole
+ * work (the size of a gzip member is known only after compressing): *size is always the exact
+ * size; a capacity below it returns CSM_E_CAPACITY with *size set and nothing written, and so
+ * does a message of 2^31 bytes or more.  The handle is left unchanged, and no insert may be in
+ * flight on it. */
+
+/* ProbabilityGrid::DrawToSubmapTexture or TSDF2D::DrawToSubmapTexture (probability_grid.cc:109-147,
+ * internal/2d/tsdf_2d.cc:137-181) with the submap's local pose, as Submap2D::ToResponseProto
+ * calls it: the cells of Grid2D::ComputeCroppedLimits (the known-cells box, or 1 x 1 at offset 0
+ * when it is empty).  ProbabilityGrid: delta = 128 - ProbabilityToLogOddsInteger(probability);
+ * TSDF2D: delta = round(weight / max_weight * (pow(|tsd| / max_tsd, 0.5f) * 255. - 128.)), the
+ * powers from the host's powf.  One or two stream synchronisations (the known-cells box of a
+ * handle made from cells, the cells). */
+csm_status csm_rt_grid2d_to_texture(const csm_rt_grid2d* grid, const double local_pose[7],
+                                    uint8_t* buf, int64_t capacity, int64_t* size);
+/* AddToTextureProto (mapping/3d/submap_3d.cc:51-176) with the global submap pose, as
+ * Submap3D::ToResponseProto calls it for the high- and then the low-resolution grid: an X-ray
+ * view of the voxels with probability >= 0.501f, transformed by the pose cast to float, rounded
+ * to pixels and accumulated per pixel in HybridGrid's iteration order.  A grid with no such
+ * voxel gives what x86-64 gives the reference: the pixel box stays (INT_MAX, INT_MIN), its
+ * width and height wrap to 2, the 2 x 2 pixels are (0, 0) and the slice pose is built from
+ * INT_MIN * resolution.  A pixel box of 2^30 pixels or more returns CSM_E_CAPACITY (the
+ * reference would allocate 20 bytes per pixel).  Four stream synchronisations (the non-zero box,
+ * the voxel count, the pixel box, the pixels; one when the grid has no non-zero voxel). */
+csm_status csm_grid3d_to_texture(const csm_grid3d* grid, const double global_submap_pose[7],
+                                 uint8_t* buf, int64_t capacity, int64_t* size);
+
 /* ---- map writing in 2D: ProbabilityGridRangeDataInserter2D on device grids ------------ */
 /* ProbabilityGridRangeDataInserter2D (mapping/2d/probability_grid_range_data_inserter_2d.cc)
  * applied in place to a ProbabilityGrid csm_rt_grid2d, so that a 2D submap lives on the device
