@@ -1848,14 +1848,6 @@ struct BatchPlan {
 
 struct TieLeaf { int scan, xo, yo; };
 
-// Kernel forms that can be forced.  A match takes them from CSM_NO_LATTICE / CSM_LAT_UNROLL,
-// the test hooks csm_score_top2d / csm_branch_step2d from their arguments.
-struct Forms2D {
-  const char* top = nullptr;  // "small" | "gather" | "tile" | "dense"; nullptr = by size
-  int lattice_min = INT_MAX;  // smallest frontier the lattice kernel takes (INT_MAX: none)
-  int unroll = 8;             // k_expand_lattice<4 | 8 | 16>
-};
-
 // The branch-and-bound sweep.  The first sweep hmax -> 1 is a static stream of launches:
 // every level takes a chunk of <= kChunk nodes from the end of its queue (k_level_begin),
 // picks the kernel form on the device and appends the survivors to the next queue; nothing
@@ -1871,6 +1863,22 @@ constexpr int kLatticeMin = 16384;  // smaller frontiers: the warp-per-parent ke
 constexpr int kInlineBest = 4096;   // optimal leaves read back with the first (usually only) sync
 // Dives start only from scans whose best lowest-resolution sum is within 3 % of their job's best.
 constexpr float kDiveRatio = 0.97f;
+// Discrete-scan points per sub-batch of csm_match2d_batch (~4 GB of short2).
+constexpr long long kMaxPoints = 1LL << 30;
+
+// Kernel forms and sweep limits that can be forced.  A match takes the forms from
+// CSM_NO_LATTICE / CSM_LAT_UNROLL and the limits from the constants above; the test hooks
+// take them from their arguments.  A limit below its constant changes only the control
+// flow: every buffer is still reserved at the constant's size.
+struct Forms2D {
+  const char* top = nullptr;  // "small" | "gather" | "tile" | "dense"; nullptr = by size
+  int lattice_min = INT_MAX;  // smallest frontier the lattice kernel takes (INT_MAX: none)
+  int unroll = 8;             // k_expand_lattice<4 | 8 | 16>
+  int chunk = kChunk;              // nodes per level chunk (k_level_begin)
+  int leaf_cap = kLeafCap;         // leaves recorded before the queue-overflow error
+  int inline_best = kInlineBest;   // optimal leaves read back with each collect
+  float dive_ratio = kDiveRatio;   // k_dive's gate; > 1 runs no dive
+};
 
 double NowMs() {
   return std::chrono::duration<double, std::milli>(
@@ -1916,6 +1924,9 @@ struct Batch2D {
   const unsigned* lbh = nullptr;
   const Node* best_inline = nullptr;
   int host_syncs = 0;
+  // sweep trace: collects (1 + continuation sweeps), leaf compactions between sweeps, most
+  // leaves held at a collect, optimal leaves
+  int sweeps = 0, compactions = 0, max_leaves = 0, n_best = 0;
   unsigned long long prof_c0 = 0;
   double t_phase = 0.;
 
@@ -2258,7 +2269,7 @@ csm_status Dives2D(Batch2D& b) {
   k_dive<<<grid, 256, 0, b.s>>>(
       b.d_jobs->as<JobDev>(), b.d_info->as<ScanInfo>(), b.d_dscan->as<short2>(),
       b.d_top->as<int>(), b.d_slot_base->as<long long>(), b.total_scans, b.d_job_best->as<int>(),
-      kDiveRatio, b.d_lb->as<unsigned>(), b.ctr);
+      b.forms.dive_ratio, b.d_lb->as<unsigned>(), b.ctr);
   CSM_LAUNCH_CHECK();
   if (g_profile_on.load()) {
     ProfStop(b.ctx);
@@ -2317,7 +2328,7 @@ csm_status FilterTop2D(Batch2D& b) {
   if (hmax == 0) {
     k_top_as_leaves<<<b.ctx->sm_count * 4, 256, 0, b.s>>>(b.d_info->as<ScanInfo>(), b.Queue(0),
                                                           b.ictr, b.d_lb->as<unsigned>(),
-                                                          b.d_leaves->as<Node>(), kLeafCap);
+                                                          b.d_leaves->as<Node>(), b.forms.leaf_cap);
     CSM_LAUNCH_CHECK();
   }
   return CSM_OK;
@@ -2331,7 +2342,8 @@ csm_status LevelStep2D(Batch2D& b, int h) {
   const int total_scans = b.total_scans;
   const int nb = DivUp(total_scans, 1024);
   const int sort_grid = ctx->sm_count * 8;
-  const int max_items = kChunk / 32 + std::min(kChunk, total_scans) + 1;
+  const int chunk = b.forms.chunk, leaf_cap = b.forms.leaf_cap;
+  const int max_items = chunk / 32 + std::min(chunk, total_scans) + 1;
   int* ictr = b.ictr;
   int* scan_cnt = b.d_scan_cnt->as<int>();
   int* cursor = scan_cnt + total_scans;
@@ -2340,7 +2352,7 @@ csm_status LevelStep2D(Batch2D& b, int h) {
   int* part_b = part_a + nb;
   Node* next = h - 1 >= 1 ? b.Queue(h - 1) : nullptr;
   int* next_count = ictr + (h - 1 >= 1 ? h - 1 : 31);
-  k_level_begin<<<1, 32, 0, s>>>(ictr, h, kChunk, b.forms.lattice_min);
+  k_level_begin<<<1, 32, 0, s>>>(ictr, h, chunk, b.forms.lattice_min);
   CSM_LAUNCH_CHECK();
   CSM_CUDA(cudaMemsetAsync(b.d_scan_cnt->p, 0, sizeof(int) * 2 * total_scans, s));
   ProfBegin(ctx);
@@ -2366,7 +2378,7 @@ csm_status LevelStep2D(Batch2D& b, int h) {
       b.d_jobs->as<JobDev>(), b.d_info->as<ScanInfo>(), b.d_dscan->as<short2>(),              \
       b.d_sorted->as<Node>(), b.d_items->as<WorkItem>(), ictr + kCtlItems, h,                 \
       b.d_lb->as<unsigned>(), next, next_count, kQueueCap, b.d_leaves->as<Node>(),            \
-      ictr + kCtlLeaf, kLeafCap, ictr + kCtlOverflow, b.ctr)
+      ictr + kCtlLeaf, leaf_cap, ictr + kCtlOverflow, b.ctr)
   if (b.forms.unroll <= 4) CSM_LATTICE(4);
   else if (b.forms.unroll <= 8) CSM_LATTICE(8);
   else CSM_LATTICE(16);
@@ -2381,7 +2393,7 @@ csm_status LevelStep2D(Batch2D& b, int h) {
   k_expand<<<kLatticeMin * 32 / 256, 256, 0, s>>>(
       b.d_jobs->as<JobDev>(), b.d_info->as<ScanInfo>(), b.d_dscan->as<short2>(), b.Queue(h),
       ictr, h, b.d_lb->as<unsigned>(), next, next_count, kQueueCap, b.d_leaves->as<Node>(),
-      ictr + kCtlLeaf, kLeafCap, ictr + kCtlOverflow, b.ctr);
+      ictr + kCtlLeaf, leaf_cap, ictr + kCtlOverflow, b.ctr);
   CSM_LAUNCH_CHECK();
   if (g_profile_on.load()) {
     ProfStop(ctx);
@@ -2396,10 +2408,11 @@ csm_status Collect2D(Batch2D& b) {
   cudaStream_t s = b.s;
   int* best_count = b.ictr + kCtlBest;
   char* pin = b.pin->as<char>();
+  const int leaf_cap = b.forms.leaf_cap;
   CSM_CUDA(cudaMemsetAsync(best_count, 0, sizeof(int), s));
   k_compact_leaves<<<b.ctx->sm_count * 4, 256, 0, s>>>(
-      b.d_info->as<ScanInfo>(), b.d_leaves->as<Node>(), b.ictr + kCtlLeaf, kLeafCap,
-      b.d_lb->as<unsigned>(), b.d_best->as<Node>(), best_count, kLeafCap, b.ictr + kCtlOverflow);
+      b.d_info->as<ScanInfo>(), b.d_leaves->as<Node>(), b.ictr + kCtlLeaf, leaf_cap,
+      b.d_lb->as<unsigned>(), b.d_best->as<Node>(), best_count, leaf_cap, b.ictr + kCtlOverflow);
   CSM_LAUNCH_CHECK();
   CSM_CUDA(cudaEventRecord(b.ctx->ev1, s));
   CSM_CUDA(cudaMemcpyAsync(pin, b.ictr, b.rb_ctr, cudaMemcpyDeviceToHost, s));
@@ -2407,10 +2420,13 @@ csm_status Collect2D(Batch2D& b) {
                            cudaMemcpyDeviceToHost, s));
   CSM_CUDA(cudaMemcpyAsync(pin + b.rb_lb, b.d_lb->p, sizeof(unsigned) * b.num_jobs,
                            cudaMemcpyDeviceToHost, s));
-  CSM_CUDA(cudaMemcpyAsync(pin + b.rb_best, b.d_best->p, sizeof(Node) * kInlineBest,
-                           cudaMemcpyDeviceToHost, s));
+  if (b.forms.inline_best > 0)
+    CSM_CUDA(cudaMemcpyAsync(pin + b.rb_best, b.d_best->p, sizeof(Node) * b.forms.inline_best,
+                             cudaMemcpyDeviceToHost, s));
   CSM_CUDA(cudaStreamSynchronize(s));
   ++b.host_syncs;
+  ++b.sweeps;
+  b.max_leaves = std::max(b.max_leaves, b.hp[kCtlLeaf]);
   return CSM_OK;
 }
 
@@ -2429,14 +2445,16 @@ csm_status Sweep2D(Batch2D& b) {
     for (int l = 1; l <= b.hmax; ++l)
       if (b.hp[l] > 0) { h = l; break; }
     if (h < 0) break;
-    if (b.hp[kCtlLeaf] > kLeafCap / 2) {
+    const int leaf_cap = b.forms.leaf_cap;
+    if (b.hp[kCtlLeaf] > leaf_cap / 2) {
       // drop the leaves that are already below their job's bound (d_best holds them
-      // after Collect2D); more than kLeafCap / 2 exactly tied optima are not supported
-      if (b.hp[kCtlBest] > kLeafCap / 2) { SetError("too many tied leaves"); return CSM_E_CAPACITY; }
+      // after Collect2D); more than leaf_cap / 2 exactly tied optima are not supported
+      if (b.hp[kCtlBest] > leaf_cap / 2) { SetError("too many tied leaves"); return CSM_E_CAPACITY; }
       CSM_CUDA(cudaMemcpyAsync(b.d_leaves->p, b.d_best->p, sizeof(Node) * b.hp[kCtlBest],
                                cudaMemcpyDeviceToDevice, b.s));
       CSM_CUDA(cudaMemcpyAsync(b.ictr + kCtlLeaf, b.ictr + kCtlBest, sizeof(int),
                                cudaMemcpyDeviceToDevice, b.s));
+      ++b.compactions;
     }
     CSM_TRY(LevelStep2D(b, h));
     for (int l = h - 1; l >= 1; --l) CSM_TRY(LevelStep2D(b, l));  // its children fit one chunk each
@@ -2612,8 +2630,9 @@ csm_status MatchBatch2D(Batch2D& b, const HostSearch* search, csm_result2d* resu
     SetError("internal: a scan's lowest-resolution lattice exceeds its reserved slots");
     return CSM_E_CAPACITY;
   }
-  std::vector<Node> best(b.best_inline, b.best_inline + std::min(n_best, kInlineBest));
-  if (n_best > kInlineBest) {  // many exactly tied optima
+  b.n_best = n_best;
+  std::vector<Node> best(b.best_inline, b.best_inline + std::min(n_best, b.forms.inline_best));
+  if (n_best > b.forms.inline_best) {  // many exactly tied optima
     best.resize(n_best);
     CSM_CUDA(cudaMemcpyAsync(best.data(), b.d_best->p, sizeof(Node) * n_best,
                              cudaMemcpyDeviceToHost, b.s));
@@ -2688,13 +2707,51 @@ csm_status ReadInfo2D(const Batch2D& b, std::vector<ScanInfo>* info) {
 
 extern "C" {
 
+void csm_sweep_limits2d_default(csm_sweep_limits2d* out) {
+  if (!out) return;
+  static const int lattice_min = getenv("CSM_NO_LATTICE") ? INT_MAX : kLatticeMin;
+  // k_expand_lattice<U> is launched with the smallest U in {4, 8, 16} that is >= the value
+  static const int unroll = [] {
+    const int v = getenv("CSM_LAT_UNROLL") ? atoi(getenv("CSM_LAT_UNROLL")) : 8;
+    return v <= 4 ? 4 : (v <= 8 ? 8 : 16);
+  }();
+  out->chunk = kChunk;
+  out->leaf_cap = kLeafCap;
+  out->inline_best = kInlineBest;
+  out->lattice_min = lattice_min;
+  out->unroll = unroll;
+  out->dive_ratio = kDiveRatio;
+  out->max_points = kMaxPoints;
+}
+
 csm_status csm_match2d_batch(const csm_stack2d* const* stacks, int32_t num_stacks,
                              const csm_cloud* const* clouds, int32_t num_clouds,
                              const csm_job2d* jobs, int32_t num_jobs, double linear_window,
                              double angular_window, csm_result2d* results, csm_stats* total) {
+  return csm_match2d_batch_limits(stacks, num_stacks, clouds, num_clouds, jobs, num_jobs,
+                                  linear_window, angular_window, nullptr, results, total, nullptr);
+}
+
+csm_status csm_match2d_batch_limits(const csm_stack2d* const* stacks, int32_t num_stacks,
+                                    const csm_cloud* const* clouds, int32_t num_clouds,
+                                    const csm_job2d* jobs, int32_t num_jobs, double linear_window,
+                                    double angular_window, const csm_sweep_limits2d* limits,
+                                    csm_result2d* results, csm_stats* total, int32_t trace[4]) {
   CSM_REQUIRE(stacks && clouds && jobs && results, "null pointer");
   CSM_REQUIRE(num_jobs >= 1 && num_stacks >= 1 && num_clouds >= 1, "empty batch");
   CSM_REQUIRE(stacks[0] != nullptr, "null stack");
+  csm_sweep_limits2d lim;
+  csm_sweep_limits2d_default(&lim);
+  if (limits) {
+    lim = *limits;
+    CSM_REQUIRE(lim.chunk >= 1 && lim.chunk <= kChunk, "limits: chunk");
+    CSM_REQUIRE(lim.leaf_cap >= 2 && lim.leaf_cap <= kLeafCap, "limits: leaf_cap");
+    CSM_REQUIRE(lim.inline_best >= 0 && lim.inline_best <= kInlineBest, "limits: inline_best");
+    CSM_REQUIRE(lim.lattice_min >= 1, "limits: lattice_min");
+    CSM_REQUIRE(lim.unroll == 4 || lim.unroll == 8 || lim.unroll == 16, "limits: unroll");
+    CSM_REQUIRE(std::isfinite(lim.dive_ratio) && lim.dive_ratio >= 0.f, "limits: dive_ratio");
+    CSM_REQUIRE(lim.max_points >= 1, "limits: max_points");
+  }
   bool one_depth = true;
   for (int j = 0; j < num_jobs; ++j) {
     const csm_job2d& jb = jobs[j];
@@ -2704,16 +2761,22 @@ csm_status csm_match2d_batch(const csm_stack2d* const* stacks, int32_t num_stack
     one_depth = one_depth &&
                 stacks[jb.stack_index]->h.depth == stacks[jobs[0].stack_index]->h.depth;
   }
-  static const Forms2D env_forms{nullptr, getenv("CSM_NO_LATTICE") ? INT_MAX : kLatticeMin,
-                                 getenv("CSM_LAT_UNROLL") ? atoi(getenv("CSM_LAT_UNROLL")) : 8};
+  Forms2D forms;
+  forms.lattice_min = lim.lattice_min;
+  forms.unroll = lim.unroll;
+  forms.chunk = lim.chunk;
+  forms.leaf_cap = lim.leaf_cap;
+  forms.inline_best = lim.inline_best;
+  forms.dive_ratio = lim.dive_ratio;
+  const long long max_points = lim.max_points;
   LaneGuard guard;
   CSM_TRY(AcquireLane(stacks[0]->ctx->device, &guard));
   Ctx* ctx = guard.lane;
   if (total) std::memset(total, 0, sizeof(*total));
+  if (trace) std::memset(trace, 0, sizeof(int32_t) * 4);
   // Runs jobs[0..n) (one branch_and_bound_depth) in sub-batches whose discrete-scan buffer
-  // stays below ~4 GB.
+  // stays below max_points points.
   auto run = [&](const csm_job2d* js, int n, csm_result2d* rs) -> csm_status {
-    const long long kMaxPoints = 1LL << 30;
     std::vector<HostSearch> search(n);
     for (int j = 0; j < n; ++j)
       search[j] = JobSearch(stacks[js[j].stack_index], clouds[js[j].cloud_index], js[j],
@@ -2725,12 +2788,18 @@ csm_status csm_match2d_batch(const csm_stack2d* const* stacks, int32_t num_stack
       while (j1 < n) {
         const long long add =
             static_cast<long long>(search[j1].num_scans) * clouds[js[j1].cloud_index]->n;
-        if (j1 > j0 && pts + add > kMaxPoints) break;
+        if (j1 > j0 && pts + add > max_points) break;
         pts += add;
         ++j1;
       }
-      Batch2D b(ctx, stacks, clouds, js + j0, j1 - j0, env_forms);
+      Batch2D b(ctx, stacks, clouds, js + j0, j1 - j0, forms);
       CSM_TRY(MatchBatch2D(b, search.data() + j0, rs + j0, total));
+      if (trace) {
+        trace[0] += b.sweeps;
+        trace[1] += b.compactions;
+        trace[2] = std::max(trace[2], b.max_leaves);
+        trace[3] += b.n_best;
+      }
       j0 = j1;
     }
     return CSM_OK;
@@ -2926,6 +2995,66 @@ csm_status csm_branch_step2d(const csm_stack2d* stack, const float* xyz, int32_t
   *final_bound = OrderedToFloat(lb_out);
   counters[0] = static_cast<int64_t>(c[0]);
   counters[1] = static_cast<int64_t>(c[1]);
+  return CSM_OK;
+}
+
+csm_status csm_dives2d(const csm_stack2d* stack, const float* xyz, int32_t n,
+                       const double initial_pose[3], int32_t full_submap, double linear_window,
+                       double angular_window, float min_score, float dive_ratio,
+                       int32_t* job_best, float bounds[2], int64_t counters[2],
+                       csm_node2d* top_queue, int32_t top_capacity, int32_t* top_count) {
+  static_assert(sizeof(csm_node2d) == sizeof(Node), "csm_node2d is Node");
+  CSM_REQUIRE(job_best && bounds && counters && top_count, "null pointer");
+  CSM_REQUIRE(top_capacity >= 0, "top_capacity");
+  CSM_REQUIRE(top_queue || top_capacity == 0, "null top_queue");
+  CSM_REQUIRE(std::isfinite(dive_ratio) && dive_ratio >= 0.f, "dive_ratio");
+  CSM_REQUIRE(full_submap || initial_pose, "null initial pose");
+  Hook2D hk;
+  CSM_TRY(MakeHook2D(hk, stack, xyz, n, initial_pose, full_submap, linear_window, angular_window,
+                     min_score));
+  Forms2D forms;
+  forms.dive_ratio = dive_ratio;
+  CSM_TRY(PlanHook2D(hk, forms));
+  Batch2D& b = hk.b;
+  cudaStream_t s = b.s;
+  // the batch's own launches up to the level loop
+  CSM_TRY(Upload2D(b));
+  CSM_TRY(TopPass2D(b));
+  CSM_TRY(Dives2D(b));
+  unsigned lb_dives = 0;
+  CSM_CUDA(cudaMemcpyAsync(&lb_dives, b.d_lb->p, sizeof(unsigned), cudaMemcpyDeviceToHost, s));
+  CSM_CUDA(cudaStreamSynchronize(s));
+  CSM_TRY(PrepareLevels2D(b));
+  CSM_TRY(FilterTop2D(b));
+  int ctl[kCtlInts];
+  unsigned long long c[8];
+  unsigned lb_top = 0;
+  int jb = 0;
+  CSM_CUDA(cudaMemcpyAsync(ctl, b.ictr, sizeof(ctl), cudaMemcpyDeviceToHost, s));
+  CSM_CUDA(cudaMemcpyAsync(c, b.ctr, sizeof(c), cudaMemcpyDeviceToHost, s));
+  CSM_CUDA(cudaMemcpyAsync(&lb_top, b.d_lb->p, sizeof(unsigned), cudaMemcpyDeviceToHost, s));
+  CSM_CUDA(cudaMemcpyAsync(&jb, b.d_job_best->p, sizeof(int), cudaMemcpyDeviceToHost, s));
+  CSM_CUDA(cudaStreamSynchronize(s));
+  if (c[6] || c[7]) {
+    SetError("a scan's lattice or cell indices exceed the engine's limits");
+    return CSM_E_CAPACITY;
+  }
+  if (ctl[kCtlOverflow]) {
+    SetError("top queue or leaf list overflow");
+    return CSM_E_CAPACITY;
+  }
+  // depth 1: the queue's candidates are the leaves, in queue order
+  const int count = ctl[b.hmax];
+  const Node* src = b.hmax == 0 ? b.d_leaves->as<Node>() : b.Queue(b.hmax);
+  const int copy = std::min(count, top_capacity);
+  if (copy > 0)
+    CSM_CUDA(cudaMemcpy(top_queue, src, sizeof(Node) * copy, cudaMemcpyDeviceToHost));
+  *job_best = jb;
+  bounds[0] = OrderedToFloat(lb_dives);
+  bounds[1] = OrderedToFloat(lb_top);
+  counters[0] = static_cast<int64_t>(c[0] - c[3]);  // the top pass scores every slot once
+  counters[1] = static_cast<int64_t>(c[2]);
+  *top_count = count;
   return CSM_OK;
 }
 

@@ -216,6 +216,43 @@ class FastCorrelativeScanMatcher2D:
             ptr(ctr, C.c_int64)))
         return out[:count.value].copy(), np.float32(final.value), (int(ctr[0]), int(ctr[1]))
 
+    def dives(self, point_cloud, initial_pose_estimate, full_submap, min_score, dive_ratio):
+        """csm_dives2d: the match's greedy dives and top-queue filter.
+        -> (job_best, (bound after the dives, bound after the filter),
+            (candidates the dives scored, dives run), top queue in queue order)."""
+        xyz = _f32(point_cloud)
+        ip = np.ascontiguousarray(initial_pose_estimate, dtype=np.float64)
+        job_best, count = C.c_int32(0), C.c_int32(0)
+        bounds = np.zeros(2, np.float32)
+        ctr = np.zeros(2, np.int64)
+        out = np.zeros(4096, NODE2D_DTYPE)
+        while True:
+            check(lib().csm_dives2d(
+                self._h, ptr(xyz, C.c_float), C.c_int32(len(xyz)), ptr(ip, C.c_double),
+                C.c_int32(int(full_submap)), C.c_double(self.options.linear_search_window),
+                C.c_double(self.options.angular_search_window), C.c_float(min_score),
+                C.c_float(dive_ratio), C.byref(job_best), ptr(bounds, C.c_float),
+                ptr(ctr, C.c_int64), out.ctypes.data_as(C.c_void_p), C.c_int32(len(out)),
+                C.byref(count)))
+            if count.value <= len(out):
+                break
+            out = np.zeros(count.value, NODE2D_DTYPE)
+        return (int(job_best.value), (bounds[0], bounds[1]), (int(ctr[0]), int(ctr[1])),
+                out[:count.value].copy())
+
+
+class SweepLimits2D(C.Structure):
+    """csm_sweep_limits2d: limits of the batched 2D branch-and-bound sweep."""
+    _fields_ = [("chunk", C.c_int32), ("leaf_cap", C.c_int32), ("inline_best", C.c_int32),
+                ("lattice_min", C.c_int32), ("unroll", C.c_int32), ("dive_ratio", C.c_float),
+                ("max_points", C.c_int64)]
+
+    @classmethod
+    def default(cls):
+        out = cls()
+        lib().csm_sweep_limits2d_default(C.byref(out))
+        return out
+
 
 def load_pbstream_matchers2d(path, options, device=0):
     """csm_pbstream_load_stacks2d: one FastCorrelativeScanMatcher2D per 2D submap of a
@@ -235,23 +272,35 @@ def load_pbstream_matchers2d(path, options, device=0):
     return matchers, [(int(a), int(b)) for a, b in ids[:count]]
 
 
-def match_batch(matchers, clouds, jobs, linear_search_window, angular_search_window):
-    """Batched FastCorrelativeScanMatcher2D searches (csm_match2d_batch).
+def match_batch(matchers, clouds, jobs, linear_search_window, angular_search_window,
+                limits=None):
+    """Batched FastCorrelativeScanMatcher2D searches (csm_match2d_batch_limits).
 
     matchers: list of FastCorrelativeScanMatcher2D; clouds: list of DeviceCloud;
-    jobs: numpy array of JOB2D_DTYPE.  Returns (results[RESULT2D_DTYPE], stats dict).
+    jobs: numpy array of JOB2D_DTYPE; limits: None (the defaults), a SweepLimits2D, or a
+    dict of SweepLimits2D fields that override the defaults.  Returns
+    (results[RESULT2D_DTYPE], stats dict); stats["sweep_trace"] is (collects, leaf
+    compactions, most leaves held at a collect, optimal leaves).
     """
     jobs = np.ascontiguousarray(jobs, dtype=JOB2D_DTYPE)
     hs = (C.c_void_p * len(matchers))(*[m._h for m in matchers])
     cs = (C.c_void_p * len(clouds))(*[c._h for c in clouds])
     results = np.zeros(len(jobs), RESULT2D_DTYPE)
     stats = CsmStats()
-    check(lib().csm_match2d_batch(hs, C.c_int32(len(matchers)), cs, C.c_int32(len(clouds)),
-                                  jobs.ctypes.data_as(C.c_void_p), C.c_int32(len(jobs)),
-                                  C.c_double(linear_search_window),
-                                  C.c_double(angular_search_window),
-                                  results.ctypes.data_as(C.c_void_p), C.byref(stats)))
-    return results, stats.as_dict()
+    if isinstance(limits, dict):
+        lim = SweepLimits2D.default()
+        for k, v in limits.items():
+            setattr(lim, k, v)
+        limits = lim
+    trace = np.zeros(4, np.int32)
+    check(lib().csm_match2d_batch_limits(
+        hs, C.c_int32(len(matchers)), cs, C.c_int32(len(clouds)),
+        jobs.ctypes.data_as(C.c_void_p), C.c_int32(len(jobs)), C.c_double(linear_search_window),
+        C.c_double(angular_search_window), C.byref(limits) if limits is not None else None,
+        results.ctypes.data_as(C.c_void_p), C.byref(stats), ptr(trace, C.c_int32)))
+    out = stats.as_dict()
+    out["sweep_trace"] = tuple(int(v) for v in trace)
+    return results, out
 
 
 class RealTimeCorrelativeScanMatcher2D:

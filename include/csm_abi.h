@@ -176,6 +176,30 @@ csm_status csm_match2d_batch(const csm_stack2d* const* stacks, int32_t num_stack
                              double linear_search_window, double angular_search_window,
                              csm_result2d* results, csm_stats* total /* may be NULL */);
 
+/* Limits of the batched 2D branch-and-bound sweep.  csm_sweep_limits2d_default gives the
+ * values csm_match2d_batch runs with (lattice_min and unroll follow CSM_NO_LATTICE and
+ * CSM_LAT_UNROLL).  Smaller limits change only the control flow: every buffer keeps its
+ * default size, and a limit too small for a search ends in CSM_E_CAPACITY. */
+typedef struct csm_sweep_limits2d {
+  int32_t chunk;        /* nodes per level chunk, 1 .. 1 << 23 */
+  int32_t leaf_cap;     /* leaf buffer capacity, 2 .. 1 << 22 */
+  int32_t inline_best;  /* optimal leaves read back with the first sync, 0 .. 4096 */
+  int32_t lattice_min;  /* smallest chunk k_expand_lattice takes; INT32_MAX = never */
+  int32_t unroll;       /* 4 | 8 | 16 */
+  float dive_ratio;     /* >= 0, finite; > 1 disables the dives */
+  int64_t max_points;   /* discrete-scan points per sub-batch, >= 1 */
+} csm_sweep_limits2d;
+void csm_sweep_limits2d_default(csm_sweep_limits2d* out);
+/* csm_match2d_batch under `limits` (NULL: the defaults).  trace (may be NULL) receives
+ * {collects, i.e. 1 + continuation sweeps, summed over sub-batches; leaf compactions between
+ * sweeps, summed; most leaves held at any collect; optimal leaves, summed}. */
+csm_status csm_match2d_batch_limits(const csm_stack2d* const* stacks, int32_t num_stacks,
+                                    const csm_cloud* const* clouds, int32_t num_clouds,
+                                    const csm_job2d* jobs, int32_t num_jobs,
+                                    double linear_search_window, double angular_search_window,
+                                    const csm_sweep_limits2d* limits, csm_result2d* results,
+                                    csm_stats* total /* may be NULL */, int32_t trace[4]);
+
 /* ---- test hooks ("visible for testing" in the reference) ------------------ */
 /* FastCorrelativeScanMatcher2D::ScoreCandidates (fast...2d.cc:314-333) without
  * the sort: candidates are {scan_index, x_index_offset, y_index_offset} triples,
@@ -227,6 +251,19 @@ csm_status csm_branch_step2d(const csm_stack2d* stack, const float* xyz, int32_t
                              int32_t num_parents, float bound, int32_t form, int32_t unroll,
                              csm_node2d* children, int32_t* num_children, float* final_bound,
                              int64_t counters[2]);
+/* The same match's phases between the lowest-resolution pass and the level loop, run by
+ * the batch's own launch code with k_dive's gate at `dive_ratio`: job_best is the largest
+ * lowest-resolution sum; bounds = {the job's bound after the dives, after the top-queue
+ * filter} (they differ only at depth 1, where every queued candidate is a leaf);
+ * counters = {candidates the dives scored, dives run}.  top_queue receives the first
+ * top_capacity records of the top queue in queue order (at depth 1, of the leaves, which
+ * are the queue's copy) and *top_count the queue's length. */
+csm_status csm_dives2d(const csm_stack2d* stack, const float* xyz, int32_t num_points,
+                       const double initial_pose[3], int32_t full_submap,
+                       double linear_search_window, double angular_search_window,
+                       float min_score, float dive_ratio, int32_t* job_best, float bounds[2],
+                       int64_t counters[2], csm_node2d* top_queue, int32_t top_capacity,
+                       int32_t* top_count);
 
 /* ---- RealTimeCorrelativeScanMatcher2D::Match ------------------------------ */
 /* real_time_correlative_scan_matcher_2d.cc:117-149 on a ProbabilityGrid (the
