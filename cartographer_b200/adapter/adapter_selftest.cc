@@ -20,7 +20,7 @@ static unsigned Bits(float f) {
   return u;
 }
 
-// Host-only part (runs everywhere): the builder's gating and WhenDone cycle when no
+// Host-only part (runs everywhere): the builders' gating and WhenDone cycle when no
 // pair survives the gates — nothing reaches the device — and the sampler's sequence
 // (common/fixed_ratio_sampler_test.cc).
 // A serialised grid (DeviceHybridGrid / DeviceGrid2D::ToProto, the bytes in this stand-in
@@ -54,6 +54,19 @@ static int HostOnlyChecks() {
   size_t constraints = 99;
   builder.WhenDone([&](const ConstraintBuilder2D::Result& r) { ++calls; constraints = r.size(); });
   if (calls != 1 || constraints != 0 || builder.GetNumFinishedNodes() != 1) return 1;
+  // the same cycle through ConstraintBuilder3D
+  using mapping::constraints::ConstraintBuilder3D;
+  ConstraintBuilder3D builder3d(bo, &pool);
+  const mapping::Submap3D submap3d(nullptr, nullptr, nullptr);  // never read: the pair is gated
+  builder3d.MaybeAddConstraint(mapping::SubmapId{0, 0}, &submap3d, mapping::NodeId{0, 0}, &node,
+                               transform::Rigid3d({{5., 0., 0.}},  // beyond max_constraint_distance
+                                                  transform::Quaterniond{1., 0., 0., 0.}),
+                               transform::Rigid3d());
+  builder3d.NotifyEndOfNode();
+  calls = 0;
+  constraints = 99;
+  builder3d.WhenDone([&](const ConstraintBuilder3D::Result& r) { ++calls; constraints = r.size(); });
+  if (calls != 1 || constraints != 0 || builder3d.GetNumFinishedNodes() != 1) return 1;
   // Rigid2d algebra used for the constraint transform
   const transform::Rigid2d a({1., 2.}, 0.3);
   const transform::Rigid2d id = a.inverse() * a;

@@ -59,10 +59,122 @@ struct DeviceSubmap2D {
   transform::Rigid2d local_pose_2d;          // ComputeSubmapPose(submap)
 };
 
-class ConstraintBuilder2D {
+namespace b200_internal {
+// What ConstraintBuilder2D and ConstraintBuilder3D share (constraint_builder_2d.cc:68-75,
+// 139-163, 279-316): the queue of pairs, the per-submap FixedRatioSamplers and matchers, the
+// node counters and the WhenDone cycle.  A builder gates a pair with Sample, queues it with Push
+// and turns the whole queue into constraints in Match, which runs on the pool thread under the
+// mutex; the callback runs after it, outside the lock.
+template <typename Pending, typename SubmapMatcher>
+class ConstraintQueue {
  public:
   using Constraint = PoseGraphInterface::Constraint;
   using Result = std::vector<Constraint>;
+
+  virtual ~ConstraintQueue() {
+    std::lock_guard<std::mutex> lock(mutex_);
+    Require(pending_.empty(), "WhenDone() was not called");
+    Require(num_started_nodes_ == num_finished_nodes_, "unfinished nodes");
+    Require(when_done_ == nullptr, "callback still pending");
+  }
+  ConstraintQueue(const ConstraintQueue&) = delete;
+  ConstraintQueue& operator=(const ConstraintQueue&) = delete;
+
+  void NotifyEndOfNode() {  // :139-151
+    std::lock_guard<std::mutex> lock(mutex_);
+    ++num_started_nodes_;
+  }
+
+  // :153-163; `callback` runs in the thread pool after the queue has been drained.
+  void WhenDone(const std::function<void(const Result&)>& callback) {
+    {
+      std::lock_guard<std::mutex> lock(mutex_);
+      Require(when_done_ == nullptr, "WhenDone called twice");
+      when_done_.reset(new std::function<void(const Result&)>(callback));
+    }
+    std::unique_ptr<common::Task> task(new common::Task);
+    task->SetWorkItem([this] { Drain(); });
+    thread_pool_->Schedule(std::move(task));
+  }
+
+  int GetNumFinishedNodes() {
+    std::lock_guard<std::mutex> lock(mutex_);
+    return num_finished_nodes_;
+  }
+
+  void DeleteScanMatcher(const SubmapId& submap_id) {  // :307-316
+    std::lock_guard<std::mutex> lock(mutex_);
+    matchers_.erase(submap_id);
+    samplers_.erase(submap_id);
+  }
+
+ protected:
+  ConstraintQueue(common::ThreadPoolInterface* thread_pool, double sampling_ratio)
+      : thread_pool_(thread_pool), sampling_ratio_(sampling_ratio) {}
+
+  // The per-submap FixedRatioSampler of a pair that passed the distance gate (:85-90).
+  bool Sample(const SubmapId& submap_id) {
+    std::lock_guard<std::mutex> lock(mutex_);
+    return samplers_
+        .emplace(std::piecewise_construct, std::forward_as_tuple(submap_id),
+                 std::forward_as_tuple(sampling_ratio_))
+        .first->second.Pulse();
+  }
+  void Push(const Pending& pending) {
+    std::lock_guard<std::mutex> lock(mutex_);
+    pending_.push_back(pending);
+  }
+  // The constraints of the queued pairs, in queue order.
+  virtual Result Match(const std::deque<Pending>& pending) = 0;
+
+  std::map<SubmapId, SubmapMatcher> matchers_;   // DispatchScanMatcherConstruction (:165-186)
+
+ private:
+  void Drain() {
+    Result result;
+    std::unique_ptr<std::function<void(const Result&)>> callback;
+    {
+      std::lock_guard<std::mutex> lock(mutex_);
+      Require(when_done_ != nullptr, "no callback");
+      result = Match(pending_);
+      pending_.clear();
+      num_finished_nodes_ = num_started_nodes_;
+      callback = std::move(when_done_);
+    }
+    (*callback)(result);
+  }
+
+  common::ThreadPoolInterface* const thread_pool_;
+  const double sampling_ratio_;
+  std::mutex mutex_;
+  std::unique_ptr<std::function<void(const Result&)>> when_done_;
+  int num_started_nodes_ = 0;
+  int num_finished_nodes_ = 0;
+  std::deque<Pending> pending_;
+  std::map<SubmapId, common::FixedRatioSampler> samplers_;
+};
+
+struct Pending2D {
+  SubmapId submap_id;
+  const Submap2D* submap;                 // one of the two is set
+  const DeviceSubmap2D* device_submap;
+  NodeId node_id;
+  const TrajectoryNodeData* constant_data;
+  transform::Rigid2d initial_pose;
+  bool full;
+  float min_score;
+};
+struct SubmapMatcher2D {
+  std::unique_ptr<scan_matching::FastCorrelativeScanMatcher2D> matcher;
+  // the refinement's upload of a host submap's grid; a device submap's is its own
+  std::unique_ptr<scan_matching::DeviceGrid2D> device_grid;
+};
+}  // namespace b200_internal
+
+class ConstraintBuilder2D
+    : public b200_internal::ConstraintQueue<b200_internal::Pending2D,
+                                            b200_internal::SubmapMatcher2D> {
+ public:
   // (pose_estimate, point cloud, grid) -> refined pose; identity when unset.
   using Refiner = std::function<transform::Rigid2d(
       const transform::Rigid2d&, const sensor::PointCloud&, const Grid2D&)>;
@@ -74,20 +186,13 @@ class ConstraintBuilder2D {
   ConstraintBuilder2D(const proto::ConstraintBuilderOptions& options,
                       common::ThreadPoolInterface* thread_pool, int device = 0,
                       csm_ctx* multi_gpu = nullptr)
-      : options_(options), thread_pool_(thread_pool), device_(device), ctx_(multi_gpu) {
+      : ConstraintQueue(thread_pool, options.sampling_ratio()),
+        options_(options),
+        device_(device),
+        ctx_(multi_gpu) {
     if (ctx_ != nullptr)
       scan_matching::b200_internal::Check(csm_ctx_info(ctx_, &world_, &rank_, nullptr));
   }
-
-  ~ConstraintBuilder2D() {  // constraint_builder_2d.cc:68-75
-    std::lock_guard<std::mutex> lock(mutex_);
-    b200_internal::Require(pending_.empty(), "WhenDone() was not called");
-    b200_internal::Require(num_started_nodes_ == num_finished_nodes_, "unfinished nodes");
-    b200_internal::Require(when_done_ == nullptr, "callback still pending");
-    for (auto& kv : stacks_) csm_stack2d_destroy(kv.second.stack);
-  }
-  ConstraintBuilder2D(const ConstraintBuilder2D&) = delete;
-  ConstraintBuilder2D& operator=(const ConstraintBuilder2D&) = delete;
 
   void set_refiner(const Refiner& refiner) { refiner_ = refiner; }
   // constraint_builder_2d.cc:245-249 on the device.  Single-GPU builders only: with a
@@ -125,58 +230,11 @@ class ConstraintBuilder2D {
     AddGlobal(submap_id, nullptr, submap, node_id, constant_data);
   }
 
-  void NotifyEndOfNode() {  // :139-151
-    std::lock_guard<std::mutex> lock(mutex_);
-    ++num_started_nodes_;
-  }
-
-  // :153-163; `callback` runs in the thread pool after the queue has been drained.
-  void WhenDone(const std::function<void(const Result&)>& callback) {
-    {
-      std::lock_guard<std::mutex> lock(mutex_);
-      b200_internal::Require(when_done_ == nullptr, "WhenDone called twice");
-      when_done_.reset(new std::function<void(const Result&)>(callback));
-    }
-    std::unique_ptr<common::Task> task(new common::Task);
-    task->SetWorkItem([this] { Drain(); });
-    thread_pool_->Schedule(std::move(task));
-  }
-
-  int GetNumFinishedNodes() {
-    std::lock_guard<std::mutex> lock(mutex_);
-    return num_finished_nodes_;
-  }
-
-  void DeleteScanMatcher(const SubmapId& submap_id) {  // :307-316
-    std::lock_guard<std::mutex> lock(mutex_);
-    auto it = stacks_.find(submap_id);
-    if (it != stacks_.end()) {
-      csm_stack2d_destroy(it->second.stack);
-      stacks_.erase(it);
-    }
-    per_submap_sampler_.erase(submap_id);
-  }
-
   // device counters of the last drained queue
   const csm_stats& last_stats() const { return last_stats_; }
 
  private:
-  struct Pending {
-    SubmapId submap_id;
-    const Submap2D* submap;                 // one of the two is set
-    const DeviceSubmap2D* device_submap;
-    NodeId node_id;
-    const TrajectoryNodeData* constant_data;
-    transform::Rigid2d initial_pose;
-    bool full;
-    float min_score;
-  };
-  struct SubmapStack {
-    const Grid2D* grid = nullptr;
-    csm_stack2d* stack = nullptr;
-    // the refinement's upload of a host submap's grid; a device submap's is its own
-    std::unique_ptr<scan_matching::DeviceGrid2D> device_grid;
-  };
+  using Pending = b200_internal::Pending2D;
 
   // Refusals for a device submap, before anything is queued: its handle exists only in this
   // process and on the device it was made on, and only a ProbabilityGrid has a stack.
@@ -201,188 +259,160 @@ class ConstraintBuilder2D {
                 const TrajectoryNodeData* constant_data,
                 const transform::Rigid2d& initial_relative_pose) {
     if (initial_relative_pose.translation().norm() > options_.max_constraint_distance()) return;
-    if (!per_submap_sampler_
-             .emplace(std::piecewise_construct, std::forward_as_tuple(submap_id),
-                      std::forward_as_tuple(options_.sampling_ratio()))
-             .first->second.Pulse()) {
-      return;
-    }
-    std::lock_guard<std::mutex> lock(mutex_);
+    if (!Sample(submap_id)) return;
     // initial_pose = ComputeSubmapPose(*submap) * initial_relative_pose (:196-197)
-    Push(submap_id, submap, device_submap, node_id, constant_data,
-         LocalPose(submap, device_submap) * initial_relative_pose, false,
-         static_cast<float>(options_.min_score()));
+    Queue(Pending{submap_id, submap, device_submap, node_id, constant_data,
+                  LocalPose(submap, device_submap) * initial_relative_pose, false,
+                  static_cast<float>(options_.min_score())});
   }
 
   void AddGlobal(const SubmapId& submap_id, const Submap2D* submap,
                  const DeviceSubmap2D* device_submap, const NodeId& node_id,
                  const TrajectoryNodeData* constant_data) {
-    std::lock_guard<std::mutex> lock(mutex_);
-    Push(submap_id, submap, device_submap, node_id, constant_data,
-         transform::Rigid2d::Identity(), true,
-         static_cast<float>(options_.global_localization_min_score()));
+    Queue(Pending{submap_id, submap, device_submap, node_id, constant_data,
+                  transform::Rigid2d::Identity(), true,
+                  static_cast<float>(options_.global_localization_min_score())});
   }
 
-  void Push(const SubmapId& submap_id, const Submap2D* submap,
-            const DeviceSubmap2D* device_submap, const NodeId& node_id,
-            const TrajectoryNodeData* constant_data, const transform::Rigid2d& initial_pose,
-            bool full, float min_score) {
-    if (device_submap == nullptr)
-      b200_internal::Require(submap != nullptr && submap->grid() != nullptr, "grid");  // :167
-    pending_.push_back(Pending{submap_id, submap, device_submap, node_id, constant_data,
-                               initial_pose, full, min_score});
+  void Queue(const Pending& p) {
+    if (p.device_submap == nullptr)
+      b200_internal::Require(p.submap != nullptr && p.submap->grid() != nullptr, "grid");  // :167
+    Push(p);
   }
 
-  // DispatchScanMatcherConstruction (:165-186): one device stack per submap, built once; a
-  // device submap's from its grid, device to device.
-  csm_stack2d* StackFor(const Pending& p) {
-    SubmapStack& entry = stacks_[p.submap_id];
+  // One matcher per submap, built once; a device submap's from its grid, device to device.
+  const csm_stack2d* StackFor(const Pending& p) {
+    std::unique_ptr<scan_matching::FastCorrelativeScanMatcher2D>& m =
+        matchers_[p.submap_id].matcher;
     const auto& fo = options_.fast_correlative_scan_matcher_options();
-    if (entry.stack == nullptr && p.device_submap != nullptr) {
-      scan_matching::b200_internal::Check(csm_stack2d_create_from_rt_grid2d(
-          p.device_submap->grid->handle(), fo.branch_and_bound_depth(), &entry.stack));
-    } else if (entry.stack == nullptr) {
-      const Grid2D* grid = p.submap->grid();
-      const MapLimits& l = grid->limits();
-      scan_matching::b200_internal::Check(csm_stack2d_create(
-          grid->correspondence_cost_cells().data(), l.cell_limits().num_x_cells,
-          l.cell_limits().num_y_cells, l.resolution(), l.max().x(), l.max().y(),
-          grid->GetMinCorrespondenceCost(), grid->GetMaxCorrespondenceCost(),
-          fo.branch_and_bound_depth(), device_, &entry.stack));
-      entry.grid = grid;
-    }
-    return entry.stack;
+    if (m == nullptr && p.device_submap != nullptr)
+      m.reset(new scan_matching::FastCorrelativeScanMatcher2D(*p.device_submap->grid, fo));
+    else if (m == nullptr)
+      m.reset(new scan_matching::FastCorrelativeScanMatcher2D(*p.submap->grid(), fo, device_));
+    return m->stack();
   }
 
-  void Drain() {
-    Result result;
-    std::unique_ptr<std::function<void(const Result&)>> callback;
-    {
-      std::lock_guard<std::mutex> lock(mutex_);
-      b200_internal::Require(when_done_ != nullptr, "no callback");
-      if (refiner_) {   // Refiner takes a host Grid2D, which a device submap does not have
-        for (const Pending& p : pending_)
-          b200_internal::Require(p.device_submap == nullptr,
-                                 "set_refiner cannot refine on a device submap");
-      }
-      const auto& fo = options_.fast_correlative_scan_matcher_options();
-      // distinct stacks / clouds of this queue
-      std::vector<const csm_stack2d*> stacks;
-      std::vector<int32_t> owners;
-      std::map<SubmapId, int> stack_index;
-      std::vector<csm_cloud*> clouds;
-      std::map<const TrajectoryNodeData*, int> cloud_index;
-      std::vector<csm_job2d> jobs(pending_.size());
-      for (size_t i = 0; i < pending_.size(); ++i) {
-        const Pending& p = pending_[i];
-        auto si = stack_index.find(p.submap_id);
-        if (si == stack_index.end()) {
-          si = stack_index.emplace(p.submap_id, static_cast<int>(stacks.size())).first;
-          const int owner = OwnerOf(p.submap_id);
-          owners.push_back(owner);
-          stacks.push_back(owner == rank_ ? StackFor(p) : nullptr);
-        }
-        auto ci = cloud_index.find(p.constant_data);
-        if (ci == cloud_index.end()) {
-          const sensor::PointCloud& pc = p.constant_data->filtered_gravity_aligned_point_cloud;
-          const std::vector<float> xyz = scan_matching::b200_internal::Flatten(pc);
-          csm_cloud* cloud = nullptr;
-          scan_matching::b200_internal::Check(
-              csm_cloud_create(xyz.data(), static_cast<int32_t>(pc.size()), device_, &cloud));
-          ci = cloud_index.emplace(p.constant_data, static_cast<int>(clouds.size())).first;
-          clouds.push_back(cloud);
-        }
-        csm_job2d& j = jobs[i];
-        j = csm_job2d{};
-        j.stack_index = si->second;
-        j.cloud_index = ci->second;
-        j.full_submap = p.full ? 1 : 0;
-        j.initial_pose[0] = p.initial_pose.translation().x();
-        j.initial_pose[1] = p.initial_pose.translation().y();
-        j.initial_pose[2] = p.initial_pose.rotation().angle();
-        j.min_score = p.min_score;
-      }
-      std::vector<csm_result2d> results(jobs.size());
-      if (!jobs.empty()) {
-        const auto run = [&](const csm_job2d* js, int32_t n, csm_result2d* rs) {
-          const csm_cloud* const* cl = const_cast<const csm_cloud* const*>(clouds.data());
-          if (ctx_ != nullptr)
-            return csm_cb_batch2d_run(ctx_, stacks.data(), static_cast<int32_t>(stacks.size()), cl,
-                                      static_cast<int32_t>(clouds.size()), js, n, owners.data(),
-                                      fo.linear_search_window(), fo.angular_search_window(), rs,
-                                      &last_stats_);
-          return csm_match2d_batch(stacks.data(), static_cast<int32_t>(stacks.size()), cl,
-                                   static_cast<int32_t>(clouds.size()), js, n,
-                                   fo.linear_search_window(), fo.angular_search_window(), rs,
-                                   &last_stats_);
-        };
-        if (!scan_matching::b200_internal::Check(
-                run(jobs.data(), static_cast<int32_t>(jobs.size()), results.data()))) {
-          // An engine capacity limit was hit somewhere in the batch: run the pairs one by
-          // one; a pair that still exceeds it yields no constraint (the reference would
-          // have produced a match or none — it never aborts here).
-          for (size_t i = 0; i < jobs.size(); ++i) {
-            results[i] = csm_result2d{};
-            if (!scan_matching::b200_internal::Check(run(&jobs[i], 1, &results[i])))
-              results[i].found = 0;
-          }
-        }
-      }
-      for (csm_cloud* c : clouds) csm_cloud_destroy(c);
-      // ceres_scan_matcher_.Match(pose_estimate.translation(), pose_estimate, cloud, grid,
-      // &pose_estimate, ...) for every found match (:245-249), one launch for the queue
-      std::vector<transform::Rigid2d> refined;
-      std::vector<size_t> refined_of(pending_.size(), 0);
-      if (device_refinement_) {
-        std::vector<scan_matching::CeresScanMatcher2D::Job> rjobs;
-        for (size_t i = 0; i < pending_.size(); ++i) {
-          if (!results[i].found) continue;
-          const Pending& p = pending_[i];
-          const scan_matching::DeviceGrid2D* grid = nullptr;
-          if (p.device_submap != nullptr) {   // the submap's own grid
-            grid = p.device_submap->grid;
-          } else {
-            SubmapStack& entry = stacks_[p.submap_id];
-            if (entry.device_grid == nullptr)
-              entry.device_grid.reset(new scan_matching::DeviceGrid2D(*p.submap->grid(), device_));
-            grid = entry.device_grid.get();
-          }
-          refined_of[i] = rjobs.size();
-          rjobs.push_back(scan_matching::CeresScanMatcher2D::Job{
-              {results[i].pose_estimate[0], results[i].pose_estimate[1]},
-              transform::Rigid2d({results[i].pose_estimate[0], results[i].pose_estimate[1]},
-                                 results[i].pose_estimate[2]),
-              &p.constant_data->filtered_gravity_aligned_point_cloud, grid});
-        }
-        scan_matching::CeresScanMatcher2D(options_.ceres_scan_matcher_options(), device_)
-            .MatchBatch(rjobs, &refined, nullptr);
-      }
-      for (size_t i = 0; i < pending_.size(); ++i) {
-        if (!results[i].found) continue;  // below min_score: no constraint (:253-261)
-        const Pending& p = pending_[i];
-        transform::Rigid2d pose_estimate({results[i].pose_estimate[0], results[i].pose_estimate[1]},
-                                         results[i].pose_estimate[2]);
-        if (device_refinement_) pose_estimate = refined[refined_of[i]];
-        if (refiner_)
-          pose_estimate = refiner_(pose_estimate,
-                                   p.constant_data->filtered_gravity_aligned_point_cloud,
-                                   *p.submap->grid());
-        // constraint_transform = ComputeSubmapPose(*submap).inverse() * pose_estimate (:251-252)
-        const transform::Rigid2d constraint_transform =
-            LocalPose(p.submap, p.device_submap).inverse() * pose_estimate;
-        result.push_back(Constraint{p.submap_id,
-                                    p.node_id,
-                                    {b200_internal::Embed3D(constraint_transform),
-                                     options_.loop_closure_translation_weight(),
-                                     options_.loop_closure_rotation_weight()},
-                                    Constraint::INTER_SUBMAP});
-      }
-      pending_.clear();
-      num_finished_nodes_ = num_started_nodes_;
-      callback = std::move(when_done_);
-      when_done_.reset();
+  Result Match(const std::deque<Pending>& pending) override {
+    if (refiner_) {   // Refiner takes a host Grid2D, which a device submap does not have
+      for (const Pending& p : pending)
+        b200_internal::Require(p.device_submap == nullptr,
+                               "set_refiner cannot refine on a device submap");
     }
-    (*callback)(result);
+    const auto& fo = options_.fast_correlative_scan_matcher_options();
+    // distinct stacks / clouds of this queue
+    std::vector<const csm_stack2d*> stacks;
+    std::vector<int32_t> owners;
+    std::map<SubmapId, int> stack_index;
+    std::vector<csm_cloud*> clouds;
+    std::map<const TrajectoryNodeData*, int> cloud_index;
+    std::vector<csm_job2d> jobs(pending.size());
+    for (size_t i = 0; i < pending.size(); ++i) {
+      const Pending& p = pending[i];
+      auto si = stack_index.find(p.submap_id);
+      if (si == stack_index.end()) {
+        si = stack_index.emplace(p.submap_id, static_cast<int>(stacks.size())).first;
+        const int owner = OwnerOf(p.submap_id);
+        owners.push_back(owner);
+        stacks.push_back(owner == rank_ ? StackFor(p) : nullptr);
+      }
+      auto ci = cloud_index.find(p.constant_data);
+      if (ci == cloud_index.end()) {
+        const sensor::PointCloud& pc = p.constant_data->filtered_gravity_aligned_point_cloud;
+        const std::vector<float> xyz = scan_matching::b200_internal::Flatten(pc);
+        csm_cloud* cloud = nullptr;
+        scan_matching::b200_internal::Check(
+            csm_cloud_create(xyz.data(), static_cast<int32_t>(pc.size()), device_, &cloud));
+        ci = cloud_index.emplace(p.constant_data, static_cast<int>(clouds.size())).first;
+        clouds.push_back(cloud);
+      }
+      csm_job2d& j = jobs[i];
+      j = csm_job2d{};
+      j.stack_index = si->second;
+      j.cloud_index = ci->second;
+      j.full_submap = p.full ? 1 : 0;
+      j.initial_pose[0] = p.initial_pose.translation().x();
+      j.initial_pose[1] = p.initial_pose.translation().y();
+      j.initial_pose[2] = p.initial_pose.rotation().angle();
+      j.min_score = p.min_score;
+    }
+    std::vector<csm_result2d> results(jobs.size());
+    if (!jobs.empty()) {
+      const auto run = [&](const csm_job2d* js, int32_t n, csm_result2d* rs) {
+        const csm_cloud* const* cl = const_cast<const csm_cloud* const*>(clouds.data());
+        if (ctx_ != nullptr)
+          return csm_cb_batch2d_run(ctx_, stacks.data(), static_cast<int32_t>(stacks.size()), cl,
+                                    static_cast<int32_t>(clouds.size()), js, n, owners.data(),
+                                    fo.linear_search_window(), fo.angular_search_window(), rs,
+                                    &last_stats_);
+        return csm_match2d_batch(stacks.data(), static_cast<int32_t>(stacks.size()), cl,
+                                 static_cast<int32_t>(clouds.size()), js, n,
+                                 fo.linear_search_window(), fo.angular_search_window(), rs,
+                                 &last_stats_);
+      };
+      if (!scan_matching::b200_internal::Check(
+              run(jobs.data(), static_cast<int32_t>(jobs.size()), results.data()))) {
+        // An engine capacity limit was hit somewhere in the batch: run the pairs one by
+        // one; a pair that still exceeds it yields no constraint (the reference would
+        // have produced a match or none — it never aborts here).
+        for (size_t i = 0; i < jobs.size(); ++i) {
+          results[i] = csm_result2d{};
+          if (!scan_matching::b200_internal::Check(run(&jobs[i], 1, &results[i])))
+            results[i].found = 0;
+        }
+      }
+    }
+    for (csm_cloud* c : clouds) csm_cloud_destroy(c);
+    // ceres_scan_matcher_.Match(pose_estimate.translation(), pose_estimate, cloud, grid,
+    // &pose_estimate, ...) for every found match (:245-249), one launch for the queue
+    std::vector<transform::Rigid2d> refined;
+    std::vector<size_t> refined_of(pending.size(), 0);
+    if (device_refinement_) {
+      std::vector<scan_matching::CeresScanMatcher2D::Job> rjobs;
+      for (size_t i = 0; i < pending.size(); ++i) {
+        if (!results[i].found) continue;
+        const Pending& p = pending[i];
+        const scan_matching::DeviceGrid2D* grid = nullptr;
+        if (p.device_submap != nullptr) {   // the submap's own grid
+          grid = p.device_submap->grid;
+        } else {
+          std::unique_ptr<scan_matching::DeviceGrid2D>& upload =
+              matchers_[p.submap_id].device_grid;
+          if (upload == nullptr)
+            upload.reset(new scan_matching::DeviceGrid2D(*p.submap->grid(), device_));
+          grid = upload.get();
+        }
+        refined_of[i] = rjobs.size();
+        rjobs.push_back(scan_matching::CeresScanMatcher2D::Job{
+            {results[i].pose_estimate[0], results[i].pose_estimate[1]},
+            transform::Rigid2d({results[i].pose_estimate[0], results[i].pose_estimate[1]},
+                               results[i].pose_estimate[2]),
+            &p.constant_data->filtered_gravity_aligned_point_cloud, grid});
+      }
+      scan_matching::CeresScanMatcher2D(options_.ceres_scan_matcher_options(), device_)
+          .MatchBatch(rjobs, &refined, nullptr);
+    }
+    Result result;
+    for (size_t i = 0; i < pending.size(); ++i) {
+      if (!results[i].found) continue;  // below min_score: no constraint (:253-261)
+      const Pending& p = pending[i];
+      transform::Rigid2d pose_estimate({results[i].pose_estimate[0], results[i].pose_estimate[1]},
+                                       results[i].pose_estimate[2]);
+      if (device_refinement_) pose_estimate = refined[refined_of[i]];
+      if (refiner_)
+        pose_estimate = refiner_(pose_estimate,
+                                 p.constant_data->filtered_gravity_aligned_point_cloud,
+                                 *p.submap->grid());
+      // constraint_transform = ComputeSubmapPose(*submap).inverse() * pose_estimate (:251-252)
+      const transform::Rigid2d constraint_transform =
+          LocalPose(p.submap, p.device_submap).inverse() * pose_estimate;
+      result.push_back(Constraint{p.submap_id,
+                                  p.node_id,
+                                  {b200_internal::Embed3D(constraint_transform),
+                                   options_.loop_closure_translation_weight(),
+                                   options_.loop_closure_rotation_weight()},
+                                  Constraint::INTER_SUBMAP});
+    }
+    return result;
   }
 
   // submap-major ownership, stable across drains
@@ -393,17 +423,9 @@ class ConstraintBuilder2D {
   }
 
   const proto::ConstraintBuilderOptions options_;
-  common::ThreadPoolInterface* thread_pool_;
   const int device_;
   csm_ctx* const ctx_;
   int32_t world_ = 1, rank_ = 0;
-  std::mutex mutex_;
-  std::unique_ptr<std::function<void(const Result&)>> when_done_;
-  int num_started_nodes_ = 0;
-  int num_finished_nodes_ = 0;
-  std::deque<Pending> pending_;
-  std::map<SubmapId, SubmapStack> stacks_;
-  std::map<SubmapId, common::FixedRatioSampler> per_submap_sampler_;
   Refiner refiner_;
   bool device_refinement_ = false;
   csm_stats last_stats_{};
@@ -421,24 +443,33 @@ struct DeviceSubmap3D {
   int grid_size_in_voxels = 0;   // HybridGrid::grid_size(); 0 derives it from the grid
 };
 
-class ConstraintBuilder3D {
- public:
-  using Constraint = PoseGraphInterface::Constraint;
-  using Result = std::vector<Constraint>;
+namespace b200_internal {
+struct Pending3D {
+  SubmapId submap_id;
+  const Submap3D* submap;                 // one of the two is set
+  const DeviceSubmap3D* device_submap;
+  NodeId node_id;
+  const TrajectoryNodeData* constant_data;
+  transform::Rigid3d global_node_pose, global_submap_pose;
+  bool full;
+  float min_score;
+};
+struct SubmapMatcher3D {
+  std::unique_ptr<scan_matching::FastCorrelativeScanMatcher3D> matcher;
+  // the refinement's uploads of a host submap's high / low resolution grids
+  std::unique_ptr<scan_matching::DeviceHybridGrid> high, low;
+};
+}  // namespace b200_internal
 
+class ConstraintBuilder3D
+    : public b200_internal::ConstraintQueue<b200_internal::Pending3D,
+                                            b200_internal::SubmapMatcher3D> {
+ public:
   ConstraintBuilder3D(const proto::ConstraintBuilderOptions& options,
                       common::ThreadPoolInterface* thread_pool, int device = 0)
-      : options_(options), thread_pool_(thread_pool), device_(device) {}
-
-  ~ConstraintBuilder3D() {  // constraint_builder_3d.cc:70-77
-    std::lock_guard<std::mutex> lock(mutex_);
-    b200_internal::Require(pending_.empty(), "WhenDone() was not called");
-    b200_internal::Require(num_started_nodes_ == num_finished_nodes_, "unfinished nodes");
-    b200_internal::Require(when_done_ == nullptr, "callback still pending");
-    for (auto& kv : matchers_) csm_matcher3d_destroy(kv.second);
-  }
-  ConstraintBuilder3D(const ConstraintBuilder3D&) = delete;
-  ConstraintBuilder3D& operator=(const ConstraintBuilder3D&) = delete;
+      : ConstraintQueue(thread_pool, options.sampling_ratio()),
+        options_(options),
+        device_(device) {}
 
   // constraint_builder_3d.cc:265-275 on the device: every found match of a drained queue is
   // refined by CeresScanMatcher3D (options.ceres_scan_matcher_options_3d()) in one launch.
@@ -478,49 +509,8 @@ class ConstraintBuilder3D {
               global_submap_rotation);
   }
 
-  void NotifyEndOfNode() {
-    std::lock_guard<std::mutex> lock(mutex_);
-    ++num_started_nodes_;
-  }
-
-  void WhenDone(const std::function<void(const Result&)>& callback) {
-    {
-      std::lock_guard<std::mutex> lock(mutex_);
-      b200_internal::Require(when_done_ == nullptr, "WhenDone called twice");
-      when_done_.reset(new std::function<void(const Result&)>(callback));
-    }
-    std::unique_ptr<common::Task> task(new common::Task);
-    task->SetWorkItem([this] { Drain(); });
-    thread_pool_->Schedule(std::move(task));
-  }
-
-  int GetNumFinishedNodes() {
-    std::lock_guard<std::mutex> lock(mutex_);
-    return num_finished_nodes_;
-  }
-
-  void DeleteScanMatcher(const SubmapId& submap_id) {  // constraint_builder_3d.cc:312-321
-    std::lock_guard<std::mutex> lock(mutex_);
-    auto it = matchers_.find(submap_id);
-    if (it != matchers_.end()) {
-      csm_matcher3d_destroy(it->second);
-      matchers_.erase(it);
-    }
-    device_grids_.erase(submap_id);
-    per_submap_sampler_.erase(submap_id);
-  }
-
  private:
-  struct Pending {
-    SubmapId submap_id;
-    const Submap3D* submap;                 // one of the two is set
-    const DeviceSubmap3D* device_submap;
-    NodeId node_id;
-    const TrajectoryNodeData* constant_data;
-    transform::Rigid3d global_node_pose, global_submap_pose;
-    bool full;
-    float min_score;
-  };
+  using Pending = b200_internal::Pending3D;
 
   void AddLocal(const SubmapId& submap_id, const Submap3D* submap,
                 const DeviceSubmap3D* device_submap, const NodeId& node_id,
@@ -532,16 +522,9 @@ class ConstraintBuilder3D {
     const double dy = global_node_pose.translation().y() - global_submap_pose.translation().y();
     const double dz = global_node_pose.translation().z() - global_submap_pose.translation().z();
     if (std::sqrt(dx * dx + dy * dy + dz * dz) > options_.max_constraint_distance()) return;
-    if (!per_submap_sampler_
-             .emplace(std::piecewise_construct, std::forward_as_tuple(submap_id),
-                      std::forward_as_tuple(options_.sampling_ratio()))
-             .first->second.Pulse()) {
-      return;
-    }
-    std::lock_guard<std::mutex> lock(mutex_);
-    pending_.push_back(Pending{submap_id, submap, device_submap, node_id, constant_data,
-                               global_node_pose, global_submap_pose, false,
-                               static_cast<float>(options_.min_score())});
+    if (!Sample(submap_id)) return;
+    Push(Pending{submap_id, submap, device_submap, node_id, constant_data, global_node_pose,
+                 global_submap_pose, false, static_cast<float>(options_.min_score())});
   }
 
   void AddGlobal(const SubmapId& submap_id, const Submap3D* submap,
@@ -549,196 +532,130 @@ class ConstraintBuilder3D {
                  const TrajectoryNodeData* constant_data,
                  const transform::Quaterniond& global_node_rotation,
                  const transform::Quaterniond& global_submap_rotation) {
-    std::lock_guard<std::mutex> lock(mutex_);
-    pending_.push_back(Pending{submap_id, submap, device_submap, node_id, constant_data,
-                               transform::Rigid3d({{0., 0., 0.}}, global_node_rotation),
-                               transform::Rigid3d({{0., 0., 0.}}, global_submap_rotation), true,
-                               static_cast<float>(options_.global_localization_min_score())});
+    Push(Pending{submap_id, submap, device_submap, node_id, constant_data,
+                 transform::Rigid3d({{0., 0., 0.}}, global_node_rotation),
+                 transform::Rigid3d({{0., 0., 0.}}, global_submap_rotation), true,
+                 static_cast<float>(options_.global_localization_min_score())});
   }
 
-  static void Flatten(const HybridGrid& grid, std::vector<int32_t>* idx,
-                      std::vector<uint16_t>* val) {
-    for (const auto& v : grid.voxels()) {
-      idx->push_back(v.x);
-      idx->push_back(v.y);
-      idx->push_back(v.z);
-      val->push_back(v.value);
-    }
-  }
-  static void Pose7(const transform::Rigid3d& p, double out[7]) {
-    out[0] = p.translation().x(); out[1] = p.translation().y(); out[2] = p.translation().z();
-    out[3] = p.rotation().w(); out[4] = p.rotation().x(); out[5] = p.rotation().y();
-    out[6] = p.rotation().z();
-  }
-
-  // DispatchScanMatcherConstruction (constraint_builder_3d.cc:172-198)
-  csm_matcher3d* MatcherFor(const Pending& p) {
-    csm_matcher3d*& m = matchers_[p.submap_id];
+  // One matcher per submap, built once (constraint_builder_3d.cc:172-198); a device submap's
+  // from its grids, device to device.
+  const csm_matcher3d* MatcherFor(const Pending& p) {
+    std::unique_ptr<scan_matching::FastCorrelativeScanMatcher3D>& m =
+        matchers_[p.submap_id].matcher;
+    const auto& fo = options_.fast_correlative_scan_matcher_options_3d();
     if (m == nullptr && p.device_submap != nullptr) {
       const DeviceSubmap3D& d = *p.device_submap;
-      const csm_options3d o = scan_matching::b200_internal::Options3D(
-          options_.fast_correlative_scan_matcher_options_3d());
-      scan_matching::b200_internal::Check(csm_matcher3d_create_from_grid3d(
-          d.high_resolution_hybrid_grid->handle(), d.grid_size_in_voxels,
-          d.low_resolution_hybrid_grid->handle(), d.rotational_scan_matcher_histogram->data(),
-          static_cast<int32_t>(d.rotational_scan_matcher_histogram->size()), &o, &m));
+      m.reset(new scan_matching::FastCorrelativeScanMatcher3D(
+          *d.high_resolution_hybrid_grid, d.low_resolution_hybrid_grid,
+          d.rotational_scan_matcher_histogram, fo, d.grid_size_in_voxels));
     } else if (m == nullptr) {
-      const Submap3D* submap = p.submap;
-      std::vector<int32_t> hi_idx, lo_idx;
-      std::vector<uint16_t> hi_val, lo_val;
-      Flatten(submap->high_resolution_hybrid_grid(), &hi_idx, &hi_val);
-      Flatten(submap->low_resolution_hybrid_grid(), &lo_idx, &lo_val);
-      const csm_options3d o = scan_matching::b200_internal::Options3D(
-          options_.fast_correlative_scan_matcher_options_3d());
-      const std::vector<float>& hist = submap->rotational_scan_matcher_histogram();
-      scan_matching::b200_internal::Check(csm_matcher3d_create(
-          hi_idx.data(), hi_val.data(), static_cast<int64_t>(hi_val.size()),
-          submap->high_resolution_hybrid_grid().resolution(),
-          submap->high_resolution_hybrid_grid().grid_size(), lo_idx.data(), lo_val.data(),
-          static_cast<int64_t>(lo_val.size()), submap->low_resolution_hybrid_grid().resolution(),
-          hist.data(), static_cast<int32_t>(hist.size()), &o, device_, &m));
+      m.reset(new scan_matching::FastCorrelativeScanMatcher3D(
+          p.submap->high_resolution_hybrid_grid(), &p.submap->low_resolution_hybrid_grid(),
+          &p.submap->rotational_scan_matcher_histogram(), fo, device_));
     }
-    return m;
+    return m->matcher();
   }
 
-  void Drain() {
-    Result result;
-    std::unique_ptr<std::function<void(const Result&)>> callback;
-    {
-      std::lock_guard<std::mutex> lock(mutex_);
-      b200_internal::Require(when_done_ != nullptr, "no callback");
-      std::vector<const csm_matcher3d*> matchers;
-      std::map<SubmapId, int> matcher_index;
-      std::vector<csm_node3d> nodes;
-      std::deque<std::vector<float>> buffers;  // keeps the flattened clouds alive
-      std::map<const TrajectoryNodeData*, int> node_index;
-      std::vector<csm_job3d> jobs(pending_.size());
-      for (size_t i = 0; i < pending_.size(); ++i) {
-        const Pending& p = pending_[i];
-        auto mi = matcher_index.find(p.submap_id);
-        if (mi == matcher_index.end()) {
-          mi = matcher_index.emplace(p.submap_id, static_cast<int>(matchers.size())).first;
-          matchers.push_back(MatcherFor(p));
-        }
-        auto ni = node_index.find(p.constant_data);
-        if (ni == node_index.end()) {
-          const TrajectoryNodeData& d = *p.constant_data;
-          buffers.push_back(scan_matching::b200_internal::Flatten(d.high_resolution_point_cloud));
-          const float* hi = buffers.back().data();
-          buffers.push_back(scan_matching::b200_internal::Flatten(d.low_resolution_point_cloud));
-          const float* lo = buffers.back().data();
-          csm_node3d n;
-          n.high_resolution_point_cloud = hi;
-          n.num_high = static_cast<int32_t>(d.high_resolution_point_cloud.size());
-          n.low_resolution_point_cloud = lo;
-          n.num_low = static_cast<int32_t>(d.low_resolution_point_cloud.size());
-          n.rotational_scan_matcher_histogram = d.rotational_scan_matcher_histogram.data();
-          n.histogram_size = static_cast<int32_t>(d.rotational_scan_matcher_histogram.size());
-          n.gravity_alignment[0] = d.gravity_alignment.w();
-          n.gravity_alignment[1] = d.gravity_alignment.x();
-          n.gravity_alignment[2] = d.gravity_alignment.y();
-          n.gravity_alignment[3] = d.gravity_alignment.z();
-          ni = node_index.emplace(p.constant_data, static_cast<int>(nodes.size())).first;
-          nodes.push_back(n);
-        }
-        csm_job3d& j = jobs[i];
-        j.matcher_index = mi->second;
-        j.node_index = ni->second;
-        j.full_submap = p.full ? 1 : 0;
-        j.min_score = p.min_score;
-        Pose7(p.global_node_pose, j.global_node_pose);
-        Pose7(p.global_submap_pose, j.global_submap_pose);
+  Result Match(const std::deque<Pending>& pending) override {
+    std::vector<const csm_matcher3d*> matchers;
+    std::map<SubmapId, int> matcher_index;
+    std::vector<csm_node3d> nodes;
+    std::deque<std::vector<float>> buffers;  // keeps the flattened clouds alive
+    std::map<const TrajectoryNodeData*, int> node_index;
+    std::vector<csm_job3d> jobs(pending.size());
+    for (size_t i = 0; i < pending.size(); ++i) {
+      const Pending& p = pending[i];
+      auto mi = matcher_index.find(p.submap_id);
+      if (mi == matcher_index.end()) {
+        mi = matcher_index.emplace(p.submap_id, static_cast<int>(matchers.size())).first;
+        matchers.push_back(MatcherFor(p));
       }
-      std::vector<csm_result3d> results(jobs.size());
-      if (!jobs.empty()) {
-        scan_matching::b200_internal::Check(csm_match3d_batch(
-            matchers.data(), static_cast<int32_t>(matchers.size()), nodes.data(),
-            static_cast<int32_t>(nodes.size()), jobs.data(), static_cast<int32_t>(jobs.size()),
-            0, results.data(), nullptr));
+      auto ni = node_index.find(p.constant_data);
+      if (ni == node_index.end()) {
+        buffers.emplace_back();
+        std::vector<float>* high = &buffers.back();
+        buffers.emplace_back();
+        ni = node_index.emplace(p.constant_data, static_cast<int>(nodes.size())).first;
+        nodes.push_back(
+            scan_matching::b200_internal::Node3D(*p.constant_data, high, &buffers.back()));
       }
-      // ceres_scan_matcher_.Match(pose_estimate.translation(), pose_estimate, {{high cloud,
-      // high grid}, {low cloud, low grid}}, &constraint_transform, ...) for every found
-      // match (constraint_builder_3d.cc:265-275), one launch for the queue
-      std::vector<transform::Rigid3d> refined;
-      std::vector<size_t> refined_of(pending_.size(), 0);
-      if (device_refinement_) {
-        std::vector<scan_matching::CeresScanMatcher3D::Job> rjobs;
-        for (size_t i = 0; i < pending_.size(); ++i) {
-          if (!results[i].found) continue;
-          const Pending& p = pending_[i];
-          const scan_matching::DeviceHybridGrid* high;
-          const scan_matching::DeviceHybridGrid* low;
-          if (p.device_submap != nullptr) {   // the submap's own grids
-            high = p.device_submap->high_resolution_hybrid_grid;
-            low = p.device_submap->low_resolution_hybrid_grid;
-          } else {
-            auto& grids = device_grids_[p.submap_id];
-            if (grids.first == nullptr) {
-              grids.first.reset(new scan_matching::DeviceHybridGrid(
-                  p.submap->high_resolution_hybrid_grid(), device_));
-              grids.second.reset(new scan_matching::DeviceHybridGrid(
-                  p.submap->low_resolution_hybrid_grid(), device_));
-            }
-            high = grids.first.get();
-            low = grids.second.get();
-          }
-          const csm_result3d& r = results[i];
-          scan_matching::CeresScanMatcher3D::Job job;
-          for (int k = 0; k < 3; ++k) job.target_translation[k] = r.pose_estimate[k];
-          job.initial_pose_estimate = transform::Rigid3d(
-              {{r.pose_estimate[0], r.pose_estimate[1], r.pose_estimate[2]}},
-              transform::Quaterniond{r.pose_estimate[3], r.pose_estimate[4], r.pose_estimate[5],
-                                     r.pose_estimate[6]});
-          job.point_clouds_and_hybrid_grids = {
-              {&p.constant_data->high_resolution_point_cloud, high},
-              {&p.constant_data->low_resolution_point_cloud, low}};
-          refined_of[i] = rjobs.size();
-          rjobs.push_back(job);
-        }
-        scan_matching::CeresScanMatcher3D(options_.ceres_scan_matcher_options_3d())
-            .MatchBatch(rjobs, &refined, nullptr);
-      }
-      for (size_t i = 0; i < pending_.size(); ++i) {
-        const csm_result3d& r = results[i];
-        if (!r.found) continue;
-        // constraint_transform = the matcher's pose_estimate, refined when
-        // set_device_refinement(true) (constraint_builder_3d.cc:261-275)
-        const transform::Rigid3d pose_estimate =
-            device_refinement_
-                ? refined[refined_of[i]]
-                : transform::Rigid3d(
-                      {{r.pose_estimate[0], r.pose_estimate[1], r.pose_estimate[2]}},
-                      transform::Quaterniond{r.pose_estimate[3], r.pose_estimate[4],
-                                             r.pose_estimate[5], r.pose_estimate[6]});
-        result.push_back(Constraint{
-            pending_[i].submap_id,
-            pending_[i].node_id,
-            {pose_estimate, options_.loop_closure_translation_weight(),
-             options_.loop_closure_rotation_weight()},
-            Constraint::INTER_SUBMAP});
-      }
-      pending_.clear();
-      num_finished_nodes_ = num_started_nodes_;
-      callback = std::move(when_done_);
-      when_done_.reset();
+      csm_job3d& j = jobs[i];
+      j.matcher_index = mi->second;
+      j.node_index = ni->second;
+      j.full_submap = p.full ? 1 : 0;
+      j.min_score = p.min_score;
+      scan_matching::b200_internal::Pose7(p.global_node_pose, j.global_node_pose);
+      scan_matching::b200_internal::Pose7(p.global_submap_pose, j.global_submap_pose);
     }
-    (*callback)(result);
+    std::vector<csm_result3d> results(jobs.size());
+    if (!jobs.empty()) {
+      scan_matching::b200_internal::Check(csm_match3d_batch(
+          matchers.data(), static_cast<int32_t>(matchers.size()), nodes.data(),
+          static_cast<int32_t>(nodes.size()), jobs.data(), static_cast<int32_t>(jobs.size()),
+          0, results.data(), nullptr));
+    }
+    // ceres_scan_matcher_.Match(pose_estimate.translation(), pose_estimate, {{high cloud,
+    // high grid}, {low cloud, low grid}}, &constraint_transform, ...) for every found
+    // match (constraint_builder_3d.cc:265-275), one launch for the queue
+    std::vector<transform::Rigid3d> refined;
+    std::vector<size_t> refined_of(pending.size(), 0);
+    if (device_refinement_) {
+      std::vector<scan_matching::CeresScanMatcher3D::Job> rjobs;
+      for (size_t i = 0; i < pending.size(); ++i) {
+        if (!results[i].found) continue;
+        const Pending& p = pending[i];
+        const scan_matching::DeviceHybridGrid* high;
+        const scan_matching::DeviceHybridGrid* low;
+        if (p.device_submap != nullptr) {   // the submap's own grids
+          high = p.device_submap->high_resolution_hybrid_grid;
+          low = p.device_submap->low_resolution_hybrid_grid;
+        } else {
+          b200_internal::SubmapMatcher3D& uploads = matchers_[p.submap_id];
+          if (uploads.high == nullptr) {
+            uploads.high.reset(new scan_matching::DeviceHybridGrid(
+                p.submap->high_resolution_hybrid_grid(), device_));
+            uploads.low.reset(new scan_matching::DeviceHybridGrid(
+                p.submap->low_resolution_hybrid_grid(), device_));
+          }
+          high = uploads.high.get();
+          low = uploads.low.get();
+        }
+        const csm_result3d& r = results[i];
+        scan_matching::CeresScanMatcher3D::Job job;
+        for (int k = 0; k < 3; ++k) job.target_translation[k] = r.pose_estimate[k];
+        job.initial_pose_estimate = scan_matching::b200_internal::FromPose7(r.pose_estimate);
+        job.point_clouds_and_hybrid_grids = {
+            {&p.constant_data->high_resolution_point_cloud, high},
+            {&p.constant_data->low_resolution_point_cloud, low}};
+        refined_of[i] = rjobs.size();
+        rjobs.push_back(job);
+      }
+      scan_matching::CeresScanMatcher3D(options_.ceres_scan_matcher_options_3d())
+          .MatchBatch(rjobs, &refined, nullptr);
+    }
+    Result result;
+    for (size_t i = 0; i < pending.size(); ++i) {
+      const csm_result3d& r = results[i];
+      if (!r.found) continue;
+      // constraint_transform = the matcher's pose_estimate, refined when
+      // set_device_refinement(true) (constraint_builder_3d.cc:261-275)
+      const transform::Rigid3d pose_estimate =
+          device_refinement_ ? refined[refined_of[i]]
+                             : scan_matching::b200_internal::FromPose7(r.pose_estimate);
+      result.push_back(Constraint{
+          pending[i].submap_id,
+          pending[i].node_id,
+          {pose_estimate, options_.loop_closure_translation_weight(),
+           options_.loop_closure_rotation_weight()},
+          Constraint::INTER_SUBMAP});
+    }
+    return result;
   }
 
   const proto::ConstraintBuilderOptions options_;
-  common::ThreadPoolInterface* thread_pool_;
   const int device_;
-  std::mutex mutex_;
-  std::unique_ptr<std::function<void(const Result&)>> when_done_;
-  int num_started_nodes_ = 0;
-  int num_finished_nodes_ = 0;
-  std::deque<Pending> pending_;
-  std::map<SubmapId, csm_matcher3d*> matchers_;
-  std::map<SubmapId, std::pair<std::unique_ptr<scan_matching::DeviceHybridGrid>,
-                               std::unique_ptr<scan_matching::DeviceHybridGrid>>>
-      device_grids_;   // high / low resolution grids for the refinement
   bool device_refinement_ = false;
-  std::map<SubmapId, common::FixedRatioSampler> per_submap_sampler_;
 };
 #endif  // !CSM_ADAPTER_REAL_CARTOGRAPHER
 

@@ -68,6 +68,12 @@ inline std::vector<float> Flatten(const sensor::PointCloud& point_cloud) {
   }
   return xyz;
 }
+// A Rigid3d as the ABI's pose[7] (tx, ty, tz, qw, qx, qy, qz); FromPose7 is the way back.
+inline void Pose7(const transform::Rigid3d& p, double out[7]) {
+  out[0] = p.translation().x(); out[1] = p.translation().y(); out[2] = p.translation().z();
+  out[3] = p.rotation().w(); out[4] = p.rotation().x(); out[5] = p.rotation().y();
+  out[6] = p.rotation().z();
+}
 // The serialised message of one *_to_proto entry point (sized by a first call).  A message
 // of 2 GiB or more, which protobuf cannot hold, aborts as the reference's serialiser does.
 template <typename Handle>
@@ -107,9 +113,8 @@ template <typename Handle>
 std::string DrawTexture(csm_status (*to_texture)(const Handle*, const double*, uint8_t*, int64_t,
                                                  int64_t*),
                         const Handle* handle, const transform::Rigid3d& pose) {
-  const double p[7] = {pose.translation().x(), pose.translation().y(), pose.translation().z(),
-                       pose.rotation().w(),    pose.rotation().x(),    pose.rotation().y(),
-                       pose.rotation().z()};
+  double p[7];
+  Pose7(pose, p);
   std::string bytes(size_t(1) << 16, '\0');
   int64_t size = 0;
   csm_status st = to_texture(handle, p, reinterpret_cast<uint8_t*>(&bytes[0]),
@@ -553,6 +558,38 @@ inline csm_options3d Options3D(const proto::FastCorrelativeScanMatcherOptions3D&
   o.angular_search_window = options.angular_search_window();
   return o;
 }
+inline transform::Rigid3d FromPose7(const double p[7]) {
+  return transform::Rigid3d({{p[0], p[1], p[2]}}, transform::Quaterniond{p[3], p[4], p[5], p[6]});
+}
+// A HybridGrid's voxels as the ABI takes them: (x, y, z) index triples and their values.
+inline void Flatten(const HybridGrid& grid, std::vector<int32_t>* idx,
+                    std::vector<uint16_t>* val) {
+  for (const auto& v : grid.voxels()) {
+    idx->push_back(v.x);
+    idx->push_back(v.y);
+    idx->push_back(v.z);
+    val->push_back(v.value);
+  }
+}
+// The csm_node3d of a node's data.  Its clouds are flattened into `high` and `low`, which must
+// outlive it.
+inline csm_node3d Node3D(const TrajectoryNodeData& data, std::vector<float>* high,
+                         std::vector<float>* low) {
+  *high = Flatten(data.high_resolution_point_cloud);
+  *low = Flatten(data.low_resolution_point_cloud);
+  csm_node3d node;
+  node.high_resolution_point_cloud = high->data();
+  node.num_high = static_cast<int32_t>(data.high_resolution_point_cloud.size());
+  node.low_resolution_point_cloud = low->data();
+  node.num_low = static_cast<int32_t>(data.low_resolution_point_cloud.size());
+  node.rotational_scan_matcher_histogram = data.rotational_scan_matcher_histogram.data();
+  node.histogram_size = static_cast<int32_t>(data.rotational_scan_matcher_histogram.size());
+  node.gravity_alignment[0] = data.gravity_alignment.w();
+  node.gravity_alignment[1] = data.gravity_alignment.x();
+  node.gravity_alignment[2] = data.gravity_alignment.y();
+  node.gravity_alignment[3] = data.gravity_alignment.z();
+  return node;
+}
 }  // namespace b200_internal
 
 class DeviceHybridGrid;
@@ -585,8 +622,8 @@ class FastCorrelativeScanMatcher3D {
                                int device = 0) {
     std::vector<int32_t> hi_idx, lo_idx;
     std::vector<uint16_t> hi_val, lo_val;
-    Flatten(hybrid_grid, &hi_idx, &hi_val);
-    Flatten(*low_resolution_hybrid_grid, &lo_idx, &lo_val);
+    b200_internal::Flatten(hybrid_grid, &hi_idx, &hi_val);
+    b200_internal::Flatten(*low_resolution_hybrid_grid, &lo_idx, &lo_val);
     const csm_options3d o = b200_internal::Options3D(options);
     b200_internal::Check(csm_matcher3d_create(
         hi_idx.data(), hi_val.data(), static_cast<int64_t>(hi_val.size()),
@@ -613,50 +650,23 @@ class FastCorrelativeScanMatcher3D {
                min_score);
   }
 
+  const csm_matcher3d* matcher() const { return matcher_; }  // for the batched ConstraintBuilder
+
  private:
-  static void Flatten(const HybridGrid& grid, std::vector<int32_t>* idx,
-                      std::vector<uint16_t>* val) {
-    for (const auto& v : grid.voxels()) {
-      idx->push_back(v.x);
-      idx->push_back(v.y);
-      idx->push_back(v.z);
-      val->push_back(v.value);
-    }
-  }
-  static void Pose7(const transform::Rigid3d& p, double out[7]) {
-    out[0] = p.translation().x(); out[1] = p.translation().y(); out[2] = p.translation().z();
-    out[3] = p.rotation().w(); out[4] = p.rotation().x(); out[5] = p.rotation().y();
-    out[6] = p.rotation().z();
-  }
   std::unique_ptr<Result> Run(int full, const transform::Rigid3d& node_pose,
                               const transform::Rigid3d& submap_pose,
                               const TrajectoryNodeData& data, float min_score) const {
-    const std::vector<float> hi = b200_internal::Flatten(data.high_resolution_point_cloud);
-    const std::vector<float> lo = b200_internal::Flatten(data.low_resolution_point_cloud);
-    csm_node3d node;
-    node.high_resolution_point_cloud = hi.data();
-    node.num_high = static_cast<int32_t>(data.high_resolution_point_cloud.size());
-    node.low_resolution_point_cloud = lo.data();
-    node.num_low = static_cast<int32_t>(data.low_resolution_point_cloud.size());
-    node.rotational_scan_matcher_histogram = data.rotational_scan_matcher_histogram.data();
-    node.histogram_size = static_cast<int32_t>(data.rotational_scan_matcher_histogram.size());
-    node.gravity_alignment[0] = data.gravity_alignment.w();
-    node.gravity_alignment[1] = data.gravity_alignment.x();
-    node.gravity_alignment[2] = data.gravity_alignment.y();
-    node.gravity_alignment[3] = data.gravity_alignment.z();
+    std::vector<float> hi, lo;
+    const csm_node3d node = b200_internal::Node3D(data, &hi, &lo);
     double np[7], sp[7];
-    Pose7(node_pose, np);
-    Pose7(submap_pose, sp);
+    b200_internal::Pose7(node_pose, np);
+    b200_internal::Pose7(submap_pose, sp);
     csm_result3d r;
     if (!b200_internal::Check(csm_match3d(matcher_, &node, np, sp, full, min_score, &r, nullptr)))
       return nullptr;
     if (!r.found) return nullptr;  // fast_correlative_scan_matcher_3d.cc:197
-    return std::unique_ptr<Result>(new Result{
-        r.score,
-        transform::Rigid3d({{r.pose_estimate[0], r.pose_estimate[1], r.pose_estimate[2]}},
-                           transform::Quaterniond{r.pose_estimate[3], r.pose_estimate[4],
-                                                  r.pose_estimate[5], r.pose_estimate[6]}),
-        r.rotational_score, r.low_resolution_score});
+    return std::unique_ptr<Result>(new Result{r.score, b200_internal::FromPose7(r.pose_estimate),
+                                              r.rotational_score, r.low_resolution_score});
   }
   csm_matcher3d* matcher_ = nullptr;
 };
@@ -671,12 +681,7 @@ class DeviceHybridGrid {
   explicit DeviceHybridGrid(const HybridGrid& grid, int device = 0) {
     std::vector<int32_t> idx;
     std::vector<uint16_t> val;
-    for (const auto& v : grid.voxels()) {
-      idx.push_back(v.x);
-      idx.push_back(v.y);
-      idx.push_back(v.z);
-      val.push_back(v.value);
-    }
+    b200_internal::Flatten(grid, &idx, &val);
     b200_internal::Check(csm_grid3d_create(idx.data(), val.data(),
                                            static_cast<int64_t>(val.size()), grid.resolution(),
                                            device, &grid_));
@@ -810,13 +815,8 @@ class RealTimeCorrelativeScanMatcher3D {
               transform::Rigid3d* pose_estimate) const {
     if (pose_estimate == nullptr) std::abort();  // CHECK(:38)
     const std::vector<float> xyz = b200_internal::Flatten(point_cloud);
-    const double init[7] = {initial_pose_estimate.translation().x(),
-                            initial_pose_estimate.translation().y(),
-                            initial_pose_estimate.translation().z(),
-                            initial_pose_estimate.rotation().w(),
-                            initial_pose_estimate.rotation().x(),
-                            initial_pose_estimate.rotation().y(),
-                            initial_pose_estimate.rotation().z()};
+    double init[7];
+    b200_internal::Pose7(initial_pose_estimate, init);
     float score = -1.f;
     double pose[7] = {0., 0., 0., 1., 0., 0., 0.};
     if (!b200_internal::Check(csm_rt_match3d(
@@ -825,8 +825,7 @@ class RealTimeCorrelativeScanMatcher3D {
             options_.translation_delta_cost_weight(), options_.rotation_delta_cost_weight(),
             &score, pose, nullptr)))
       return -1.f;
-    *pose_estimate = transform::Rigid3d(
-        {{pose[0], pose[1], pose[2]}}, transform::Quaterniond{pose[3], pose[4], pose[5], pose[6]});
+    *pose_estimate = b200_internal::FromPose7(pose);
     return score;
   }
 
@@ -901,11 +900,7 @@ class CeresScanMatcher3D {
         }
       }
       for (int k = 0; k < 3; ++k) cj[i].target_translation[k] = job.target_translation[k];
-      const transform::Rigid3d& p = job.initial_pose_estimate;
-      const double init[7] = {p.translation().x(), p.translation().y(), p.translation().z(),
-                              p.rotation().w(), p.rotation().x(), p.rotation().y(),
-                              p.rotation().z()};
-      for (int k = 0; k < 7; ++k) cj[i].initial_pose[k] = init[k];
+      b200_internal::Pose7(job.initial_pose_estimate, cj[i].initial_pose);
     }
     csm_ceres_options3d o{};
     o.occupied_space_weight[0] = options_.occupied_space_weight(0);
@@ -933,10 +928,7 @@ class CeresScanMatcher3D {
                                                    &o, res.data(), nullptr));
     }
     for (const csm_ceres_result3d& r : res) {
-      poses->push_back(transform::Rigid3d(
-          {{r.pose_estimate[0], r.pose_estimate[1], r.pose_estimate[2]}},
-          transform::Quaterniond{r.pose_estimate[3], r.pose_estimate[4], r.pose_estimate[5],
-                                 r.pose_estimate[6]}));
+      poses->push_back(b200_internal::FromPose7(r.pose_estimate));
       if (summaries != nullptr) {
         Summary s;
         s.initial_cost = r.initial_cost;

@@ -231,23 +231,27 @@ class CudaExecutor:
         self.clouds = {}
 
 
-class ConstraintBuilder2D:
-    """constraint_builder_2d.h:60-107.  `executor.run(jobs, submaps, clouds)` does the
-    matching (CudaExecutor in production); `process_group` (torch.distributed) turns
-    on submap-major sharding + the single all_gather of constraint records."""
+class _ConstraintQueue:
+    """What ConstraintBuilder2D and ConstraintBuilder3D share: the queue of (submap, node)
+    pairs, the per-submap FixedRatioSamplers, the node counters and the WhenDone drain.
 
-    def __init__(self, options, executor=None, process_group=None, device=0, context=None):
-        """`context` (scan_matching.MultiGpuContext): the library's own NCCL communicator;
-        when given, the single all-gather runs inside libcsm_b200.so (csm_ctx_allgather ->
-        ncclAllGather) and no torch.distributed group is needed."""
+    With a `process_group` (torch.distributed) or a `context` (scan_matching.MultiGpuContext)
+    the queue is sharded submap-major: rank r runs the pairs of the submaps whose first-use
+    order % world == r, and one all-gather of fixed-size records (RECORD) gives every rank the
+    whole Result in queue order.  A dimension supplies its record dtype, `_fill` (one executor
+    result -> one record), `_is_device` and its MaybeAdd*Constraint gates."""
+
+    RECORD = None
+
+    def __init__(self, options, executor, process_group, device, context=None):
         self.options = options
-        self.executor = executor if executor is not None else CudaExecutor(options, device)
+        self.executor = executor
         self.pg = process_group
         self.ctx = context
         self.device = device
         self._jobs = []
         self._submaps = {}
-        self._clouds = {}
+        self._constant_data = {}   # id(constant_data) -> the node's cloud / data
         self._submap_order = {}
         self._samplers = {}
         self._when_done = None
@@ -255,45 +259,34 @@ class ConstraintBuilder2D:
         self.num_finished_nodes = 0
         self.last_records = None
 
+    def _world(self):
+        if self.ctx is not None:
+            return self.ctx.rank, self.ctx.world_size
+        if self.pg is None:
+            return 0, 1
+        import torch.distributed as dist
+        return dist.get_rank(self.pg), dist.get_world_size(self.pg)
+
     # -- queue --------------------------------------------------------------------
     def _check_submap(self, submap):
-        """Refuses, before anything is queued, a device submap the builder cannot use: a TSDF
-        handle, a handle on another device, or any device submap when the queue is sharded
-        over several ranks (a device submap stays on the GPU that inserted it)."""
-        device = getattr(self.executor, "device", self.device)
-        if _is_device_grid(submap.grid, device) and self._world()[1] > 1:
+        """Refuses, before any gate, a device submap the builder cannot use (see `_is_device`),
+        or any device submap when the queue is sharded over several ranks (a device submap
+        stays on the GPU that inserted it)."""
+        if self._is_device(submap) and self._world()[1] > 1:
             raise ValueError("device-resident submaps are not sharded over several ranks")
+
+    def _pulse(self, submap_id):
+        """The per-submap FixedRatioSampler of constraint_builder_2d.cc:85-90."""
+        sampler = self._samplers.setdefault(submap_id,
+                                            FixedRatioSampler(self.options.sampling_ratio))
+        return sampler.Pulse()
 
     def _register(self, submap_id, submap, constant_data):
         self._submaps[submap_id] = submap
         self._submap_order.setdefault(submap_id, len(self._submap_order))
         key = id(constant_data)
-        self._clouds[key] = constant_data
+        self._constant_data[key] = constant_data
         return key
-
-    def MaybeAddConstraint(self, submap_id, submap, node_id, constant_data,
-                           initial_relative_pose):
-        """constraint_builder_2d.cc:77-112.  constant_data is the node's
-        filtered_gravity_aligned_point_cloud (N x 3 float32)."""
-        self._check_submap(submap)
-        if math.hypot(initial_relative_pose[0], initial_relative_pose[1]) > \
-                self.options.max_constraint_distance:
-            return
-        sampler = self._samplers.setdefault(submap_id,
-                                            FixedRatioSampler(self.options.sampling_ratio))
-        if not sampler.Pulse():
-            return
-        key = self._register(submap_id, submap, constant_data)
-        initial_pose = _compose(tuple(submap.local_pose), tuple(initial_relative_pose))  # :196-197
-        self._jobs.append(_Job(submap_id, node_id, key, initial_pose, False,
-                               self.options.min_score))
-
-    def MaybeAddGlobalConstraint(self, submap_id, submap, node_id, constant_data):
-        """constraint_builder_2d.cc:114-137."""
-        self._check_submap(submap)
-        key = self._register(submap_id, submap, constant_data)
-        self._jobs.append(_Job(submap_id, node_id, key, (0.0, 0.0, 0.0), True,
-                               self.options.global_localization_min_score))
 
     def NotifyEndOfNode(self):
         """constraint_builder_2d.cc:139-151 (the node finishes when WhenDone drains)."""
@@ -309,14 +302,6 @@ class ConstraintBuilder2D:
         self._samplers.pop(submap_id, None)
 
     # -- drain ---------------------------------------------------------------------
-    def _world(self):
-        if self.ctx is not None:
-            return self.ctx.rank, self.ctx.world_size
-        if self.pg is None:
-            return 0, 1
-        import torch.distributed as dist
-        return dist.get_rank(self.pg), dist.get_world_size(self.pg)
-
     def WhenDone(self, callback):
         """constraint_builder_2d.cc:153-163 + RunWhenDoneCallback :279-300: runs the
         queue, then calls callback(Result) with the found constraints in queue order."""
@@ -327,31 +312,23 @@ class ConstraintBuilder2D:
         jobs = self._jobs
         owner = [self._submap_order[j.submap_id] % world for j in jobs]
         mine = [i for i, o in enumerate(owner) if o == rank]
-        out = self.executor.run([jobs[i] for i in mine], self._submaps, self._clouds)
-        local = np.zeros(len(mine), RECORD_DTYPE)
-        for rec, i, (found, score, pose) in zip(local, mine, out):
+        out = self.executor.run([jobs[i] for i in mine], self._submaps, self._constant_data)
+        local = np.zeros(len(mine), self.RECORD)
+        for rec, i, r in zip(local, mine, out):
             j = jobs[i]
             rec["submap_trajectory"], rec["submap_index"] = j.submap_id
             rec["node_trajectory"], rec["node_index"] = j.node_id
-            rec["found"] = int(found)
-            if found:
-                rec["score"] = score
-                # constraint_transform = ComputeSubmapPose(submap)^-1 * pose_estimate (:251-252)
-                rec["pose"] = _compose(_inverse(tuple(self._submaps[j.submap_id].local_pose)), pose)
-        records = self._allgather(local, mine, len(jobs), rank, world)
+            self._fill(rec, j, r)
+        records = self._exchange(local, owner, world)
         self.last_records = records
-        result = []
-        for rec in records:
-            if rec["found"]:
-                result.append(Constraint(
-                    (int(rec["submap_trajectory"]), int(rec["submap_index"])),
-                    (int(rec["node_trajectory"]), int(rec["node_index"])),
-                    tuple(float(v) for v in rec["pose"]),
-                    self.options.loop_closure_translation_weight,
-                    self.options.loop_closure_rotation_weight, "INTER_SUBMAP",
-                    float(rec["score"])))
+        result = [Constraint((int(r["submap_trajectory"]), int(r["submap_index"])),
+                             (int(r["node_trajectory"]), int(r["node_index"])),
+                             tuple(float(v) for v in r["pose"]),
+                             self.options.loop_closure_translation_weight,
+                             self.options.loop_closure_rotation_weight, "INTER_SUBMAP",
+                             float(r["score"])) for r in records if r["found"]]
         self._jobs = []
-        self._clouds = {}
+        self._constant_data = {}
         if hasattr(self.executor, "release_clouds"):
             self.executor.release_clouds()
         self.num_finished_nodes = self.num_started_nodes
@@ -359,44 +336,84 @@ class ConstraintBuilder2D:
         cb(result)
         return result
 
-    def _allgather(self, local, mine, total, rank, world):
-        """The path's single collective: fixed-size records, padded to the largest
-        shard, gathered to every rank and re-ordered into queue order."""
+    def _exchange(self, local, owner, world):
+        """The queue's single collective: every rank's records, padded to the largest shard,
+        gathered to every rank (ncclAllGather inside the library with a `context`, else
+        all_gather_into_tensor on the process group) and put back in queue order."""
         if world == 1:
             return local
-        counts = [sum(1 for j in self._jobs if self._submap_order[j.submap_id] % world == r)
-                  for r in range(world)]
-        cap = max(1, max(counts))
-        if self.ctx is not None:   # ncclAllGather inside the library
-            send = np.zeros(cap, RECORD_DTYPE)
-            send[:len(local)] = local
-            parts = self.ctx.allgather(send.tobytes())
-            allrec = np.stack([np.frombuffer(p, dtype=RECORD_DTYPE) for p in parts])
-            out = np.zeros(total, RECORD_DTYPE)
-            cursor = [0] * world
-            for i, j in enumerate(self._jobs):
-                r = self._submap_order[j.submap_id] % world
-                out[i] = allrec[r, cursor[r]]
-                cursor[r] += 1
-            return out
-        import torch
-        import torch.distributed as dist
-        backend = dist.get_backend(self.pg)
-        dev = torch.device("cuda", self.device) if backend == "nccl" else torch.device("cpu")
-        send = np.zeros(cap, RECORD_DTYPE)
+        cap = max(1, max(owner.count(r) for r in range(world)))
+        send = np.zeros(cap, local.dtype)
         send[:len(local)] = local
-        t_send = torch.from_numpy(send.view(np.uint8).reshape(-1).copy()).to(dev)
-        t_recv = torch.empty(world * cap * RECORD_DTYPE.itemsize, dtype=torch.uint8, device=dev)
-        dist.all_gather_into_tensor(t_recv, t_send, group=self.pg)
-        allrec = np.frombuffer(t_recv.cpu().numpy().tobytes(), dtype=RECORD_DTYPE).reshape(
-            world, cap)
-        out = np.zeros(total, RECORD_DTYPE)
+        if self.ctx is not None:
+            raw = b"".join(self.ctx.allgather(send.tobytes()))
+        else:
+            import torch
+            import torch.distributed as dist
+            dev = (torch.device("cuda", self.device) if dist.get_backend(self.pg) == "nccl"
+                   else torch.device("cpu"))
+            t_send = torch.from_numpy(send.view(np.uint8).reshape(-1).copy()).to(dev)
+            t_recv = torch.empty(world * send.nbytes, dtype=torch.uint8, device=dev)
+            dist.all_gather_into_tensor(t_recv, t_send, group=self.pg)
+            raw = t_recv.cpu().numpy().tobytes()
+        allrec = np.frombuffer(raw, dtype=local.dtype).reshape(world, cap)
+        out = np.zeros(len(owner), local.dtype)
         cursor = [0] * world
-        for i, j in enumerate(self._jobs):
-            r = self._submap_order[j.submap_id] % world
+        for i, r in enumerate(owner):
             out[i] = allrec[r, cursor[r]]
             cursor[r] += 1
         return out
+
+
+class ConstraintBuilder2D(_ConstraintQueue):
+    """constraint_builder_2d.h:60-107.  `executor.run(jobs, submaps, clouds)` does the
+    matching (CudaExecutor in production); `process_group` (torch.distributed) turns
+    on submap-major sharding + the single all_gather of constraint records."""
+
+    RECORD = RECORD_DTYPE
+
+    def __init__(self, options, executor=None, process_group=None, device=0, context=None):
+        """`context` (scan_matching.MultiGpuContext): the library's own NCCL communicator;
+        when given, the single all-gather runs inside libcsm_b200.so (csm_ctx_allgather ->
+        ncclAllGather) and no torch.distributed group is needed."""
+        super().__init__(options,
+                         executor if executor is not None else CudaExecutor(options, device),
+                         process_group, device, context)
+
+    def _is_device(self, submap):
+        """_is_device_grid against the executor's device: ValueError for a TSDF handle or one
+        on another device."""
+        return _is_device_grid(submap.grid, getattr(self.executor, "device", self.device))
+
+    def MaybeAddConstraint(self, submap_id, submap, node_id, constant_data,
+                           initial_relative_pose):
+        """constraint_builder_2d.cc:77-112.  constant_data is the node's
+        filtered_gravity_aligned_point_cloud (N x 3 float32)."""
+        self._check_submap(submap)
+        if math.hypot(initial_relative_pose[0], initial_relative_pose[1]) > \
+                self.options.max_constraint_distance:
+            return
+        if not self._pulse(submap_id):
+            return
+        key = self._register(submap_id, submap, constant_data)
+        initial_pose = _compose(tuple(submap.local_pose), tuple(initial_relative_pose))  # :196-197
+        self._jobs.append(_Job(submap_id, node_id, key, initial_pose, False,
+                               self.options.min_score))
+
+    def MaybeAddGlobalConstraint(self, submap_id, submap, node_id, constant_data):
+        """constraint_builder_2d.cc:114-137."""
+        self._check_submap(submap)
+        key = self._register(submap_id, submap, constant_data)
+        self._jobs.append(_Job(submap_id, node_id, key, (0.0, 0.0, 0.0), True,
+                               self.options.global_localization_min_score))
+
+    def _fill(self, rec, job, result):
+        found, score, pose = result
+        rec["found"] = int(found)
+        if found:
+            rec["score"] = score
+            # constraint_transform = ComputeSubmapPose(submap)^-1 * pose_estimate (:251-252)
+            rec["pose"] = _compose(_inverse(tuple(self._submaps[job.submap_id].local_pose)), pose)
 
 
 # ===========================================================================
@@ -567,47 +584,31 @@ class CudaExecutor3D:
         return out
 
 
-class ConstraintBuilder3D:
+class ConstraintBuilder3D(_ConstraintQueue):
     """constraint_builder_3d.h:59-114 over the 3D engine; same sharding / single
     all_gather scheme as ConstraintBuilder2D.  Constraint poses are the fast
     matcher's pose_estimate (submap <- node); with
     ConstraintBuilderOptions3D.ceres_scan_matcher_options_3d set they are first refined as
     constraint_builder_3d.cc:265-275 does (one csm_ceres_match3d_batch launch per drain)."""
 
-    def __init__(self, options, executor=None, process_group=None, device=0):
-        self.options = options
-        self.executor = executor if executor is not None else CudaExecutor3D(options, device)
-        self.pg = process_group
-        self.device = device
-        self._jobs, self._submaps, self._nodes = [], {}, {}
-        self._submap_order, self._samplers = {}, {}
-        self._when_done = None
-        self.num_started_nodes = 0
-        self.num_finished_nodes = 0
-        self.last_records = None
+    RECORD = RECORD3D_DTYPE
 
-    def _register(self, submap_id, submap, constant_data):
-        if self.pg is not None and _is_device_submap(submap):
-            import torch.distributed as dist
-            if dist.get_world_size(self.pg) > 1:
-                # the queue is sharded submap-major, but a device submap stays on the GPU that
-                # inserted it
-                raise ValueError("device-resident submaps are not sharded over several ranks")
-        self._submaps[submap_id] = submap
-        self._submap_order.setdefault(submap_id, len(self._submap_order))
-        key = id(constant_data)
-        self._nodes[key] = constant_data
-        return key
+    def __init__(self, options, executor=None, process_group=None, device=0):
+        super().__init__(options,
+                         executor if executor is not None else CudaExecutor3D(options, device),
+                         process_group, device)
+
+    def _is_device(self, submap):
+        return _is_device_submap(submap)
 
     def MaybeAddConstraint(self, submap_id, submap, node_id, constant_data, global_node_pose,
                            global_submap_pose):
         """constraint_builder_3d.cc:79-114; poses are [tx,ty,tz,qw,qx,qy,qz]."""
+        self._check_submap(submap)
         d = np.asarray(global_node_pose[:3], float) - np.asarray(global_submap_pose[:3], float)
         if float(np.sqrt((d * d).sum())) > self.options.max_constraint_distance:
             return
-        sampler = self._samplers.setdefault(submap_id,
-                                            FixedRatioSampler(self.options.sampling_ratio))
-        if not sampler.Pulse():
+        if not self._pulse(submap_id):
             return
         key = self._register(submap_id, submap, constant_data)
         self._jobs.append(_Job3(submap_id, node_id, key, tuple(global_node_pose),
@@ -616,79 +617,16 @@ class ConstraintBuilder3D:
     def MaybeAddGlobalConstraint(self, submap_id, submap, node_id, constant_data,
                                  global_node_rotation, global_submap_rotation):
         """constraint_builder_3d.cc:116-142; rotations are [qw,qx,qy,qz]."""
+        self._check_submap(submap)
         key = self._register(submap_id, submap, constant_data)
         self._jobs.append(_Job3(submap_id, node_id, key, (0, 0, 0) + tuple(global_node_rotation),
                                 (0, 0, 0) + tuple(global_submap_rotation), True,
                                 self.options.global_localization_min_score))
 
-    def NotifyEndOfNode(self):
-        self.num_started_nodes += 1
-
-    def GetNumFinishedNodes(self):
-        return self.num_finished_nodes
-
-    def DeleteScanMatcher(self, submap_id):
-        if hasattr(self.executor, "delete_matcher"):
-            self.executor.delete_matcher(submap_id)
-        self._samplers.pop(submap_id, None)
-
-    def WhenDone(self, callback):
-        if self._when_done is not None:
-            raise RuntimeError("WhenDone called twice")
-        self._when_done = callback
-        rank, world = (0, 1)
-        if self.pg is not None:
-            import torch.distributed as dist
-            rank, world = dist.get_rank(self.pg), dist.get_world_size(self.pg)
-        jobs = self._jobs
-        mine = [i for i, j in enumerate(jobs) if self._submap_order[j.submap_id] % world == rank]
-        out = self.executor.run([jobs[i] for i in mine], self._submaps, self._nodes)
-        local = np.zeros(len(mine), RECORD3D_DTYPE)
-        for rec, i, r in zip(local, mine, out):
-            j = jobs[i]
-            rec["submap_trajectory"], rec["submap_index"] = j.submap_id
-            rec["node_trajectory"], rec["node_index"] = j.node_id
-            if r is not None:
-                rec["found"] = 1
-                rec["score"] = r["score"]
-                rec["pose"] = r["pose_estimate"]
-                rec["rotational_score"] = r["rotational_score"]
-                rec["low_resolution_score"] = r["low_resolution_score"]
-        records = _allgather_records(self, local, len(jobs), rank, world, RECORD3D_DTYPE)
-        self.last_records = records
-        result = [Constraint((int(r["submap_trajectory"]), int(r["submap_index"])),
-                             (int(r["node_trajectory"]), int(r["node_index"])),
-                             tuple(float(v) for v in r["pose"]),
-                             self.options.loop_closure_translation_weight,
-                             self.options.loop_closure_rotation_weight, "INTER_SUBMAP",
-                             float(r["score"])) for r in records if r["found"]]
-        self._jobs, self._nodes = [], {}
-        self.num_finished_nodes = self.num_started_nodes
-        cb, self._when_done = self._when_done, None
-        cb(result)
-        return result
-
-
-def _allgather_records(builder, local, total, rank, world, dtype):
-    """Shared single-collective exchange (see ConstraintBuilder2D._allgather)."""
-    if world == 1:
-        return local
-    import torch
-    import torch.distributed as dist
-    owner = [builder._submap_order[j.submap_id] % world for j in builder._jobs]
-    counts = [owner.count(r) for r in range(world)]
-    cap = max(1, max(counts))
-    backend = dist.get_backend(builder.pg)
-    dev = torch.device("cuda", builder.device) if backend == "nccl" else torch.device("cpu")
-    send = np.zeros(cap, dtype)
-    send[:len(local)] = local
-    t_send = torch.from_numpy(send.view(np.uint8).reshape(-1).copy()).to(dev)
-    t_recv = torch.empty(world * cap * dtype.itemsize, dtype=torch.uint8, device=dev)
-    dist.all_gather_into_tensor(t_recv, t_send, group=builder.pg)
-    allrec = np.frombuffer(t_recv.cpu().numpy().tobytes(), dtype=dtype).reshape(world, cap)
-    out = np.zeros(total, dtype)
-    cursor = [0] * world
-    for i, r in enumerate(owner):
-        out[i] = allrec[r, cursor[r]]
-        cursor[r] += 1
-    return out
+    def _fill(self, rec, job, result):
+        if result is not None:
+            rec["found"] = 1
+            rec["score"] = result["score"]
+            rec["pose"] = result["pose_estimate"]
+            rec["rotational_score"] = result["rotational_score"]
+            rec["low_resolution_score"] = result["low_resolution_score"]

@@ -11,6 +11,7 @@
 #include <dlfcn.h>
 #include <nccl.h>
 
+#include <algorithm>
 #include <chrono>
 
 #include "engine2d.cuh"
@@ -81,6 +82,66 @@ struct csm_ctx {
 };
 
 static_assert(sizeof(ncclUniqueId) == CSM_COMM_ID_BYTES, "CSM_COMM_ID_BYTES");
+
+namespace {
+// What both csm_cb_batch*_run do with the WHOLE queue (identical on every rank): job j belongs
+// to submap submap_of(jobs[j]) and runs on rank submap_owner[that submap] (NULL => submap %
+// world_size); `run(jobs, n, results)` runs this rank's share locally.  With more than one rank,
+// ONE allgather of fixed-size {job index, result} records, padded to the largest shard, then
+// leaves results[0 .. num_jobs) in job order on every rank.
+template <typename Job, typename Result, typename SubmapOf, typename HasSubmap, typename Run>
+csm_status ShardedQueue(csm_ctx* ctx, const Job* jobs, int32_t num_jobs, int32_t num_submaps,
+                        const int32_t* submap_owner, Result* results, csm_stats* stats,
+                        SubmapOf submap_of, const char* bad_index, HasSubmap has_submap,
+                        const char* not_held, Run run) {
+  if (stats) std::memset(stats, 0, sizeof(*stats));
+  if (num_jobs == 0) return CSM_OK;
+  const int W = ctx->world;
+  std::vector<int> mine;
+  std::vector<int> per_rank(W, 0);
+  for (int j = 0; j < num_jobs; ++j) {
+    const int s = submap_of(jobs[j]);
+    CSM_REQUIRE(s >= 0 && s < num_submaps, bad_index);
+    const int o = submap_owner ? submap_owner[s] : s % W;
+    CSM_REQUIRE(o >= 0 && o < W, "submap owner out of range");
+    ++per_rank[o];
+    if (o == ctx->rank) mine.push_back(j);
+  }
+  // local searches
+  std::vector<Job> my_jobs(mine.size());
+  std::vector<Result> my_results(mine.size());
+  for (size_t i = 0; i < mine.size(); ++i) {
+    my_jobs[i] = jobs[mine[i]];
+    CSM_REQUIRE(has_submap(submap_of(my_jobs[i])), not_held);
+  }
+  if (!mine.empty())
+    CSM_TRY(run(my_jobs.data(), static_cast<int32_t>(my_jobs.size()), my_results.data()));
+  if (W == 1) {
+    for (size_t i = 0; i < mine.size(); ++i) results[mine[i]] = my_results[i];
+    return CSM_OK;
+  }
+  const int max_per_rank = *std::max_element(per_rank.begin(), per_rank.end());
+  struct Record { int32_t job; int32_t pad; Result r; };
+  static_assert(sizeof(Record) == 8 + sizeof(Result), "record layout");
+  std::vector<Record> send(static_cast<size_t>(max_per_rank));
+  for (size_t i = 0; i < send.size(); ++i) {
+    send[i].job = i < mine.size() ? mine[i] : -1;
+    send[i].pad = 0;
+    if (i < mine.size()) send[i].r = my_results[i];
+    else std::memset(&send[i].r, 0, sizeof(Result));
+  }
+  std::vector<Record> recv(static_cast<size_t>(max_per_rank) * W);
+  const auto t0 = std::chrono::steady_clock::now();
+  CSM_TRY(csm_ctx_allgather(ctx, send.data(), static_cast<int64_t>(sizeof(Record)) * max_per_rank,
+                            recv.data()));
+  if (stats)
+    stats->collective_ms +=
+        std::chrono::duration<float, std::milli>(std::chrono::steady_clock::now() - t0).count();
+  for (const Record& rec : recv)
+    if (rec.job >= 0 && rec.job < num_jobs) results[rec.job] = rec.r;
+  return CSM_OK;
+}
+}  // namespace
 
 extern "C" {
 
@@ -176,64 +237,21 @@ csm_status csm_cb_batch2d_run(csm_ctx* ctx, const csm_stack2d* const* stacks, in
                               double angular_window, csm_result2d* results, csm_stats* stats) {
   CSM_REQUIRE(ctx && stacks && clouds && jobs && results, "null pointer");
   CSM_REQUIRE(num_jobs >= 0 && num_stacks >= 1 && num_clouds >= 1, "sizes");
-  if (stats) std::memset(stats, 0, sizeof(*stats));
-  if (num_jobs == 0) return CSM_OK;
-  const int W = ctx->world;
-  auto owner = [&](int stack) { return submap_owner ? submap_owner[stack] : stack % W; };
-  std::vector<int> mine;
-  std::vector<int> per_rank(W, 0);
-  for (int j = 0; j < num_jobs; ++j) {
-    CSM_REQUIRE(jobs[j].stack_index >= 0 && jobs[j].stack_index < num_stacks, "stack index");
-    const int o = owner(jobs[j].stack_index);
-    CSM_REQUIRE(o >= 0 && o < W, "submap owner out of range");
-    ++per_rank[o];
-    if (o == ctx->rank) mine.push_back(j);
-  }
-  int max_per_rank = 0;
-  for (int r = 0; r < W; ++r) max_per_rank = std::max(max_per_rank, per_rank[r]);
-  // local searches
-  std::vector<csm_job2d> my_jobs(mine.size());
-  std::vector<csm_result2d> my_results(mine.size());
-  for (size_t i = 0; i < mine.size(); ++i) {
-    my_jobs[i] = jobs[mine[i]];
-    CSM_REQUIRE(stacks[my_jobs[i].stack_index] != nullptr, "an owned submap has no stack");
-  }
-  if (!mine.empty()) {
-    // the batch entry needs stacks[0] for its device: pass a dense view of owned stacks
-    std::vector<const csm_stack2d*> dense(num_stacks, nullptr);
-    const csm_stack2d* any = nullptr;
-    for (int s = 0; s < num_stacks; ++s)
-      if (stacks[s]) { dense[s] = stacks[s]; any = stacks[s]; }
-    for (int s = 0; s < num_stacks; ++s)
-      if (!dense[s]) dense[s] = any;  // never dereferenced: no local job points at it
-    CSM_TRY(csm_match2d_batch(dense.data(), num_stacks, clouds, num_clouds, my_jobs.data(),
-                              static_cast<int32_t>(my_jobs.size()), linear_window,
-                              angular_window, my_results.data(), stats));
-  }
-  if (W == 1) {
-    for (size_t i = 0; i < mine.size(); ++i) results[mine[i]] = my_results[i];
-    return CSM_OK;
-  }
-  // ONE allgather of fixed-size records {job index, result}, padded to the largest shard
-  struct Record { int32_t job; int32_t pad; csm_result2d r; };
-  static_assert(sizeof(Record) == 56, "record layout");
-  std::vector<Record> send(static_cast<size_t>(max_per_rank));
-  for (size_t i = 0; i < send.size(); ++i) {
-    send[i].job = i < mine.size() ? mine[i] : -1;
-    send[i].pad = 0;
-    if (i < mine.size()) send[i].r = my_results[i];
-    else std::memset(&send[i].r, 0, sizeof(csm_result2d));
-  }
-  std::vector<Record> recv(static_cast<size_t>(max_per_rank) * W);
-  const auto t0 = std::chrono::steady_clock::now();
-  CSM_TRY(csm_ctx_allgather(ctx, send.data(), static_cast<int64_t>(sizeof(Record)) * max_per_rank,
-                            recv.data()));
-  if (stats)
-    stats->collective_ms +=
-        std::chrono::duration<float, std::milli>(std::chrono::steady_clock::now() - t0).count();
-  for (const Record& rec : recv)
-    if (rec.job >= 0 && rec.job < num_jobs) results[rec.job] = rec.r;
-  return CSM_OK;
+  return ShardedQueue(
+      ctx, jobs, num_jobs, num_stacks, submap_owner, results, stats,
+      [](const csm_job2d& j) { return j.stack_index; }, "stack index",
+      [&](int s) { return stacks[s] != nullptr; }, "an owned submap has no stack",
+      [&](const csm_job2d* my_jobs, int32_t n, csm_result2d* my_results) {
+        // the batch entry needs stacks[0] for its device: pass a dense view of owned stacks
+        std::vector<const csm_stack2d*> dense(num_stacks, nullptr);
+        const csm_stack2d* any = nullptr;
+        for (int s = 0; s < num_stacks; ++s)
+          if (stacks[s]) { dense[s] = stacks[s]; any = stacks[s]; }
+        for (int s = 0; s < num_stacks; ++s)
+          if (!dense[s]) dense[s] = any;  // never dereferenced: no local job points at it
+        return csm_match2d_batch(dense.data(), num_stacks, clouds, num_clouds, my_jobs, n,
+                                 linear_window, angular_window, my_results, stats);
+      });
 }
 
 // The sharded 3D queue (constraint_builder_3d.cc:107-116): same ownership rule on
@@ -245,50 +263,14 @@ csm_status csm_cb_batch3d_run(csm_ctx* ctx, const csm_matcher3d* const* matchers
                               csm_result3d* results, csm_stats* stats) {
   CSM_REQUIRE(ctx && matchers && nodes && jobs && results, "null pointer");
   CSM_REQUIRE(num_jobs >= 0 && num_matchers >= 1 && num_nodes >= 1, "sizes");
-  if (stats) std::memset(stats, 0, sizeof(*stats));
-  if (num_jobs == 0) return CSM_OK;
-  const int W = ctx->world;
-  auto owner = [&](int m) { return submap_owner ? submap_owner[m] : m % W; };
-  std::vector<int> mine;
-  std::vector<int> per_rank(W, 0);
-  for (int j = 0; j < num_jobs; ++j) {
-    CSM_REQUIRE(jobs[j].matcher_index >= 0 && jobs[j].matcher_index < num_matchers,
-                "matcher index");
-    const int o = owner(jobs[j].matcher_index);
-    CSM_REQUIRE(o >= 0 && o < W, "submap owner out of range");
-    ++per_rank[o];
-    if (o == ctx->rank) mine.push_back(j);
-  }
-  int max_per_rank = 0;
-  for (int r = 0; r < W; ++r) max_per_rank = std::max(max_per_rank, per_rank[r]);
-  std::vector<csm_job3d> my_jobs(mine.size());
-  std::vector<csm_result3d> my_results(mine.size());
-  for (size_t i = 0; i < mine.size(); ++i) {
-    my_jobs[i] = jobs[mine[i]];
-    CSM_REQUIRE(matchers[my_jobs[i].matcher_index] != nullptr, "an owned submap has no matcher");
-  }
-  if (!mine.empty())
-    CSM_TRY(csm_match3d_batch(matchers, num_matchers, nodes, num_nodes, my_jobs.data(),
-                              static_cast<int32_t>(my_jobs.size()), max_concurrency,
-                              my_results.data(), stats));
-  if (W == 1) {
-    for (size_t i = 0; i < mine.size(); ++i) results[mine[i]] = my_results[i];
-    return CSM_OK;
-  }
-  struct Record { int32_t job; int32_t pad; csm_result3d r; };
-  std::vector<Record> send(static_cast<size_t>(max_per_rank));
-  for (size_t i = 0; i < send.size(); ++i) {
-    send[i].job = i < mine.size() ? mine[i] : -1;
-    send[i].pad = 0;
-    if (i < mine.size()) send[i].r = my_results[i];
-    else std::memset(&send[i].r, 0, sizeof(csm_result3d));
-  }
-  std::vector<Record> recv(static_cast<size_t>(max_per_rank) * W);
-  CSM_TRY(csm_ctx_allgather(ctx, send.data(), static_cast<int64_t>(sizeof(Record)) * max_per_rank,
-                            recv.data()));
-  for (const Record& rec : recv)
-    if (rec.job >= 0 && rec.job < num_jobs) results[rec.job] = rec.r;
-  return CSM_OK;
+  return ShardedQueue(
+      ctx, jobs, num_jobs, num_matchers, submap_owner, results, stats,
+      [](const csm_job3d& j) { return j.matcher_index; }, "matcher index",
+      [&](int m) { return matchers[m] != nullptr; }, "an owned submap has no matcher",
+      [&](const csm_job3d* my_jobs, int32_t n, csm_result3d* my_results) {
+        return csm_match3d_batch(matchers, num_matchers, nodes, num_nodes, my_jobs, n,
+                                 max_concurrency, my_results, stats);
+      });
 }
 
 }  // extern "C"
