@@ -7,6 +7,7 @@
 #include <cstring>
 
 #include "constraint_builder_b200.h"
+#include "pose_graph_trimmer_b200.h"
 #include "scan_matchers_b200.h"
 #include "voxel_filter_b200.h"
 
@@ -76,6 +77,221 @@ static int HostOnlyChecks() {
   std::printf("adapter_selftest: host-only checks passed\n");
   return 0;
 }
+
+// ---- OverlappingSubmapsTrimmer2D: the reference's overlapping_submaps_trimmer_2d_test.cc cases
+// on device grids, and one random map whose inputs and outcome are printed ----
+namespace trimmer_cases {
+using mapping::NodeId;
+using mapping::PoseGraphInterface;
+using mapping::SubmapId;
+using mapping::scan_matching::DeviceGrid2D;
+
+transform::Rigid3d Embed3D(double x, double y, double theta) {
+  return transform::Rigid3d({{x, y, 0.}}, transform::Quaterniond{std::cos(theta / 2), 0., 0.,
+                                                                  std::sin(theta / 2)});
+}
+
+class FakeTrimmable : public mapping::Trimmable {
+ public:
+  mapping::MapById<SubmapId, PoseGraphInterface::SubmapData> GetOptimizedSubmapData()
+      const override {
+    return submap_data;
+  }
+  const mapping::MapById<NodeId, mapping::TrajectoryNode>& GetTrajectoryNodes() const override {
+    return nodes;
+  }
+  const std::vector<PoseGraphInterface::Constraint>& GetConstraints() const override {
+    return constraints;
+  }
+  void TrimSubmap(const SubmapId& id) override { trimmed.push_back(id); }
+
+  // AddSquareSubmap: num_cells x num_cells cells of value 1, resolution 1, max = corner
+  void AddSquareSubmap(const transform::Rigid3d& global, const transform::Rigid3d& local,
+                       double corner_x, double corner_y, int index, int num_cells,
+                       bool finished) {
+    const mapping::Grid2D grid(
+        mapping::MapLimits(1.0, corner_x, corner_y, mapping::CellLimits{num_cells, num_cells}),
+        0.1f, 0.9f, std::vector<uint16_t>(num_cells * num_cells, 1));
+    grids[SubmapId{0, index}] = std::make_shared<DeviceGrid2D>(grid);
+    submap_data.Insert(SubmapId{0, index},
+                       {std::make_shared<const mapping::Submap2D>(local, finished), global});
+  }
+  void AddNode(int index, int64_t time) {
+    mapping::TrajectoryNode n;
+    n.time_.ticks = time;
+    nodes.Insert(NodeId{0, index}, n);
+  }
+  void AddConstraint(int submap, int node, bool intra) {
+    PoseGraphInterface::Constraint c;
+    c.submap_id = SubmapId{0, submap};
+    c.node_id = NodeId{0, node};
+    c.tag = intra ? PoseGraphInterface::Constraint::INTRA_SUBMAP
+                  : PoseGraphInterface::Constraint::INTER_SUBMAP;
+    constraints.push_back(c);
+  }
+  mapping::OverlappingSubmapsTrimmer2D::DeviceGridOf DeviceGrids() {
+    return [this](const SubmapId& id, const mapping::Submap2D&) -> const DeviceGrid2D& {
+      return *grids.at(id);
+    };
+  }
+  std::string Trimmed() const {
+    std::string s;
+    for (const SubmapId& id : trimmed) s += std::to_string(id.submap_index) + ",";
+    return s;
+  }
+
+  mapping::MapById<SubmapId, PoseGraphInterface::SubmapData> submap_data;
+  mapping::MapById<NodeId, mapping::TrajectoryNode> nodes;
+  std::vector<PoseGraphInterface::Constraint> constraints;
+  std::vector<SubmapId> trimmed;
+  std::map<SubmapId, std::shared_ptr<DeviceGrid2D>> grids;
+};
+
+int Expect(const char* name, const FakeTrimmable& g, const char* want) {
+  const bool ok = g.Trimmed() == want;
+  std::printf("RESULT trimmer2d_%s %s %s\n", name, ok ? "ok" : "FAILED", g.Trimmed().c_str());
+  return ok ? 0 : 1;
+}
+
+void TwoOverlapping(FakeTrimmable* g, bool finished0) {
+  const transform::Rigid3d id;
+  g->AddSquareSubmap(id, id, 1., 1., 0, 1, finished0);
+  g->AddSquareSubmap(id, id, 1., 1., 1, 1, true);
+  g->AddNode(0, 1000);
+  g->AddNode(1, 2000);
+  g->AddConstraint(0, 0, true);
+  g->AddConstraint(1, 1, true);
+}
+
+int Run() {
+  using Trimmer = mapping::OverlappingSubmapsTrimmer2D;
+  const transform::Rigid3d id;
+  int failed = 0;
+  {
+    FakeTrimmable g;
+    Trimmer t(1, 0, 0, g.DeviceGrids());
+    t.Trim(&g);
+    failed += Expect("EmptyPoseGraph", g, "");
+  }
+  {
+    FakeTrimmable g;
+    TwoOverlapping(&g, true);
+    Trimmer t(1, 0, 0, g.DeviceGrids());
+    t.Trim(&g);
+    failed += Expect("TrimOneOfTwoOverlappingSubmaps", g, "0,");
+  }
+  {
+    FakeTrimmable g;
+    TwoOverlapping(&g, true);
+    Trimmer t(1, 0, 2, g.DeviceGrids());
+    t.Trim(&g);
+    failed += Expect("TestMinAddedSubmapsCountParam_first", g, "");
+    g.AddSquareSubmap(id, id, 1., 1., 2, 1, true);
+    g.AddNode(2, 3000);
+    g.AddConstraint(2, 2, true);
+    t.Trim(&g);
+    failed += Expect("TestMinAddedSubmapsCountParam", g, "0,1,");
+  }
+  {
+    FakeTrimmable g;
+    TwoOverlapping(&g, false);
+    Trimmer t(1, 0, 0, g.DeviceGrids());
+    t.Trim(&g);
+    failed += Expect("DoNotTrimUnfinishedSubmap", g, "");
+  }
+  {
+    FakeTrimmable g;
+    g.AddSquareSubmap(id, id, 1., 1., 0, 1, true);
+    g.AddSquareSubmap(id, id, 1., 1., 1, 1, true);
+    g.AddNode(0, 1000);
+    g.AddNode(1, 2000);
+    g.AddNode(2, 3000);
+    g.AddConstraint(0, 0, false);
+    g.AddConstraint(0, 2, true);
+    g.AddConstraint(1, 1, true);
+    Trimmer t(1, 0, 0, g.DeviceGrids());
+    t.Trim(&g);
+    failed += Expect("UseOnlyIntraSubmapsToComputeFreshness", g, "1,");
+  }
+  {
+    FakeTrimmable g;
+    g.AddSquareSubmap(id, id, 1., 1., 0, 2, true);
+    g.AddSquareSubmap(Embed3D(1., 1., 0.), id, 1., 1., 1, 2, true);
+    g.AddNode(0, 1000);
+    g.AddNode(1, 2000);
+    g.AddConstraint(0, 0, true);
+    g.AddConstraint(1, 1, true);
+    Trimmer t(1, 4, 0, g.DeviceGrids());
+    t.Trim(&g);
+    failed += Expect("TrimSubmapWithLowCoveredCellsCount", g, "0,");
+  }
+  {
+    FakeTrimmable g;
+    g.AddSquareSubmap(id, id, 1., 1., 0, 1, true);
+    const transform::Rigid3d transform = Embed3D(1., 1., M_PI / 2);
+    g.AddSquareSubmap(transform, transform, 1., 1., 1, 1, true);
+    g.AddNode(0, 1000);
+    g.AddNode(1, 2000);
+    g.AddConstraint(0, 0, true);
+    g.AddConstraint(1, 1, true);
+    Trimmer t(1, 0, 0, g.DeviceGrids());
+    t.Trim(&g);
+    failed += Expect("TestTransformations", g, "0,");
+  }
+  {
+    // 40 random 60 x 60 submaps at 5 cm along a circle with random yaw, a few shared times
+    FakeTrimmable g;
+    uint64_t state = 12345;
+    auto next = [&state]() {
+      state = state * 6364136223846793005ull + 1442695040888963407ull;
+      return static_cast<double>(state >> 11) / 9007199254740992.;
+    };
+    const int n = 40, size = 60;
+    std::vector<std::vector<uint16_t>> cells(n);
+    std::vector<transform::Rigid3d> composed(n);
+    std::vector<double> limits(3 * n);
+    for (int i = 0; i < n; ++i) {
+      const double a = 2 * M_PI * i / 12, x = 1.0 * std::cos(a), y = 1.0 * std::sin(a);
+      cells[i].resize(size * size);
+      for (auto& c : cells[i]) c = next() < 0.7 ? static_cast<uint16_t>(1 + next() * 32766) : 0;
+      const double mx = x + size / 2 * 0.05, my = y + size / 2 * 0.05;
+      limits[3 * i] = mx;
+      limits[3 * i + 1] = my;
+      limits[3 * i + 2] = 0.05;
+      const mapping::Grid2D grid(mapping::MapLimits(0.05, mx, my, mapping::CellLimits{size, size}),
+                                 0.1f, 0.9f, cells[i]);
+      g.grids[SubmapId{0, i}] = std::make_shared<DeviceGrid2D>(grid);
+      const transform::Rigid3d local = Embed3D(x, y, 2 * M_PI * next());
+      const transform::Rigid3d global = Embed3D(x + 0.1 * next(), y - 0.1 * next(), 2 * M_PI * next());
+      g.submap_data.Insert(SubmapId{0, i},
+                           {std::make_shared<const mapping::Submap2D>(local, true), global});
+      composed[i] = global * local.inverse();
+      g.AddNode(i, i % 9 == 4 ? 1000 * (i - 1) : 1000 * i);
+      g.AddConstraint(i, i, true);
+    }
+    Trimmer t(2, 0.5, 0, g.DeviceGrids());
+    t.Trim(&g);
+    // the inputs of the coverage pass and its outcome, which the GPU test checks against the
+    // CPU restatement (tests/trimmer2d_oracle.cc)
+    for (int i = 0; i < n; ++i) {
+      const auto& tr = composed[i].translation();
+      const auto& q = composed[i].rotation();
+      std::printf("RESULT trimmer2d_random_submap %d %lld %.17g %.17g %.17g %.17g %.17g %.17g "
+                  "%.17g %.17g %.17g %.17g %d ",
+                  i, static_cast<long long>(i % 9 == 4 ? 1000 * (i - 1) : 1000 * i),
+                  limits[3 * i], limits[3 * i + 1], limits[3 * i + 2], tr.x(), tr.y(), tr.z(),
+                  q.w(), q.x(), q.y(), q.z(), size);
+      for (uint16_t c : cells[i]) std::printf("%04x", c);
+      std::printf("\n");
+    }
+    std::printf("RESULT trimmer2d_random_map %s\n", g.Trimmed().c_str());
+    std::printf("RESULT trimmer2d_random_map_stats %lld %lld\n",
+                static_cast<long long>(t.last_stats().entries),
+                static_cast<long long>(t.last_stats().coverage_cells));
+  }
+  return failed;
+}
+}  // namespace trimmer_cases
 
 int main() {
   if (HostOnlyChecks() != 0) {
@@ -779,5 +995,6 @@ int main() {
     for (float v : b.intensities()) std::printf(" %d", int(v));
     std::printf("\n");
   }
+  if (trimmer_cases::Run() != 0) return 1;
   return 0;
 }

@@ -12,6 +12,7 @@
 #include <cmath>
 #include <cstdint>
 #include <functional>
+#include <map>
 #include <memory>
 #include <utility>
 #include <vector>
@@ -189,7 +190,35 @@ class Rigid3d {
   Rigid3d(const Vector& t, const Quaterniond& q) : t_(t), q_(q) {}
   const Vector& translation() const { return t_; }
   const Quaterniond& rotation() const { return q_; }
+  // :159-163 and :184-189, with Eigen's Quaternion * Vector3 (_transformVector) and
+  // quaternion product in their scalar order
+  Rigid3d inverse() const {
+    const Quaterniond q{q_.w_, -q_.x_, -q_.y_, -q_.z_};
+    const Vector t = Rotate(q, t_);
+    return Rigid3d({{-t.v[0], -t.v[1], -t.v[2]}}, q);
+  }
+  friend Rigid3d operator*(const Rigid3d& a, const Rigid3d& b) {
+    Vector t = Rotate(a.q_, b.t_);
+    for (int k = 0; k < 3; ++k) t.v[k] = t.v[k] + a.t_.v[k];
+    const Quaterniond& p = a.q_;
+    const Quaterniond& q = b.q_;
+    const double w = p.w_ * q.w_ - p.x_ * q.x_ - p.y_ * q.y_ - p.z_ * q.z_;
+    const double x = p.w_ * q.x_ + p.x_ * q.w_ + p.y_ * q.z_ - p.z_ * q.y_;
+    const double y = p.w_ * q.y_ + p.y_ * q.w_ + p.z_ * q.x_ - p.x_ * q.z_;
+    const double z = p.w_ * q.z_ + p.z_ * q.w_ + p.x_ * q.y_ - p.y_ * q.x_;
+    const double n = std::sqrt(w * w + x * x + y * y + z * z);
+    return Rigid3d(t, Quaterniond{w / n, x / n, y / n, z / n});
+  }
  private:
+  static Vector Rotate(const Quaterniond& q, const Vector& c) {
+    const double* v = c.v;
+    double uv[3] = {q.y_ * v[2] - q.z_ * v[1], q.z_ * v[0] - q.x_ * v[2], q.x_ * v[1] - q.y_ * v[0]};
+    for (double& u : uv) u += u;
+    const double x[3] = {q.y_ * uv[2] - q.z_ * uv[1], q.z_ * uv[0] - q.x_ * uv[2],
+                         q.x_ * uv[1] - q.y_ * uv[0]};
+    return Vector{{v[0] + q.w_ * uv[0] + x[0], v[1] + q.w_ * uv[1] + x[1],
+                   v[2] + q.w_ * uv[2] + x[2]}};
+  }
   Vector t_;
   Quaterniond q_;
 };
@@ -525,12 +554,20 @@ class Submap2D {
  public:
   Submap2D(const Grid2D* grid, const transform::Rigid2d& local_pose_2d)
       : grid_(grid), local_pose_2d_(local_pose_2d) {}
+  // what OverlappingSubmapsTrimmer2D reads (mapping/submaps.h:61-80): local_pose() and
+  // insertion_finished(); the grid lives on the device
+  Submap2D(const transform::Rigid3d& local_pose, bool insertion_finished)
+      : grid_(nullptr), local_pose_(local_pose), insertion_finished_(insertion_finished) {}
   const Grid2D* grid() const { return grid_; }
   // stands for transform::Project2D(local_pose()) = ComputeSubmapPose (submap_2d.h, constraint_builder_2d.cc:48-50)
   const transform::Rigid2d& local_pose_2d() const { return local_pose_2d_; }
+  const transform::Rigid3d& local_pose() const { return local_pose_; }
+  bool insertion_finished() const { return insertion_finished_; }
  private:
   const Grid2D* grid_;
   transform::Rigid2d local_pose_2d_;
+  transform::Rigid3d local_pose_;
+  bool insertion_finished_ = false;
 };
 class Submap3D {
  public:
@@ -556,6 +593,10 @@ struct PoseGraphInterface {
     NodeId node_id;
     Pose pose;
     enum Tag { INTRA_SUBMAP, INTER_SUBMAP } tag;
+  };
+  struct SubmapData {   // :55-58
+    std::shared_ptr<const Submap2D> submap;
+    transform::Rigid3d pose;
   };
 };
 namespace constraints {
@@ -588,6 +629,69 @@ struct ConstraintBuilderOptions {
 };
 }  // namespace proto
 }  // namespace constraints
+
+// mapping/id.h:194-428: the read-only part of MapById that the trimmer uses (ordered iteration
+// with .id and .data, size(), Contains(), at()).
+template <typename IdType, typename DataType>
+class MapById {
+ public:
+  struct IdDataReference {
+    const IdType& id;
+    const DataType& data;
+  };
+  class ConstIterator {
+   public:
+    explicit ConstIterator(typename std::map<IdType, DataType>::const_iterator it) : it_(it) {}
+    IdDataReference operator*() const { return IdDataReference{it_->first, it_->second}; }
+    ConstIterator& operator++() {
+      ++it_;
+      return *this;
+    }
+    bool operator!=(const ConstIterator& o) const { return it_ != o.it_; }
+   private:
+    typename std::map<IdType, DataType>::const_iterator it_;
+  };
+  void Insert(const IdType& id, const DataType& data) { map_[id] = data; }
+  void Trim(const IdType& id) { map_.erase(id); }
+  size_t size() const { return map_.size(); }
+  bool Contains(const IdType& id) const { return map_.count(id) != 0; }
+  const DataType& at(const IdType& id) const { return map_.at(id); }
+  ConstIterator begin() const { return ConstIterator(map_.begin()); }
+  ConstIterator end() const { return ConstIterator(map_.end()); }
+ private:
+  std::map<IdType, DataType> map_;
+};
+
+// mapping/trajectory_node.h:35-72: the node's time (common::Time, whose ticks the trimmer
+// reads through time_since_epoch().count()).
+struct TrajectoryNode {
+  struct Time {
+    struct Ticks {
+      int64_t ticks;
+      int64_t count() const { return ticks; }
+    };
+    int64_t ticks;
+    Ticks time_since_epoch() const { return Ticks{ticks}; }
+  };
+  Time time_;
+  Time time() const { return time_; }
+};
+
+// mapping/pose_graph_trimmer.h:27-61
+class Trimmable {
+ public:
+  virtual ~Trimmable() {}
+  virtual MapById<SubmapId, PoseGraphInterface::SubmapData> GetOptimizedSubmapData() const = 0;
+  virtual const MapById<NodeId, TrajectoryNode>& GetTrajectoryNodes() const = 0;
+  virtual const std::vector<PoseGraphInterface::Constraint>& GetConstraints() const = 0;
+  virtual void TrimSubmap(const SubmapId& submap_id) = 0;
+};
+class PoseGraphTrimmer {
+ public:
+  virtual ~PoseGraphTrimmer() {}
+  virtual void Trim(Trimmable* pose_graph) = 0;
+  virtual bool IsFinished() = 0;
+};
 }  // namespace mapping
 }  // namespace cartographer
 

@@ -478,6 +478,19 @@ csm_status csm_rt_grid2d_read(const csm_rt_grid2d* grid, csm_rt_grid2d_info* inf
   return CSM_OK;
 }
 
+csm_status csm_rt_grid2d_limits(const csm_rt_grid2d* grid, double* resolution, double* max_x,
+                                double* max_y, int32_t* num_x_cells, int32_t* num_y_cells) {
+  CSM_REQUIRE(grid != nullptr, "null pointer");
+  std::lock_guard<std::mutex> lock(grid->ctx->mu);   // an insert may be growing the limits
+  const RtGridDev& d = grid->g;
+  if (resolution) *resolution = d.resolution;
+  if (max_x) *max_x = d.max_x;
+  if (max_y) *max_y = d.max_y;
+  if (num_x_cells) *num_x_cells = d.nx;
+  if (num_y_cells) *num_y_cells = d.ny;
+  return CSM_OK;
+}
+
 csm_status csm_rt_grid2d_read_weights(const csm_rt_grid2d* grid, uint16_t* weight_cells,
                                       int64_t capacity) {
   CSM_REQUIRE(grid != nullptr && weight_cells != nullptr, "null pointer");

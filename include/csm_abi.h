@@ -850,6 +850,48 @@ csm_status csm_rt_grid2d_to_texture(const csm_rt_grid2d* grid, const double loca
 csm_status csm_grid3d_to_texture(const csm_grid3d* grid, const double global_submap_pose[7],
                                  uint8_t* buf, int64_t capacity, int64_t* size);
 
+/* ---- lifelong mapping in 2D: OverlappingSubmapsTrimmer2D's coverage pass ------------------- */
+/* One finished submap with a freshness (overlapping_submaps_trimmer_2d.cc:62-64: the caller
+ * leaves out unfinished submaps and submaps without one).  grid: the submap's ProbabilityGrid or
+ * TSDF2D handle (IsKnown reads the cell alone); translation and rotation (w, x, y, z):
+ * global_frame_from_local_frame = global_pose * local_pose().inverse(), composed by the caller;
+ * freshness: the common::Time ticks of the submap's latest intra-submap node. */
+typedef struct csm_coverage_submap2d {
+  const csm_rt_grid2d* grid;
+  double translation[3];
+  double rotation[4];
+  int64_t freshness;
+} csm_coverage_submap2d;
+typedef struct csm_coverage_stats2d {
+  int64_t entries;             /* (submap, known cell) entries of the coverage grid */
+  int64_t coverage_cells;      /* distinct global cells */
+  int64_t device_tie_cells;    /* cells of <= 16 entries with a tie between submaps across the
+                                  cut, settled in list order (libstdc++'s insertion sort) */
+  int64_t host_sorted_cells;   /* cells of > 16 entries with such a tie, std::sort'ed on the host */
+  int32_t host_syncs;          /* stream synchronisations */
+  int32_t reserved;
+} csm_coverage_stats2d;
+/* AddSubmapsToSubmapCoverageGrid2D + FindSubmapIdsToTrim (overlapping_submaps_trimmer_2d.cc:55-102,
+ * 145-182) over the submaps' device grids: every known cell of each submap's cropped limits (the
+ * known-cells box, 1 x 1 at offset 0 when it is empty), x fastest, its centre moved into the
+ * global frame in double (no FMA) and keyed by lround((first_max - p) / first_resolution) per
+ * axis; per global cell the fresh_submaps_count freshest entries, chosen as the reference's
+ * std::sort chooses them, count for their submaps.  trim[i] = 1 iff submap i gets no covered
+ * entry or uint16(covered_entries[i]) < min_covered_cells_count (the reference's
+ * std::map<SubmapId, uint16>, whose counts wrap at 65536); covered_entries[i] is the count before
+ * the wrap.  The handles are read and left unchanged; no insert may be in flight on them.
+ * CSM_E_INVALID for null pointers, a null grid, non-finite poses or limits, a resolution <= 0 or
+ * handles on more than one device; CSM_E_CAPACITY, with nothing written, for a global cell key
+ * outside int32 or entries that do not fit the device.  n == 0 does nothing.  At most three stream
+ * synchronisations (the entry total; the counts; the cells left to the host, if any). */
+csm_status csm_trim_overlapping_submaps2d(const csm_coverage_submap2d* submaps, int32_t n,
+                                          double first_max_x, double first_max_y,
+                                          double first_resolution, uint16_t fresh_submaps_count,
+                                          uint16_t min_covered_cells_count,
+                                          uint8_t* trim /* n */,
+                                          uint32_t* covered_entries /* n */,
+                                          csm_coverage_stats2d* stats /* may be NULL */);
+
 /* ---- map writing in 2D: ProbabilityGridRangeDataInserter2D on device grids ------------ */
 /* ProbabilityGridRangeDataInserter2D (mapping/2d/probability_grid_range_data_inserter_2d.cc)
  * applied in place to a ProbabilityGrid csm_rt_grid2d, so that a 2D submap lives on the device
@@ -908,6 +950,11 @@ typedef struct csm_rt_grid2d_info {
 } csm_rt_grid2d_info;
 csm_status csm_rt_grid2d_read(const csm_rt_grid2d* grid, csm_rt_grid2d_info* info,
                               uint16_t* cells, int64_t capacity);
+/* A handle's MapLimits alone (resolution, max and cell counts; any pointer but grid may be NULL),
+ * read on the host: no stream synchronisation, even when the known-cells box of a handle made from
+ * cells has not been computed yet. */
+csm_status csm_rt_grid2d_limits(const csm_rt_grid2d* grid, double* resolution, double* max_x,
+                                double* max_y, int32_t* num_x_cells, int32_t* num_y_cells);
 
 /* ---- map writing in 2D: TSDFRangeDataInserter2D on device grids ----------------------- */
 /* TSDFRangeDataInserter2D (mapping/internal/2d/tsdf_range_data_inserter_2d.cc) applied in place
