@@ -1471,6 +1471,14 @@ struct Match3 {
   const unsigned long long* hctr = nullptr;
   const BestLeaf3* best_inline = nullptr;
   int host_syncs = 0;
+  // Sweep limits (csm_sweep_limits3d).  A limit below its constant changes only the control
+  // flow: every buffer is still reserved at the constant's size.
+  int chunk = kChunk;              // nodes per level chunk (k3_level_begin)
+  int leaf_cap = kLeafCap;         // leaves recorded before the capacity error
+  int inline_best = kInlineBest;   // optimal leaves read back with each collect
+  float dive_ratio = kDiveRatio;   // k3_dive's gate; > 1 runs no dive
+  // sweep trace: collects (1 + continuation sweeps), most leaves recorded at a collect
+  int collects = 0, max_leaves = 0;
 
   Node3* Queue(int h) const {
     return h == hmax ? d_qtop->as<Node3>() : d_q->as<Node3>() + static_cast<size_t>(kQueueCap) * h;
@@ -1618,7 +1626,8 @@ csm_status TopDive3D(Match3& x) {
   CSM_LAUNCH_CHECK();
   ProfEnd(ctx, "k3_score_top", static_cast<double>(x.max_top));
   ProfBegin(ctx);
-  k3_dive<<<x.plan.num_angles, kT3, 0, x.s>>>(x.jb, x.d_top->as<int>(), kDiveRatio, x.lb, x.ctr);
+  k3_dive<<<x.plan.num_angles, kT3, 0, x.s>>>(x.jb, x.d_top->as<int>(), x.dive_ratio, x.lb,
+                                               x.ctr);
   CSM_LAUNCH_CHECK();
   ProfEnd(ctx, "k3_dive", static_cast<double>(x.plan.num_angles) * 8 * x.hmax);
   return CSM_OK;
@@ -1640,13 +1649,13 @@ csm_status FilterTop3D(Match3& x, long long top_queue) {
 
 // One level step of the device-driven level loop (see engine2d.cu).
 csm_status LevelStep3D(Match3& x, int h) {
-  k3_level_begin<<<1, 32, 0, x.s>>>(x.ictr, h, kChunk);
+  k3_level_begin<<<1, 32, 0, x.s>>>(x.ictr, h, x.chunk);
   CSM_LAUNCH_CHECK();
   ProfBegin(x.ctx);
   k3_expand<<<x.ctx->sm_count * 4, kT3, 0, x.s>>>(x.jb, x.Queue(h), x.ictr, h,
                                                    h - 1 >= 1 ? x.Queue(h - 1) : nullptr,
                                                    x.ictr + (h - 1 >= 1 ? h - 1 : 23), kQueueCap,
-                                                   x.d_leaves->as<Leaf3>(), kLeafCap, x.ctr);
+                                                   x.d_leaves->as<Leaf3>(), x.leaf_cap, x.ctr);
   CSM_LAUNCH_CHECK();
   ProfEnd(x.ctx, "k3_expand", 0.);
   return CSM_OK;
@@ -1658,16 +1667,19 @@ csm_status Collect3D(Match3& x) {
   char* pin = x.pin->as<char>();
   CSM_CUDA(cudaMemsetAsync(x.ictr + kC3Best, 0, 4, s));
   k3_collect<<<x.ctx->sm_count, 256, 0, s>>>(x.d_leaves->as<Leaf3>(), x.d_scans->as<Scan3>(),
-                                             x.d_sel->as<int>(), x.ictr, kLeafCap,
-                                             x.d_best->as<BestLeaf3>(), kLeafCap);
+                                             x.d_sel->as<int>(), x.ictr, x.leaf_cap,
+                                             x.d_best->as<BestLeaf3>(), x.leaf_cap);
   CSM_LAUNCH_CHECK();
   CSM_CUDA(cudaEventRecord(x.ctx->ev1, s));
   CSM_CUDA(cudaMemcpyAsync(pin, x.ictr, kRbCtr, cudaMemcpyDeviceToHost, s));
   CSM_CUDA(cudaMemcpyAsync(pin + kRbCtr, x.ctr, 8 * 8, cudaMemcpyDeviceToHost, s));
-  CSM_CUDA(cudaMemcpyAsync(pin + kRbBest, x.d_best->p, sizeof(BestLeaf3) * kInlineBest,
-                           cudaMemcpyDeviceToHost, s));
+  if (x.inline_best > 0)
+    CSM_CUDA(cudaMemcpyAsync(pin + kRbBest, x.d_best->p, sizeof(BestLeaf3) * x.inline_best,
+                             cudaMemcpyDeviceToHost, s));
   CSM_CUDA(cudaStreamSynchronize(s));
   ++x.host_syncs;
+  ++x.collects;
+  x.max_leaves = std::max(x.max_leaves, x.hp[kC3Leaf]);
   return CSM_OK;
 }
 
@@ -1815,11 +1827,20 @@ void Result3D(const Match3& x, const std::vector<BestLeaf3>& ties, int host_reso
 }
 
 // One match = one stream of launches + one synchronisation.  `dev` (optional) carries the
-// node's clouds already on the device.
+// node's clouds already on the device; `lim` (NULL: the defaults) the sweep limits, already
+// validated.  trace (may be NULL) receives {collects, most leaves recorded at a collect,
+// optimal leaves}.
 csm_status Match3D(Ctx* ctx, const csm_matcher3d* m, const csm_node3d* node,
                    const NodeDev3* dev, const double node_pose[7], const double submap_pose[7],
-                   int full, float min_score, csm_result3d* result, csm_stats* stats) {
+                   int full, float min_score, csm_result3d* result, csm_stats* stats,
+                   const csm_sweep_limits3d* lim = nullptr, int32_t trace[3] = nullptr) {
   Match3 x;
+  if (lim) {
+    x.chunk = lim->chunk;
+    x.leaf_cap = lim->leaf_cap;
+    x.inline_best = lim->inline_best;
+    x.dive_ratio = lim->dive_ratio;
+  }
   CSM_TRY(Plan3D(x, ctx, m, node, dev, node_pose, submap_pose, full, min_score));
   std::memset(result, 0, sizeof(*result));
   if (stats) std::memset(stats, 0, sizeof(*stats));
@@ -1830,8 +1851,13 @@ csm_status Match3D(Ctx* ctx, const csm_matcher3d* m, const csm_node3d* node,
   CSM_TRY(FilterTop3D(x, x.max_top));
   CSM_TRY(Sweep3D(x));
   const int n_best = x.hp[kC3Best];
-  std::vector<BestLeaf3> ties(x.best_inline, x.best_inline + std::min(n_best, kInlineBest));
-  if (n_best > kInlineBest) {
+  if (trace) {
+    trace[0] = x.collects;
+    trace[1] = x.max_leaves;
+    trace[2] = n_best;
+  }
+  std::vector<BestLeaf3> ties(x.best_inline, x.best_inline + std::min(n_best, x.inline_best));
+  if (n_best > x.inline_best) {
     ties.resize(n_best);
     CSM_CUDA(cudaMemcpy(ties.data(), x.d_best->p, sizeof(BestLeaf3) * n_best, cudaMemcpyDeviceToHost));
     ++x.host_syncs;
@@ -1883,12 +1909,39 @@ csm_status csm_match3d(const csm_matcher3d* m, const csm_node3d* node, const dou
   return Match3D(guard.lane, m, node, nullptr, node_pose, submap_pose, full, min_score, result,
                  stats);
 }
+void csm_sweep_limits3d_default(csm_sweep_limits3d* out) {
+  if (!out) return;
+  out->chunk = kChunk;
+  out->leaf_cap = kLeafCap;
+  out->inline_best = kInlineBest;
+  out->dive_ratio = kDiveRatio;
+}
+
 csm_status csm_match3d_batch(const csm_matcher3d* const* matchers, int32_t num_matchers,
                              const csm_node3d* nodes, int32_t num_nodes, const csm_job3d* jobs,
                              int32_t num_jobs, int32_t max_concurrency, csm_result3d* results,
                              csm_stats* stats) {
+  return csm_match3d_batch_limits(matchers, num_matchers, nodes, num_nodes, jobs, num_jobs,
+                                  max_concurrency, nullptr, results, stats, nullptr);
+}
+
+csm_status csm_match3d_batch_limits(const csm_matcher3d* const* matchers, int32_t num_matchers,
+                                    const csm_node3d* nodes, int32_t num_nodes,
+                                    const csm_job3d* jobs, int32_t num_jobs,
+                                    int32_t max_concurrency, const csm_sweep_limits3d* limits,
+                                    csm_result3d* results, csm_stats* stats, int32_t trace[3]) {
+  csm_sweep_limits3d lim;
+  csm_sweep_limits3d_default(&lim);
+  if (limits) {
+    lim = *limits;
+    CSM_REQUIRE(lim.chunk >= 1 && lim.chunk <= kChunk, "limits: chunk");
+    CSM_REQUIRE(lim.leaf_cap >= 1 && lim.leaf_cap <= kLeafCap, "limits: leaf_cap");
+    CSM_REQUIRE(lim.inline_best >= 0 && lim.inline_best <= kInlineBest, "limits: inline_best");
+    CSM_REQUIRE(std::isfinite(lim.dive_ratio) && lim.dive_ratio >= 0.f, "limits: dive_ratio");
+  }
   CSM_REQUIRE(num_jobs >= 0 && num_matchers >= 0 && num_nodes >= 0, "negative count");
   if (stats) std::memset(stats, 0, sizeof(*stats));
+  if (trace) std::memset(trace, 0, sizeof(int32_t) * 3);
   if (num_jobs == 0) return CSM_OK;
   CSM_REQUIRE(matchers && nodes && jobs && results, "null pointer");
   int device = -1;
@@ -1959,6 +2012,7 @@ csm_status csm_match3d_batch(const csm_matcher3d* const* matchers, int32_t num_m
       const csm_job3d& jb = jobs[j];
       csm_stats st;
       std::memset(&st, 0, sizeof(st));
+      int32_t tr[3] = {0, 0, 0};
       csm_status rc;
       {
         LaneGuard guard;
@@ -1966,7 +2020,7 @@ csm_status csm_match3d_batch(const csm_matcher3d* const* matchers, int32_t num_m
         if (rc == CSM_OK)
           rc = Match3D(guard.lane, matchers[jb.matcher_index], &nodes[jb.node_index],
                        &ndev[jb.node_index], jb.global_node_pose, jb.global_submap_pose,
-                       jb.full_submap, jb.min_score, &results[j], &st);
+                       jb.full_submap, jb.min_score, &results[j], &st, &lim, tr);
       }
       std::lock_guard<std::mutex> lock(mu);
       if (rc != CSM_OK) {
@@ -1983,6 +2037,11 @@ csm_status csm_match3d_batch(const csm_matcher3d* const* matchers, int32_t num_m
       total.host_tie_resolves += st.host_tie_resolves;
       total.host_syncs += st.host_syncs;
       total.device_ms += st.device_ms;
+      if (trace) {
+        trace[0] += tr[0];
+        trace[1] = std::max(trace[1], tr[1]);
+        trace[2] += tr[2];
+      }
     }
   };
   std::vector<std::thread> pool;
@@ -2097,6 +2156,31 @@ csm_status csm_score_top3d(const csm_matcher3d* m, const csm_node3d* node,
     counters[0] = static_cast<int64_t>(c[0]);
     counters[1] = static_cast<int64_t>(c[2]);
   }
+  return CSM_OK;
+}
+
+csm_status csm_top_queue3d(const csm_matcher3d* m, const csm_node3d* node,
+                           const double node_pose[7], const double submap_pose[7],
+                           int32_t full_submap, float min_score, float dive_ratio, float* bound,
+                           csm_bnb_node3d* queue, int32_t capacity, int32_t* count) {
+  static_assert(sizeof(csm_bnb_node3d) == sizeof(Node3), "csm_bnb_node3d is Node3");
+  CSM_REQUIRE(bound && count, "null pointer");
+  CSM_REQUIRE(capacity >= 0, "capacity");
+  CSM_REQUIRE(queue || capacity == 0, "null queue");
+  CSM_REQUIRE(std::isfinite(dive_ratio) && dive_ratio >= 0.f, "dive_ratio");
+  Hook3D hk;
+  Match3& x = hk.x;
+  x.dive_ratio = dive_ratio;
+  CSM_TRY(StartHook3D(hk, m, node, node_pose, submap_pose, full_submap, min_score));
+  CSM_TRY(TopDive3D(x));
+  CSM_TRY(FilterTop3D(x, x.max_top));
+  CSM_TRY(ReadCtl3D(x));
+  const int n = x.hp[x.hmax];
+  const int copy = std::min(n, capacity);
+  if (copy > 0)
+    CSM_CUDA(cudaMemcpy(queue, x.Queue(x.hmax), sizeof(Node3) * copy, cudaMemcpyDeviceToHost));
+  *bound = OrderedToFloat(static_cast<unsigned>(x.hp[kC3Bound]));
+  *count = n;
   return CSM_OK;
 }
 

@@ -1131,6 +1131,35 @@ class FastCorrelativeScanMatcher3D:
             C.byref(count), C.byref(final), ptr(ctr, C.c_int64)))
         return out[:count.value].copy(), np.float32(final.value), tuple(int(c) for c in ctr)
 
+    def top_queue(self, full, node_pose, submap_pose, constant_data, min_score, dive_ratio):
+        """csm_top_queue3d: the match through its dives (at `dive_ratio`) and its top-queue
+        filter.  -> (bound the level loop starts from, top queue as BNB_NODE3D_DTYPE records).
+        The queue is filled by atomic appends: its order is not deterministic."""
+        holder = _NodeHolder(constant_data)
+        args = self._probe_args(full, node_pose, submap_pose, holder) + (
+            C.c_float(min_score), C.c_float(dive_ratio))
+        bound, count = C.c_float(0.0), C.c_int32(0)
+        out = np.zeros(1024, BNB_NODE3D_DTYPE)
+        while True:
+            check(lib().csm_top_queue3d(*args, C.byref(bound), out.ctypes.data_as(C.c_void_p),
+                                        C.c_int32(len(out)), C.byref(count)))
+            if count.value <= len(out):
+                break
+            out = np.zeros(count.value, BNB_NODE3D_DTYPE)
+        return np.float32(bound.value), out[:count.value].copy()
+
+
+class SweepLimits3D(C.Structure):
+    """csm_sweep_limits3d: limits of the 3D branch-and-bound sweep."""
+    _fields_ = [("chunk", C.c_int32), ("leaf_cap", C.c_int32), ("inline_best", C.c_int32),
+                ("dive_ratio", C.c_float)]
+
+    @classmethod
+    def default(cls):
+        out = cls()
+        lib().csm_sweep_limits3d_default(C.byref(out))
+        return out
+
 
 class CsmJob3D(C.Structure):
     _fields_ = [("matcher_index", C.c_int32), ("node_index", C.c_int32),
@@ -1148,13 +1177,20 @@ def _result3d_dict(res):
                 leaves_tied=res.leaves_tied)
 
 
-def match_batch3d(matchers, nodes, jobs, max_concurrency=0, ctx=None, submap_owner=None):
+def match_batch3d(matchers, nodes, jobs, max_concurrency=0, ctx=None, submap_owner=None,
+                  limits=None):
     """csm_match3d_batch: a queue of ConstraintBuilder3D searches in one call.
     jobs: iterable of (matcher_index, node_index, full_submap, global_node_pose[7],
     global_submap_pose[7], min_score).  -> ([Result dict or None per job], stats dict).
     With `ctx` (MultiGpuContext) the queue is sharded over the GPUs (csm_cb_batch3d_run:
     matcher m runs on rank submap_owner[m], default m % world_size; matchers[m] may be None
-    elsewhere) and every rank gets all results after one ncclAllGather."""
+    elsewhere) and every rank gets all results after one ncclAllGather.
+    limits: None (the defaults), a SweepLimits3D, or a dict of SweepLimits3D fields that
+    override the defaults (csm_match3d_batch_limits; not with `ctx`); then
+    stats["sweep_trace"] is (collects summed over the jobs, most leaves recorded by one
+    match, optimal leaves summed)."""
+    if limits is not None and ctx is not None:
+        raise ValueError("sweep limits apply to the unsharded batch only")
     jobs = list(jobs)
     holders = [_NodeHolder(n) for n in nodes]
     c_nodes = (CsmNode3D * max(1, len(holders)))(*[h.c for h in holders])
@@ -1170,7 +1206,19 @@ def match_batch3d(matchers, nodes, jobs, max_concurrency=0, ctx=None, submap_own
         c_jobs[k].global_submap_pose = (C.c_double * 7)(*[float(v) for v in spose])
     c_res = (CsmResult3D * max(1, len(jobs)))()
     stats = CsmStats()
-    if ctx is None:
+    trace = None
+    if limits is not None:
+        if isinstance(limits, dict):
+            lim = SweepLimits3D.default()
+            for k, v in limits.items():
+                setattr(lim, k, v)
+            limits = lim
+        trace = np.zeros(3, np.int32)
+        check(lib().csm_match3d_batch_limits(
+            c_matchers, C.c_int32(len(matchers)), c_nodes, C.c_int32(len(holders)), c_jobs,
+            C.c_int32(len(jobs)), C.c_int32(int(max_concurrency)), C.byref(limits), c_res,
+            C.byref(stats), ptr(trace, C.c_int32)))
+    elif ctx is None:
         check(lib().csm_match3d_batch(c_matchers, C.c_int32(len(matchers)), c_nodes,
                                       C.c_int32(len(holders)), c_jobs, C.c_int32(len(jobs)),
                                       C.c_int32(int(max_concurrency)), c_res, C.byref(stats)))
@@ -1183,7 +1231,10 @@ def match_batch3d(matchers, nodes, jobs, max_concurrency=0, ctx=None, submap_own
                                        C.c_int32(len(holders)), c_jobs, C.c_int32(len(jobs)),
                                        owner, C.c_int32(int(max_concurrency)), c_res,
                                        C.byref(stats)))
-    return [_result3d_dict(c_res[k]) for k in range(len(jobs))], stats.as_dict()
+    out = stats.as_dict()
+    if trace is not None:
+        out["sweep_trace"] = tuple(int(v) for v in trace)
+    return [_result3d_dict(c_res[k]) for k in range(len(jobs))], out
 
 
 def rotational_match(submap_histogram, histogram, initial_angle, angles, device=0):

@@ -544,6 +544,27 @@ csm_status csm_match3d_batch(const csm_matcher3d* const* matchers, int32_t num_m
                              int32_t num_jobs, int32_t max_concurrency, csm_result3d* results,
                              csm_stats* stats /* may be NULL */);
 
+/* Limits of the 3D branch-and-bound sweep.  csm_sweep_limits3d_default gives the values
+ * csm_match3d and csm_match3d_batch run with.  Smaller limits change only the control flow:
+ * every buffer keeps its default size, and a limit too small for a search ends in
+ * CSM_E_CAPACITY. */
+typedef struct csm_sweep_limits3d {
+  int32_t chunk;        /* nodes per level chunk, 1 .. 1 << 16 */
+  int32_t leaf_cap;     /* leaves a match may record, 1 .. 1 << 20 */
+  int32_t inline_best;  /* optimal leaves read back with each collect, 0 .. 256 */
+  float dive_ratio;     /* >= 0, finite; > 1 disables the dives */
+} csm_sweep_limits3d;
+void csm_sweep_limits3d_default(csm_sweep_limits3d* out);
+/* csm_match3d_batch under `limits` (NULL: the defaults), validated before any device is
+ * used.  trace (may be NULL) receives {collects, i.e. 1 + continuation sweeps, summed over
+ * the jobs; most leaves recorded by one match at a collect; optimal leaves, summed}. */
+csm_status csm_match3d_batch_limits(const csm_matcher3d* const* matchers, int32_t num_matchers,
+                                    const csm_node3d* nodes, int32_t num_nodes,
+                                    const csm_job3d* jobs, int32_t num_jobs,
+                                    int32_t max_concurrency, const csm_sweep_limits3d* limits,
+                                    csm_result3d* results, csm_stats* stats /* may be NULL */,
+                                    int32_t trace[3]);
+
 /* Test hooks: RotationalScanMatcher::Match (rotational_scan_matcher.cc:178-189) and
  * the discrete scans of a match (GenerateDiscreteScans, :246-295): full-resolution
  * cell indices (num_scans x n x 3), scan poses (num_scans x 7 float: t, q wxyz) and
@@ -606,6 +627,15 @@ csm_status csm_branch_step3d(const csm_matcher3d* matcher, const csm_node3d* nod
                              int32_t num_parents, float bound, csm_bnb_node3d* children,
                              csm_bnb_leaf3d* leaves, int32_t* num_out, float* final_bound,
                              int64_t counters[3]);
+/* The same match through its dives (k3_dive's gate at `dive_ratio`) and its top-queue filter:
+ * *bound is the bound the level loop starts from, *count the length of the top queue (the
+ * lowest-resolution candidates with score > min_score and score >= *bound) and queue its
+ * first `capacity` records.  The queue is filled by atomic appends, so its order is not
+ * deterministic: compare it as a set. */
+csm_status csm_top_queue3d(const csm_matcher3d* matcher, const csm_node3d* node,
+                           const double global_node_pose[7], const double global_submap_pose[7],
+                           int32_t full_submap, float min_score, float dive_ratio, float* bound,
+                           csm_bnb_node3d* queue, int32_t capacity, int32_t* count);
 
 /* ==== RealTimeCorrelativeScanMatcher3D ======================================== */
 /* A HybridGrid resident on the device (dense uint16 box over its non-zero voxels; reads

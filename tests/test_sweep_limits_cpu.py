@@ -1,7 +1,8 @@
-"""CPU-side checks of the 2D sweep-limit hooks (csm_sweep_limits2d,
-csm_match2d_batch_limits, csm_dives2d): exported, laid out as the C compiler lays them
-out, defaulting to the engine's constants, and refusing every out-of-range limit and
-null pointer with CSM_E_INVALID before any device is needed."""
+"""CPU-side checks of the 2D and 3D sweep-limit hooks (csm_sweep_limits2d,
+csm_match2d_batch_limits, csm_dives2d; csm_sweep_limits3d, csm_match3d_batch_limits,
+csm_top_queue3d): exported, laid out as the C compiler lays them out, defaulting to the
+engines' constants, and refusing every out-of-range limit and null pointer with
+CSM_E_INVALID before any device is needed."""
 import ctypes as C
 import math
 import os
@@ -35,10 +36,10 @@ def test_symbols_exported(csm):
         assert hasattr(lib, name), name
 
 
-def _c_layout(fields):
+def _c_layout(fields, struct="csm_sweep_limits2d"):
     src = ('#include <stdio.h>\n#include <stddef.h>\n#include "include/csm_abi.h"\nint main(){'
-           'printf("%zu\\n", sizeof(csm_sweep_limits2d));' +
-           "".join('printf("%%zu\\n", offsetof(csm_sweep_limits2d, %s));' % f for f in fields) + "}")
+           'printf("%%zu\\n", sizeof(%s));' % struct +
+           "".join('printf("%%zu\\n", offsetof(%s, %s));' % (struct, f) for f in fields) + "}")
     with tempfile.TemporaryDirectory() as d:
         open(os.path.join(d, "lim.c"), "w").write(src)
         subprocess.check_call(["gcc", "-I", ROOT, os.path.join(d, "lim.c"), "-o",
@@ -156,3 +157,117 @@ def test_null_pointers_are_refused(csm, sm):
                          ctr.ctypes.data_as(C.POINTER(C.c_int64)), None, C.c_int32(0),
                          C.byref(cnt))
     assert st == 1
+
+
+# ---- 3D: csm_sweep_limits3d, csm_match3d_batch_limits, csm_top_queue3d --------------------
+def test_symbols_exported_3d(csm):
+    lib = csm.lib()
+    for name in ("csm_sweep_limits3d_default", "csm_match3d_batch_limits", "csm_top_queue3d"):
+        assert hasattr(lib, name), name
+
+
+def test_struct_layout_3d(sm):
+    fields = [f for f, _ in sm.SweepLimits3D._fields_]
+    assert fields == ["chunk", "leaf_cap", "inline_best", "dive_ratio"]
+    got = _c_layout(fields, "csm_sweep_limits3d")
+    assert got[0] == C.sizeof(sm.SweepLimits3D) == 16
+    assert got[1:] == [getattr(sm.SweepLimits3D, f).offset for f in fields]
+
+
+def test_defaults_are_the_engine_constants_3d(sm):
+    d = sm.SweepLimits3D.default()
+    assert (d.chunk, d.leaf_cap, d.inline_best) == (1 << 16, 1 << 20, 256)
+    assert d.dive_ratio == np.float32(0.97)
+
+
+def _batch3d_args(sm, limits, matchers=True, nodes=True, jobs=True, results=True,
+                  matcher_index=0, num_jobs=1):
+    # the matcher handle is never dereferenced: validation fails first
+    hs = (C.c_void_p * 1)(C.c_void_p(0x10))
+    cloud = np.zeros((4, 3), np.float32)
+    nd = (sm.CsmNode3D * 1)()
+    nd[0].high_resolution_point_cloud = cloud.ctypes.data_as(C.POINTER(C.c_float))
+    nd[0].num_high = 4
+    js = (sm.CsmJob3D * 1)()
+    js[0].matcher_index = matcher_index
+    res = (sm.CsmResult3D * 1)()
+    trace = np.zeros(3, np.int32)
+    keep = (hs, cloud, nd, js, res, trace)
+    args = (hs if matchers else None, C.c_int32(1), nd if nodes else None, C.c_int32(1),
+            js if jobs else None, C.c_int32(num_jobs), C.c_int32(0),
+            C.byref(limits) if limits is not None else None, res if results else None, None,
+            trace.ctypes.data_as(C.POINTER(C.c_int32)))
+    return args, keep
+
+
+BAD_LIMITS_3D = [("chunk", 0), ("chunk", (1 << 16) + 1), ("chunk", -5),
+                 ("leaf_cap", 0), ("leaf_cap", (1 << 20) + 1), ("leaf_cap", -1),
+                 ("inline_best", -1), ("inline_best", 257),
+                 ("dive_ratio", -0.5), ("dive_ratio", math.inf), ("dive_ratio", math.nan)]
+
+
+@pytest.mark.parametrize("field,value", BAD_LIMITS_3D)
+def test_out_of_range_limit_is_refused_3d(csm, sm, field, value):
+    """Refused before anything else, even for an empty batch."""
+    lim = sm.SweepLimits3D.default()
+    setattr(lim, field, value)
+    for n in (1, 0):
+        args, keep = _batch3d_args(sm, lim, num_jobs=n)
+        assert csm.lib().csm_match3d_batch_limits(*args) == 1
+        assert field.encode() in csm.lib().csm_last_error_string()
+
+
+@pytest.mark.parametrize("field,value", [("chunk", 1), ("chunk", 1 << 16), ("leaf_cap", 1),
+                                         ("leaf_cap", 1 << 20), ("inline_best", 0),
+                                         ("inline_best", 256), ("dive_ratio", 0.0),
+                                         ("dive_ratio", 1e30)])
+def test_limits_at_their_ends_pass_validation_3d(csm, sm, field, value):
+    """A limit at the end of its range gets past the limit checks, which come before the
+    jobs' checks: the call then fails on the job's matcher index, not on the limit.  An
+    empty batch under the same limits succeeds and leaves a zero trace."""
+    lim = sm.SweepLimits3D.default()
+    setattr(lim, field, value)
+    args, keep = _batch3d_args(sm, lim, matcher_index=5)
+    assert csm.lib().csm_match3d_batch_limits(*args) == 1
+    assert b"matcher_index out of range" in csm.lib().csm_last_error_string()
+    args, keep = _batch3d_args(sm, lim, num_jobs=0)
+    keep[-1][:] = 7
+    assert csm.lib().csm_match3d_batch_limits(*args) == 0
+    assert list(keep[-1]) == [0, 0, 0]
+
+
+def test_null_pointers_are_refused_3d(csm, sm):
+    lib = csm.lib()
+    lim = sm.SweepLimits3D.default()
+    for kw in ({"matchers": False}, {"nodes": False}, {"jobs": False}, {"results": False}):
+        args, keep = _batch3d_args(sm, lim, **kw)
+        assert lib.csm_match3d_batch_limits(*args) == 1, kw
+        assert b"null" in lib.csm_last_error_string(), kw
+    # csm_top_queue3d: every output pointer, a queue without storage and the dive ratio are
+    # checked before the handle is used
+    cloud = np.zeros((4, 3), np.float32)
+    nd = sm.CsmNode3D()
+    nd.high_resolution_point_cloud = cloud.ctypes.data_as(C.POINTER(C.c_float))
+    nd.num_high = 4
+    pose = np.array([0, 0, 0, 1, 0, 0, 0], np.float64)
+    bound, cnt = C.c_float(), C.c_int32()
+    q = np.zeros(4, sm.BNB_NODE3D_DTYPE)
+
+    def top_queue(matcher=True, node=True, npose=True, spose=True, b=True, queue=True, cap=4,
+                  count=True, ratio=0.97):
+        pp = pose.ctypes.data_as(C.POINTER(C.c_double))
+        return lib.csm_top_queue3d(
+            C.c_void_p(0x10) if matcher else None, C.byref(nd) if node else None,
+            pp if npose else None, pp if spose else None, C.c_int32(0), C.c_float(0.1),
+            C.c_float(ratio), C.byref(bound) if b else None,
+            q.ctypes.data_as(C.c_void_p) if queue else None, C.c_int32(cap),
+            C.byref(cnt) if count else None)
+
+    for kw in ({"b": False}, {"count": False}, {"queue": False}, {"cap": -1}, {"ratio": -1.0},
+               {"ratio": math.nan}, {"ratio": math.inf}):
+        assert top_queue(**kw) == 1, kw
+        assert lib.csm_last_error_string(), kw
+    # with every output valid, the null inputs (the fake handle is never reached)
+    for kw in ({"matcher": False}, {"node": False}, {"npose": False}, {"spose": False}):
+        assert top_queue(**kw) == 1, kw
+        assert b"null" in lib.csm_last_error_string(), kw
