@@ -473,3 +473,29 @@ def node_intensities(world, node, seed=0):
     c, s = math.cos(yaw), math.sin(yaw)
     w = node["cloud"].astype(np.float64) @ np.array([[c, -s, 0], [s, c, 0], [0, 0, 1]]).T + p[:3]
     return surface_intensity(world, w, seed)
+
+
+def moving_box_scans(seed, num_scans, size_m=16.0, height_m=4.0, rings=16, azimuths=512,
+                     max_range=12.0, box_m=1.2):
+    """Lidar scans of make_building(seed) from seeded free poses while a box of side `box_m`
+    crosses the ground floor, one step per scan: the input of OutlierRemovingPointsProcessor,
+    whose rays through the box's earlier places mark those hits as moving.  Returns
+    num_scans (origin (3,), world-frame points (n, 3)) float32 pairs."""
+    occ, cell, origin = make_building(seed, size_m=size_m, height_m=height_m)
+    rng = np.random.RandomState(seed + 101)
+    nz, ny, nx = occ.shape
+    b = max(1, int(round(box_m / cell)))
+    y0 = ny // 2 - b // 2
+    scans = []
+    for k in range(num_scans):
+        pose = random_free_pose_3d(occ, cell, origin, rng, margin_m=min(4.0, size_m / 4))
+        world = occ.copy()
+        x0 = int(round((0.15 + 0.7 * k / max(1, num_scans - 1)) * (nx - b)))
+        world[1:1 + b, y0:y0 + b, x0:x0 + b] = True
+        pts = cast_lidar_3d(world, cell, origin, pose, rings=rings, azimuths=azimuths,
+                            max_range=max_range, seed=seed * 1000 + k)
+        c, s = math.cos(pose[3]), math.sin(pose[3])
+        R = np.array([[c, -s, 0], [s, c, 0], [0, 0, 1]])
+        scans.append((pose[:3].astype(np.float32),
+                      (pts.astype(np.float64) @ R.T + pose[:3]).astype(np.float32)))
+    return scans

@@ -7,6 +7,7 @@
 #include <cstring>
 
 #include "constraint_builder_b200.h"
+#include "points_processor_b200.h"
 #include "pose_graph_trimmer_b200.h"
 #include "scan_matchers_b200.h"
 #include "voxel_filter_b200.h"
@@ -994,6 +995,60 @@ int main() {
     std::printf("RESULT vf_adaptive");
     for (float v : b.intensities()) std::printf(" %d", int(v));
     std::printf("\n");
+  }
+  {
+    // io::OutlierRemovingPointsProcessor on three batches streamed three times (the fixture of
+    // tests/test_gpu_adapter_outlier_removal.py): a wall at x = 5 and, per batch, a patch in front
+    // of it that the other batches' rays cross.  Intensities carry each point's index and colors
+    // its index and batch, so the RESULT lines show that the payloads follow the kept points.
+    struct Sink : io::PointsProcessor {
+      std::vector<std::unique_ptr<io::PointsBatch>> batches;
+      void Process(std::unique_ptr<io::PointsBatch> b) override { batches.push_back(std::move(b)); }
+      FlushResult Flush() override { return FlushResult::kFinished; }
+    } sink;
+    auto make = [](int b) {
+      auto batch = std::make_unique<io::PointsBatch>();
+      batch->origin.v[0] = float(b) * 0.3f;
+      batch->origin.v[1] = float(b) * -0.2f;
+      batch->origin.v[2] = 1.f;
+      for (int i = 0; i < 600; ++i) {
+        sensor::RangefinderPoint p;
+        if (i < 400) {
+          p = {{{5.f, float(i % 20) * 0.1f - 1.f, float(i / 20) * 0.1f}}};
+        } else {
+          p = {{{2.f + float(b), float(i % 10) * 0.1f - 0.5f, float((i / 10) % 10) * 0.1f}}};
+        }
+        batch->points.push_back(p);
+        batch->intensities.push_back(float(i));
+        batch->colors.push_back({float(i), float(b), 0.f});
+      }
+      return batch;
+    };
+    io::OutlierRemovingPointsProcessor processor(0.1, 3.0, &sink);
+    std::printf("RESULT or_action %s\n",
+                io::OutlierRemovingPointsProcessor::kConfigurationFileActionName);
+    std::printf("RESULT or_flush");
+    for (int pass = 0; pass < 3; ++pass) {
+      for (int b = 0; b < 3; ++b) processor.Process(make(b));
+      std::printf(" %d", processor.Flush() == io::PointsProcessor::FlushResult::kFinished);
+    }
+    std::printf("\n");
+    for (const auto& batch : sink.batches) {
+      std::printf("RESULT or_kept_%d", int(batch->colors.empty() ? -1 : batch->colors[0][1]));
+      for (float v : batch->intensities) std::printf(" %d", int(v));
+      std::printf("\nRESULT or_colors_%d", int(batch->colors.empty() ? -1 : batch->colors[0][1]));
+      for (const auto& c : batch->colors) std::printf(" %d", int(c[0]));
+      // 1 where a kept point is the input point its intensity names
+      const int b = int(batch->colors.empty() ? 0 : batch->colors[0][1]);
+      const auto input = make(b);
+      std::printf("\nRESULT or_points_%d", b);
+      for (size_t i = 0; i < batch->points.size(); ++i) {
+        const auto& q = input->points[int(batch->intensities[i])].position;
+        const auto& p = batch->points[i].position;
+        std::printf(" %d", p.x() == q.x() && p.y() == q.y() && p.z() == q.z());
+      }
+      std::printf("\n");
+    }
   }
   if (trimmer_cases::Run() != 0) return 1;
   return 0;

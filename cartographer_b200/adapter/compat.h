@@ -9,11 +9,14 @@
 #ifndef CSM_ADAPTER_COMPAT_H_
 #define CSM_ADAPTER_COMPAT_H_
 
+#include <array>
 #include <cmath>
 #include <cstdint>
 #include <functional>
 #include <map>
 #include <memory>
+#include <string>
+#include <unordered_set>
 #include <utility>
 #include <vector>
 
@@ -693,6 +696,51 @@ class PoseGraphTrimmer {
   virtual bool IsFinished() = 0;
 };
 }  // namespace mapping
+}  // namespace cartographer
+
+// ---- points processing (io/points_batch.h, io/points_processor.h) ----
+namespace absl {
+// The set type io::RemovePoints takes (absl/container/flat_hash_set.h).
+template <class T>
+using flat_hash_set = std::unordered_set<T>;
+}  // namespace absl
+
+namespace cartographer {
+namespace io {
+using FloatColor = std::array<float, 3>;   // io/color.h
+// io/points_batch.h:31-66 (origin is an Eigen::Vector3f there, zero by default).
+struct PointsBatch {
+  struct { float v[3] = {0.f, 0.f, 0.f}; float x() const { return v[0]; } float y() const { return v[1]; } float z() const { return v[2]; } } origin;
+  std::string frame_id;
+  int trajectory_id = 0;
+  std::vector<sensor::RangefinderPoint> points;
+  std::vector<float> intensities;   // empty, or one per point
+  std::vector<FloatColor> colors;   // empty, or one per point
+};
+// io/points_batch.cc:22-49: the points whose indices are not in to_remove, in order, with their
+// intensities and colors where the batch has them.
+inline void RemovePoints(absl::flat_hash_set<int> to_remove, PointsBatch* batch) {
+  PointsBatch kept;
+  for (size_t i = 0; i < batch->points.size(); ++i) {
+    if (to_remove.count(static_cast<int>(i))) continue;
+    kept.points.push_back(batch->points[i]);
+    if (!batch->intensities.empty()) kept.intensities.push_back(batch->intensities[i]);
+    if (!batch->colors.empty()) kept.colors.push_back(batch->colors[i]);
+  }
+  batch->points = std::move(kept.points);
+  batch->intensities = std::move(kept.intensities);
+  batch->colors = std::move(kept.colors);
+}
+// io/points_processor.h:27-52.
+class PointsProcessor {
+ public:
+  enum class FlushResult { kRestartStream, kFinished };
+  PointsProcessor() {}
+  virtual ~PointsProcessor() {}
+  virtual void Process(std::unique_ptr<PointsBatch> points_batch) = 0;
+  virtual FlushResult Flush() = 0;
+};
+}  // namespace io
 }  // namespace cartographer
 
 #endif  // CSM_ADAPTER_COMPAT_H_

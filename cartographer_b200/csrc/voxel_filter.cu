@@ -27,6 +27,7 @@
 #include <cub/iterator/counting_input_iterator.cuh>
 
 #include "common.cuh"
+#include "point_batch.cuh"
 
 namespace csm {
 namespace {
@@ -62,36 +63,12 @@ __device__ inline uint64_t Past(int k) {
   return uk * (kUrngRange / uk);
 }
 
-// common::RoundToInt = std::lround narrowed to int: half away from zero; an integer at or
-// beyond 2^63 in magnitude is LONG_MIN on x86-64, whose low 32 bits are 0.
-__device__ inline int RoundToInt(float v) {
-  if (!(fabsf(roundf(v)) < 9.223372036854775808e18f)) return 0;
-  return static_cast<int>(lroundf(v));
-}
-
 // GetVoxelCellIndex (voxel_filter.cc:79-86), wrapping.
 __device__ inline unsigned long long VoxelKey(const float* p, float resolution) {
   const uint64_t x = static_cast<uint64_t>(static_cast<int64_t>(RoundToInt(p[0] / resolution)));
   const uint64_t y = static_cast<uint64_t>(static_cast<int64_t>(RoundToInt(p[1] / resolution)));
   const uint64_t z = static_cast<uint64_t>(static_cast<int64_t>(RoundToInt(p[2] / resolution)));
   return (x << 42) + (y << 21) + z;
-}
-
-__device__ inline int CloudOf(const int* off, int num_clouds, int i) {
-  int lo = 0, hi = num_clouds;                    // last c with off[c] <= i
-  while (hi - lo > 1) {
-    const int mid = (lo + hi) / 2;
-    if (off[mid] <= i) lo = mid; else hi = mid;
-  }
-  return lo;
-}
-
-__device__ inline uint64_t Mix(unsigned long long k) {
-  k ^= k >> 33;
-  k *= 0xff51afd7ed558ccdull;
-  k ^= k >> 33;
-  k *= 0xc4ceb9fe1a85ec53ull;
-  return k ^ (k >> 33);
 }
 
 // Per-cloud search state (voxel_filter.cc:38-75).  The output is VoxelFilter(length) of the
@@ -401,20 +378,6 @@ __global__ void k_vf_localize(const int* __restrict__ off, int nc, const int* __
 struct MaxOp {
   __device__ unsigned long long operator()(unsigned long long a, unsigned long long b) const {
     return a > b ? a : b;
-  }
-};
-
-size_t Align(size_t b) { return (b + 255) / 256 * 256; }
-
-// Carves typed arrays out of one workspace.
-struct Carver {
-  size_t at = 0;
-  char* base = nullptr;
-  template <typename T>
-  T* take(size_t count) {
-    T* p = reinterpret_cast<T*>(base + at);
-    at += Align(sizeof(T) * std::max<size_t>(count, 1));
-    return p;
   }
 };
 

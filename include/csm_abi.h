@@ -1067,6 +1067,57 @@ csm_status csm_adaptive_voxel_filter_batch(const float* const* xyz, const int32_
                                            int32_t* kept_indices, int32_t* num_kept,
                                            csm_stats* stats /* may be NULL */);
 
+/* ---- map assets: OutlierRemovingPointsProcessor ------------------------------------------ */
+/* io::OutlierRemovingPointsProcessor (io/outlier_removing_points_processor.cc:53-129), the
+ * assets writer's voxel_filter_and_remove_moving_objects stage, with its voxel map on one
+ * device.  Three phases, each over every batch of the stream: add_hits counts hits per voxel
+ * (GetCellIndex = lround(p / (float)voxel_size), narrowed to int); count_rays samples every ray
+ * from its batch's origin at x = 0, x += voxel_size (x a float, voxel_size a double) while
+ * x < |point - origin|, and counts a ray in each sampled voxel that has hits; filter keeps a point
+ * iff rays < miss_per_hit_limit * hits of its voxel (in double; a voxel never hit reads {0, 0}).
+ * Every count and kept index is bit for bit the reference's, however the batches are grouped
+ * into calls.  Phases only move forward: a call of an earlier phase than one already begun
+ * returns CSM_E_INVALID.  Batch b has num_points[b] x {x, y, z} in xyz[b]; a call takes any
+ * number of batches.  Every call checks all its input first, and a refused call changes nothing:
+ * CSM_E_INVALID for a null pointer where data is required, a negative count, a non-finite
+ * coordinate or origin, more than 2^30 points in one call, a hit outside the [-8192, 8192)^3
+ * voxels the reference's grid can grow to (its CHECK), or a ray longer than the point where
+ * x += voxel_size stops growing (the reference would loop forever).  One stream synchronisation
+ * per call with points (none without); stats (may be NULL) gets host_syncs and device_ms.
+ * Counts are int32, as in the reference, whose overflow is undefined behaviour. */
+typedef struct csm_outlier_remover csm_outlier_remover;
+/* CSM_E_INVALID for a voxel_size that is not finite and > 0, or a non-finite limit. */
+csm_status csm_outlier_remover_create(double voxel_size, double miss_per_hit_limit, int32_t device,
+                                      csm_outlier_remover** out);
+csm_status csm_outlier_remover_destroy(csm_outlier_remover* remover);
+/* Phase 1 (ProcessInPhaseOne).  The voxel map grows (a device rehash) at the start of a call
+ * that would fill it past one half; CSM_E_CAPACITY, with the map unchanged, when the device has
+ * not the memory for that. */
+csm_status csm_outlier_remover_add_hits(csm_outlier_remover* remover, const float* const* xyz,
+                                        const int32_t* num_points, int32_t num_batches,
+                                        csm_stats* stats /* may be NULL */);
+/* Phase 2 (ProcessInPhaseTwo); origins holds num_batches x {x, y, z}. */
+csm_status csm_outlier_remover_count_rays(csm_outlier_remover* remover, const float* origins,
+                                          const float* const* xyz, const int32_t* num_points,
+                                          int32_t num_batches, csm_stats* stats /* may be NULL */);
+/* Phase 3 (ProcessInPhaseThree): kept_indices (capacity sum of num_points) receives the batches'
+ * kept indices in input order, one batch after another, each index into its own batch;
+ * num_kept[b] their count.  The removed points are the others (RemovePoints). */
+csm_status csm_outlier_remover_filter(csm_outlier_remover* remover, const float* const* xyz,
+                                      const int32_t* num_points, int32_t num_batches,
+                                      int32_t* kept_indices, int32_t* num_kept,
+                                      csm_stats* stats /* may be NULL */);
+/* Test hook: every voxel with hits in ascending (z, y, x): indices (n x {x, y, z}), hits, rays
+ * (each may be NULL).  With all three NULL only *num_voxels is written, without a stream
+ * synchronisation; a capacity below it returns CSM_E_CAPACITY with *num_voxels set. */
+csm_status csm_outlier_remover_voxels(const csm_outlier_remover* remover, int32_t* indices,
+                                      int32_t* hits, int32_t* rays, int64_t capacity,
+                                      int64_t* num_voxels);
+/* The current phase (1, 2 or 3), the voxel count and the map's slot count (a power of two),
+ * read on the host. */
+csm_status csm_outlier_remover_info(const csm_outlier_remover* remover, int32_t* phase,
+                                    int64_t* num_voxels, int64_t* slots);
+
 /* Test hook: as csm_ceres_evaluate3d, in the problem's residual-block order — per cloud its
  * occupied-space residuals, then its intensity residuals if it has a grid; then 3
  * translation and 3 rotation residuals.  Residuals and rows are uncorrected by the loss, as
