@@ -5,6 +5,7 @@
 
 #include <cuda_runtime.h>
 
+#include <algorithm>
 #include <atomic>
 #include <cmath>
 #include <cstdarg>
@@ -50,6 +51,11 @@ extern std::atomic<int64_t> g_launches;
   } while (0)
 
 inline int DivUp(long long a, long long b) { return static_cast<int>((a + b - 1) / b); }
+
+// Blocks of 256 threads for `work` items, at least one and at most `cap`.
+inline unsigned Blocks(long long work, long long cap = 1 << 16) {
+  return static_cast<unsigned>(std::max(1LL, std::min(cap, (work + 255) / 256)));
+}
 
 // The engines' order-preserving float <-> unsigned map (bounds are kept as unsigned so that
 // atomicMax on them orders like the float scores).

@@ -10,16 +10,11 @@
 // on the host, as in the 2D path; every float expression that reaches an output
 // uses round-to-nearest intrinsics in the reference's operation order.
 #include <algorithm>
-#include <climits>
 #include <cmath>
 #include <functional>
 
-#include <cub/block/block_scan.cuh>
-#include <cub/device/device_scan.cuh>
-
 #include "common.cuh"
 #include "grid3d.cuh"
-#include "proto_write.h"
 #include "rigid3f.h"
 #include "value_conversion.h"
 
@@ -42,12 +37,6 @@ struct Stack3Dev {
   int depth, frd;
   float resolution;
 };
-struct Low3Dev {
-  const uint16_t* p;
-  int lo[3];
-  int n[3];
-  float resolution, k_scale, bias, min_probability;
-};
 struct Scan3 {
   float tx, ty, tz, qw, qx, qy, qz;  // DiscreteScan3D::pose
   float nw, nx, ny, nz;              // rotation of GetPoseFromCandidate (normalised)
@@ -55,7 +44,7 @@ struct Scan3 {
 };
 struct Job3 {
   const Stack3Dev* stack;
-  const Low3Dev* low;
+  const Grid3Dev* low;
   const float* hi_xyz;
   const float* lo_xyz;
   const Scan3* scans;  // the scans that passed the rotational filter (written on the device)
@@ -102,80 +91,9 @@ __global__ void k3_scatter_u8(const int* __restrict__ idx, const uint16_t* __res
   const int x = idx[3 * i] - v.lo[0], y = idx[3 * i + 1] - v.lo[1], z = idx[3 * i + 2] - v.lo[2];
   out[(static_cast<size_t>(z) * v.n[1] + y) * v.n[0] + x] = lut[values[i]];
 }
-__global__ void k3_scatter_u16(const int* __restrict__ idx, const uint16_t* __restrict__ values,
-                               long long n, Low3Dev v, uint16_t* __restrict__ out) {
-  const long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x;
-  if (i >= n) return;
-  const int x = idx[3 * i] - v.lo[0], y = idx[3 * i + 1] - v.lo[1], z = idx[3 * i + 2] - v.lo[2];
-  out[(static_cast<size_t>(z) * v.n[1] + y) * v.n[0] + x] = values[i];
-}
 
 // ---- the same from a csm_grid3d's dense box (csm_matcher3d_create_from_grid3d) ----
-// Launch shape of the three kernels below: x along a row of the box they walk (coalesced),
-// blockIdx.y strides over the rows (y + n1 * z).
-struct Box16 {
-  const uint16_t* p;
-  int lo[3];
-  int n[3];
-};
-
-// The bounding box of the non-zero cells of `b`, as offsets from b.lo: mn[0..2] receives the
-// min (atomicMin; the caller sets them to 0xffffffff), mx[0..2] the max + 1 (atomicMax; the
-// caller zeroes them), so mx[0] != 0 is the "any non-zero cell" flag.  Per thread, then per
-// block (warp reductions + shared memory), then six atomics per block that saw a cell.
-__global__ void __launch_bounds__(256)
-k3_nonzero_box(Box16 b, unsigned* __restrict__ mn_out, unsigned* __restrict__ mx_out) {
-  __shared__ unsigned s[6][8];
-  unsigned mn[3] = {0xffffffffu, 0xffffffffu, 0xffffffffu}, mx[3] = {0u, 0u, 0u};
-  const int x = blockIdx.x * blockDim.x + threadIdx.x;
-  const long long rows = static_cast<long long>(b.n[1]) * b.n[2];
-  if (x < b.n[0]) {
-    for (long long r = blockIdx.y; r < rows; r += gridDim.y) {
-      if (__ldg(b.p + r * b.n[0] + x) == 0) continue;
-      const unsigned y = static_cast<unsigned>(r % b.n[1]), z = static_cast<unsigned>(r / b.n[1]);
-      const unsigned c[3] = {static_cast<unsigned>(x), y, z};
-#pragma unroll
-      for (int a = 0; a < 3; ++a) {
-        mn[a] = min(mn[a], c[a]);
-        mx[a] = max(mx[a], c[a] + 1u);
-      }
-    }
-  }
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-#pragma unroll
-  for (int a = 0; a < 3; ++a) {
-    mn[a] = __reduce_min_sync(0xffffffffu, mn[a]);
-    mx[a] = __reduce_max_sync(0xffffffffu, mx[a]);
-    if (lane == 0) {
-      s[a][warp] = mn[a];
-      s[3 + a][warp] = mx[a];
-    }
-  }
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    unsigned v[6];
-    for (int a = 0; a < 6; ++a) {
-      v[a] = s[a][0];
-      for (int w = 1; w < static_cast<int>(blockDim.x >> 5); ++w)
-        v[a] = a < 3 ? min(v[a], s[a][w]) : max(v[a], s[a][w]);
-    }
-    if (v[3] != 0u)
-      for (int a = 0; a < 3; ++a) {
-        atomicMin(&mn_out[a], v[a]);
-        atomicMax(&mx_out[a], v[3 + a]);
-      }
-  }
-}
-
-// The value of cell (x, y, z) of the source box, 0 outside it.
-__device__ __forceinline__ uint16_t Val16(const Box16& b, int x, int y, int z) {
-  const int lx = x - b.lo[0], ly = y - b.lo[1], lz = z - b.lo[2];
-  if (static_cast<unsigned>(lx) >= static_cast<unsigned>(b.n[0]) ||
-      static_cast<unsigned>(ly) >= static_cast<unsigned>(b.n[1]) ||
-      static_cast<unsigned>(lz) >= static_cast<unsigned>(b.n[2]))
-    return 0;
-  return __ldg(b.p + (static_cast<size_t>(lz) * b.n[1] + ly) * b.n[0] + lx);
-}
+// Both kernels are launched with RowGrid (grid3d.cuh).
 
 // Depth 0 (ConvertToPrecomputationGrid) in gather form: one thread per level-0 cell.  A cell
 // outside the source box reads 0, which the LUT maps to 0 as the scatter form's memset leaves it.
@@ -192,99 +110,13 @@ k3_gather_u8(Box16 src, const uint8_t* __restrict__ lut, Vol8 v, uint8_t* __rest
 
 // The low-resolution volume: the cells of the source box inside `v`, copied as they are.
 __global__ void __launch_bounds__(256)
-k3_gather_u16(Box16 src, Low3Dev v, uint16_t* __restrict__ out) {
+k3_gather_u16(Box16 src, Grid3Dev v, uint16_t* __restrict__ out) {
   const int x = blockIdx.x * blockDim.x + threadIdx.x;
   if (x >= v.n[0]) return;
   const long long rows = static_cast<long long>(v.n[1]) * v.n[2];
   for (long long r = blockIdx.y; r < rows; r += gridDim.y) {
     const int y = static_cast<int>(r % v.n[1]), z = static_cast<int>(r / v.n[1]);
     out[r * v.n[0] + x] = Val16(src, x + v.lo[0], y + v.lo[1], z + v.lo[2]);
-  }
-}
-
-// ---- the non-zero voxels of a csm_grid3d in HybridGrid's iteration order (csm_grid3d_voxels) ----
-// HybridGrid is DynamicGrid<NestedGrid<FlatGrid<uint16, 3>, 3>> (hybrid_grid.h), and each level
-// walks its cells in ToFlatIndex order, z outermost (:40-43), skipping null meta cells and value 0
-// (:57, :106-115).  The DynamicGrid shifts an index by grid_size() / 2 = 2^(bits - 1) * 64, a
-// multiple of 64 (:263-264), so its meta cells are the 64^3 blocks floor(index / 64) in z, y, x
-// order, whatever bits_ is and however the grid grew; inside them come the NestedGrid's 8^3 blocks
-// and inside those the cells, both in z, y, x order.  The kernels below enumerate the 64-aligned
-// cover of the non-zero box in that blocked order and compact the non-zero cells stably: tile t is
-// kVoxTile consecutive cells of the enumeration (4 of the 8^3 blocks, 128 tiles per 64^3 block),
-// and thread k of a tile holds the x-row (z & 7, y & 7) = ((k & 63) >> 3, k & 7) of its block
-// k >> 6.  No sort is needed.
-constexpr int kVoxThreads = 256;
-constexpr int kVoxTile = 8 * kVoxThreads;
-
-struct VoxCover {
-  Box16 src;
-  int lo[3];   // multiples of 64
-  int nb[3];   // 64^3 blocks per axis
-};
-
-// The 8 cells x .. x + 7 of this thread's row in tile t, and their values in v.
-__device__ __forceinline__ void VoxRow(const VoxCover& c, long long t, int* x, int* y, int* z,
-                                       uint16_t v[8]) {
-  const long long m = t >> 7;                                          // the 64^3 block
-  const int f = static_cast<int>(t & 127) * 4 + (threadIdx.x >> 6);    // the 8^3 block in it
-  const int r = threadIdx.x & 63;
-  const long long bxy = static_cast<long long>(c.nb[0]) * c.nb[1];
-  const int bz = static_cast<int>(m / bxy);
-  const int by = static_cast<int>((m % bxy) / c.nb[0]);
-  const int bx = static_cast<int>(m % c.nb[0]);
-  *x = c.lo[0] + 64 * bx + 8 * (f & 7);
-  *y = c.lo[1] + 64 * by + 8 * ((f >> 3) & 7) + (r & 7);
-  *z = c.lo[2] + 64 * bz + 8 * (f >> 6) + (r >> 3);
-#pragma unroll
-  for (int i = 0; i < 8; ++i) v[i] = Val16(c.src, *x + i, *y, *z);
-}
-
-// Pass 1: counts[t] = the non-zero cells of tile t.
-__global__ void __launch_bounds__(kVoxThreads)
-k3_voxel_count(VoxCover c, long long* __restrict__ counts) {
-  __shared__ int s[kVoxThreads / 32];
-  int x, y, z;
-  uint16_t v[8];
-  VoxRow(c, blockIdx.x, &x, &y, &z, v);
-  int n = 0;
-#pragma unroll
-  for (int i = 0; i < 8; ++i) n += v[i] != 0;
-  n = __reduce_add_sync(0xffffffffu, n);
-  if ((threadIdx.x & 31) == 0) s[threadIdx.x >> 5] = n;
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    int total = 0;
-    for (int w = 0; w < kVoxThreads / 32; ++w) total += s[w];
-    counts[blockIdx.x] = total;
-  }
-}
-
-// Pass 2: the non-zero cells of tile t written from offsets[t] on, in enumeration order:
-// idx as {x, y, z}, val as held.
-__global__ void __launch_bounds__(kVoxThreads)
-k3_voxel_write(VoxCover c, const long long* __restrict__ counts,
-               const long long* __restrict__ offsets, int* __restrict__ idx,
-               uint16_t* __restrict__ val) {
-  typedef cub::BlockScan<int, kVoxThreads> Scan;
-  __shared__ typename Scan::TempStorage scan;
-  if (counts[blockIdx.x] == 0) return;   // uniform over the block
-  int x, y, z;
-  uint16_t v[8];
-  VoxRow(c, blockIdx.x, &x, &y, &z, v);
-  int n = 0;
-#pragma unroll
-  for (int i = 0; i < 8; ++i) n += v[i] != 0;
-  int before;
-  Scan(scan).ExclusiveSum(n, before);
-  long long o = offsets[blockIdx.x] + before;
-#pragma unroll
-  for (int i = 0; i < 8; ++i) {
-    if (v[i] == 0) continue;
-    idx[3 * o] = x + i;
-    idx[3 * o + 1] = y;
-    idx[3 * o + 2] = z;
-    val[o] = v[i];
-    ++o;
   }
 }
 
@@ -521,7 +353,7 @@ __device__ float LowResScore(const Job3& jb, int scan, int ox, int oy, int oz, f
                            __fadd_rn(sc.ty, __fmul_rn(res, __int2float_rn(oy))),
                            __fadd_rn(sc.tz, __fmul_rn(res, __int2float_rn(oz)))},
                      Quatf{sc.nw, sc.nx, sc.ny, sc.nz}};
-  const Low3Dev& lg = *jb.low;
+  const Grid3Dev& lg = *jb.low;
   __shared__ float s_sum;
   __syncthreads();  // a previous call's readers of s_sum are done
   if (threadIdx.x == 0) s_sum = 0.f;
@@ -790,8 +622,8 @@ struct csm_matcher3d {
   Ctx* ctx = nullptr;
   Stack3Dev hs;            // host copy (device pointers inside)
   Stack3Dev* d_stack = nullptr;
-  Low3Dev hl;
-  Low3Dev* d_low = nullptr;
+  Grid3Dev hl;
+  Grid3Dev* d_low = nullptr;
   uint8_t* d_levels = nullptr;
   uint16_t* d_lowvol = nullptr;
   float* d_hist = nullptr;
@@ -843,32 +675,25 @@ csm_status CheckOptions3D(const csm_options3d* options) {
   return CSM_OK;
 }
 
-// The inclusive bounding box of a set of voxels; {0, 0, 0} for an empty set.
-struct VoxelBox3 {
-  int lo[3] = {0, 0, 0};
-  int hi[3] = {0, 0, 0};
-};
-
 // What the two ways to build a csm_matcher3d differ in: how depth 0 and the low-resolution
 // volume are filled, on the context's stream, into volumes already zeroed.  Each gets the
 // box it fills and its destination; FillDepth0 also gets the device LUT of
 // ConvertToPrecomputationGrid (precomputation_grid_3d.cc:49-61).
 using FillDepth0 = std::function<csm_status(const Vol8& level0, uint8_t* dst, const uint8_t* lut)>;
-using FillLow = std::function<csm_status(const Low3Dev& low, uint16_t* dst)>;
+using FillLow = std::function<csm_status(const Grid3Dev& low, uint16_t* dst)>;
 
 // FastCorrelativeScanMatcher3D's ctor over voxel boxes that are already known: level
 // geometry, the 24 GB guard, the allocations, the precomputation chain, the low-resolution
 // volume and the upload of the records and histogram; one stream synchronisation at the end.
 // The caller holds ctx->mu, has made the context's device current and checked `options`.
-csm_status BuildMatcher3D(Ctx* ctx, const VoxelBox3& hi_box, float hi_res, int32_t hi_grid_size,
-                          const VoxelBox3& lo_box, float lo_res, const float* submap_hist,
+csm_status BuildMatcher3D(Ctx* ctx, const TightBox3& hi_box, float hi_res, int32_t hi_grid_size,
+                          const TightBox3& lo_box, float lo_res, const float* submap_hist,
                           int32_t hist_n, const csm_options3d* options,
                           const FillDepth0& fill_depth0, const FillLow& fill_low,
                           csm_matcher3d** out) {
   const int* lo0 = hi_box.lo;
   const int* hi0 = hi_box.hi;
-  for (int a = 0; a < 3; ++a)
-    CSM_REQUIRE(lo0[a] >= -8192 && hi0[a] < 8192, "voxel index outside the 2^14 cube");  // :387
+  CSM_REQUIRE(hi_box.InCube(), "voxel index outside the 2^14 cube");
   cudaStream_t s = ctx->stream;
   std::unique_ptr<csm_matcher3d> m(new csm_matcher3d);
   m->ctx = ctx;
@@ -941,30 +766,18 @@ csm_status BuildMatcher3D(Ctx* ctx, const VoxelBox3& hi_box, float hi_res, int32
   }
 
   // ---- low-resolution grid ----
-  Low3Dev& hl = m->hl;
-  std::memset(&hl, 0, sizeof(hl));
-  for (int a = 0; a < 3; ++a) {
-    hl.lo[a] = lo_box.lo[a];
-    hl.n[a] = lo_box.hi[a] - lo_box.lo[a] + 1;
-  }
-  const size_t lvox = static_cast<size_t>(hl.n[0]) * hl.n[1] * hl.n[2];
+  const Box3 lbox = lo_box.Dense();
+  const size_t lvox = lbox.Volume();
   CSM_REQUIRE(lvox < (size_t(4) << 30), "dense low-resolution volume too large");
   CSM_CUDA(cudaMalloc(&m->d_lowvol, std::max<size_t>(lvox * 2, 256)));
   CSM_CUDA(cudaMemsetAsync(m->d_lowvol, 0, std::max<size_t>(lvox * 2, 256), s));
-  hl.p = m->d_lowvol;
-  hl.resolution = lo_res;
-  {
-    const ValueConversion probability = MakeValueConversion(kMinProbability, kMaxProbability);
-    hl.k_scale = probability.scale;
-    hl.bias = probability.bias;
-    hl.min_probability = kMinProbability;
-  }
-  CSM_TRY(fill_low(hl, m->d_lowvol));
+  m->hl = MakeGrid3Dev(m->d_lowvol, lbox, lo_res);
+  CSM_TRY(fill_low(m->hl, m->d_lowvol));
   CSM_CUDA(cudaMalloc(&m->d_stack, sizeof(Stack3Dev)));
-  CSM_CUDA(cudaMalloc(&m->d_low, sizeof(Low3Dev)));
+  CSM_CUDA(cudaMalloc(&m->d_low, sizeof(Grid3Dev)));
   CSM_CUDA(cudaMalloc(&m->d_hist, sizeof(float) * std::max(1, hist_n)));
   CSM_CUDA(cudaMemcpyAsync(m->d_stack, &hs, sizeof(hs), cudaMemcpyHostToDevice, s));
-  CSM_CUDA(cudaMemcpyAsync(m->d_low, &hl, sizeof(hl), cudaMemcpyHostToDevice, s));
+  CSM_CUDA(cudaMemcpyAsync(m->d_low, &m->hl, sizeof(Grid3Dev), cudaMemcpyHostToDevice, s));
   if (hist_n)
     CSM_CUDA(cudaMemcpyAsync(m->d_hist, m->hist.data(), sizeof(float) * hist_n,
                              cudaMemcpyHostToDevice, s));
@@ -973,117 +786,7 @@ csm_status BuildMatcher3D(Ctx* ctx, const VoxelBox3& hi_box, float hi_res, int32
   return CSM_OK;
 }
 
-VoxelBox3 ListBox3(const int32_t* idx, int64_t n) {
-  VoxelBox3 b;
-  if (n == 0) return b;
-  for (int a = 0; a < 3; ++a) { b.lo[a] = INT_MAX; b.hi[a] = INT_MIN; }
-  for (int64_t i = 0; i < n; ++i)
-    for (int a = 0; a < 3; ++a) {
-      b.lo[a] = std::min(b.lo[a], idx[3 * i + a]);
-      b.hi[a] = std::max(b.hi[a], idx[3 * i + a]);
-    }
-  return b;
-}
-
-Box16 HandleBox(const csm_grid3d* g) {
-  Box16 b;
-  b.p = g->g.p;
-  for (int a = 0; a < 3; ++a) {
-    b.lo[a] = g->g.lo[a];
-    b.n[a] = g->g.n[a];
-  }
-  return b;
-}
-
-// Launch shape of k3_nonzero_box / k3_gather_*: x along the rows of a box of n[0] x rows
-// cells, blockIdx.y over the rows, at most `max_blocks` blocks in all.
-dim3 RowGrid(int nx, long long rows, int max_blocks) {
-  const int bx = DivUp(nx, 256);
-  const long long by = std::max<long long>(1, std::min<long long>(rows, max_blocks / bx));
-  return dim3(bx, static_cast<unsigned>(std::min<long long>(by, 65535)));
-}
-
-// The number *n of non-zero voxels of `g` and, when it is at most list_capacity, the voxels in
-// HybridGrid's iteration order (k3_voxel_*) in the device workspaces "g3v_idx" ({x, y, z} each)
-// and "g3v_val" (*d_idx, *d_val), ready on the stream.  Caller holds ctx->mu.  One stream synchronisation for
-// the non-zero box and, if the grid has a non-zero voxel, one for the count.
-csm_status DeviceVoxels3D(const csm_grid3d* g, long long list_capacity, long long* n,
-                          const int** d_idx, const uint16_t** d_val) {
-  Ctx* ctx = g->ctx;
-  cudaStream_t s = ctx->stream;
-  VoxCover c;
-  c.src = HandleBox(g);
-  DevBuf* d_box;
-  CSM_TRY(ctx->Reserve("g3v_box", 6 * sizeof(unsigned), &d_box));
-  unsigned* box = d_box->as<unsigned>();
-  CSM_CUDA(cudaMemsetAsync(box, 0xff, 3 * sizeof(unsigned), s));
-  CSM_CUDA(cudaMemsetAsync(box + 3, 0, 3 * sizeof(unsigned), s));
-  const long long rows = static_cast<long long>(c.src.n[1]) * c.src.n[2];
-  k3_nonzero_box<<<RowGrid(c.src.n[0], rows, ctx->sm_count * 8), 256, 0, s>>>(c.src, box, box + 3);
-  CSM_LAUNCH_CHECK();
-  PinnedBuf& pin = ctx->P("g3v_box");
-  CSM_TRY(pin.Reserve(6 * sizeof(unsigned) + sizeof(long long)));
-  unsigned* h = pin.as<unsigned>();
-  CSM_CUDA(cudaMemcpyAsync(h, box, 6 * sizeof(unsigned), cudaMemcpyDeviceToHost, s));
-  CSM_CUDA(cudaStreamSynchronize(s));
-  *n = 0;
-  if (h[3] == 0u) return CSM_OK;   // no non-zero cell
-  // the 64-aligned cover of the non-zero box (floor division: indices may be negative)
-  long long tiles = static_cast<long long>(262144 / kVoxTile);
-  for (int a = 0; a < 3; ++a) {
-    const int b0 = (c.src.lo[a] + static_cast<int>(h[a]) + 8192) / 64 - 128;
-    const int b1 = (c.src.lo[a] + static_cast<int>(h[3 + a]) - 1 + 8192) / 64 - 128;
-    c.lo[a] = 64 * b0;
-    c.nb[a] = b1 - b0 + 1;
-    tiles *= c.nb[a];
-  }
-  if (tiles >= INT_MAX) {   // one block per tile
-    SetError("the non-zero box of the grid is too large to enumerate");
-    return CSM_E_CAPACITY;
-  }
-  // counts[tiles] stays 0, so that the exclusive scan's last entry is the total
-  size_t scan_bytes = 0;
-  CSM_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, scan_bytes, static_cast<long long*>(nullptr),
-                                         static_cast<long long*>(nullptr), tiles + 1, s));
-  const size_t o_off = (sizeof(long long) * (tiles + 1) + 255) / 256 * 256;
-  const size_t o_temp = 2 * o_off;
-  DevBuf* d_work;
-  CSM_TRY(ctx->Reserve("g3v_scan", o_temp + scan_bytes, &d_work));
-  long long* counts = d_work->as<long long>();
-  long long* offsets = reinterpret_cast<long long*>(d_work->as<char>() + o_off);
-  CSM_CUDA(cudaMemsetAsync(counts + tiles, 0, sizeof(long long), s));
-  k3_voxel_count<<<static_cast<unsigned>(tiles), kVoxThreads, 0, s>>>(c, counts);
-  CSM_LAUNCH_CHECK();
-  CSM_CUDA(cub::DeviceScan::ExclusiveSum(d_work->as<char>() + o_temp, scan_bytes, counts, offsets,
-                                         tiles + 1, s));
-  g_launches.fetch_add(1, std::memory_order_relaxed);
-  long long* h_n = reinterpret_cast<long long*>(h + 6);
-  CSM_CUDA(cudaMemcpyAsync(h_n, offsets + tiles, sizeof(long long), cudaMemcpyDeviceToHost, s));
-  CSM_CUDA(cudaStreamSynchronize(s));
-  *n = *h_n;
-  if (*n > list_capacity) return CSM_OK;
-  DevBuf* out_idx;
-  DevBuf* out_val;
-  CSM_TRY(ctx->Reserve("g3v_idx", sizeof(int) * 3 * *n, &out_idx));
-  CSM_TRY(ctx->Reserve("g3v_val", sizeof(uint16_t) * *n, &out_val));
-  k3_voxel_write<<<static_cast<unsigned>(tiles), kVoxThreads, 0, s>>>(
-      c, counts, offsets, out_idx->as<int>(), out_val->as<uint16_t>());
-  CSM_LAUNCH_CHECK();
-  *d_idx = out_idx->as<int>();
-  *d_val = out_val->as<uint16_t>();
-  return CSM_OK;
-}
-
 }  // namespace
-
-namespace csm {
-
-csm_status NonZeroVoxels3D(const csm_grid3d* g, long long list_capacity, long long* n,
-                           const int** d_idx, const uint16_t** d_val) {
-  return DeviceVoxels3D(g, list_capacity, n, d_idx, d_val);
-}
-
-}  // namespace csm
 
 extern "C" {
 
@@ -1106,8 +809,7 @@ csm_status csm_matcher3d_create(const int32_t* hi_idx, const uint16_t* hi_val, i
   cudaStream_t s = ctx->stream;
   DevBuf& d_idx = ctx->D("m3_idx");
   DevBuf& d_val = ctx->D("m3_val");
-  // depth 0 and the low-resolution volume scattered from the lists; both lists go through
-  // the same staging, so the second waits until the first has been read
+  // depth 0 and the low-resolution volume scattered from the lists
   auto fill_depth0 = [&](const Vol8& level0, uint8_t* dst, const uint8_t* lut) -> csm_status {
     if (hi_n == 0) return CSM_OK;
     CSM_TRY(d_idx.Reserve(sizeof(int) * 3 * hi_n));
@@ -1119,17 +821,8 @@ csm_status csm_matcher3d_create(const int32_t* hi_idx, const uint16_t* hi_val, i
     CSM_LAUNCH_CHECK();
     return CSM_OK;
   };
-  auto fill_low = [&](const Low3Dev& low, uint16_t* dst) -> csm_status {
-    CSM_CUDA(cudaStreamSynchronize(s));
-    if (lo_n == 0) return CSM_OK;
-    CSM_TRY(d_idx.Reserve(sizeof(int) * 3 * lo_n));
-    CSM_TRY(d_val.Reserve(sizeof(uint16_t) * lo_n));
-    CSM_CUDA(cudaMemcpyAsync(d_idx.p, lo_idx, sizeof(int) * 3 * lo_n, cudaMemcpyHostToDevice, s));
-    CSM_CUDA(cudaMemcpyAsync(d_val.p, lo_val, sizeof(uint16_t) * lo_n, cudaMemcpyHostToDevice, s));
-    k3_scatter_u16<<<DivUp(lo_n, 256), 256, 0, s>>>(d_idx.as<int>(), d_val.as<uint16_t>(), lo_n,
-                                                     low, dst);
-    CSM_LAUNCH_CHECK();
-    return CSM_OK;
+  auto fill_low = [&](const Grid3Dev& low, uint16_t* dst) -> csm_status {
+    return ScatterVoxels3(ctx, lo_idx, lo_val, lo_n, BoxOf(low), dst);
   };
   return BuildMatcher3D(ctx, ListBox3(hi_idx, hi_n), hi_res, hi_grid_size, ListBox3(lo_idx, lo_n),
                         lo_res, submap_hist, hist_n, options, fill_depth0, fill_low, out);
@@ -1157,15 +850,11 @@ csm_status csm_matcher3d_create_from_grid3d(const csm_grid3d* hybrid_grid,
   // with csm_profile_enable, the device spans of this call are recorded as "m3g_nonzero_box"
   // (the two passes) and "m3g_build" (everything after the read-back)
   ProfBegin(ctx);
-  CSM_CUDA(cudaMemsetAsync(box, 0xff, 6 * sizeof(unsigned), s));
-  CSM_CUDA(cudaMemsetAsync(box + 6, 0, 6 * sizeof(unsigned), s));
+  const csm_grid3d* grids[2] = {hybrid_grid, low_resolution_hybrid_grid};
   double cells = 0.;
   for (int k = 0; k < 2; ++k) {
-    const long long rows = static_cast<long long>(src[k].n[1]) * src[k].n[2];
-    k3_nonzero_box<<<RowGrid(src[k].n[0], rows, ctx->sm_count * 8), 256, 0, s>>>(
-        src[k], box + 3 * k, box + 6 + 3 * k);
-    CSM_LAUNCH_CHECK();
-    cells += static_cast<double>(rows) * src[k].n[0];
+    CSM_TRY(QueueNonZeroBox3(grids[k], box + 3 * k, box + 6 + 3 * k));
+    cells += static_cast<double>(src[k].n[1]) * src[k].n[2] * src[k].n[0];
   }
   ProfEnd(ctx, "m3g_nonzero_box", cells);
   PinnedBuf& pin = ctx->P("m3g_box");
@@ -1173,9 +862,10 @@ csm_status csm_matcher3d_create_from_grid3d(const csm_grid3d* hybrid_grid,
   unsigned* h = pin.as<unsigned>();
   CSM_CUDA(cudaMemcpyAsync(h, box, 12 * sizeof(unsigned), cudaMemcpyDeviceToHost, s));
   CSM_CUDA(cudaStreamSynchronize(s));
-  VoxelBox3 vb[2];
+  TightBox3 vb[2];
   for (int k = 0; k < 2; ++k) {
     if (h[6 + 3 * k] == 0u) continue;   // no non-zero cell: the empty list's box
+    vb[k].empty = false;
     for (int a = 0; a < 3; ++a) {
       vb[k].lo[a] = src[k].lo[a] + static_cast<int>(h[3 * k + a]);
       vb[k].hi[a] = src[k].lo[a] + static_cast<int>(h[6 + 3 * k + a]) - 1;
@@ -1188,7 +878,7 @@ csm_status csm_matcher3d_create_from_grid3d(const csm_grid3d* hybrid_grid,
     CSM_LAUNCH_CHECK();
     return CSM_OK;
   };
-  auto fill_low = [&](const Low3Dev& low, uint16_t* dst) -> csm_status {
+  auto fill_low = [&](const Grid3Dev& low, uint16_t* dst) -> csm_status {
     const long long rows = static_cast<long long>(low.n[1]) * low.n[2];
     k3_gather_u16<<<RowGrid(low.n[0], rows, 1 << 16), 256, 0, s>>>(src[1], low, dst);
     CSM_LAUNCH_CHECK();
@@ -1199,88 +889,6 @@ csm_status csm_matcher3d_create_from_grid3d(const csm_grid3d* hybrid_grid,
                          low_resolution_hybrid_grid->g.resolution, submap_hist, hist_n, options,
                          fill_depth0, fill_low, out));
   ProfEnd(ctx, "m3g_build", 0.);
-  return CSM_OK;
-}
-
-csm_status csm_grid3d_voxels(const csm_grid3d* grid, int32_t* indices, uint16_t* values,
-                             int64_t capacity, int64_t* num_voxels) {
-  CSM_REQUIRE(grid && num_voxels, "null pointer");
-  CSM_REQUIRE((indices == nullptr) == (values == nullptr), "indices and values go together");
-  Ctx* ctx = grid->ctx;
-  std::lock_guard<std::mutex> lock(ctx->mu);
-  CSM_CUDA(cudaSetDevice(ctx->device));
-  long long n = 0;
-  const int* d_idx = nullptr;
-  const uint16_t* d_val = nullptr;
-  CSM_TRY(DeviceVoxels3D(grid, indices ? capacity : -1, &n, &d_idx, &d_val));
-  *num_voxels = n;
-  if (!indices || n == 0) return CSM_OK;
-  if (capacity < n) {
-    SetError("capacity %lld is below the %lld non-zero voxels", static_cast<long long>(capacity), n);
-    return CSM_E_CAPACITY;
-  }
-  cudaStream_t s = ctx->stream;
-  CSM_CUDA(cudaMemcpyAsync(indices, d_idx, sizeof(int) * 3 * n, cudaMemcpyDeviceToHost, s));
-  CSM_CUDA(cudaMemcpyAsync(values, d_val, sizeof(uint16_t) * n, cudaMemcpyDeviceToHost, s));
-  CSM_CUDA(cudaStreamSynchronize(s));
-  return CSM_OK;
-}
-
-csm_status csm_grid3d_to_proto(const csm_grid3d* grid, uint8_t* buf, int64_t capacity,
-                               int64_t* size) {
-  using namespace wire;
-  CSM_REQUIRE(grid && size, "null pointer");
-  Ctx* ctx = grid->ctx;
-  std::lock_guard<std::mutex> lock(ctx->mu);
-  CSM_CUDA(cudaSetDevice(ctx->device));
-  long long n = 0;
-  const int* d_idx = nullptr;
-  const uint16_t* d_val = nullptr;
-  CSM_TRY(DeviceVoxels3D(grid, LLONG_MAX, &n, &d_idx, &d_val));
-  PinnedBuf& h_idx = ctx->P("g3v_idx");
-  PinnedBuf& h_val = ctx->P("g3v_val");
-  if (n > 0) {
-    CSM_TRY(h_idx.Reserve(sizeof(int) * 3 * n));
-    CSM_TRY(h_val.Reserve(sizeof(uint16_t) * n));
-    cudaStream_t s = ctx->stream;
-    CSM_CUDA(cudaMemcpyAsync(h_idx.p, d_idx, sizeof(int) * 3 * n, cudaMemcpyDeviceToHost, s));
-    CSM_CUDA(cudaMemcpyAsync(h_val.p, d_val, sizeof(uint16_t) * n, cudaMemcpyDeviceToHost, s));
-    CSM_CUDA(cudaStreamSynchronize(s));
-  }
-  const int* idx = h_idx.as<int>();
-  const uint16_t* val = h_val.as<uint16_t>();
-  // proto::HybridGrid (hybrid_grid.proto): resolution = 1, packed sint32 x / y / z_indices =
-  // 3 / 4 / 5, packed int32 values = 6; HybridGrid::ToProto adds the voxels in iteration order
-  int64_t len[4] = {0, 0, 0, 0};
-  for (long long i = 0; i < n; ++i) {
-    for (int a = 0; a < 3; ++a) len[a] += VarintSize(ZigZag32(idx[3 * i + a]));
-    len[3] += VarintSize(val[i]);
-  }
-  const float resolution = grid->g.resolution;
-  int64_t total = FloatFieldSize(resolution);
-  if (n > 0)
-    for (int f = 0; f < 4; ++f) total += DelimitedSize(len[f]);
-  *size = total;
-  if (total >= (int64_t(1) << 31)) {
-    SetError("a serialized HybridGrid of %lld bytes exceeds protobuf's 2 GiB limit",
-             static_cast<long long>(total));
-    return CSM_E_CAPACITY;
-  }
-  if (!buf) return CSM_OK;
-  if (capacity < total) {
-    SetError("capacity %lld is below the %lld bytes of the message",
-             static_cast<long long>(capacity), static_cast<long long>(total));
-    return CSM_E_CAPACITY;
-  }
-  uint8_t* p = PutFloatField(buf, 1, resolution);
-  if (n > 0) {
-    for (int a = 0; a < 3; ++a) {
-      p = PutDelimitedHeader(p, 3 + a, len[a]);
-      for (long long i = 0; i < n; ++i) p = PutVarint(p, ZigZag32(idx[3 * i + a]));
-    }
-    p = PutDelimitedHeader(p, 6, len[3]);
-    for (long long i = 0; i < n; ++i) p = PutVarint(p, val[i]);
-  }
   return CSM_OK;
 }
 

@@ -97,11 +97,6 @@ __device__ __forceinline__ void RayToPixelMask2(int2 b, int2 e, Emit&& emit) {
   }
 }
 
-// Blocks of 256 threads for `work` items, at least one and at most `cap`.
-inline unsigned Blocks(long long work, long long cap = 1 << 16) {
-  return static_cast<unsigned>(std::max(1LL, std::min(cap, (work + 255) / 256)));
-}
-
 }  // namespace csm
 
 #endif  // CSM_INSERT2D_CUH_

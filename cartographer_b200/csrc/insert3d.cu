@@ -10,6 +10,8 @@
 // inside each phase.  Here:
 //   * the host computes every cell (GetCellIndex, :428-433) and checks them, so an invalid
 //     call changes nothing and the box an insert needs is known before any launch;
+//   * GridInsert3 (grid3d.cu) grows the handles' volumes, and installs them only after the
+//     insert's one synchronisation;
 //   * k_ins3_hits (one thread per return), then k_ins3_misses (one per (return, sample)):
 //     a 16-bit atomicCAS applies the table only while the marker is clear; the thread whose
 //     CAS set the marker appends the cell to the insert's touched list;
@@ -37,16 +39,6 @@ struct csm_range_inserter3d {
 
 namespace csm {
 
-struct Box3 {
-  int lo[3];
-  int n[3];
-};
-
-__device__ __forceinline__ unsigned long long BoxIndex(const Box3& b, int x, int y, int z) {
-  return (static_cast<unsigned long long>(z - b.lo[2]) * b.n[1] + (y - b.lo[1])) * b.n[0] +
-         (x - b.lo[0]);
-}
-
 __device__ __forceinline__ void Touched(unsigned long long idx, unsigned long long* list,
                                         unsigned long long* count) {
   list[atomicAdd(count, 1ull)] = idx;
@@ -57,7 +49,7 @@ __global__ void k_ins3_hits(const int* __restrict__ cells, int n, Box3 box, uint
                             unsigned long long* count) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
-  const unsigned long long idx = BoxIndex(box, cells[3 * i], cells[3 * i + 1], cells[3 * i + 2]);
+  const unsigned long long idx = box.Index(cells[3 * i], cells[3 * i + 1], cells[3 * i + 2]);
   if (ApplyTable(vol + idx, hit_table)) Touched(idx, list, count);
 }
 
@@ -77,7 +69,7 @@ __global__ void k_ins3_misses(const int* __restrict__ cells, int n, int per_retu
     if (position < max(0, num_samples - num_free_space_voxels)) continue;
     // origin_cell + delta * position / num_samples: truncating integer division per axis
     const unsigned long long idx =
-        BoxIndex(box, ox + dx * position / num_samples, oy + dy * position / num_samples,
+        box.Index(ox + dx * position / num_samples, oy + dy * position / num_samples,
                  oz + dz * position / num_samples);
     if (ApplyTable(vol + idx, miss_table)) Touched(idx, list, count);
   }
@@ -97,7 +89,7 @@ __global__ void k_ins3_intensity_keys(const int* __restrict__ cells, int m, Box3
                                       unsigned* __restrict__ keys) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= m) return;
-  keys[i] = static_cast<unsigned>(BoxIndex(box, cells[3 * i], cells[3 * i + 1], cells[3 * i + 2]));
+  keys[i] = static_cast<unsigned>(box.Index(cells[3 * i], cells[3 * i + 1], cells[3 * i + 2]));
 }
 
 // One thread per run of equal voxels of the sorted pairs: AddIntensity in return order.
@@ -118,33 +110,6 @@ __global__ void k_ins3_intensity_runs(const unsigned* __restrict__ keys,
   mean[k] = __fdiv_rn(s, __int2float_rn(c));
 }
 
-// Copies the part of box `from` that lies in box `to` (`to` already zero-filled).
-template <typename T>
-__global__ void k_ins3_copy(const T* __restrict__ src, Box3 from, T* __restrict__ dst, Box3 to) {
-  const unsigned long long total =
-      static_cast<unsigned long long>(from.n[0]) * from.n[1] * from.n[2];
-  for (unsigned long long i = blockIdx.x * static_cast<unsigned long long>(blockDim.x) + threadIdx.x;
-       i < total; i += static_cast<unsigned long long>(gridDim.x) * blockDim.x) {
-    const int x = from.lo[0] + static_cast<int>(i % from.n[0]);
-    const int y = from.lo[1] + static_cast<int>(i / from.n[0] % from.n[1]);
-    const int z = from.lo[2] + static_cast<int>(i / (static_cast<unsigned long long>(from.n[0]) * from.n[1]));
-    if (x < to.lo[0] || x >= to.lo[0] + to.n[0] || y < to.lo[1] || y >= to.lo[1] + to.n[1] ||
-        z < to.lo[2] || z >= to.lo[2] + to.n[2])
-      continue;
-    dst[BoxIndex(to, x, y, z)] = src[i];
-  }
-}
-
-__global__ void k_ins3_scatter_made(const int* __restrict__ idx, const float* __restrict__ s,
-                                    const int32_t* __restrict__ c, long long m, Box3 box,
-                                    float* sum, int32_t* count) {
-  const long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x;
-  if (i >= m) return;
-  const unsigned long long k = BoxIndex(box, idx[3 * i], idx[3 * i + 1], idx[3 * i + 2]);
-  sum[k] = s[i];
-  count[k] = c[i];
-}
-
 }  // namespace csm
 
 using namespace csm;
@@ -156,59 +121,10 @@ namespace {
 bool CellIndex(const float* p, float resolution, int* cell) {
   for (int a = 0; a < 3; ++a) {
     const float q = p[a] / resolution;
-    if (!(q > -8192.5f && q < 8191.5f)) return false;
+    if (!(q > -kCube - 0.5f && q < kCube - 0.5f)) return false;
     cell[a] = static_cast<int>(std::lround(q));
   }
   return true;
-}
-
-void Include(TightBox3* t, const int* c) {
-  for (int a = 0; a < 3; ++a) {
-    if (t->empty || c[a] < t->lo[a]) t->lo[a] = c[a];
-    if (t->empty || c[a] > t->hi[a]) t->hi[a] = c[a];
-  }
-  t->empty = false;
-}
-
-bool Covers(const Box3& b, const TightBox3& t) {
-  if (t.empty) return true;
-  for (int a = 0; a < 3; ++a)
-    if (t.lo[a] < b.lo[a] || t.hi[a] >= b.lo[a] + b.n[a]) return false;
-  return true;
-}
-
-// The box a handle grows to (DESIGN §9): the tight box plus extent / 8 voxels on each side of
-// every axis, inside the 2^14 cube — at most 1.25^3 < 2x the tight box's volume, and every
-// regrowth extends some axis's tight extent by more than 1/8 since the last one.
-Box3 SlackBox(const TightBox3& t) {
-  Box3 b;
-  for (int a = 0; a < 3; ++a) {
-    const int s = (t.hi[a] - t.lo[a] + 1) / 8;
-    b.lo[a] = std::max(-8192, t.lo[a] - s);
-    b.n[a] = std::min(8191, t.hi[a] + s) - b.lo[a] + 1;
-  }
-  return b;
-}
-
-size_t Volume(const Box3& b) { return static_cast<size_t>(b.n[0]) * b.n[1] * b.n[2]; }
-
-unsigned Blocks(long long work, long long cap = 1 << 16) {
-  return static_cast<unsigned>(std::max(1LL, std::min(cap, (work + 255) / 256)));
-}
-
-// A zero-filled volume of box `to` holding what `old` held over box `from`.
-template <typename T>
-csm_status Regrow(T* old, const Box3& from, const Box3& to, cudaStream_t s, T** out) {
-  const size_t bytes = std::max<size_t>((Volume(to) * sizeof(T) + 3) / 4 * 4, 256);
-  T* p = nullptr;
-  CSM_CUDA(cudaMalloc(&p, bytes));
-  *out = p;
-  CSM_CUDA(cudaMemsetAsync(p, 0, bytes, s));
-  if (old) {
-    k_ins3_copy<T><<<Blocks(static_cast<long long>(Volume(from))), 256, 0, s>>>(old, from, p, to);
-    CSM_LAUNCH_CHECK();
-  }
-  return CSM_OK;
 }
 
 }  // namespace
@@ -282,10 +198,10 @@ csm_status csm_range_inserter3d_insert(const csm_range_inserter3d* inserter,
                                               std::abs(c[2] - origin_cell[2])));
     CSM_REQUIRE(num_samples < (1 << 15), "num_samples");   // range_data_inserter_3d.cc:38
     max_samples = std::max(max_samples, num_samples);
-    Include(&need, c);
+    need.Include(c);
   }
   // every miss cell lies between the origin cell and a hit cell
-  if (n > 0) Include(&need, origin_cell);
+  if (n > 0) need.Include(origin_cell);
   const bool with_intensity = intensity_grid != nullptr && intensities != nullptr;
   std::vector<int> icells;
   std::vector<float> ivalues;
@@ -300,88 +216,14 @@ csm_status csm_range_inserter3d_insert(const csm_range_inserter3d* inserter,
                   "intensity cell outside the 2^14 cube");
       icells.insert(icells.end(), c, c + 3);
       ivalues.push_back(intensities[i]);
-      Include(&ineed, c);
+      ineed.Include(c);
     }
   }
   const int m = static_cast<int>(ivalues.size());
-  Box3 box, grown;
-  std::copy(grid->g.lo, grid->g.lo + 3, box.lo);
-  std::copy(grid->g.n, grid->g.n + 3, box.n);
-  const bool grow = !Covers(box, need);
-  if (grow) {
-    grown = SlackBox(need);
-    CSM_REQUIRE(Volume(grown) < (size_t(8) << 30), "dense volume too large");
-  }
-  Box3 ibox{}, igrown{};
-  bool igrow = false;
-  if (with_intensity) {
-    std::copy(intensity_grid->lo, intensity_grid->lo + 3, ibox.lo);
-    std::copy(intensity_grid->n, intensity_grid->n + 3, ibox.n);
-    igrow = !Covers(ibox, ineed);
-    if (igrow) {
-      igrown = SlackBox(ineed);
-      CSM_REQUIRE(Volume(igrown) < (size_t(4) << 30), "dense volume too large");
-    }
-  }
-
-  CSM_CUDA(cudaSetDevice(ctx->device));
+  GridInsert3 tx(grid, with_intensity ? intensity_grid : nullptr);
+  CSM_TRY(tx.Grow(need, ineed));
+  CSM_TRY(tx.Begin());
   cudaStream_t s = ctx->stream;
-  std::vector<void*> retired;   // freed once the stream has passed the copies
-  CSM_CUDA(cudaEventRecord(ctx->ev0, s));
-  // ---- growth ----
-  if (grow) {
-    uint16_t* p;
-    CSM_TRY(Regrow<uint16_t>(grid->d_vol, box, grown, s, &p));
-    retired.push_back(grid->d_vol);
-    grid->d_vol = p;
-    grid->g.p = p;
-    std::copy(grown.lo, grown.lo + 3, grid->g.lo);
-    std::copy(grown.n, grown.n + 3, grid->g.n);
-    box = grown;
-  }
-  grid->tight = need;
-  if (with_intensity) {
-    csm_intensity_grid3d* ig = intensity_grid;
-    if (!ig->d_sum) {   // first insert: the AverageIntensityData volumes of what it was made from
-      CSM_TRY(Regrow<float>(nullptr, ibox, ibox, s, &ig->d_sum));
-      CSM_TRY(Regrow<int32_t>(nullptr, ibox, ibox, s, &ig->d_count));
-      const long long made = static_cast<long long>(ig->made_sum.size());
-      if (made > 0) {
-        DevBuf& d_made = ctx->D("ins3_made");
-        const size_t o_sum = (sizeof(int) * 3 * made + 255) / 256 * 256;
-        const size_t o_cnt = o_sum + (sizeof(float) * made + 255) / 256 * 256;
-        CSM_TRY(d_made.Reserve(o_cnt + sizeof(int32_t) * made));
-        char* d = d_made.as<char>();
-        CSM_CUDA(cudaMemcpyAsync(d, ig->made_idx.data(), sizeof(int) * 3 * made,
-                                 cudaMemcpyHostToDevice, s));
-        CSM_CUDA(cudaMemcpyAsync(d + o_sum, ig->made_sum.data(), sizeof(float) * made,
-                                 cudaMemcpyHostToDevice, s));
-        CSM_CUDA(cudaMemcpyAsync(d + o_cnt, ig->made_count.data(), sizeof(int32_t) * made,
-                                 cudaMemcpyHostToDevice, s));
-        k_ins3_scatter_made<<<Blocks(made, 1LL << 30), 256, 0, s>>>(
-            reinterpret_cast<const int*>(d), reinterpret_cast<const float*>(d + o_sum),
-            reinterpret_cast<const int32_t*>(d + o_cnt), made, ibox, ig->d_sum, ig->d_count);
-        CSM_LAUNCH_CHECK();
-      }
-    }
-    if (igrow) {
-      float *mean, *sum;
-      int32_t* count;
-      CSM_TRY(Regrow<float>(ig->d_vol, ibox, igrown, s, &mean));
-      retired.push_back(ig->d_vol);
-      ig->d_vol = mean;
-      CSM_TRY(Regrow<float>(ig->d_sum, ibox, igrown, s, &sum));
-      retired.push_back(ig->d_sum);
-      ig->d_sum = sum;
-      CSM_TRY(Regrow<int32_t>(ig->d_count, ibox, igrown, s, &count));
-      retired.push_back(ig->d_count);
-      ig->d_count = count;
-      std::copy(igrown.lo, igrown.lo + 3, ig->lo);
-      std::copy(igrown.n, igrown.n + 3, ig->n);
-      ibox = igrown;
-    }
-    ig->tight = ineed;
-  }
   // ---- upload: hit cells | intensity cells | intensities ----
   const size_t o_icell = (sizeof(int) * 3 * static_cast<size_t>(n) + 255) / 256 * 256;
   const size_t o_ival = o_icell + (sizeof(int) * 3 * static_cast<size_t>(m) + 255) / 256 * 256;
@@ -401,7 +243,7 @@ csm_status csm_range_inserter3d_insert(const csm_range_inserter3d* inserter,
     // ---- occupancy: hits, misses, FinishUpdate ----
     const int per_return = std::min(nfsv, max_samples);
     const unsigned long long list_cap = std::min<unsigned long long>(
-        static_cast<unsigned long long>(n) * (per_return + 1), Volume(box));
+        static_cast<unsigned long long>(n) * (per_return + 1), tx.box.Volume());
     DevBuf& d_list = ctx->D("ins3_touched");
     CSM_TRY(d_list.Reserve(sizeof(unsigned long long) * (list_cap + 1)));
     unsigned long long* d_count = d_list.as<unsigned long long>();
@@ -410,21 +252,21 @@ csm_status csm_range_inserter3d_insert(const csm_range_inserter3d* inserter,
     const uint16_t* hit_table = inserter->d_tables;
     const uint16_t* miss_table = inserter->d_tables + kValueCount;
     ProfBegin(ctx);
-    k_ins3_hits<<<Blocks(n, 1LL << 30), 256, 0, s>>>(d_cells, n, box, grid->d_vol, hit_table,
+    k_ins3_hits<<<Blocks(n, 1LL << 30), 256, 0, s>>>(d_cells, n, tx.box, tx.vol, hit_table,
                                                     d_touched, d_count);
     CSM_LAUNCH_CHECK();
     ProfEnd(ctx, "k_ins3_hits", n);
     if (per_return > 0) {
       ProfBegin(ctx);
       k_ins3_misses<<<Blocks(static_cast<long long>(n) * per_return), 256, 0, s>>>(
-          d_cells, n, per_return, origin_cell[0], origin_cell[1], origin_cell[2], nfsv, box,
-          grid->d_vol, miss_table, d_touched, d_count);
+          d_cells, n, per_return, origin_cell[0], origin_cell[1], origin_cell[2], nfsv, tx.box,
+          tx.vol, miss_table, d_touched, d_count);
       CSM_LAUNCH_CHECK();
       ProfEnd(ctx, "k_ins3_misses", static_cast<double>(n) * per_return);
     }
     ProfBegin(ctx);
     k_ins3_finish<<<Blocks(static_cast<long long>(list_cap)), 256, 0, s>>>(d_touched, d_count,
-                                                                         grid->d_vol);
+                                                                         tx.vol);
     CSM_LAUNCH_CHECK();
     ProfEnd(ctx, "k_ins3_finish", static_cast<double>(list_cap));
     // ---- intensities ----
@@ -432,7 +274,7 @@ csm_status csm_range_inserter3d_insert(const csm_range_inserter3d* inserter,
       const int* d_icells = reinterpret_cast<const int*>(d + o_icell);
       const float* d_ivals = reinterpret_cast<const float*>(d + o_ival);
       int end_bit = 1;
-      while (end_bit < 32 && (Volume(ibox) - 1) >> end_bit) ++end_bit;
+      while (end_bit < 32 && (tx.ibox.Volume() - 1) >> end_bit) ++end_bit;
       size_t temp_bytes = 0;
       CSM_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, temp_bytes, static_cast<unsigned*>(nullptr),
                                                static_cast<unsigned*>(nullptr),
@@ -448,80 +290,20 @@ csm_status csm_range_inserter3d_insert(const csm_range_inserter3d* inserter,
       unsigned* keys_sorted = reinterpret_cast<unsigned*>(w + o_kout);
       float* vals_sorted = reinterpret_cast<float*>(w + o_vout);
       ProfBegin(ctx);
-      k_ins3_intensity_keys<<<Blocks(m, 1LL << 30), 256, 0, s>>>(d_icells, m, ibox, keys);
+      k_ins3_intensity_keys<<<Blocks(m, 1LL << 30), 256, 0, s>>>(d_icells, m, tx.ibox, keys);
       CSM_LAUNCH_CHECK();
       CSM_CUDA(cub::DeviceRadixSort::SortPairs(w + o_temp, temp_bytes, keys, keys_sorted, d_ivals,
                                                vals_sorted, m, 0, end_bit, s));
       g_launches.fetch_add(1, std::memory_order_relaxed);
       k_ins3_intensity_runs<<<Blocks(m, 1LL << 30), 256, 0, s>>>(
-          keys_sorted, vals_sorted, m, intensity_grid->d_sum, intensity_grid->d_count,
-          intensity_grid->d_vol);
+          keys_sorted, vals_sorted, m, tx.sum, tx.count, tx.mean);
       CSM_LAUNCH_CHECK();
       ProfEnd(ctx, "k_ins3_intensity", m);
     }
   }
   CSM_CUDA(cudaEventRecord(ctx->ev1, s));
   CSM_CUDA(cudaStreamSynchronize(s));
-  for (void* p : retired) CSM_CUDA(cudaFree(p));
-  if (with_intensity && !intensity_grid->made_sum.empty()) {
-    // the volumes hold it now
-    std::vector<int32_t>().swap(intensity_grid->made_idx);
-    std::vector<int32_t>().swap(intensity_grid->made_count);
-    std::vector<float>().swap(intensity_grid->made_sum);
-  }
-  if (stats) {
-    std::memset(stats, 0, sizeof(*stats));
-    stats->host_syncs = 1;
-    cudaEventElapsedTime(&stats->device_ms, ctx->ev0, ctx->ev1);
-  }
-  return CSM_OK;
-}
-
-csm_status csm_grid3d_read(const csm_grid3d* grid, int32_t lo[3], int32_t dims[3],
-                           uint16_t* out) {
-  CSM_REQUIRE(grid && lo && dims, "null pointer");
-  std::lock_guard<std::mutex> lock(grid->ctx->mu);
-  for (int a = 0; a < 3; ++a) {
-    lo[a] = grid->g.lo[a];
-    dims[a] = grid->g.n[a];
-  }
-  if (!out) return CSM_OK;
-  CSM_CUDA(cudaSetDevice(grid->ctx->device));
-  const size_t vox = static_cast<size_t>(dims[0]) * dims[1] * dims[2];
-  CSM_CUDA(cudaMemcpyAsync(out, grid->d_vol, vox * sizeof(uint16_t), cudaMemcpyDeviceToHost,
-                           grid->ctx->stream));
-  CSM_CUDA(cudaStreamSynchronize(grid->ctx->stream));
-  return CSM_OK;
-}
-
-csm_status csm_intensity_grid3d_read(const csm_intensity_grid3d* grid, int32_t lo[3],
-                                     int32_t dims[3], float* mean, float* sum, int32_t* count) {
-  CSM_REQUIRE(grid && lo && dims, "null pointer");
-  std::lock_guard<std::mutex> lock(grid->ctx->mu);
-  for (int a = 0; a < 3; ++a) {
-    lo[a] = grid->lo[a];
-    dims[a] = grid->n[a];
-  }
-  if (!mean) return CSM_OK;
-  CSM_CUDA(cudaSetDevice(grid->ctx->device));
-  cudaStream_t s = grid->ctx->stream;
-  const size_t vox = static_cast<size_t>(dims[0]) * dims[1] * dims[2];
-  CSM_CUDA(cudaMemcpyAsync(mean, grid->d_vol, vox * sizeof(float), cudaMemcpyDeviceToHost, s));
-  if (grid->d_sum) {
-    if (sum) CSM_CUDA(cudaMemcpyAsync(sum, grid->d_sum, vox * 4, cudaMemcpyDeviceToHost, s));
-    if (count) CSM_CUDA(cudaMemcpyAsync(count, grid->d_count, vox * 4, cudaMemcpyDeviceToHost, s));
-  } else {   // never inserted into: the list it was made from
-    if (sum) std::fill(sum, sum + vox, 0.f);
-    if (count) std::fill(count, count + vox, 0);
-    for (size_t i = 0; i < grid->made_sum.size(); ++i) {
-      const int* c = &grid->made_idx[3 * i];
-      const size_t k = (static_cast<size_t>(c[2] - lo[2]) * dims[1] + (c[1] - lo[1])) * dims[0] +
-                       (c[0] - lo[0]);
-      if (sum) sum[k] = grid->made_sum[i];
-      if (count) count[k] = grid->made_count[i];
-    }
-  }
-  CSM_CUDA(cudaStreamSynchronize(s));
+  tx.Commit(stats);
   return CSM_OK;
 }
 

@@ -693,8 +693,8 @@ void FillIntensity3(const csm_ceres_job3d& j, const csm_ceres_intensity_job3d* i
     Ref3IntensityCloud& c = d->c[b];
     c.ivol = g->d_vol;
     for (int a = 0; a < 3; ++a) {
-      c.ilo[a] = g->lo[a];
-      c.in[a] = g->n[a];
+      c.ilo[a] = g->box.lo[a];
+      c.in[a] = g->box.n[a];
     }
     c.iresolution = g->resolution;
     c.intensity_threshold = o->intensity_threshold[b];
@@ -750,15 +750,6 @@ void Stage3(const csm_ceres_job3d* jobs, const csm_ceres_intensity_job3d* ij,
       std::memcpy(f + hi->c[b].intensity_off, ij[j].intensities[b],
                   sizeof(float) * static_cast<size_t>(job.num_points[b]));
   }
-}
-
-__global__ void k_intensity_scatter(const int* __restrict__ idx, const float* __restrict__ v,
-                                    long long n, int lo0, int lo1, int lo2, int n0, int n1,
-                                    float* __restrict__ vol) {
-  const long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x;
-  if (i >= n) return;
-  const long long x = idx[3 * i] - lo0, y = idx[3 * i + 1] - lo1, z = idx[3 * i + 2] - lo2;
-  vol[(z * n1 + y) * n0 + x] = v[i];
 }
 
 csm_status MatchBatch3(const csm_ceres_job3d* jobs, const csm_ceres_intensity_job3d* ij,
@@ -925,75 +916,6 @@ csm_status csm_ceres_evaluate3d_intensity(const csm_ceres_job3d* job,
                                           double* jacobian) {
   CSM_REQUIRE(intensity_job != nullptr, "null pointer");
   return Evaluate3(job, intensity_job, options, intensity_options, pose, residuals, jacobian);
-}
-
-csm_status csm_intensity_grid3d_create(const int32_t* idx, const float* sum, const int32_t* count,
-                                       int64_t n, float resolution, int32_t device,
-                                       csm_intensity_grid3d** out) {
-  CSM_REQUIRE(out != nullptr, "null pointer");
-  CSM_REQUIRE(n >= 0 && (n == 0 || (idx && sum && count)), "voxel list");
-  CSM_REQUIRE(resolution > 0.f, "resolution");
-  Ctx* ctx;
-  CSM_TRY(GetCtx(device, &ctx));
-  std::lock_guard<std::mutex> lock(ctx->mu);
-  CSM_CUDA(cudaSetDevice(device));
-  cudaStream_t s = ctx->stream;
-  std::unique_ptr<csm_intensity_grid3d> g(new csm_intensity_grid3d);
-  g->ctx = ctx;
-  int lo[3] = {0, 0, 0}, hi[3] = {0, 0, 0};
-  for (int64_t i = 0; i < n; ++i)
-    for (int a = 0; a < 3; ++a) {
-      const int v = idx[3 * i + a];
-      if (i == 0 || v < lo[a]) lo[a] = v;
-      if (i == 0 || v > hi[a]) hi[a] = v;
-    }
-  for (int a = 0; a < 3; ++a) {
-    CSM_REQUIRE(lo[a] >= -8192 && hi[a] < 8192, "voxel index outside the 2^14 cube");  // hybrid_grid.h:387
-    g->lo[a] = lo[a];
-    g->n[a] = hi[a] - lo[a] + 1;
-    g->tight.lo[a] = lo[a];
-    g->tight.hi[a] = hi[a];
-  }
-  g->tight.empty = n == 0;
-  const size_t vox = static_cast<size_t>(g->n[0]) * g->n[1] * g->n[2];
-  CSM_REQUIRE(vox < (size_t(4) << 30), "dense volume too large");
-  // IntensityHybridGrid::GetIntensity (hybrid_grid.h:562-569): the float mean, 0 where no
-  // intensity was added
-  std::vector<float> value(static_cast<size_t>(n));
-  for (int64_t i = 0; i < n; ++i) {
-    CSM_REQUIRE(count[i] >= 0, "negative intensity count");
-    value[i] = count[i] == 0 ? 0.f : sum[i] / static_cast<float>(count[i]);
-  }
-  CSM_CUDA(cudaMalloc(&g->d_vol, std::max<size_t>(vox * 4, 256)));
-  CSM_CUDA(cudaMemsetAsync(g->d_vol, 0, std::max<size_t>(vox * 4, 256), s));
-  g->resolution = resolution;
-  if (n > 0) {
-    DevBuf& d_idx = ctx->D("g3i_idx");
-    DevBuf& d_val = ctx->D("g3i_val");
-    CSM_TRY(d_idx.Reserve(sizeof(int) * 3 * n));
-    CSM_TRY(d_val.Reserve(sizeof(float) * n));
-    CSM_CUDA(cudaMemcpyAsync(d_idx.p, idx, sizeof(int) * 3 * n, cudaMemcpyHostToDevice, s));
-    CSM_CUDA(cudaMemcpyAsync(d_val.p, value.data(), sizeof(float) * n, cudaMemcpyHostToDevice, s));
-    k_intensity_scatter<<<static_cast<unsigned>((n + 255) / 256), 256, 0, s>>>(
-        d_idx.as<int>(), d_val.as<float>(), n, lo[0], lo[1], lo[2], g->n[0], g->n[1], g->d_vol);
-    CSM_LAUNCH_CHECK();
-  }
-  CSM_CUDA(cudaStreamSynchronize(s));
-  // what a first insert fills its sum / count volumes from (insert3d.cu)
-  g->made_idx.assign(idx, idx + 3 * n);
-  g->made_sum.assign(sum, sum + n);
-  g->made_count.assign(count, count + n);
-  *out = g.release();
-  return CSM_OK;
-}
-
-csm_status csm_intensity_grid3d_destroy(csm_intensity_grid3d* grid) {
-  if (!grid) return CSM_OK;
-  std::lock_guard<std::mutex> lock(grid->ctx->mu);
-  cudaSetDevice(grid->ctx->device);
-  cudaStreamSynchronize(grid->ctx->stream);
-  delete grid;
-  return CSM_OK;
 }
 
 }  // extern "C"

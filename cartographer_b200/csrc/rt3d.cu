@@ -22,7 +22,6 @@
 #include "common.cuh"
 #include "grid3d.cuh"
 #include "rigid3f.h"
-#include "value_conversion.h"
 
 namespace csm {
 
@@ -30,14 +29,6 @@ struct Rt3Params {
   int n;          // points
   int T, R;       // translations, rotations
 };
-
-__global__ void k_rt3_scatter(const int* __restrict__ idx, const uint16_t* __restrict__ values,
-                              long long n, Grid3Dev g, uint16_t* __restrict__ out) {
-  const long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x;
-  if (i >= n) return;
-  const int x = idx[3 * i] - g.lo[0], y = idx[3 * i + 1] - g.lo[1], z = idx[3 * i + 2] - g.lo[2];
-  out[(static_cast<size_t>(z) * g.n[1] + y) * g.n[0] + x] = values[i];
-}
 
 constexpr int kRt3Chunk = 256;
 
@@ -111,78 +102,6 @@ k_rt3_match(const Grid3Dev G, const Rt3Params P, const float* __restrict__ xyz,
 }  // namespace csm
 
 using namespace csm;
-
-extern "C" {
-
-csm_status csm_grid3d_create(const int32_t* idx, const uint16_t* values, int64_t n,
-                             float resolution, int32_t device, csm_grid3d** out) {
-  CSM_REQUIRE(out != nullptr, "null pointer");
-  CSM_REQUIRE(n >= 0 && (n == 0 || (idx && values)), "voxel list");
-  CSM_REQUIRE(resolution > 0.f, "resolution");
-  Ctx* ctx;
-  CSM_TRY(GetCtx(device, &ctx));
-  std::lock_guard<std::mutex> lock(ctx->mu);
-  CSM_CUDA(cudaSetDevice(device));
-  cudaStream_t s = ctx->stream;
-  std::unique_ptr<csm_grid3d> g(new csm_grid3d);
-  g->ctx = ctx;
-  Grid3Dev& d = g->g;
-  std::memset(&d, 0, sizeof(d));
-  int lo[3] = {0, 0, 0}, hi[3] = {0, 0, 0};
-  for (int64_t i = 0; i < n; ++i)
-    for (int a = 0; a < 3; ++a) {
-      const int v = idx[3 * i + a];
-      if (i == 0 || v < lo[a]) lo[a] = v;
-      if (i == 0 || v > hi[a]) hi[a] = v;
-    }
-  for (int a = 0; a < 3; ++a) {
-    CSM_REQUIRE(lo[a] >= -8192 && hi[a] < 8192, "voxel index outside the 2^14 cube");  // hybrid_grid.h:387
-    d.lo[a] = lo[a];
-    d.n[a] = hi[a] - lo[a] + 1;
-    g->tight.lo[a] = lo[a];
-    g->tight.hi[a] = hi[a];
-  }
-  g->tight.empty = n == 0;
-  const size_t vox = static_cast<size_t>(d.n[0]) * d.n[1] * d.n[2];
-  CSM_REQUIRE(vox < (size_t(8) << 30), "dense volume too large");
-  // whole 32-bit words: the inserter clears update markers with 32-bit atomics (insert3d.cu)
-  const size_t bytes = std::max<size_t>((vox * 2 + 3) / 4 * 4, 256);
-  CSM_CUDA(cudaMalloc(&g->d_vol, bytes));
-  CSM_CUDA(cudaMemsetAsync(g->d_vol, 0, bytes, s));
-  d.p = g->d_vol;
-  d.resolution = resolution;
-  {
-    const ValueConversion probability = MakeValueConversion(kMinProbability, kMaxProbability);
-    d.k_scale = probability.scale;
-    d.bias = probability.bias;
-    d.min_probability = kMinProbability;
-  }
-  if (n > 0) {
-    DevBuf& d_idx = ctx->D("g3_idx");
-    DevBuf& d_val = ctx->D("g3_val");
-    CSM_TRY(d_idx.Reserve(sizeof(int) * 3 * n));
-    CSM_TRY(d_val.Reserve(sizeof(uint16_t) * n));
-    CSM_CUDA(cudaMemcpyAsync(d_idx.p, idx, sizeof(int) * 3 * n, cudaMemcpyHostToDevice, s));
-    CSM_CUDA(cudaMemcpyAsync(d_val.p, values, sizeof(uint16_t) * n, cudaMemcpyHostToDevice, s));
-    k_rt3_scatter<<<DivUp(n, 256), 256, 0, s>>>(d_idx.as<int>(), d_val.as<uint16_t>(), n, d,
-                                                 g->d_vol);
-    CSM_LAUNCH_CHECK();
-  }
-  CSM_CUDA(cudaStreamSynchronize(s));
-  *out = g.release();
-  return CSM_OK;
-}
-
-csm_status csm_grid3d_destroy(csm_grid3d* grid) {
-  if (!grid) return CSM_OK;
-  std::lock_guard<std::mutex> lock(grid->ctx->mu);
-  cudaSetDevice(grid->ctx->device);
-  cudaStreamSynchronize(grid->ctx->stream);
-  delete grid;
-  return CSM_OK;
-}
-
-}  // extern "C"
 
 namespace {
 

@@ -305,7 +305,7 @@ csm_status csm_grid3d_to_texture(const csm_grid3d* grid, const double global_sub
   long long n = 0;
   const int* d_idx = nullptr;
   const uint16_t* d_val = nullptr;
-  CSM_TRY(NonZeroVoxels3D(grid, LLONG_MAX, &n, &d_idx, &d_val));
+  CSM_TRY(DeviceVoxels3D(grid, LLONG_MAX, &n, &d_idx, &d_val));
   if (n >= INT_MAX) {   // the sort's item count
     SetError("%lld non-zero voxels are too many to draw", n);
     return CSM_E_CAPACITY;

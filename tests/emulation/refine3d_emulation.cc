@@ -63,7 +63,7 @@ void FillEmuJob(int num_clouds, const uint16_t* const* vol, const int32_t* lo, c
       c.n[a] = n[3 * b + a];
     }
     c.resolution = resolution[b];
-    // as rt3d.cu fills them
+    // as MakeGrid3Dev (grid3d.cu) fills them
     const csm::ValueConversion probability =
         csm::MakeValueConversion(csm::kMinProbability, csm::kMaxProbability);
     c.k_scale = probability.scale;
