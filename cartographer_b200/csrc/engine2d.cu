@@ -1300,10 +1300,18 @@ k_expand_lattice(const JobDev* __restrict__ jobs, const ScanInfo* __restrict__ i
   int i0 = (nd.xo - si.min_x) >> h, j0 = (nd.yo - si.min_y) >> h;  // parent lattice coords
   int toff = j0 * ids + i0;
   bool x2 = !(nd.xo + s > si.max_x), y2 = !(nd.yo + s > si.max_y);
-  if (live && sub == 0) {
-    // a parent ruled out early still counts: the bound decided all its children
-    atomicAdd(&counters[0], 1ull + y2 + x2 + (x2 && y2));
-    atomicAdd(&counters[1], 1ull);
+  {
+    // a parent ruled out early still counts: the bound decided all its children.  The
+    // warp's counts are summed first: one atomic per counter and item instead of one per
+    // parent, which all went to the same two addresses.
+    const bool counted = live && sub == 0;
+    const unsigned scored =
+        __reduce_add_sync(0xffffffffu, counted ? 1u + y2 + x2 + (x2 && y2) : 0u);
+    const unsigned parents = __popc(__ballot_sync(0xffffffffu, counted));
+    if (lane == 0 && parents) {
+      atomicAdd(&counters[0], static_cast<unsigned long long>(scored));
+      atomicAdd(&counters[1], static_cast<unsigned long long>(parents));
+    }
   }
   unsigned sum0 = 0, sum1 = 0, sum2 = 0, sum3 = 0;  // slots 2*ix+iy: 00, 01, 10, 11
   // Early exit.  Every child window lies inside the parent's, so at each point the
