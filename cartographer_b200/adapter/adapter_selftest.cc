@@ -1050,6 +1050,70 @@ int main() {
       std::printf("\n");
     }
   }
+  {
+    // io::XRayPointsProcessor on three batches in three floors (the fixture of
+    // tests/test_gpu_adapter_xray.py): batch b has start_time b, batch 1 has no colours, floor 0
+    // holds times 0..1, floor 1 times 1..2 and floor 2 none.  The stand-in Image writes its
+    // cairo words, so the RESULT lines list every floor's pixels.
+    struct Writer : io::FileWriter {
+      std::map<std::string, std::string>* files;
+      std::string name, data;
+      bool WriteHeader(const char* d, size_t n) override { data.insert(0, d, n); return true; }
+      bool Write(const char* d, size_t n) override { data.append(d, n); return true; }
+      bool Close() override { (*files)[name] = data; return true; }
+      std::string GetFilename() override { return name; }
+    };
+    struct Sink : io::PointsProcessor {
+      int batches = 0;
+      void Process(std::unique_ptr<io::PointsBatch>) override { ++batches; }
+      FlushResult Flush() override { return FlushResult::kFinished; }
+    } sink;
+    std::map<std::string, std::string> files;
+    const io::FileWriterFactory factory = [&files](const std::string& name) {
+      auto w = std::make_unique<Writer>();
+      w->files = &files;
+      w->name = name;
+      return std::unique_ptr<io::FileWriter>(std::move(w));
+    };
+    std::vector<mapping::Floor> floors(3);
+    floors[0].timespans = {{0, 1}};
+    floors[1].timespans = {{1, 2}};
+    floors[2].timespans = {{5, 6}};
+    const transform::Rigid3f transform({0.5f, -0.25f, 0.125f}, {0.8f, 0.f, 0.6f, 0.f});
+    io::XRayPointsProcessor processor(0.25, 1.5, transform, floors,
+                                      io::XRayPointsProcessor::DrawTrajectories::kNo, "xray", {},
+                                      factory, &sink);
+    std::printf("RESULT xr_action %s\n", io::XRayPointsProcessor::kConfigurationFileActionName);
+    for (int b = 0; b < 3; ++b) {
+      auto batch = std::make_unique<io::PointsBatch>();
+      batch->start_time = b;
+      for (int i = 0; i < 300; ++i) {
+        sensor::RangefinderPoint p{{{float((i * 7) % 23) * 0.1f,
+                                     float((i * 11) % 17) * 0.1f - 0.8f,
+                                     float(i % 9) * 0.15f + float(b) * 0.2f}}};
+        batch->points.push_back(p);
+        if (b != 1) {
+          batch->colors.push_back(
+              {float(i % 10) * 0.1f, float(b) * 0.3f, float((i * 3) % 7) / 7.f});
+        }
+      }
+      processor.Process(std::move(batch));
+    }
+    std::printf("RESULT xr_flush %d %d\n",
+                processor.Flush() == io::PointsProcessor::FlushResult::kFinished, sink.batches);
+    const auto box = processor.bounding_box();
+    std::printf("RESULT xr_box %d %d %d %d %d %d %d\n", int(box.empty), box.min[0], box.min[1],
+                box.min[2], box.max[0], box.max[1], box.max[2]);
+    for (const auto& file : files) {
+      std::printf("RESULT xr_file_%s", file.first.c_str());
+      for (size_t i = 0; i + 4 <= file.second.size(); i += 4) {
+        uint32_t word;
+        std::memcpy(&word, file.second.data() + i, 4);
+        std::printf(" %u", word);
+      }
+      std::printf("\n");
+    }
+  }
   if (trimmer_cases::Run() != 0) return 1;
   return 0;
 }

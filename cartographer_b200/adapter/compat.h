@@ -706,11 +706,74 @@ using flat_hash_set = std::unordered_set<T>;
 }  // namespace absl
 
 namespace cartographer {
+namespace common {
+using Time = int64_t;   // common/time.h: a std::chrono time point there, compared the same way
+}  // namespace common
+namespace transform {
+// transform/rigid_transform.h:116-196 (Rigid3<float>): the accessors the X-ray adapter reads.
+class Rigid3f {
+ public:
+  struct Vector { float x_, y_, z_; float x() const { return x_; } float y() const { return y_; } float z() const { return z_; } };
+  struct Quaternion { float w_, x_, y_, z_; float w() const { return w_; } float x() const { return x_; } float y() const { return y_; } float z() const { return z_; } };
+  Rigid3f(const Vector& t, const Quaternion& q) : t_(t), q_(q) {}
+  const Vector& translation() const { return t_; }
+  const Quaternion& rotation() const { return q_; }
+ private:
+  Vector t_;
+  Quaternion q_;
+};
+}  // namespace transform
+namespace mapping {
+// mapping/detect_floors.h:26-39.
+struct Timespan {
+  common::Time start;
+  common::Time end;
+};
+struct Floor {
+  std::vector<Timespan> timespans;
+  double z;
+};
+namespace proto {
+struct Trajectory {};   // mapping/proto/trajectory.proto: not drawn outside a checkout
+}  // namespace proto
+}  // namespace mapping
 namespace io {
 using FloatColor = std::array<float, 3>;   // io/color.h
+using Uint8Color = std::array<uint8_t, 3>;
+// io/file_writer.h:28-65.
+class FileWriter {
+ public:
+  virtual ~FileWriter() {}
+  virtual bool WriteHeader(const char* data, size_t len) = 0;
+  virtual bool Write(const char* data, size_t len) = 0;
+  virtual bool Close() = 0;
+  virtual std::string GetFilename() = 0;
+};
+using FileWriterFactory = std::function<std::unique_ptr<FileWriter>(const std::string& filename)>;
+// io/image.h:30-61 without cairo: the pixels as cairo ARGB32 words, row-major.  A checkout's
+// WritePng encodes a PNG through cairo; this stand-in writes the words themselves
+// (little-endian), which is what the self-test compares.
+class Image {
+ public:
+  Image(int width, int height) : width_(width), height_(height), pixels_(width * height, 0) {}
+  int width() const { return width_; }
+  int height() const { return height_; }
+  void SetPixel(int x, int y, const Uint8Color& color) {
+    pixels_[y * width_ + x] = static_cast<uint32_t>(255) << 24 |
+                              static_cast<uint32_t>(color[0]) << 16 |
+                              static_cast<uint32_t>(color[1]) << 8 | color[2];
+  }
+  void WritePng(FileWriter* const file_writer) {
+    file_writer->Write(reinterpret_cast<const char*>(pixels_.data()), 4 * pixels_.size());
+  }
+ private:
+  int width_, height_;
+  std::vector<uint32_t> pixels_;
+};
 // io/points_batch.h:31-66 (origin is an Eigen::Vector3f there, zero by default).
 struct PointsBatch {
   struct { float v[3] = {0.f, 0.f, 0.f}; float x() const { return v[0]; } float y() const { return v[1]; } float z() const { return v[2]; } } origin;
+  common::Time start_time = 0;
   std::string frame_id;
   int trajectory_id = 0;
   std::vector<sensor::RangefinderPoint> points;

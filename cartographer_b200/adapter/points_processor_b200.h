@@ -1,9 +1,10 @@
 // io::OutlierRemovingPointsProcessor (io/outlier_removing_points_processor.h/.cc) over the
-// csm_outlier_remover entry points, on device 0 like the other adapter defaults: the same
-// constructor, action name, Process / Flush state machine and CHECK, with the voxel map on the
-// device.  Every count and kept point is bit for bit the reference's.  In a checkout this class
-// replaces the processor's header and body; the pipeline builder
-// (points_processor_pipeline_builder.cc) registers it by kConfigurationFileActionName and
+// csm_outlier_remover entry points, and io::XRayPointsProcessor (io/xray_points_processor.h/.cc)
+// over the csm_xray entry points, on device 0 like the other adapter defaults: the same
+// constructors, action names, Process / Flush and CHECKs, with the voxel maps on the device.
+// Every count, kept point and pixel is bit for bit the reference's.  In a checkout these classes
+// replace the processors' headers and bodies; the pipeline builder
+// (points_processor_pipeline_builder.cc) registers them by kConfigurationFileActionName and
 // FromDictionary as before (INTEGRATION.md §3).
 #ifndef CSM_ADAPTER_POINTS_PROCESSOR_B200_H_
 #define CSM_ADAPTER_POINTS_PROCESSOR_B200_H_
@@ -11,6 +12,7 @@
 #include <cstdio>
 #include <cstdlib>
 #include <memory>
+#include <string>
 #include <vector>
 
 #include "../../include/csm_abi.h"
@@ -21,6 +23,17 @@
 #include "cartographer/common/lua_parameter_dictionary.h"
 #include "cartographer/io/points_batch.h"
 #include "cartographer/io/points_processor.h"
+#include "absl/strings/str_cat.h"
+#include "cartographer/common/math.h"
+#include "cartographer/io/color.h"
+#include "cartographer/io/draw_trajectories.h"
+#include "cartographer/io/file_writer.h"
+#include "cartographer/io/image.h"
+#include "cartographer/mapping/detect_floors.h"
+#include "cartographer/mapping/proto/trajectory.pb.h"
+#include "cartographer/transform/rigid_transform.h"
+#include "cartographer/transform/transform.h"
+#include "glog/logging.h"
 #define CSM_B200_IO_CHECKOUT 1
 #else
 #include "compat.h"
@@ -132,6 +145,201 @@ class OutlierRemovingPointsProcessor : public PointsProcessor {
   PointsProcessor* const next_;
   State state_ = State::kPhase1;
   csm_outlier_remover* remover_ = nullptr;
+};
+
+// Creates X-ray cuts through the points with pixels being 'voxel_size' big: per floor (or one)
+// aggregation the voxels and column colour sums live on the device, and Flush draws each image
+// there.
+class XRayPointsProcessor : public PointsProcessor {
+ public:
+  constexpr static const char* kConfigurationFileActionName = "write_xray_image";
+  enum class DrawTrajectories { kNo, kYes };
+
+  XRayPointsProcessor(double voxel_size, double saturation_factor,
+                      const transform::Rigid3f& transform,
+                      const std::vector<mapping::Floor>& floors,
+                      const DrawTrajectories& draw_trajectories,
+                      const std::string& output_filename,
+                      const std::vector<mapping::proto::Trajectory>& trajectories,
+                      FileWriterFactory file_writer_factory, PointsProcessor* const next)
+      : draw_trajectories_(draw_trajectories),
+        trajectories_(trajectories),
+        file_writer_factory_(file_writer_factory),
+        next_(next),
+        floors_(floors),
+        output_filename_(output_filename),
+        transform_(transform),
+        resolution_(static_cast<float>(voxel_size)) {
+    const float t[7] = {transform.translation().x(), transform.translation().y(),
+                        transform.translation().z(), transform.rotation().w(),
+                        transform.rotation().x(),    transform.rotation().y(),
+                        transform.rotation().z()};
+    const int32_t num_aggregations = floors_.empty() ? 1 : static_cast<int32_t>(floors_.size());
+    Check(csm_xray_create(voxel_size, saturation_factor, t, num_aggregations, 0, &xray_));
+  }
+
+#if CSM_B200_IO_CHECKOUT
+  static std::unique_ptr<XRayPointsProcessor> FromDictionary(
+      const std::vector<mapping::proto::Trajectory>& trajectories,
+      FileWriterFactory file_writer_factory, common::LuaParameterDictionary* const dictionary,
+      PointsProcessor* const next) {
+    std::vector<mapping::Floor> floors;
+    const bool separate_floor =
+        dictionary->HasKey("separate_floors") && dictionary->GetBool("separate_floors");
+    const auto draw_trajectories =
+        (!dictionary->HasKey("draw_trajectories") || dictionary->GetBool("draw_trajectories"))
+            ? DrawTrajectories::kYes
+            : DrawTrajectories::kNo;
+    const double saturation_factor =
+        dictionary->HasKey("saturation_factor") ? dictionary->GetDouble("saturation_factor") : 1.;
+    if (separate_floor) {
+      CHECK_EQ(trajectories.size(), 1) << "Can only detect floors with a single trajectory.";
+      floors = mapping::DetectFloors(trajectories.at(0));
+    }
+    return absl::make_unique<XRayPointsProcessor>(
+        dictionary->GetDouble("voxel_size"), saturation_factor,
+        transform::FromDictionary(dictionary->GetDictionary("transform").get()).cast<float>(),
+        floors, draw_trajectories, dictionary->GetString("filename"), trajectories,
+        file_writer_factory, next);
+  }
+#endif
+
+  ~XRayPointsProcessor() override { csm_xray_destroy(xray_); }
+
+  XRayPointsProcessor(const XRayPointsProcessor&) = delete;
+  XRayPointsProcessor& operator=(const XRayPointsProcessor&) = delete;
+
+  void Process(std::unique_ptr<PointsBatch> batch) override {
+    if (floors_.empty()) {
+      Insert(*batch, 0);
+    } else {
+      for (size_t i = 0; i < floors_.size(); ++i) {
+        if (!ContainedIn(batch->start_time, floors_[i].timespans)) continue;
+        Insert(*batch, static_cast<int32_t>(i));
+      }
+    }
+    next_->Process(std::move(batch));
+  }
+
+  FlushResult Flush() override {
+    if (floors_.empty()) {
+      WriteVoxels(0, file_writer_factory_(output_filename_ + ".png").get());
+    } else {
+      for (size_t i = 0; i < floors_.size(); ++i) {
+        WriteVoxels(static_cast<int32_t>(i),
+                    file_writer_factory_(output_filename_ + std::to_string(i) + ".png").get());
+      }
+    }
+    switch (next_->Flush()) {
+      case FlushResult::kRestartStream:
+        std::fprintf(stderr,
+                     "X-Ray generation must be configured to occur after any stages that "
+                     "require multiple passes.\n");
+        std::abort();
+      case FlushResult::kFinished:
+        return FlushResult::kFinished;
+    }
+    std::abort();
+  }
+
+  // The shared box of cell indices as {empty, min, max} (the reference returns an
+  // Eigen::AlignedBox3i, empty until the first point).
+  struct Box {
+    bool empty;
+    int32_t min[3], max[3];
+  };
+  Box bounding_box() const {
+    Box box;
+    int32_t empty = 0;
+    Check(csm_xray_bounding_box(xray_, box.min, box.max, &empty));
+    box.empty = empty != 0;
+    return box;
+  }
+
+ private:
+  static bool ContainedIn(const common::Time& time,
+                          const std::vector<mapping::Timespan>& timespans) {
+    for (const mapping::Timespan& timespan : timespans) {
+      if (timespan.start <= time && time <= timespan.end) return true;
+    }
+    return false;
+  }
+
+  void Insert(const PointsBatch& batch, int32_t aggregation) {
+    const int32_t n = static_cast<int32_t>(batch.points.size());
+    std::vector<float> xyz, rgb;
+    xyz.reserve(3 * static_cast<size_t>(n));
+    for (const auto& p : batch.points) {
+      xyz.push_back(p.position.x());
+      xyz.push_back(p.position.y());
+      xyz.push_back(p.position.z());
+    }
+    for (size_t i = 0; i < batch.colors.size(); ++i) {
+      for (int c = 0; c < 3; ++c) rgb.push_back(batch.colors.at(i)[c]);
+    }
+    const float* points[1] = {xyz.data()};
+    const float* colors[1] = {batch.colors.empty() ? nullptr : rgb.data()};
+    Check(csm_xray_insert(xray_, aggregation, points, colors, &n, 1, nullptr));
+  }
+
+  void WriteVoxels(int32_t aggregation, FileWriter* const file_writer) {
+    int32_t width = 0, height = 0;
+    Check(csm_xray_draw(xray_, aggregation, nullptr, 0, &width, &height, nullptr));
+    if (width == 0) {
+      std::fprintf(stderr, "Not writing output: bounding box is empty.\n");
+      return;
+    }
+    std::vector<uint32_t> pixels(static_cast<size_t>(width) * height);
+    Check(csm_xray_draw(xray_, aggregation, pixels.data(), static_cast<int64_t>(pixels.size()),
+                        &width, &height, nullptr));
+    Image image(width, height);
+    for (int y = 0; y < height; ++y) {
+      for (int x = 0; x < width; ++x) {
+        const uint32_t word = pixels[static_cast<size_t>(y) * width + x];
+        image.SetPixel(x, y, {{static_cast<uint8_t>(word >> 16), static_cast<uint8_t>(word >> 8),
+                               static_cast<uint8_t>(word)}});
+      }
+    }
+#if CSM_B200_IO_CHECKOUT
+    if (draw_trajectories_ == DrawTrajectories::kYes) {
+      const Box box = bounding_box();
+      // voxel_index_to_pixel of the cell of the pose's transformed translation
+      const auto pose_to_pixel = [&box, this](const transform::Rigid3d& pose) -> Eigen::Array2i {
+        const Eigen::Vector3f p = (transform_ * pose.cast<float>()).translation();
+        return Eigen::Array2i(box.max[1] - common::RoundToInt(p.y() / resolution_),
+                              box.max[2] - common::RoundToInt(p.z() / resolution_));
+      };
+      for (size_t i = 0; i < trajectories_.size(); ++i) {
+        DrawTrajectory(trajectories_[i], GetColor(i), pose_to_pixel,
+                       image.GetCairoSurface().get());
+      }
+    }
+#endif
+    image.WritePng(file_writer);
+    if (!file_writer->Close()) {
+      std::fprintf(stderr, "Check failed: file_writer->Close()\n");
+      std::abort();
+    }
+  }
+
+  // Refusals and CUDA failures keep the reference's CHECK semantics (abort with the message).
+  static void Check(csm_status s) {
+    if (s != CSM_OK) {
+      std::fprintf(stderr, "libcsm_b200: %s\n", csm_last_error_string());
+      std::abort();
+    }
+  }
+
+  const DrawTrajectories draw_trajectories_;
+  const std::vector<mapping::proto::Trajectory> trajectories_;
+  FileWriterFactory file_writer_factory_;
+  PointsProcessor* const next_;
+  // If empty, we do not separate into floors.
+  const std::vector<mapping::Floor> floors_;
+  const std::string output_filename_;
+  const transform::Rigid3f transform_;
+  const float resolution_;
+  csm_xray* xray_ = nullptr;
 };
 
 }  // namespace io

@@ -36,8 +36,6 @@
 
 namespace {
 
-constexpr int kCubeHalf = 8192;                     // DynamicGrid: indices in [-8192, 8192)^3
-constexpr unsigned long long kEmptyKey = ~0ull;     // no packed key has bits above 41 set
 constexpr long long kInitialSlots = 1 << 12;
 constexpr int kThreads = 256;
 
@@ -71,14 +69,6 @@ struct csm_outlier_remover {
 namespace csm {
 namespace {
 
-__host__ __device__ inline bool InCube(int v) { return v >= -kCubeHalf && v < kCubeHalf; }
-
-__host__ __device__ inline unsigned long long Pack(int x, int y, int z) {
-  return (static_cast<unsigned long long>(z + kCubeHalf) << 28) |
-         (static_cast<unsigned long long>(y + kCubeHalf) << 14) |
-         static_cast<unsigned long long>(x + kCubeHalf);
-}
-
 // GetCellIndex (hybrid_grid.h:428-433) of (x, y, z) and its packed key; false outside the cube.
 __device__ inline bool VoxelKey(float x, float y, float z, float resolution,
                                 unsigned long long* key) {
@@ -88,40 +78,6 @@ __device__ inline bool VoxelKey(float x, float y, float z, float resolution,
   if (!InCube(ix) || !InCube(iy) || !InCube(iz)) return false;
   *key = Pack(ix, iy, iz);
   return true;
-}
-
-// The slot of `key`, or -1 when the voxel was never hit.
-__device__ inline long long Find(const unsigned long long* __restrict__ keys,
-                                 unsigned long long mask, unsigned long long key) {
-  unsigned long long h = Mix(key) & mask;
-  for (;;) {
-    const unsigned long long k = keys[h];
-    if (k == key) return static_cast<long long>(h);
-    if (k == kEmptyKey) return -1;
-    h = (h + 1) & mask;
-  }
-}
-
-__device__ inline unsigned long long Insert(unsigned long long* keys, unsigned long long mask,
-                                            unsigned long long key, bool* inserted) {
-  unsigned long long h = Mix(key) & mask;
-  for (;;) {
-    const unsigned long long old = atomicCAS(&keys[h], kEmptyKey, key);
-    if (old == kEmptyKey || old == key) {
-      *inserted = old == kEmptyKey;
-      return h;
-    }
-    h = (h + 1) & mask;
-  }
-}
-
-__global__ void k_or_rehash(const unsigned long long* __restrict__ old_keys,
-                            const int2* __restrict__ old_vals, long long old_slots,
-                            unsigned long long* keys, int2* vals, unsigned long long mask) {
-  const long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
-  if (i >= old_slots || old_keys[i] == kEmptyKey) return;
-  bool inserted;
-  vals[Insert(keys, mask, old_keys[i], &inserted)] = old_vals[i];
 }
 
 // Phase 1 (ProcessInPhaseOne): every point is inside the cube (checked on the host).
@@ -284,8 +240,8 @@ csm_status Reserve(csm_outlier_remover* h, long long incoming) {
   CSM_CUDA(cudaMemsetAsync(keys, 0xff, sizeof(unsigned long long) * slots, s));
   CSM_CUDA(cudaMemsetAsync(vals, 0, sizeof(int2) * slots, s));
   if (h->slots > 0) {
-    k_or_rehash<<<DivUp(h->slots, kThreads), kThreads, 0, s>>>(h->keys, h->vals, h->slots, keys,
-                                                              vals, slots - 1);
+    k_rehash<<<DivUp(h->slots, kThreads), kThreads, 0, s>>>(h->keys, h->vals, h->slots, keys,
+                                                           vals, slots - 1);
     CSM_LAUNCH_CHECK();
     CSM_CUDA(cudaFreeAsync(h->keys, s));
     CSM_CUDA(cudaFreeAsync(h->vals, s));

@@ -1,11 +1,13 @@
 """cartographer::io points processing on the device: OutlierRemovingPointsProcessor
 (io/outlier_removing_points_processor.cc), the assets writer's
 voxel_filter_and_remove_moving_objects stage, with its voxel map on the GPU and every count and
-kept point bit for bit the reference's.
+kept point bit for bit the reference's; and XRayPointsProcessor (io/xray_points_processor.cc),
+its write_xray_image stage, with its voxels, column sums and image on the GPU and every pixel the
+reference's.
 
-OutlierRemover is the device handle (csm_outlier_remover_*): its three phases each take many
-batches per call.  OutlierRemovingPointsProcessor is the pipeline stage with the reference's
-Process / Flush state machine over it.  Points are (n, 3) float32 arrays.
+OutlierRemover and XRay are the device handles (csm_outlier_remover_*, csm_xray_*): each call
+takes many batches.  OutlierRemovingPointsProcessor and XRayPointsProcessor are the pipeline
+stages with the reference's Process / Flush over them.  Points are (n, 3) float32 arrays.
 """
 import ctypes as C
 import enum
@@ -166,4 +168,208 @@ class OutlierRemovingPointsProcessor:
         if self.next is not None and self.next.Flush() != FlushResult.kFinished:
             raise RuntimeError("Voxel filtering and outlier removal must be configured to occur "
                                "after any stages that require multiple passes.")
+        return FlushResult.kFinished
+
+
+def _colors(colors_list, pts):
+    out = []
+    for c, p in zip(colors_list, pts):
+        if c is None or len(c) == 0:
+            out.append(None)
+        else:
+            c = np.ascontiguousarray(np.asarray(c, np.float32).reshape(-1, 3))
+            if len(c) != len(p):
+                raise ValueError("one colour per point, or none")
+            out.append(c)
+    return out
+
+
+class XRay:
+    """The device aggregations of one XRayPointsProcessor (csm_xray_*): per aggregation (one per
+    floor, or one) its voxels and per (y, z) column the float sums and count of its colours, and
+    one bounding box shared by all.  `transform` is (t x, y, z, q w, x, y, z), a Rigid3f.  Each
+    insert takes any number of batches and makes one stream synchronisation.  Refusals raise
+    _lib.CsmError and change nothing."""
+
+    def __init__(self, voxel_size, transform=(0.0, 0.0, 0.0, 1.0, 0.0, 0.0, 0.0),
+                 saturation_factor=1.0, num_aggregations=1, device=0):
+        self._L = _lib.lib()
+        t = np.ascontiguousarray(np.asarray(transform, np.float32).reshape(7))
+        h = C.c_void_p()
+        _lib.check(self._L.csm_xray_create(C.c_double(voxel_size), C.c_double(saturation_factor),
+                                           _lib.ptr(t, C.c_float), num_aggregations, device,
+                                           C.byref(h)))
+        self._h = h
+
+    def close(self):
+        if getattr(self, "_h", None):
+            self._L.csm_xray_destroy(self._h)
+            self._h = None
+
+    __del__ = close
+
+    def insert(self, points_list, colors_list=None, aggregation=0):
+        """Inserts the batches, in order; colors_list[b] is None (black) or (n, 3) float32.
+        Returns the call's stats."""
+        pts, counts, ptrs = _batches(points_list)
+        cols = _colors(colors_list if colors_list is not None else [None] * len(pts), pts)
+        rgb = (C.POINTER(C.c_float) * max(len(pts), 1))(
+            *[_lib.ptr(c, C.c_float) if c is not None else None for c in cols])
+        stats = _lib.CsmStats()
+        _lib.check(self._L.csm_xray_insert(self._h, aggregation, ptrs, rgb,
+                                           _lib.ptr(counts, C.c_int32), len(pts),
+                                           C.byref(stats)))
+        return stats.as_dict()
+
+    def bounding_box(self):
+        """(min (3,), max (3,), empty) of the shared box of cell indices."""
+        lo, hi, empty = np.zeros(3, np.int32), np.zeros(3, np.int32), C.c_int32()
+        _lib.check(self._L.csm_xray_bounding_box(self._h, _lib.ptr(lo, C.c_int32),
+                                                 _lib.ptr(hi, C.c_int32), C.byref(empty)))
+        return lo, hi, bool(empty.value)
+
+    def draw(self, aggregation=0):
+        """(pixels, stats): the aggregation's image as a (height, width) uint32 array of cairo
+        ARGB32 words, or None when nothing was ever inserted."""
+        w, ht = C.c_int32(), C.c_int32()
+        _lib.check(self._L.csm_xray_draw(self._h, aggregation, None, C.c_int64(0), C.byref(w),
+                                         C.byref(ht), None))
+        if w.value == 0:
+            return None, {"host_syncs": 0, "device_ms": 0.0}
+        px = np.empty((ht.value, w.value), np.uint32)
+        stats = _lib.CsmStats()
+        _lib.check(self._L.csm_xray_draw(self._h, aggregation, _lib.ptr(px, C.c_uint32),
+                                         C.c_int64(px.size), C.byref(w), C.byref(ht),
+                                         C.byref(stats)))
+        return px, stats.as_dict()
+
+    def voxels(self, aggregation=0):
+        """(n, 3) cell indices of the aggregation's voxels in ascending (z, y, x)."""
+        n = C.c_int64()
+        _lib.check(self._L.csm_xray_voxels(self._h, aggregation, None, C.c_int64(0), C.byref(n)))
+        idx = np.zeros((max(n.value, 1), 3), np.int32)
+        _lib.check(self._L.csm_xray_voxels(self._h, aggregation, _lib.ptr(idx, C.c_int32),
+                                           C.c_int64(len(idx)), C.byref(n)))
+        return idx[:n.value]
+
+    def columns(self, aggregation=0):
+        """(yz (n, 2), sums (n, 3) float32, counts (n,) uint32) in ascending (y, z)."""
+        n = C.c_int64()
+        _lib.check(self._L.csm_xray_columns(self._h, aggregation, None, None, None, C.c_int64(0),
+                                            C.byref(n)))
+        m = max(n.value, 1)
+        yz, sums, counts = np.zeros((m, 2), np.int32), np.zeros((m, 3), np.float32), \
+            np.zeros(m, np.uint32)
+        _lib.check(self._L.csm_xray_columns(self._h, aggregation, _lib.ptr(yz, C.c_int32),
+                                            _lib.ptr(sums, C.c_float),
+                                            _lib.ptr(counts, C.c_uint32), C.c_int64(m),
+                                            C.byref(n)))
+        k = n.value
+        return yz[:k], sums[:k], counts[:k]
+
+
+def cairo_to_rgb(pixels):
+    """(height, width, 3) uint8 of cairo ARGB32 words (0xFF << 24 | r << 16 | g << 8 | b)."""
+    p = np.asarray(pixels, np.uint32)
+    return np.stack([(p >> 16) & 0xFF, (p >> 8) & 0xFF, p & 0xFF], -1).astype(np.uint8)
+
+
+def encode_png(pixels):
+    """An 8-bit RGB PNG of cairo ARGB32 words: IHDR, one IDAT holding one zlib stream of the
+    unfiltered scanlines, IEND.  The pixels are the reference's; the bytes are not cairo's (which
+    writes RGBA with its own filters and compression), so compare decoded pixels, not files."""
+    import struct
+    import zlib
+    rgb = cairo_to_rgb(pixels)
+    height, width = rgb.shape[:2]
+    raw = np.concatenate([np.zeros((height, 1), np.uint8), rgb.reshape(height, 3 * width)], 1)
+
+    def chunk(kind, data):
+        return struct.pack(">I", len(data)) + kind + data + \
+            struct.pack(">I", zlib.crc32(kind + data) & 0xFFFFFFFF)
+    return (b"\x89PNG\r\n\x1a\n" +
+            chunk(b"IHDR", struct.pack(">IIBBBBB", width, height, 8, 2, 0, 0, 0)) +
+            chunk(b"IDAT", zlib.compress(raw.tobytes())) + chunk(b"IEND", b""))
+
+
+def decode_png(data):
+    """(height, width, 3) uint8 of a PNG that encode_png wrote."""
+    import struct
+    import zlib
+    assert data[:8] == b"\x89PNG\r\n\x1a\n"
+    at, idat, width, height = 8, b"", 0, 0
+    while at < len(data):
+        n, = struct.unpack(">I", data[at:at + 4])
+        kind, body = data[at + 4:at + 8], data[at + 8:at + 8 + n]
+        if kind == b"IHDR":
+            width, height = struct.unpack(">II", body[:8])
+            assert body[8:] == bytes([8, 2, 0, 0, 0])
+        elif kind == b"IDAT":
+            idat += body
+        at += 12 + n
+    raw = np.frombuffer(zlib.decompress(idat), np.uint8).reshape(height, 1 + 3 * width)
+    assert not raw[:, 0].any()
+    return raw[:, 1:].reshape(height, width, 3)
+
+
+def _file_writer(filename):
+    return open(filename, "wb")
+
+
+class XRayPointsProcessor:
+    """io::XRayPointsProcessor: X-ray cuts through the points with pixels voxel_size big, drawn
+    on the device.  Process inserts the batch into every floor whose timespans contain its
+    start_time (or into the one aggregation without floors) and passes it on; Flush writes
+    filename + ".png", or filename + str(i) + ".png" per floor, and then flushes `next`.
+    `floors` is a list of floors, each a list of (start, end) timespans compared with
+    PointsBatch.start_time; `file_writer_factory(name)` returns an object with write and close
+    (a binary file by default).  The PNG carries the pixels only (see encode_png); trajectories
+    are not drawn here.  With next=None the batches collect in `.output`."""
+
+    kConfigurationFileActionName = "write_xray_image"
+
+    def __init__(self, voxel_size, transform, filename, saturation_factor=1.0, floors=None,
+                 file_writer_factory=None, next=None, device=0):
+        self.floors = [list(f) for f in floors] if floors else []
+        self.xray = XRay(voxel_size, transform, saturation_factor,
+                         max(1, len(self.floors)), device)
+        self.filename = filename
+        self.file_writer_factory = file_writer_factory or _file_writer
+        self.next = next
+        self.output = []
+
+    def bounding_box(self):
+        return self.xray.bounding_box()
+
+    def Process(self, batch):
+        if not self.floors:
+            self.xray.insert([batch.points], [batch.colors])
+        else:
+            for i, spans in enumerate(self.floors):
+                if any(start <= batch.start_time <= end for start, end in spans):
+                    self.xray.insert([batch.points], [batch.colors], aggregation=i)
+        if self.next is None:
+            self.output.append(batch)
+        else:
+            self.next.Process(batch)
+
+    def _write(self, aggregation, name):
+        pixels, _ = self.xray.draw(aggregation)
+        if pixels is None:
+            import warnings
+            warnings.warn("Not writing output: bounding box is empty.")
+            return
+        f = self.file_writer_factory(name)
+        f.write(encode_png(pixels))
+        f.close()
+
+    def Flush(self):
+        if not self.floors:
+            self._write(0, self.filename + ".png")
+        else:
+            for i in range(len(self.floors)):
+                self._write(i, self.filename + str(i) + ".png")
+        if self.next is not None and self.next.Flush() != FlushResult.kFinished:
+            raise RuntimeError("X-Ray generation must be configured to occur after any stages "
+                               "that require multiple passes.")
         return FlushResult.kFinished

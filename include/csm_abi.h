@@ -1118,6 +1118,59 @@ csm_status csm_outlier_remover_voxels(const csm_outlier_remover* remover, int32_
 csm_status csm_outlier_remover_info(const csm_outlier_remover* remover, int32_t* phase,
                                     int64_t* num_voxels, int64_t* slots);
 
+/* ---- map assets: XRayPointsProcessor ----------------------------------------------------- */
+/* io::XRayPointsProcessor (io/xray_points_processor.cc), the assets writer's write_xray_image
+ * stage, with its aggregations on one device.  Each aggregation (one per floor, or one) holds the
+ * voxels the points fall in and, per (y, z) column, the float sums of their colours and their
+ * count; one bounding box of cell indices is shared by all aggregations.  A point p goes to cell
+ * lround((transform * p) / (float)voxel_size) per axis, narrowed to int.  Every voxel, column sum
+ * and count, the box and every pixel are bit for bit the reference's, however the batches are
+ * grouped into calls.  Batch b has num_points[b] x {x, y, z} in xyz[b] and, unless rgb or rgb[b]
+ * is NULL (black, as a batch without colours), num_points[b] x {r, g, b} in rgb[b].  Every call
+ * checks its input first, and a refused call changes no voxel, column, count or box:
+ * CSM_E_INVALID for a null handle or a null pointer where data is required, an aggregation out of
+ * range, a negative count, a non-finite coordinate or colour, more than 2^30 points in one call,
+ * or a cell outside the [-8192, 8192)^3 cells the reference's grid can grow to (its CHECK).
+ * stats (may be NULL) gets host_syncs and device_ms. */
+typedef struct csm_xray csm_xray;
+/* transform = {t x, y, z, q w, x, y, z} (transform::Rigid3f).  CSM_E_INVALID for a voxel_size
+ * that is not finite and > 0 in float, a non-finite saturation_factor or transform, or
+ * num_aggregations < 1. */
+csm_status csm_xray_create(double voxel_size, double saturation_factor, const float transform[7],
+                           int32_t num_aggregations, int32_t device, csm_xray** out);
+csm_status csm_xray_destroy(csm_xray* xray);
+/* Insert (xray_points_processor.cc:221-239) of every batch, in order, into one aggregation.  The
+ * aggregation's voxel set and column map grow (a device rehash) at the start of a call that could
+ * fill them past one half; CSM_E_CAPACITY, with nothing changed, when the device has not the
+ * memory for that.  One stream synchronisation per call with points (none without). */
+csm_status csm_xray_insert(csm_xray* xray, int32_t aggregation, const float* const* xyz,
+                           const float* const* rgb, const int32_t* num_points,
+                           int32_t num_batches, csm_stats* stats /* may be NULL */);
+/* The shared bounding box (the reference's bounding_box()), read on the host: *empty = 1 while
+ * no point was inserted, and min and max are then {0, 0, 0}. */
+csm_status csm_xray_bounding_box(const csm_xray* xray, int32_t min[3], int32_t max[3],
+                                 int32_t* empty);
+/* The aggregation's image (WriteVoxels and IntoImage, xray_points_processor.cc:65-104, 170-203):
+ * width = max.y - min.y + 1 and height = max.z - min.z + 1 of the shared box, and pixel
+ * (max.y - y, max.z - z) for column (y, z), each a cairo ARGB32 word 0xFF << 24 | r << 16 |
+ * g << 8 | b, row-major with a stride of width.  An aggregation without points is all white.
+ * With pixels == NULL only *width and *height are written, without a stream synchronisation;
+ * an empty box writes 0 x 0 and returns CSM_OK (the reference writes no image); a capacity
+ * below width * height returns CSM_E_CAPACITY with *width and *height set and nothing else
+ * written.  One stream synchronisation otherwise. */
+csm_status csm_xray_draw(csm_xray* xray, int32_t aggregation, uint32_t* pixels, int64_t capacity,
+                         int32_t* width, int32_t* height, csm_stats* stats /* may be NULL */);
+/* Test hook: the aggregation's voxels in ascending (z, y, x) as n x {x, y, z}.  With
+ * indices == NULL only *num_voxels is written, without a stream synchronisation; a capacity
+ * below it returns CSM_E_CAPACITY with *num_voxels set. */
+csm_status csm_xray_voxels(const csm_xray* xray, int32_t aggregation, int32_t* indices,
+                           int64_t capacity, int64_t* num_voxels);
+/* Test hook: the aggregation's columns in ascending (y, z): yz (n x {y, z}), sums (n x {r, g, b})
+ * and counts (each may be NULL).  With all three NULL only *num_columns is written, without a
+ * stream synchronisation; a capacity below it returns CSM_E_CAPACITY with *num_columns set. */
+csm_status csm_xray_columns(const csm_xray* xray, int32_t aggregation, int32_t* yz, float* sums,
+                            uint32_t* counts, int64_t capacity, int64_t* num_columns);
+
 /* Test hook: as csm_ceres_evaluate3d, in the problem's residual-block order — per cloud its
  * occupied-space residuals, then its intensity residuals if it has a grid; then 3
  * translation and 3 rotation residuals.  Residuals and rows are uncorrected by the loss, as
