@@ -1114,6 +1114,87 @@ int main() {
       std::printf("\n");
     }
   }
+  {
+    // io::ProbabilityGridPointsProcessor (PNG and PB) and io::HybridGridPointsProcessor on the
+    // three batches of tests/test_gpu_adapter_points_to_grid.py, which reach past the initial
+    // 100 x 100 cells at 5 cm.  The stand-in Image writes its cairo words, so the RESULT lines
+    // list the image's pixels and the serialised grids' bytes.
+    struct Writer : io::FileWriter {
+      std::map<std::string, std::string>* files;
+      std::string name, data;
+      bool WriteHeader(const char* d, size_t n) override { data.insert(0, d, n); return true; }
+      bool Write(const char* d, size_t n) override { data.append(d, n); return true; }
+      bool Close() override { (*files)[name] = data; return true; }
+      std::string GetFilename() override { return name; }
+    };
+    struct Sink : io::PointsProcessor {
+      int batches = 0;
+      void Process(std::unique_ptr<io::PointsBatch>) override { ++batches; }
+      FlushResult Flush() override { return FlushResult::kFinished; }
+    } sink;
+    std::map<std::string, std::string> files;
+    const auto writer = [&files](const std::string& name) {
+      auto w = std::make_unique<Writer>();
+      w->files = &files;
+      w->name = name;
+      return std::unique_ptr<io::FileWriter>(std::move(w));
+    };
+    mapping::proto::ProbabilityGridRangeDataInserterOptions2D o2;
+    o2.set_hit_probability(0.55);
+    o2.set_miss_probability(0.49);
+    o2.set_insert_free_space(true);
+    mapping::proto::RangeDataInserterOptions3D o3;
+    o3.set_hit_probability(0.55);
+    o3.set_miss_probability(0.49);
+    o3.set_num_free_space_voxels(2);
+    o3.set_intensity_threshold(40.f);
+    using PG = io::ProbabilityGridPointsProcessor;
+    PG png(0.05, o2, PG::DrawTrajectories::kNo, PG::OutputType::kPng, writer("map.png"), {},
+           &sink);
+    PG pb(0.05, o2, PG::DrawTrajectories::kNo, PG::OutputType::kPb, writer("map.pb"), {}, &sink);
+    io::HybridGridPointsProcessor hybrid(0.1, o3, writer("map_3d"), &sink);
+    std::printf("RESULT pg_action %s %s\n", PG::kConfigurationFileActionName,
+                io::HybridGridPointsProcessor::kConfigurationFileActionName);
+    for (int b = 0; b < 3; ++b) {
+      io::PointsProcessor* const stages[3] = {&png, &pb, &hybrid};
+      for (io::PointsProcessor* stage : stages) {
+        auto batch = std::make_unique<io::PointsBatch>();
+        const float ox = float(b) * 0.7f - 0.5f, oy = float(b) * -0.4f + 0.2f;
+        batch->origin.v[0] = ox;
+        batch->origin.v[1] = oy;
+        batch->origin.v[2] = 0.25f;
+        for (int i = 0; i < 400; ++i) {
+          sensor::RangefinderPoint p{{{float((i * 37) % 161 - 80) * 0.05f + ox,
+                                       float((i * 53) % 149 - 74) * 0.05f + oy,
+                                       float(i % 5) * 0.1f}}};
+          batch->points.push_back(p);
+        }
+        stage->Process(std::move(batch));
+      }
+    }
+    Eigen::Array2i offset;
+    const std::unique_ptr<io::Image> image = io::DrawProbabilityGrid(png.probability_grid(),
+                                                                     &offset);
+    std::printf("RESULT pg_image %d %d %d %d\n", image->width(), image->height(), offset.x(),
+                offset.y());
+    int finished = 0;
+    for (io::PointsProcessor* stage : {static_cast<io::PointsProcessor*>(&png),
+                                       static_cast<io::PointsProcessor*>(&pb),
+                                       static_cast<io::PointsProcessor*>(&hybrid)})
+      finished += stage->Flush() == io::PointsProcessor::FlushResult::kFinished;
+    std::printf("RESULT pg_flush %d %d\n", finished, sink.batches);
+    std::printf("RESULT pg_file_map.png");
+    const std::string& words = files["map.png"];
+    for (size_t i = 0; i + 4 <= words.size(); i += 4) {
+      uint32_t word;
+      std::memcpy(&word, words.data() + i, 4);
+      std::printf(" %u", word);
+    }
+    std::printf("\n");
+    PrintBytes("pg_file_map.pb", files["map.pb"]);
+    PrintBytes("pg_file_map_3d", files["map_3d"]);
+    std::printf("RESULT pg_files %zu\n", files.size());
+  }
   if (trimmer_cases::Run() != 0) return 1;
   return 0;
 }

@@ -699,6 +699,17 @@ class PoseGraphTrimmer {
 }  // namespace cartographer
 
 // ---- points processing (io/points_batch.h, io/points_processor.h) ----
+namespace Eigen {
+// The Eigen::Array2i DrawProbabilityGrid fills with the offset of the cropped limits.
+struct Array2i {
+  Array2i() = default;
+  Array2i(int x, int y) : v{x, y} {}
+  int x() const { return v[0]; }
+  int y() const { return v[1]; }
+  int v[2] = {0, 0};
+};
+}  // namespace Eigen
+
 namespace absl {
 // The set type io::RemovePoints takes (absl/container/flat_hash_set.h).
 template <class T>

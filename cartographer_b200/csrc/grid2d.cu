@@ -58,6 +58,18 @@ __global__ void k_ins2_crop(const uint16_t* __restrict__ src, int src_pitch, int
   }
 }
 
+// DrawProbabilityGrid's pixel loop (probability_grid_points_processor.cc:185-194): pixel (x, y)
+// of row blockIdx.y is cell (x + ox, y + oy), its grey level looked up in the host-computed
+// colour table (entry 0, the unknown cell, is 128), written as a cairo ARGB32 word.
+__global__ void k_ins2_draw(const uint16_t* __restrict__ cells, int pitch, int ox, int oy, int w,
+                            const uint8_t* __restrict__ table, uint32_t* __restrict__ pixels) {
+  const int x = blockIdx.x * blockDim.x + threadIdx.x;
+  if (x >= w) return;
+  const int y = blockIdx.y;
+  const uint32_t v = __ldg(table + (cells[static_cast<size_t>(y + oy) * pitch + (x + ox)] & 0x7fff));
+  pixels[static_cast<size_t>(y) * w + x] = 0xFF000000u | v << 16 | v << 8 | v;
+}
+
 }  // namespace csm
 
 using namespace csm;
@@ -279,6 +291,36 @@ const std::vector<uint16_t>& CropTable() {
     return t;
   }();
   return table;
+}
+
+// ProbabilityToColor(GetProbability(v)) of every cell value (probability_grid_points_processor.cc
+// :51-56, probability_grid.cc:78-82) with the reference's float steps, and kUnknownValue = 128
+// for value 0.
+const std::vector<uint8_t>& ColorTable() {
+  static const std::vector<uint8_t> table = [] {
+    const ValueConversion cost =
+        MakeValueConversion(kMinCorrespondenceCost, kMaxCorrespondenceCost);
+    std::vector<uint8_t> t(kValueCount, 128);
+    for (int v = 1; v < kValueCount; ++v) {
+      const float probability = 1.f - (1.f - cost(v));
+      t[v] = static_cast<uint8_t>(std::lround(
+          255 * ((probability - kMinProbability) / (kMaxProbability - kMinProbability))));
+    }
+    return t;
+  }();
+  return table;
+}
+
+// Grid2D::ComputeCroppedLimits (grid_2d.cc:110-120) of a handle whose box is up to date: the
+// known-cells box, or 1 x 1 at offset (0, 0) when it is empty.
+void CroppedLimits(const csm_rt_grid2d* g, int* ox, int* oy, int* nx, int* ny) {
+  *ox = *oy = 0;
+  *nx = *ny = 1;
+  if (g->known.empty()) return;
+  *ox = g->known.lo[0];
+  *oy = g->known.lo[1];
+  *nx = g->known.hi[0] - *ox + 1;
+  *ny = g->known.hi[1] - *oy + 1;
 }
 
 }  // namespace
@@ -606,14 +648,8 @@ csm_status csm_rt_grid2d_crop(const csm_rt_grid2d* grid, csm_rt_grid2d** out) {
   std::lock_guard<std::mutex> lock(ctx->mu);
   CSM_CUDA(cudaSetDevice(ctx->device));
   CSM_TRY(KnownBox(src));
-  // ComputeCroppedLimits (grid_2d.cc:110-120)
-  int ox = 0, oy = 0, nx = 1, ny = 1;
-  if (!src->known.empty()) {
-    ox = src->known.lo[0];
-    oy = src->known.lo[1];
-    nx = src->known.hi[0] - ox + 1;
-    ny = src->known.hi[1] - oy + 1;
-  }
+  int ox, oy, nx, ny;
+  CroppedLimits(src, &ox, &oy, &nx, &ny);
   const double resolution = src->g.resolution;
   const double max_x = src->g.max_x - resolution * static_cast<double>(oy);
   const double max_y = src->g.max_y - resolution * static_cast<double>(ox);
@@ -636,6 +672,62 @@ csm_status csm_rt_grid2d_crop(const csm_rt_grid2d* grid, csm_rt_grid2d** out) {
   }
   CSM_CUDA(cudaStreamSynchronize(ctx->stream));
   *out = g.release();
+  return CSM_OK;
+}
+
+csm_status csm_rt_grid2d_draw(const csm_rt_grid2d* grid, uint32_t* pixels, int64_t capacity,
+                              int32_t* width, int32_t* height, int32_t offset[2],
+                              csm_stats* stats) {
+  CSM_REQUIRE(grid != nullptr && width != nullptr && height != nullptr && offset != nullptr,
+              "null pointer");
+  CSM_REQUIRE(grid->d_wcells == nullptr, "a TSDF2D handle is not drawn here");
+  csm_rt_grid2d* g = const_cast<csm_rt_grid2d*>(grid);   // the box is a cache
+  Ctx* ctx = g->ctx;
+  std::lock_guard<std::mutex> lock(ctx->mu);
+  if (stats) std::memset(stats, 0, sizeof(*stats));
+  CSM_CUDA(cudaSetDevice(ctx->device));
+  const int box_syncs = g->known_stale ? 1 : 0;
+  CSM_TRY(KnownBox(g));
+  int ox, oy, w, h;
+  CroppedLimits(g, &ox, &oy, &w, &h);
+  *width = w;
+  *height = h;
+  offset[0] = ox;
+  offset[1] = oy;
+  if (stats) stats->host_syncs = box_syncs;
+  if (!pixels) return CSM_OK;
+  const int64_t num_pixels = static_cast<int64_t>(w) * h;
+  if (capacity < num_pixels) {
+    SetError("a %d x %d image, capacity %lld", w, h, static_cast<long long>(capacity));
+    return CSM_E_CAPACITY;
+  }
+  const std::vector<uint8_t>& table = ColorTable();
+  DevBuf& d_table = ctx->D("ins2_draw_table");
+  DevBuf& d_pixels = ctx->D("ins2_draw_pixels");
+  CSM_TRY(d_table.Reserve(table.size()));
+  CSM_TRY(d_pixels.Reserve(sizeof(uint32_t) * num_pixels));
+  cudaStream_t s = ctx->stream;
+  CSM_CUDA(cudaMemcpyAsync(d_table.p, table.data(), table.size(), cudaMemcpyHostToDevice, s));
+  CSM_CUDA(cudaEventRecord(ctx->ev0, s));
+  k_ins2_draw<<<dim3((w + 255) / 256, h), 256, 0, s>>>(g->d_cells, g->g.pitch, ox, oy, w,
+                                                       d_table.as<uint8_t>(),
+                                                       d_pixels.as<uint32_t>());
+  CSM_LAUNCH_CHECK();
+  CSM_CUDA(cudaEventRecord(ctx->ev1, s));
+  CSM_CUDA(cudaMemcpyAsync(pixels, d_pixels.p, sizeof(uint32_t) * num_pixels,
+                           cudaMemcpyDeviceToHost, s));
+  CSM_CUDA(cudaStreamSynchronize(s));
+  if (stats) {
+    stats->host_syncs = box_syncs + 1;
+    cudaEventElapsedTime(&stats->device_ms, ctx->ev0, ctx->ev1);
+  }
+  return CSM_OK;
+}
+
+csm_status csm_rt_grid2d_draw_table(uint8_t* grey) {
+  CSM_REQUIRE(grey != nullptr, "null pointer");
+  const std::vector<uint8_t>& table = ColorTable();
+  std::memcpy(grey, table.data(), table.size());
   return CSM_OK;
 }
 

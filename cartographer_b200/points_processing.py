@@ -3,11 +3,16 @@
 voxel_filter_and_remove_moving_objects stage, with its voxel map on the GPU and every count and
 kept point bit for bit the reference's; and XRayPointsProcessor (io/xray_points_processor.cc),
 its write_xray_image stage, with its voxels, column sums and image on the GPU and every pixel the
-reference's.
+reference's; and the map-writing stages ProbabilityGridPointsProcessor
+(io/probability_grid_points_processor.cc, write_probability_grid) and HybridGridPointsProcessor
+(io/hybrid_grid_points_processor.cc, write_hybrid_grid), whose grids grow on the GPU from the first
+batch to the image or proto they save.
 
 OutlierRemover and XRay are the device handles (csm_outlier_remover_*, csm_xray_*): each call
 takes many batches.  OutlierRemovingPointsProcessor and XRayPointsProcessor are the pipeline
-stages with the reference's Process / Flush over them.  Points are (n, 3) float32 arrays.
+stages with the reference's Process / Flush over them; the map-writing stages insert into the
+device grids of scan_matching (RealTimeGrid2D, DeviceHybridGrid).  Points are (n, 3) float32
+arrays.
 """
 import ctypes as C
 import enum
@@ -372,4 +377,87 @@ class XRayPointsProcessor:
         if self.next is not None and self.next.Flush() != FlushResult.kFinished:
             raise RuntimeError("X-Ray generation must be configured to occur after any stages "
                                "that require multiple passes.")
+        return FlushResult.kFinished
+
+
+class ProbabilityGridPointsProcessor:
+    """io::ProbabilityGridPointsProcessor: every batch goes into one ProbabilityGrid on the
+    device (CreateProbabilityGrid: 100 x 100 cells, max = 0.5 * 100 * resolution on both axes)
+    as ProbabilityGridRangeDataInserter2D inserts {origin, points, no misses}, and passes on.
+    Flush writes filename + ".png", DrawProbabilityGrid's pixels (see encode_png; trajectories
+    are not drawn here), or filename + ".pb", the serialised proto::Grid2D, and then flushes
+    `next`.  The file writer is made at construction, as FromDictionary makes it.  An insert that
+    would grow the grid to 30 000 cells per axis raises _lib.CsmError and leaves the grid as it
+    was.  With next=None the batches collect in `.output`."""
+
+    kConfigurationFileActionName = "write_probability_grid"
+    kInitialProbabilityGridSize = 100
+
+    def __init__(self, resolution, range_data_inserter_options, filename, output_type="png",
+                 file_writer_factory=None, next=None, device=0):
+        from . import scan_matching as sm
+        if output_type not in ("png", "pb"):
+            raise ValueError("OutputType %s does not exist!" % output_type)
+        self.output_type = output_type
+        half = 0.5 * self.kInitialProbabilityGridSize * resolution
+        self.grid = sm.RealTimeGrid2D.empty(resolution, half, half,
+                                            self.kInitialProbabilityGridSize,
+                                            self.kInitialProbabilityGridSize, device)
+        self.inserter = sm.ProbabilityGridRangeDataInserter2D(range_data_inserter_options, device)
+        self.file_writer = (file_writer_factory or _file_writer)(filename + "." + output_type)
+        self.next = next
+        self.output = []
+
+    def Process(self, batch):
+        self.inserter.Insert(batch.origin, batch.points, self.grid)
+        if self.next is None:
+            self.output.append(batch)
+        else:
+            self.next.Process(batch)
+
+    def Flush(self):
+        if self.output_type == "png":
+            pixels, _ = self.grid.draw()
+            self.file_writer.write(encode_png(pixels))
+        else:
+            self.file_writer.write(self.grid.to_proto())
+        self.file_writer.close()
+        if self.next is not None and self.next.Flush() != FlushResult.kFinished:
+            raise RuntimeError("ProbabilityGrid generation must be configured to occur after any "
+                               "stages that require multiple passes.")
+        return FlushResult.kFinished
+
+
+class HybridGridPointsProcessor:
+    """io::HybridGridPointsProcessor: every batch goes into one HybridGrid(float(voxel_size)) on
+    the device as RangeDataInserter3D inserts {origin, points, no misses} without an intensity
+    grid, and passes on.  Flush writes the serialised proto::HybridGrid to exactly `filename`
+    and then flushes `next`.  The grid is the dense device box of DeviceHybridGrid: a cell
+    outside [-8192, 8192)^3, or a box the device cannot hold, raises _lib.CsmError and leaves
+    the grid as it was.  With next=None the batches collect in `.output`."""
+
+    kConfigurationFileActionName = "write_hybrid_grid"
+
+    def __init__(self, voxel_size, range_data_inserter_options, filename,
+                 file_writer_factory=None, next=None, device=0):
+        from . import scan_matching as sm
+        self.grid = sm.DeviceHybridGrid.empty(float(np.float32(voxel_size)), device)
+        self.inserter = sm.RangeDataInserter3D(range_data_inserter_options, device)
+        self.file_writer = (file_writer_factory or _file_writer)(filename)
+        self.next = next
+        self.output = []
+
+    def Process(self, batch):
+        self.inserter.Insert(batch.origin, batch.points, None, self.grid)
+        if self.next is None:
+            self.output.append(batch)
+        else:
+            self.next.Process(batch)
+
+    def Flush(self):
+        self.file_writer.write(self.grid.to_proto())
+        self.file_writer.close()
+        if self.next is not None and self.next.Flush() != FlushResult.kFinished:
+            raise RuntimeError("Hybrid grid generation must be configured to occur after any "
+                               "stages that require multiple passes.")
         return FlushResult.kFinished

@@ -532,6 +532,20 @@ class RealTimeGrid2D:
         adds it (csm_rt_grid2d_to_texture), as bytes."""
         return _texture(lib().csm_rt_grid2d_to_texture, self._h, local_pose)
 
+    def draw(self):
+        """io::DrawProbabilityGrid of this ProbabilityGrid (csm_rt_grid2d_draw): (pixels,
+        offset), pixels a (height, width) uint32 array of cairo ARGB32 grey words over the
+        cropped limits and offset their first cell (x, y).  An empty grid gives one pixel of
+        128 at offset (0, 0)."""
+        w, h = C.c_int32(), C.c_int32()
+        offset = np.zeros(2, np.int32)
+        check(lib().csm_rt_grid2d_draw(self._h, None, C.c_int64(0), C.byref(w), C.byref(h),
+                                       ptr(offset, C.c_int32), None))
+        pixels = np.empty((h.value, w.value), np.uint32)
+        check(lib().csm_rt_grid2d_draw(self._h, ptr(pixels, C.c_uint32), C.c_int64(pixels.size),
+                                       C.byref(w), C.byref(h), ptr(offset, C.c_int32), None))
+        return pixels, (int(offset[0]), int(offset[1]))
+
     def ComputeCroppedGrid(self):
         """ProbabilityGrid::ComputeCroppedGrid from device to device: a new RealTimeGrid2D over
         the known-cells box (csm_rt_grid2d_crop)."""

@@ -868,6 +868,25 @@ csm_status csm_rt_grid2d_to_proto(const csm_rt_grid2d* grid, uint8_t* buf, int64
  * handle made from cells, the cells). */
 csm_status csm_rt_grid2d_to_texture(const csm_rt_grid2d* grid, const double local_pose[7],
                                     uint8_t* buf, int64_t capacity, int64_t* size);
+/* io::DrawProbabilityGrid (io/probability_grid_points_processor.cc:175-196), the image the
+ * assets writer's write_probability_grid stage saves: the cells of Grid2D::ComputeCroppedLimits
+ * (the known-cells box, or 1 x 1 at offset (0, 0) when it is empty, which draws one pixel of
+ * 128), width = num_x_cells and height = num_y_cells of those limits, offset = their first cell.
+ * Pixel (x, y) is cell (offset[0] + x, offset[1] + y) at pixels[y * width + x], a cairo ARGB32
+ * grey word 0xFF << 24 | v << 16 | v << 8 | v: v = 128 for an unknown cell, else
+ * ProbabilityToColor(GetProbability(cell)) with the reference's float steps, bit for bit (a
+ * table of every cell value built on the host).  With pixels == NULL only the size and offset
+ * are written; a capacity below width * height returns CSM_E_CAPACITY with the size and offset
+ * set and no pixel written.  A TSDF2D handle returns CSM_E_INVALID.  The handle is left
+ * unchanged, and no insert may be in flight on it.  One or two stream synchronisations (the
+ * known-cells box of a handle made from cells, the pixels); stats (may be NULL) gets host_syncs
+ * and device_ms. */
+csm_status csm_rt_grid2d_draw(const csm_rt_grid2d* grid, uint32_t* pixels, int64_t capacity,
+                              int32_t* width, int32_t* height, int32_t offset[2],
+                              csm_stats* stats /* may be NULL */);
+/* Test hook, no device needed: the 32768 grey levels csm_rt_grid2d_draw looks cell values up in
+ * (grey[0] = 128, the unknown cell). */
+csm_status csm_rt_grid2d_draw_table(uint8_t* grey /* 32768 */);
 /* AddToTextureProto (mapping/3d/submap_3d.cc:51-176) with the global submap pose, as
  * Submap3D::ToResponseProto calls it for the high- and then the low-resolution grid: an X-ray
  * view of the voxels with probability >= 0.501f, transformed by the pose cast to float, rounded
