@@ -643,6 +643,80 @@ int main() {
       PrintBytes("texture_response3d_low", low_texture);
     }
   }
+  // ---- ActiveSubmaps3D over device grids: seven scans with num_range_data = 2, so submaps
+  // roll over, finish and are evicted; the active submaps' handles and histograms, and the
+  // first submap's after its eviction, which tests/test_gpu_adapter_active_submaps3d.py holds
+  // equal to scan_matching.ActiveSubmaps3D's ----
+  {
+    mapping::proto::SubmapsOptions3D so;
+    so.set_high_resolution(0.1);
+    so.set_high_resolution_max_range(4.0);
+    so.set_low_resolution(0.45);
+    so.set_num_range_data(2);
+    so.mutable_range_data_inserter_options()->set_hit_probability(0.55);
+    so.mutable_range_data_inserter_options()->set_miss_probability(0.49);
+    so.mutable_range_data_inserter_options()->set_num_free_space_voxels(2);
+    so.mutable_range_data_inserter_options()->set_intensity_threshold(40.f);
+    mapping::ActiveSubmaps3D active(so, 0);
+    std::shared_ptr<const mapping::DeviceSubmap3D> first;
+    std::vector<std::shared_ptr<const mapping::DeviceSubmap3D>> subs;
+    for (int k = 0; k < 7; ++k) {
+      sensor::RangeData range_data;
+      range_data.origin = {{0.25f * k, -0.125f * k, 0.5f}};
+      std::vector<sensor::RangefinderPoint> points;
+      std::vector<float> intensities;
+      for (int i = 0; i < 240; ++i) {
+        points.push_back({{{-3.f + 0.125f * (i % 48) + 0.25f * k, 2.f - 0.5f * (i / 48),
+                            1.5f - 0.25f * (i % 5)}}});
+        intensities.push_back(static_cast<float>(i % 60));
+      }
+      range_data.returns = sensor::PointCloud(points, intensities);
+      const transform::Quaterniond q{std::cos(0.05 * k), 0., 0., std::sin(0.05 * k)};
+      std::vector<float> histogram(8);
+      for (int i = 0; i < 8; ++i) histogram[i] = static_cast<float>(i + k);
+      subs = active.InsertData(range_data, q, histogram);
+      if (!first) first = subs.front();
+    }
+    auto print = [](const char* name, const mapping::DeviceSubmap3D& s) {
+      int32_t lo[3], dims[3];
+      for (const auto* g : {&s.high_resolution_hybrid_grid(), &s.low_resolution_hybrid_grid()}) {
+        if (csm_grid3d_read(g->handle(), lo, dims, nullptr) != CSM_OK) return false;
+        std::vector<uint16_t> v(static_cast<size_t>(dims[0]) * dims[1] * dims[2]);
+        if (csm_grid3d_read(g->handle(), lo, dims, v.data()) != CSM_OK) return false;
+        std::printf("RESULT %s_%s %d %d %d %d %d %d", name,
+                    g == &s.high_resolution_hybrid_grid() ? "high" : "low", lo[0], lo[1], lo[2],
+                    dims[0], dims[1], dims[2]);
+        for (uint16_t x : v) std::printf(" %u", x);
+        std::printf("\n");
+      }
+      std::printf("RESULT %s_state %d %d", name, s.num_range_data(), s.insertion_finished() ? 1 : 0);
+      for (float h : s.rotational_scan_matcher_histogram()) std::printf(" %08x", Bits(h));
+      std::printf("\n");
+      std::printf("RESULT %s_intensity", name);
+      if (const auto* ig = s.high_resolution_intensity_hybrid_grid()) {
+        if (csm_intensity_grid3d_read(ig->handle(), lo, dims, nullptr, nullptr, nullptr) != CSM_OK)
+          return false;
+        const size_t vox = static_cast<size_t>(dims[0]) * dims[1] * dims[2];
+        std::vector<float> mean(vox), sum(vox);
+        std::vector<int32_t> count(vox);
+        if (csm_intensity_grid3d_read(ig->handle(), lo, dims, mean.data(), sum.data(),
+                                      count.data()) != CSM_OK)
+          return false;
+        std::printf(" %d %d %d %d %d %d", lo[0], lo[1], lo[2], dims[0], dims[1], dims[2]);
+        for (size_t i = 0; i < vox; ++i)
+          std::printf(" %08x:%08x:%d", Bits(mean[i]), Bits(sum[i]), count[i]);
+      } else {
+        std::printf(" forgotten");
+      }
+      std::printf("\n");
+      return true;
+    };
+    if (subs.size() != 2 || first == subs.front()) return 1;
+    if (!print("active0", *subs[0]) || !print("active1", *subs[1]) || !print("evicted", *first))
+      return 1;
+    if (subs[0]->device_submap().high_resolution_hybrid_grid != &subs[0]->high_resolution_hybrid_grid())
+      return 1;
+  }
   // ---- FastCorrelativeScanMatcher3D and ConstraintBuilder3D on inserted device grids: the
   // axis cloud inserted twice from its sensor position into empty grids; the same built from
   // host HybridGrids of the grids' non-zero voxels prints the *_host lines, which

@@ -212,7 +212,7 @@ class Rigid3d {
     const double n = std::sqrt(w * w + x * x + y * y + z * z);
     return Rigid3d(t, Quaterniond{w / n, x / n, y / n, z / n});
   }
- private:
+  // Eigen's Quaterniond * Vector3d (_transformVector)
   static Vector Rotate(const Quaterniond& q, const Vector& c) {
     const double* v = c.v;
     double uv[3] = {q.y_ * v[2] - q.z_ * v[1], q.z_ * v[0] - q.x_ * v[2], q.x_ * v[1] - q.y_ * v[0]};
@@ -225,7 +225,62 @@ class Rigid3d {
   Vector t_;
   Quaterniond q_;
 };
+// Eigen's Quaterniond product, in its scalar order, without normalisation.
+inline Quaterniond operator*(const Quaterniond& p, const Quaterniond& q) {
+  return Quaterniond{p.w_ * q.w_ - p.x_ * q.x_ - p.y_ * q.y_ - p.z_ * q.z_,
+                     p.w_ * q.x_ + p.x_ * q.w_ + p.y_ * q.z_ - p.z_ * q.y_,
+                     p.w_ * q.y_ + p.y_ * q.w_ + p.z_ * q.x_ - p.x_ * q.z_,
+                     p.w_ * q.z_ + p.z_ * q.w_ + p.x_ * q.y_ - p.y_ * q.x_};
+}
+// transform/transform.h:42-47
+inline double GetYaw(const Quaterniond& rotation) {
+  const Rigid3d::Vector direction = Rigid3d::Rotate(rotation, {{1., 0., 0.}});
+  return std::atan2(direction.y(), direction.x());
+}
 }  // namespace transform
+
+namespace mapping {
+namespace proto {
+// mapping/proto/submaps_options_3d.proto
+class SubmapsOptions3D {
+ public:
+  double high_resolution() const { return high_resolution_; }
+  double high_resolution_max_range() const { return high_resolution_max_range_; }
+  double low_resolution() const { return low_resolution_; }
+  int32_t num_range_data() const { return num_range_data_; }
+  const RangeDataInserterOptions3D& range_data_inserter_options() const { return inserter_; }
+  RangeDataInserterOptions3D* mutable_range_data_inserter_options() { return &inserter_; }
+  void set_high_resolution(double v) { high_resolution_ = v; }
+  void set_high_resolution_max_range(double v) { high_resolution_max_range_ = v; }
+  void set_low_resolution(double v) { low_resolution_ = v; }
+  void set_num_range_data(int32_t v) { num_range_data_ = v; }
+ private:
+  double high_resolution_ = 0., high_resolution_max_range_ = 0., low_resolution_ = 0.;
+  int32_t num_range_data_ = 0;
+  RangeDataInserterOptions3D inserter_;
+};
+}  // namespace proto
+namespace scan_matching {
+// mapping/internal/3d/scan_matching/rotational_scan_matcher.cc:141-162, on the std::vector<float>
+// that stands in for Eigen::VectorXf.
+struct RotationalScanMatcher {
+  static std::vector<float> RotateHistogram(const std::vector<float>& histogram,
+                                            const float angle) {
+    const int size = static_cast<int>(histogram.size());
+    if (size == 0) return histogram;
+    const float rotate_by_buckets = -angle * size / M_PI;
+    int full_buckets = static_cast<int>(std::lround(rotate_by_buckets - 0.5f));
+    const float fraction = rotate_by_buckets - full_buckets;
+    while (full_buckets < 0) full_buckets += size;
+    std::vector<float> rotated(size);
+    for (int i = 0; i != size; ++i)
+      rotated[i] = fraction * histogram[(i + 1 + full_buckets) % size] +
+                   (1.f - fraction) * histogram[(i + full_buckets) % size];
+    return rotated;
+  }
+};
+}  // namespace scan_matching
+}  // namespace mapping
 
 namespace mapping {
 // mapping/3d/hybrid_grid.h:468-526: what the adapter needs is iteration over the

@@ -660,6 +660,123 @@ class ConstraintBuilder3D
 #endif  // !CSM_ADAPTER_REAL_CARTOGRAPHER
 
 }  // namespace constraints
+
+#ifndef CSM_ADAPTER_REAL_CARTOGRAPHER
+// A Submap3D (mapping/3d/submap_3d.h:47-103) whose grids live on the device, filled by
+// ActiveSubmaps3D below.  device_submap() is the view ConstraintBuilder3D reads; the
+// rotational scan matcher histogram is accumulated on the host.
+class DeviceSubmap3D {
+ public:
+  DeviceSubmap3D(float high_resolution, float low_resolution,
+                 const transform::Rigid3d& local_submap_pose, int histogram_size, int device)
+      : local_pose_(local_submap_pose),
+        high_(high_resolution, device),
+        low_(low_resolution, device),
+        intensity_(new scan_matching::DeviceIntensityGrid(high_resolution, device)),
+        histogram_(histogram_size, 0.f),
+        view_{&high_, &low_, &histogram_, 0} {}
+  DeviceSubmap3D(const DeviceSubmap3D&) = delete;
+  DeviceSubmap3D& operator=(const DeviceSubmap3D&) = delete;
+
+  const transform::Rigid3d& local_pose() const { return local_pose_; }
+  int num_range_data() const { return num_range_data_; }
+  bool insertion_finished() const { return insertion_finished_; }
+  const scan_matching::DeviceHybridGrid& high_resolution_hybrid_grid() const { return high_; }
+  const scan_matching::DeviceHybridGrid& low_resolution_hybrid_grid() const { return low_; }
+  const scan_matching::DeviceIntensityGrid* high_resolution_intensity_hybrid_grid() const {
+    return intensity_.get();
+  }
+  const std::vector<float>& rotational_scan_matcher_histogram() const { return histogram_; }
+  const constraints::DeviceSubmap3D& device_submap() const { return view_; }
+
+ private:
+  friend class ActiveSubmaps3D;
+  scan_matching::RangeDataInserter3D::SubmapGrids grids() {
+    return {local_pose_, &high_, &low_, intensity_.get()};
+  }
+  // submap_3d.cc:288-293, after the grids took the scan
+  void Inserted(const transform::Quaterniond& local_from_gravity_aligned,
+                const std::vector<float>& scan_histogram_in_gravity) {
+    constraints::b200_internal::Require(!insertion_finished_, "!insertion_finished()");
+    ++num_range_data_;
+    const float yaw_in_submap_from_gravity = transform::GetYaw(
+        local_pose_.inverse().rotation() * local_from_gravity_aligned);
+    const std::vector<float> rotated = scan_matching::RotationalScanMatcher::RotateHistogram(
+        scan_histogram_in_gravity, yaw_in_submap_from_gravity);
+    for (size_t i = 0; i < histogram_.size(); ++i) histogram_[i] += rotated[i];
+  }
+
+  const transform::Rigid3d local_pose_;
+  scan_matching::DeviceHybridGrid high_, low_;
+  std::unique_ptr<scan_matching::DeviceIntensityGrid> intensity_;
+  std::vector<float> histogram_;
+  const constraints::DeviceSubmap3D view_;
+  int num_range_data_ = 0;
+  bool insertion_finished_ = false;
+};
+
+// ActiveSubmaps3D (submap_3d.cc:296-351) over device grids: each scan goes into the (at most
+// two) active submaps with one csm_range_inserter3d_insert_submaps call.  Submaps are shared,
+// so one the pose graph still holds outlives its eviction.
+class ActiveSubmaps3D {
+ public:
+  ActiveSubmaps3D(const proto::SubmapsOptions3D& options, int device = 0)
+      : options_(options),
+        device_(device),
+        range_data_inserter_(options.range_data_inserter_options(), device) {}
+  ActiveSubmaps3D(const ActiveSubmaps3D&) = delete;
+  ActiveSubmaps3D& operator=(const ActiveSubmaps3D&) = delete;
+
+  std::vector<std::shared_ptr<const DeviceSubmap3D>> InsertData(
+      const sensor::RangeData& range_data,
+      const transform::Quaterniond& local_from_gravity_aligned,
+      const std::vector<float>& rotational_scan_matcher_histogram_in_gravity) {
+    if (submaps_.empty() || submaps_.back()->num_range_data() == options_.num_range_data()) {
+      AddSubmap(transform::Rigid3d({{range_data.origin.x(), range_data.origin.y(),
+                                     range_data.origin.z()}},
+                                   local_from_gravity_aligned),
+                static_cast<int>(rotational_scan_matcher_histogram_in_gravity.size()));
+    }
+    std::vector<scan_matching::RangeDataInserter3D::SubmapGrids> grids;
+    for (auto& submap : submaps_) {
+      constraints::b200_internal::Require(!submap->insertion_finished(),
+                                          "!insertion_finished()");
+      grids.push_back(submap->grids());
+    }
+    range_data_inserter_.InsertSubmaps(range_data, grids,
+                                       static_cast<float>(options_.high_resolution_max_range()));
+    for (auto& submap : submaps_)
+      submap->Inserted(local_from_gravity_aligned, rotational_scan_matcher_histogram_in_gravity);
+    if (submaps_.front()->num_range_data() == 2 * options_.num_range_data())
+      submaps_.front()->insertion_finished_ = true;   // Submap3D::Finish
+    return submaps();
+  }
+
+  std::vector<std::shared_ptr<const DeviceSubmap3D>> submaps() const {
+    return std::vector<std::shared_ptr<const DeviceSubmap3D>>(submaps_.begin(), submaps_.end());
+  }
+
+ private:
+  void AddSubmap(const transform::Rigid3d& local_submap_pose, int histogram_size) {
+    if (submaps_.size() >= 2) {
+      constraints::b200_internal::Require(submaps_.front()->insertion_finished(),
+                                          "submaps_.front()->insertion_finished()");
+      submaps_.front()->intensity_.reset();   // ForgetIntensityHybridGrid
+      submaps_.erase(submaps_.begin());
+    }
+    submaps_.emplace_back(new DeviceSubmap3D(
+        static_cast<float>(options_.high_resolution()),
+        static_cast<float>(options_.low_resolution()), local_submap_pose, histogram_size,
+        device_));
+  }
+
+  const proto::SubmapsOptions3D options_;
+  const int device_;
+  scan_matching::RangeDataInserter3D range_data_inserter_;
+  std::vector<std::shared_ptr<DeviceSubmap3D>> submaps_;
+};
+#endif  // !CSM_ADAPTER_REAL_CARTOGRAPHER
+
 }  // namespace mapping
 }  // namespace cartographer
 

@@ -791,6 +791,35 @@ class RangeDataInserter3D {
         intensity_hybrid_grid ? intensity_hybrid_grid->mutable_handle() : nullptr, nullptr));
   }
 
+  // The grids of one submap that InsertSubmaps writes, in that submap's frame.
+  struct SubmapGrids {
+    transform::Rigid3d local_pose;
+    DeviceHybridGrid* high_resolution_hybrid_grid;
+    DeviceHybridGrid* low_resolution_hybrid_grid;
+    DeviceIntensityGrid* high_resolution_intensity_hybrid_grid;   // null once forgotten
+  };
+  // Submap3D::InsertData's two inserts (submap_3d.cc:276-287) into each of `submaps`, in
+  // order, with one call (csm_range_inserter3d_insert_submaps); range_data in the local frame.
+  void InsertSubmaps(const sensor::RangeData& range_data, const std::vector<SubmapGrids>& submaps,
+                     float high_resolution_max_range) const {
+    std::vector<csm_submap_insert3d> entries(submaps.size());
+    for (size_t i = 0; i < submaps.size(); ++i) {
+      b200_internal::Pose7(submaps[i].local_pose, entries[i].local_pose);
+      entries[i].high_resolution = submaps[i].high_resolution_hybrid_grid->mutable_handle();
+      entries[i].low_resolution = submaps[i].low_resolution_hybrid_grid->mutable_handle();
+      entries[i].intensity = submaps[i].high_resolution_intensity_hybrid_grid
+                                 ? submaps[i].high_resolution_intensity_hybrid_grid->mutable_handle()
+                                 : nullptr;
+    }
+    const std::vector<float> xyz = b200_internal::Flatten(range_data.returns);
+    const float origin[3] = {range_data.origin.x(), range_data.origin.y(), range_data.origin.z()};
+    const std::vector<float>& intensities = range_data.returns.intensities();
+    b200_internal::Check(csm_range_inserter3d_insert_submaps(
+        inserter_, entries.data(), static_cast<int32_t>(entries.size()), origin, xyz.data(),
+        intensities.empty() ? nullptr : intensities.data(),
+        static_cast<int32_t>(range_data.returns.size()), high_resolution_max_range, nullptr));
+  }
+
  private:
   csm_range_inserter3d* inserter_ = nullptr;
 };

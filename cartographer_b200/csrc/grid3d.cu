@@ -406,7 +406,6 @@ csm_status GridInsert3::Begin() {
   Ctx* ctx = grid_->ctx;
   cudaStream_t s = ctx->stream;
   CSM_CUDA(cudaSetDevice(ctx->device));
-  CSM_CUDA(cudaEventRecord(ctx->ev0, s));
   if (grow_) CSM_TRY(Regrow(grid_->d_vol, BoxOf(grid_->g), box, s, &vol));
   if (!igrid_) return CSM_OK;
   const Box3& iold = igrid_->box;

@@ -152,15 +152,16 @@ csm_status DeviceVoxels3D(const csm_grid3d* g, long long list_capacity, long lon
 // The part of one 3D insert that changes the handles (caller holds ctx->mu; intensity_grid is
 // null when the insert adds no intensities):
 //   1. Grow: from the tight boxes the insert needs, the box each handle's volumes grow to;
-//   2. Begin: records ctx->ev0 and queues on the context's stream the grown volumes, with the
-//      old ones copied in, and, on the first insert into the intensity handle, its sum / count
-//      volumes at their final box with the voxel list it was made from scattered in;
+//   2. Begin: queues on the context's stream the grown volumes, with the old ones copied in,
+//      and, on the first insert into the intensity handle, its sum / count volumes at their
+//      final box with the voxel list it was made from scattered in;
 //   3. the caller's kernels write vol at `box` and mean / sum / count at `ibox`; the caller
-//      records ctx->ev1 and synchronises the stream;
+//      records ctx->ev1 (ctx->ev0 before its first device work) and synchronises the stream;
 //   4. Commit: installs the volumes, boxes and tight boxes, frees the volumes they replace,
-//      drops the voxel list the intensity handle was made from and fills stats.
+//      drops the voxel list the intensity handle was made from and fills stats (may be NULL).
 // No handle field changes before Commit.  Volumes not committed are freed when the transaction
-// ends: the handles keep their volumes, boxes and contents.
+// ends: the handles keep their volumes, boxes and contents.  Several transactions make one when
+// the caller grows all of them before it begins any, and commits all of them or none.
 class GridInsert3 {
  public:
   GridInsert3(csm_grid3d* grid, csm_intensity_grid3d* intensity_grid);

@@ -140,6 +140,21 @@ inline Quatf QuatCastInverseD(const Quatd& q) {
                static_cast<float>(inv.z)};
 }
 
+// transform::Rigid3d::inverse().cast<float>() (rigid_transform.h:148-152) of pose {t xyz,
+// q wxyz}: the conjugate, and -(conjugate * t) by Eigen 3.3's _transformVector in double.
+inline Rigid3f Rigid3dInverseCast(const double pose[7]) {
+  const double w = pose[3], x = -pose[4], y = -pose[5], z = -pose[6];
+  const double* t = pose;
+  double uv[3] = {y * t[2] - z * t[1], z * t[0] - x * t[2], x * t[1] - y * t[0]};
+  for (double& u : uv) u += u;
+  const double c[3] = {y * uv[2] - z * uv[1], z * uv[0] - x * uv[2], x * uv[1] - y * uv[0]};
+  return Rigid3f{Vec3f{static_cast<float>(-(t[0] + w * uv[0] + c[0])),
+                       static_cast<float>(-(t[1] + w * uv[1] + c[1])),
+                       static_cast<float>(-(t[2] + w * uv[2] + c[2]))},
+                 Quatf{static_cast<float>(w), static_cast<float>(x), static_cast<float>(y),
+                       static_cast<float>(z)}};
+}
+
 // Quaternionf(AngleAxisf(angle, UnitZ)): Eigen takes cos / sin of the float half angle.
 inline Quatf QuatFromAngleAxisZ(float angle) {
   const float ha = 0.5f * angle;

@@ -6,6 +6,7 @@ Reference: cartographer/mapping/internal/2d/scan_matching/
   fast_correlative_scan_matcher_2d.h:112-136, real_time_correlative_scan_matcher_2d.h:53-85.
 """
 import ctypes as C
+import math
 from dataclasses import dataclass, field
 
 import numpy as np
@@ -1444,12 +1445,178 @@ class RangeDataInserter3D:
             None if intensity_grid is None else intensity_grid._h, C.byref(stats)))
         self.last_stats = stats.as_dict()
 
+    def insert_submaps(self, submaps, origin, returns, intensities, high_resolution_max_range):
+        """Submap3D::InsertData's inserts (submap_3d.cc:271-287) into several submaps in one
+        call (csm_range_inserter3d_insert_submaps).  `submaps`: (local_pose, high_resolution,
+        low_resolution, intensity) tuples, local_pose (tx, ty, tz, qw, qx, qy, qz), the grids
+        DeviceHybridGrids and intensity a DeviceIntensityGrid or None.  origin (3), returns
+        (n x 3) and intensities (n, or None) are in the local frame."""
+        entries = (CsmSubmapInsert3D * len(submaps))()
+        for e, (pose, high, low, intensity) in zip(entries, submaps):
+            e.local_pose[:] = [float(v) for v in pose]
+            e.high_resolution = high._h
+            e.low_resolution = low._h
+            e.intensity = None if intensity is None else intensity._h
+        org = np.ascontiguousarray(origin, dtype=np.float32).reshape(3)
+        xyz = _f32(returns)
+        inten = None
+        if intensities is not None:
+            inten = np.ascontiguousarray(intensities, dtype=np.float32).reshape(-1)
+            if len(inten) != len(xyz):
+                raise ValueError("intensities and returns differ in length")
+        stats = CsmStats()
+        check(lib().csm_range_inserter3d_insert_submaps(
+            self._h, entries, C.c_int32(len(submaps)), ptr(org, C.c_float), ptr(xyz, C.c_float),
+            None if inten is None else ptr(inten, C.c_float), C.c_int32(len(xyz)),
+            C.c_float(high_resolution_max_range), C.byref(stats)))
+        self.last_stats = stats.as_dict()
+
     def close(self):
         if getattr(self, "_h", None):
             lib().csm_range_inserter3d_destroy(self._h)
             self._h = None
 
     __del__ = close
+
+
+class CsmSubmapInsert3D(C.Structure):
+    _fields_ = [("local_pose", C.c_double * 7), ("high_resolution", C.c_void_p),
+                ("low_resolution", C.c_void_p), ("intensity", C.c_void_p)]
+
+
+# ===========================================================================
+# Submap3D and ActiveSubmaps3D (mapping/3d/submap_3d.h) over device grids
+# ===========================================================================
+@dataclass
+class SubmapsOptions3D:
+    """proto SubmapsOptions3D (mapping/proto/submaps_options_3d.proto); defaults are
+    configuration_files/trajectory_builder_3d.lua's submaps."""
+    high_resolution: float = 0.10
+    high_resolution_max_range: float = 20.0
+    low_resolution: float = 0.45
+    num_range_data: int = 160
+    range_data_inserter_options: RangeDataInserterOptions3D = field(
+        default_factory=RangeDataInserterOptions3D)
+
+
+def yaw_in_submap_from_gravity(local_pose, local_from_gravity_aligned):
+    """transform::GetYaw(local_pose.inverse().rotation() * local_from_gravity_aligned) in
+    double (submap_3d.cc:289-290), as the float InsertData passes on.  Quaternions are
+    (w, x, y, z); the product and the rotation of UnitX in Eigen's scalar order."""
+    pw, px, py, pz = (float(local_pose[3]), -float(local_pose[4]), -float(local_pose[5]),
+                      -float(local_pose[6]))
+    qw, qx, qy, qz = (float(v) for v in local_from_gravity_aligned)
+    w = pw * qw - px * qx - py * qy - pz * qz
+    x = pw * qx + px * qw + py * qz - pz * qy
+    y = pw * qy + py * qw + pz * qx - px * qz
+    z = pw * qz + pz * qw + px * qy - py * qx
+    # q * UnitX (_transformVector): uv = q.vec x v, uv += uv, v + w uv + q.vec x uv, with
+    # every product of the zeros of UnitX kept (they decide the sign of a zero y)
+    v = (1.0, 0.0, 0.0)
+    uv = [y * v[2] - z * v[1], z * v[0] - x * v[2], x * v[1] - y * v[0]]
+    uv = [u + u for u in uv]
+    cross = (y * uv[2] - z * uv[1], z * uv[0] - x * uv[2], x * uv[1] - y * uv[0])
+    dx = v[0] + w * uv[0] + cross[0]
+    dy = v[1] + w * uv[1] + cross[1]
+    return np.float32(math.atan2(dy, dx))
+
+
+def rotate_histogram(histogram, angle):
+    """RotationalScanMatcher::RotateHistogram (rotational_scan_matcher.cc:141-162) in float."""
+    h = np.ascontiguousarray(histogram, np.float32).reshape(-1)
+    size = len(h)
+    if size == 0:
+        return h.copy()
+    rotate_by_buckets = np.float32(float(-np.float32(angle) * np.float32(size)) / math.pi)
+    v = np.float32(rotate_by_buckets - np.float32(0.5))
+    full = int(math.floor(abs(float(v)) + 0.5) * (1 if v >= 0 else -1))   # std::lround
+    fraction = np.float32(rotate_by_buckets - np.float32(full))
+    full %= size
+    r0 = np.roll(h, -full)
+    r1 = np.roll(h, -(full + 1))
+    return (fraction * r1 + (np.float32(1) - fraction) * r0).astype(np.float32)
+
+
+class DeviceSubmap3D:
+    """A Submap3D whose grids live on the device: local_pose (tx, ty, tz, qw, qx, qy, qz),
+    the high- and low-resolution DeviceHybridGrids, the high-resolution DeviceIntensityGrid
+    (None once forgotten), num_range_data, insertion_finished and the float32 rotational scan
+    matcher histogram, accumulated on the host."""
+
+    def __init__(self, options, local_pose, histogram_size, device=0):
+        self.local_pose = tuple(float(v) for v in local_pose)
+        self.high_resolution_hybrid_grid = DeviceHybridGrid.empty(options.high_resolution,
+                                                                  device)
+        self.low_resolution_hybrid_grid = DeviceHybridGrid.empty(options.low_resolution, device)
+        self.high_resolution_intensity_hybrid_grid = DeviceIntensityGrid.empty(
+            options.high_resolution, device)
+        self.rotational_scan_matcher_histogram = np.zeros(histogram_size, np.float32)
+        self.num_range_data = 0
+        self.insertion_finished = False
+
+    def Finish(self):
+        assert not self.insertion_finished
+        self.insertion_finished = True
+
+    def ForgetIntensityHybridGrid(self):
+        if self.high_resolution_intensity_hybrid_grid is not None:
+            self.high_resolution_intensity_hybrid_grid.close()
+        self.high_resolution_intensity_hybrid_grid = None
+
+    def constraint_builder_submap(self):
+        """The constraint_builder.Submap3D view ConstraintBuilder3D reads."""
+        from .constraint_builder import Submap3D
+        return Submap3D(self.high_resolution_hybrid_grid, self.low_resolution_hybrid_grid,
+                        self.rotational_scan_matcher_histogram)
+
+
+class ActiveSubmaps3D:
+    """ActiveSubmaps3D (submap_3d.cc:296-351) over device grids: InsertData writes each scan
+    into the (at most two) active submaps with one csm_range_inserter3d_insert_submaps call.
+    Evicted submaps are dropped from the list but stay alive while the caller holds them."""
+
+    def __init__(self, options, device=0):
+        self.options = options
+        self.device = device
+        self.range_data_inserter = RangeDataInserter3D(options.range_data_inserter_options,
+                                                       device)
+        self._submaps = []
+
+    def submaps(self):
+        return list(self._submaps)
+
+    def InsertData(self, origin, returns, intensities, local_from_gravity_aligned,
+                   rotational_scan_matcher_histogram_in_gravity):
+        """origin (3), returns (n x 3), intensities (n or None) in the local frame;
+        local_from_gravity_aligned (w, x, y, z).  Returns the active submaps."""
+        hist = np.ascontiguousarray(rotational_scan_matcher_histogram_in_gravity,
+                                    np.float32).reshape(-1)
+        if (not self._submaps or
+                self._submaps[-1].num_range_data == self.options.num_range_data):
+            org = np.asarray(origin, np.float32).reshape(3)
+            self._add_submap([float(org[0]), float(org[1]), float(org[2])] +
+                             [float(v) for v in local_from_gravity_aligned], len(hist))
+        self.range_data_inserter.insert_submaps(
+            [(s.local_pose, s.high_resolution_hybrid_grid, s.low_resolution_hybrid_grid,
+              s.high_resolution_intensity_hybrid_grid) for s in self._submaps],
+            origin, returns, intensities, self.options.high_resolution_max_range)
+        for s in self._submaps:
+            assert not s.insertion_finished
+            s.num_range_data += 1
+            yaw = yaw_in_submap_from_gravity(s.local_pose, local_from_gravity_aligned)
+            s.rotational_scan_matcher_histogram = (s.rotational_scan_matcher_histogram +
+                                                   rotate_histogram(hist, yaw))
+        if self._submaps[0].num_range_data == 2 * self.options.num_range_data:
+            self._submaps[0].Finish()
+        return self.submaps()
+
+    def _add_submap(self, local_pose, histogram_size):
+        if len(self._submaps) >= 2:
+            assert self._submaps[0].insertion_finished
+            self._submaps[0].ForgetIntensityHybridGrid()
+            del self._submaps[0]
+        self._submaps.append(DeviceSubmap3D(self.options, local_pose, histogram_size,
+                                            self.device))
 
 
 class RealTimeCorrelativeScanMatcher3D:

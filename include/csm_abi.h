@@ -783,6 +783,34 @@ csm_status csm_range_inserter3d_insert(const csm_range_inserter3d* inserter,
                                        const float* intensities, int32_t num_returns,
                                        csm_grid3d* grid, csm_intensity_grid3d* intensity_grid,
                                        csm_stats* stats /* may be NULL */);
+/* Submap3D::InsertData (mapping/3d/submap_3d.cc:271-294) into every entry of `submaps`, in
+ * order, in one call: the range data (origin, num_returns x {x, y, z} returns and, may be NULL,
+ * num_returns intensities) is in the local frame; each entry transforms it by
+ * local_pose().inverse().cast<float>(), inserts the returns within high_resolution_max_range
+ * of the transformed origin into high_resolution and, with intensities, intensity (may be NULL:
+ * ForgetIntensityHybridGrid), and every return into low_resolution.  Every handle ends
+ * bit-equal to what csm_range_inserter3d_insert leaves when it is given the transformed and
+ * filtered data of each entry in turn: voxels, intensity sums, counts and means, dense and
+ * tight boxes (the origin cell joins a handle's box only when that handle receives a return).
+ * With no returns every handle keeps its contents and boxes; the origin is still checked.
+ * CSM_E_INVALID, with every handle unchanged, for a null pointer, num_submaps outside
+ * [1, 65535], a handle that appears twice, a handle on another device than the inserter, or
+ * what csm_range_inserter3d_insert refuses for any entry: a non-finite point or an origin, hit
+ * or intensity cell outside [-8192, 8192)^3, or num_samples >= 2^15.  Two stream
+ * synchronisations however many entries; stats (may be NULL) gets host_syncs and device_ms. */
+typedef struct csm_submap_insert3d {
+  double local_pose[7];                 /* the submap's local_pose(): t xyz, q wxyz */
+  csm_grid3d* high_resolution;
+  csm_grid3d* low_resolution;
+  csm_intensity_grid3d* intensity;      /* may be NULL */
+} csm_submap_insert3d;
+csm_status csm_range_inserter3d_insert_submaps(const csm_range_inserter3d* inserter,
+                                               const csm_submap_insert3d* submaps,
+                                               int32_t num_submaps, const float origin[3],
+                                               const float* returns, const float* intensities,
+                                               int32_t num_returns,
+                                               float high_resolution_max_range,
+                                               csm_stats* stats /* may be NULL */);
 /* Test hooks: a handle's current dense box.  With out / mean == NULL only lo and dims are
  * written; otherwise the box is copied out (((z - lo.z) * dims.y + (y - lo.y)) * dims.x +
  * (x - lo.x)).  For an intensity grid, sum and count (each may be NULL) are every voxel's
