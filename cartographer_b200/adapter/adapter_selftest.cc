@@ -643,6 +643,56 @@ int main() {
       PrintBytes("texture_response3d_low", low_texture);
     }
   }
+  // ---- ActiveSubmaps2D over device grids: seven scans with num_range_data = 2, so submaps
+  // roll over, finish and are evicted; the active submaps' grids, limits, boxes, counts,
+  // finished flags and local poses, and the first submap's after its eviction, which
+  // tests/test_gpu_adapter_active_submaps2d.py holds equal to scan_matching.ActiveSubmaps2D's ----
+  {
+    mapping::proto::SubmapsOptions2D so;
+    so.set_num_range_data(2);
+    so.mutable_grid_options_2d()->set_resolution(0.05f);
+    auto* pgo = so.mutable_range_data_inserter_options()
+                    ->mutable_probability_grid_range_data_inserter_options_2d();
+    pgo->set_hit_probability(0.55);
+    pgo->set_miss_probability(0.49);
+    pgo->set_insert_free_space(true);
+    mapping::ActiveSubmaps2D active(so, 0);
+    std::shared_ptr<const mapping::DeviceSubmap2D> first;
+    std::vector<std::shared_ptr<const mapping::DeviceSubmap2D>> subs;
+    for (int k = 0; k < 7; ++k) {
+      sensor::RangeData range_data;
+      range_data.origin = {{0.3f * k, -0.2f * k, 0.f}};
+      for (int i = 0; i < 180; ++i) {
+        const double a = 0.035 * i + 0.1 * k;
+        const float r = (i % 7 == 3) ? 5.f : 2.f + 0.01f * (i % 40);
+        const sensor::RangefinderPoint p{{{range_data.origin.x() + r * static_cast<float>(std::cos(a)),
+                                           range_data.origin.y() + r * static_cast<float>(std::sin(a)),
+                                           0.f}}};
+        (i % 7 == 3 ? range_data.misses : range_data.returns).push_back(p);
+      }
+      subs = active.InsertRangeData(range_data);
+      if (!first) first = subs.front();
+    }
+    auto print = [](const char* name, const mapping::DeviceSubmap2D& s) {
+      std::vector<uint16_t> cells;
+      const csm_rt_grid2d_info info = s.grid().Read(&cells);
+      std::printf("RESULT %s_grid %d %d %.17g %.17g %.17g %d %d %d %d %d", name, info.num_x_cells,
+                  info.num_y_cells, info.resolution, info.max_x, info.max_y, info.known_empty,
+                  info.known_min_x, info.known_min_y, info.known_max_x, info.known_max_y);
+      for (uint16_t c : cells) std::printf(" %u", c);
+      std::printf("\n");
+      const transform::Rigid3d& p = s.local_pose();
+      std::printf("RESULT %s_state %d %d %.17g %.17g %.17g %.17g %.17g %.17g %.17g\n", name,
+                  s.num_range_data(), s.insertion_finished() ? 1 : 0, p.translation().x(),
+                  p.translation().y(), p.translation().z(), p.rotation().w(), p.rotation().x(),
+                  p.rotation().y(), p.rotation().z());
+    };
+    if (subs.size() != 2 || first == subs.front() || !first->insertion_finished()) return 1;
+    print("active2d0", *subs[0]);
+    print("active2d1", *subs[1]);
+    print("evicted2d", *first);
+    if (first->device_submap().grid != &first->grid()) return 1;
+  }
   // ---- ActiveSubmaps3D over device grids: seven scans with num_range_data = 2, so submaps
   // roll over, finish and are evicted; the active submaps' handles and histograms, and the
   // first submap's after its eviction, which tests/test_gpu_adapter_active_submaps3d.py holds

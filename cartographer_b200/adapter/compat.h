@@ -259,6 +259,47 @@ class SubmapsOptions3D {
   int32_t num_range_data_ = 0;
   RangeDataInserterOptions3D inserter_;
 };
+// mapping/proto/grid_2d_options.proto: the grid type and the float resolution
+class GridOptions2D {
+ public:
+  enum GridType { INVALID_GRID = 0, PROBABILITY_GRID = 1, TSDF = 2 };
+  GridType grid_type() const { return grid_type_; }
+  float resolution() const { return resolution_; }
+  void set_grid_type(GridType v) { grid_type_ = v; }
+  void set_resolution(float v) { resolution_ = v; }
+ private:
+  GridType grid_type_ = PROBABILITY_GRID;
+  float resolution_ = 0.f;
+};
+// mapping/proto/range_data_inserter_options.proto
+class RangeDataInserterOptions {
+ public:
+  enum RangeDataInserterType {
+    INVALID_INSERTER = 0, PROBABILITY_GRID_INSERTER_2D = 1, TSDF_INSERTER_2D = 2 };
+  RangeDataInserterType range_data_inserter_type() const { return type_; }
+  void set_range_data_inserter_type(RangeDataInserterType v) { type_ = v; }
+  const ProbabilityGridRangeDataInserterOptions2D&
+  probability_grid_range_data_inserter_options_2d() const { return probability_; }
+  ProbabilityGridRangeDataInserterOptions2D*
+  mutable_probability_grid_range_data_inserter_options_2d() { return &probability_; }
+ private:
+  RangeDataInserterType type_ = PROBABILITY_GRID_INSERTER_2D;
+  ProbabilityGridRangeDataInserterOptions2D probability_;
+};
+// mapping/proto/submaps_options_2d.proto
+class SubmapsOptions2D {
+ public:
+  int32_t num_range_data() const { return num_range_data_; }
+  const GridOptions2D& grid_options_2d() const { return grid_; }
+  GridOptions2D* mutable_grid_options_2d() { return &grid_; }
+  const RangeDataInserterOptions& range_data_inserter_options() const { return inserter_; }
+  RangeDataInserterOptions* mutable_range_data_inserter_options() { return &inserter_; }
+  void set_num_range_data(int32_t v) { num_range_data_ = v; }
+ private:
+  int32_t num_range_data_ = 0;
+  GridOptions2D grid_;
+  RangeDataInserterOptions inserter_;
+};
 }  // namespace proto
 namespace scan_matching {
 // mapping/internal/3d/scan_matching/rotational_scan_matcher.cc:141-162, on the std::vector<float>

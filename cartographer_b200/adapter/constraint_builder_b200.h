@@ -662,6 +662,124 @@ class ConstraintBuilder3D
 }  // namespace constraints
 
 #ifndef CSM_ADAPTER_REAL_CARTOGRAPHER
+// A ProbabilityGrid Submap2D (mapping/2d/submap_2d.h:37-71) whose grid lives on the device,
+// filled by ActiveSubmaps2D below.  grid() is the active grid until Finish, then its crop;
+// device_submap() is the view ConstraintBuilder2D reads of a finished submap.
+class DeviceSubmap2D {
+ public:
+  DeviceSubmap2D(float origin_x, float origin_y, float resolution, int device)
+      : local_pose_(transform::Rigid3d(
+            {{static_cast<double>(origin_x), static_cast<double>(origin_y), 0.}},
+            transform::Quaterniond{1., 0., 0., 0.})),   // Rigid3d::Translation
+        grid_(new scan_matching::DeviceGrid2D(CreateGridLimits(origin_x, origin_y, resolution),
+                                              device)),
+        view_{nullptr, transform::Rigid2d({static_cast<double>(origin_x),
+                                           static_cast<double>(origin_y)}, 0.)} {}
+  DeviceSubmap2D(const DeviceSubmap2D&) = delete;
+  DeviceSubmap2D& operator=(const DeviceSubmap2D&) = delete;
+
+  const transform::Rigid3d& local_pose() const { return local_pose_; }
+  int num_range_data() const { return num_range_data_; }
+  bool insertion_finished() const { return insertion_finished_; }
+  const scan_matching::DeviceGrid2D& grid() const { return *grid_; }
+  // ConstraintBuilder2D's view: the cropped grid and ComputeSubmapPose's pose.
+  const constraints::DeviceSubmap2D& device_submap() const {
+    constraints::b200_internal::Require(insertion_finished_, "insertion_finished()");
+    return view_;
+  }
+
+  // ActiveSubmaps2D::CreateGrid (submap_2d.cc:192-204): 100 x 100 cells with
+  // max = origin.cast<double>() + 0.5 * 100 * resolution, resolution the float option.
+  static MapLimits CreateGridLimits(float origin_x, float origin_y, float resolution) {
+    constexpr int kInitialSubmapSize = 100;
+    const double r = resolution;
+    return MapLimits(r, static_cast<double>(origin_x) + 0.5 * kInitialSubmapSize * r,
+                     static_cast<double>(origin_y) + 0.5 * kInitialSubmapSize * r,
+                     CellLimits{kInitialSubmapSize, kInitialSubmapSize});
+  }
+
+ private:
+  friend class ActiveSubmaps2D;
+  // Submap2D::Finish (:146-151): grid_ = grid_->ComputeCroppedGrid(), which drops the
+  // uncropped handle.
+  void Finish() {
+    constraints::b200_internal::Require(!insertion_finished_, "!insertion_finished()");
+    grid_ = grid_->ComputeCroppedGrid();
+    view_.grid = grid_.get();
+    insertion_finished_ = true;
+  }
+
+  const transform::Rigid3d local_pose_;
+  std::unique_ptr<scan_matching::DeviceGrid2D> grid_;
+  constraints::DeviceSubmap2D view_;
+  int num_range_data_ = 0;
+  bool insertion_finished_ = false;
+};
+
+// ActiveSubmaps2D (submap_2d.cc:153-236) over device grids: each scan goes into the (at most
+// two) active submaps with one csm_range_inserter2d_insert_submaps call.  ProbabilityGrid
+// submaps only: a TSDF2D crop has no device form.  Submaps are shared, so one the pose graph
+// still holds outlives its eviction.
+class ActiveSubmaps2D {
+ public:
+  ActiveSubmaps2D(const proto::SubmapsOptions2D& options, int device = 0)
+      : options_(Checked(options)),
+        device_(device),
+        range_data_inserter_(options.range_data_inserter_options()
+                                 .probability_grid_range_data_inserter_options_2d(),
+                             device) {}
+  ActiveSubmaps2D(const ActiveSubmaps2D&) = delete;
+  ActiveSubmaps2D& operator=(const ActiveSubmaps2D&) = delete;
+
+  std::vector<std::shared_ptr<const DeviceSubmap2D>> InsertRangeData(
+      const sensor::RangeData& range_data) {
+    if (submaps_.empty() || submaps_.back()->num_range_data() == options_.num_range_data())
+      AddSubmap(range_data.origin.x(), range_data.origin.y());
+    std::vector<scan_matching::DeviceGrid2D*> grids;
+    for (auto& submap : submaps_) {
+      constraints::b200_internal::Require(!submap->insertion_finished(),
+                                          "!insertion_finished()");
+      grids.push_back(submap->grid_.get());
+    }
+    range_data_inserter_.InsertSubmaps(range_data, grids);
+    for (auto& submap : submaps_) ++submap->num_range_data_;
+    if (submaps_.front()->num_range_data() == 2 * options_.num_range_data())
+      submaps_.front()->Finish();
+    return submaps();
+  }
+
+  std::vector<std::shared_ptr<const DeviceSubmap2D>> submaps() const {
+    return std::vector<std::shared_ptr<const DeviceSubmap2D>>(submaps_.begin(), submaps_.end());
+  }
+
+ private:
+  // CreateSubmapsOptions2D's checks (submap_2d.cc:45-69), and the device's grid type
+  static const proto::SubmapsOptions2D& Checked(const proto::SubmapsOptions2D& options) {
+    constraints::b200_internal::Require(options.num_range_data() > 0,
+                                        "num_range_data() > 0");
+    constraints::b200_internal::Require(
+        options.grid_options_2d().grid_type() == proto::GridOptions2D::PROBABILITY_GRID &&
+            options.range_data_inserter_options().range_data_inserter_type() ==
+                proto::RangeDataInserterOptions::PROBABILITY_GRID_INSERTER_2D,
+        "ProbabilityGrid submaps (a TSDF2D crop has no device form)");
+    return options;
+  }
+  void AddSubmap(float origin_x, float origin_y) {
+    if (submaps_.size() >= 2) {
+      constraints::b200_internal::Require(submaps_.front()->insertion_finished(),
+                                          "submaps_.front()->insertion_finished()");
+      submaps_.erase(submaps_.begin());
+    }
+    submaps_.emplace_back(new DeviceSubmap2D(origin_x, origin_y,
+                                             options_.grid_options_2d().resolution(), device_));
+  }
+
+  const proto::SubmapsOptions2D options_;
+  const int device_;
+  scan_matching::ProbabilityGridRangeDataInserter2D range_data_inserter_;
+  std::vector<std::shared_ptr<DeviceSubmap2D>> submaps_;
+};
+
 // A Submap3D (mapping/3d/submap_3d.h:47-103) whose grids live on the device, filled by
 // ActiveSubmaps3D below.  device_submap() is the view ConstraintBuilder3D reads; the
 // rotational scan matcher histogram is accumulated on the host.

@@ -418,6 +418,25 @@ class ProbabilityGridRangeDataInserter2D {
         misses.data(), static_cast<int32_t>(range_data.misses.size()), grid->mutable_handle(),
         nullptr));
   }
+  // Insert(range_data, grid) into every grid of `grids`, in one call
+  // (csm_range_inserter2d_insert_submaps): what ActiveSubmaps2D::InsertRangeData
+  // (submap_2d.cc:162-175) does to its active submaps.  Each grid ends as grids.size() Insert
+  // calls in order would leave it; range_data in the local frame.
+  void InsertSubmaps(const sensor::RangeData& range_data,
+                     const std::vector<DeviceGrid2D*>& grids) const {
+    std::vector<csm_rt_grid2d*> handles;
+    for (DeviceGrid2D* grid : grids) {
+      if (grid == nullptr) std::abort();  // CHECK(:127)
+      handles.push_back(grid->mutable_handle());
+    }
+    const std::vector<float> returns = b200_internal::Flatten(range_data.returns);
+    const std::vector<float> misses = b200_internal::Flatten(range_data.misses);
+    const float origin[3] = {range_data.origin.x(), range_data.origin.y(), range_data.origin.z()};
+    b200_internal::Check(csm_range_inserter2d_insert_submaps(
+        inserter_, origin, returns.data(), static_cast<int32_t>(range_data.returns.size()),
+        misses.data(), static_cast<int32_t>(range_data.misses.size()), handles.data(),
+        static_cast<int32_t>(handles.size()), nullptr));
+  }
 
  private:
   csm_range_inserter2d* inserter_ = nullptr;

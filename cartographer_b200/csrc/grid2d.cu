@@ -157,22 +157,30 @@ csm_status NewGrid(Ctx* ctx, int nx, int ny, double resolution, double max_x, do
   return CSM_OK;
 }
 
+// The staging of known-cells boxes: slot k is ints [4k, 4k + 4) of the device and pinned
+// "ins2_box" buffers.
+csm_status ReserveBoxSlots(Ctx* ctx, int n) {
+  CSM_TRY(ctx->D("ins2_box").Reserve(4 * sizeof(int) * static_cast<size_t>(n)));
+  CSM_TRY(ctx->P("ins2_box").Reserve(4 * sizeof(int) * static_cast<size_t>(n)));
+  return CSM_OK;
+}
+
+const int* StagedBox(Ctx* ctx, int slot) { return ctx->P("ins2_box").as<int>() + 4 * slot; }
+
 // Starts the known-box reduction of the handle's (tsd) cells and its copy (min x, min y, max x,
-// max y) into the pinned "ins2_box" buffer on the handle's stream; the caller synchronises
-// before BoxFrom reads it.
-csm_status StartKnownBox(csm_rt_grid2d* grid) {
+// max y) into slot `slot` of the pinned "ins2_box" buffer on the handle's stream; the caller
+// reserved the slot and synchronises before BoxFrom reads it.
+csm_status StartKnownBox(csm_rt_grid2d* grid, int slot) {
   Ctx* ctx = grid->ctx;
-  DevBuf& d_box = ctx->D("ins2_box");
-  PinnedBuf& h_box = ctx->P("ins2_box");
-  CSM_TRY(d_box.Reserve(4 * sizeof(int)));
-  CSM_TRY(h_box.Reserve(4 * sizeof(int)));
+  int* d_box = ctx->D("ins2_box").as<int>() + 4 * slot;
+  int* h_box = ctx->P("ins2_box").as<int>() + 4 * slot;
   const int init[4] = {INT_MAX, INT_MAX, INT_MIN, INT_MIN};
-  CSM_CUDA(cudaMemcpyAsync(d_box.p, init, sizeof(init), cudaMemcpyHostToDevice, ctx->stream));
+  CSM_CUDA(cudaMemcpyAsync(d_box, init, sizeof(init), cudaMemcpyHostToDevice, ctx->stream));
   const long long total = static_cast<long long>(grid->g.nx) * grid->g.ny;
   k_ins2_known_box<<<Blocks(total, ctx->sm_count * 8), 256, 0, ctx->stream>>>(
-      grid->d_cells, grid->g.nx, grid->g.ny, grid->g.pitch, d_box.as<int>());
+      grid->d_cells, grid->g.nx, grid->g.ny, grid->g.pitch, d_box);
   CSM_LAUNCH_CHECK();
-  CSM_CUDA(cudaMemcpyAsync(h_box.p, d_box.p, 4 * sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
+  CSM_CUDA(cudaMemcpyAsync(h_box, d_box, 4 * sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
   return CSM_OK;
 }
 
@@ -201,9 +209,10 @@ csm_status KnownBox(csm_rt_grid2d* grid) {
   if (!grid->known_stale) return CSM_OK;
   Ctx* ctx = grid->ctx;
   CSM_CUDA(cudaSetDevice(ctx->device));
-  CSM_TRY(StartKnownBox(grid));
+  CSM_TRY(ReserveBoxSlots(ctx, 1));
+  CSM_TRY(StartKnownBox(grid, 0));
   CSM_CUDA(cudaStreamSynchronize(ctx->stream));
-  grid->known = BoxFrom(ctx->P("ins2_box").as<int>());
+  grid->known = BoxFrom(StagedBox(ctx, 0));
   grid->known_stale = false;
   return CSM_OK;
 }
@@ -329,6 +338,8 @@ namespace csm {
 
 csm_status RefreshKnownBox(csm_rt_grid2d* grid) { return KnownBox(grid); }
 
+csm_status ReserveKnownBoxSlots(Ctx* ctx, int n) { return ReserveBoxSlots(ctx, n); }
+
 csm_status UploadCells(csm_rt_grid2d* g, const uint16_t* cells, const uint16_t* wcells,
                        cudaStream_t s) {
   CSM_CUDA(cudaMemcpy2DAsync(g->d_cells, static_cast<size_t>(g->g.pitch) * 2, cells,
@@ -360,10 +371,11 @@ csm_status RtGridCreate(const uint16_t* cells, const uint16_t* wcells, float tru
   return CSM_OK;
 }
 
-GridInsert2::GridInsert2(csm_rt_grid2d* grid)
+GridInsert2::GridInsert2(csm_rt_grid2d* grid, int box_slot)
     : L{grid->g.resolution, grid->g.max_x, grid->g.max_y, grid->g.nx, grid->g.ny},
       arrays{grid->d_cells, grid->d_wcells, grid->g.pitch},
-      grid_(grid) {}
+      grid_(grid),
+      box_slot_(box_slot) {}
 
 GridInsert2::~GridInsert2() {
   if (!grown_) return;
@@ -384,10 +396,12 @@ bool GridInsert2::Grow(float lo_x, float lo_y, float hi_x, float hi_y) {
 csm_status GridInsert2::Begin() {
   Ctx* ctx = grid_->ctx;
   CSM_CUDA(cudaSetDevice(ctx->device));
-  CSM_CUDA(cudaEventRecord(ctx->ev0, ctx->stream));
   // the known box of a handle made from cells, before its cells move
   box_stale_ = grid_->known_stale;
-  if (box_stale_) CSM_TRY(StartKnownBox(grid_));
+  if (box_stale_) {
+    CSM_TRY(ReserveBoxSlots(ctx, box_slot_ + 1));   // no-op once the caller reserved its slots
+    CSM_TRY(StartKnownBox(grid_, box_slot_));
+  }
   if (L.nx != grid_->g.nx) {   // the old block at the doubling offset, unknown (0) around it
     CSM_TRY(GrowCellArrays2(grid_, L, grow_x_, grow_y_, ctx->stream, &arrays));
     grown_ = true;
@@ -405,7 +419,7 @@ csm_status GridInsert2::Commit(const KnownBox2& touched, csm_stats* stats) {
     if (st != CSM_OK) return st;
   }
   // the old known box moved by the growth, plus what this insert set
-  KnownBox2 known = box_stale_ ? BoxFrom(ctx->P("ins2_box").as<int>()) : grid_->known;
+  KnownBox2 known = box_stale_ ? BoxFrom(StagedBox(ctx, box_slot_)) : grid_->known;
   if (!known.empty()) {
     known.lo[0] += grow_x_;
     known.hi[0] += grow_x_;

@@ -1,27 +1,40 @@
 // ProbabilityGridRangeDataInserter2D::Insert on the device
-// (cartographer/mapping/2d/probability_grid_range_data_inserter_2d.cc:35-133) into a
-// csm_rt_grid2d handle, growing it as Grid2D::GrowLimits (2d/grid_2d.cc:125-164) does.
+// (cartographer/mapping/2d/probability_grid_range_data_inserter_2d.cc:35-133) into one or several
+// csm_rt_grid2d handles, each growing as Grid2D::GrowLimits (2d/grid_2d.cc:125-164) does.
 //
 // The reference applies the hit table to every return's cell, then the miss table to every
 // pixel of RayToPixelMask (internal/2d/ray_to_pixel_mask.cc) of each return's ray and each
 // miss's ray.  A cell updated once carries kUpdateMarker and is skipped until FinishUpdate
 // (grid_2d.cc:99-106), so each touched cell ends at hit_table[v] & 0x7fff if a return hits it,
-// else miss_table[v] & 0x7fff, whatever the order inside each phase.  Here:
-//   * the host decides growth (it holds the limits), computes every superscaled index, and
-//     checks them all, so an invalid call changes nothing; the kernels write grown copies of
-//     the cells, installed after the insert's one synchronisation (GridInsert2, grid2d.cu);
+// else miss_table[v] & 0x7fff, whatever the order inside each phase.  Several handles take the
+// same scan independently; only their limits differ.  Here:
+//   * the host makes one pass over the points: finiteness, their bounding box (from which every
+//     handle's growth is decided, so a refused call changes nothing) and the sum of the rays'
+//     L1 lengths; it computes each handle's superscaled origin cell;
+//   * k_ins2_index (one thread per (handle, point)) computes every superscaled end index with
+//     the host's Limits2::CellIndex, flags an end outside the grown limits, writes the hit cells
+//     and each ray's pixel count, and reduces each handle's touched box: a mask contains both
+//     its end pixels and stays inside their bounding box, so the box grows by the hit pixels
+//     and, with free space on and at least one ray, by the misses' pixels and the origin's
+//     (added on the host);
 //   * each ray's mask has at most |dx| + |dy| + 1 pixels (it moves one pixel in x, in y or,
-//     across an exact corner, in both per step), so the host gives every ray a slot range by
-//     prefix sum: k_ins2_hits (one thread per return), k_ins2_rays (one thread per ray
-//     replays the reference's integer walk into its slots), k_ins2_misses (one thread per
-//     slot) and k_ins2_finish (clears the markers of the hit cells and mask pixels again);
+//     across an exact corner, in both per step).  One exclusive sum over the (handle, ray)
+//     counts gives the slot offsets; each handle's slots live in a range the host reserved
+//     from the L1 lengths (SlotReservation), and a handle whose exact total
+//     passes its range raises a flag instead of writing;
+//   * k_ins2_rays (one thread per (handle, ray) replays the reference's integer walk into its
+//     slots), k_ins2_hits, k_ins2_misses (one thread per slot) and k_ins2_finish (clears the
+//     markers of the hit cells and mask pixels again) take every handle in one launch
+//     (blockIdx.y) and write nothing once a flag is raised;
 //   * a 16-bit atomicCAS applies a table only while the marker is clear;
-//   * the known-cells box follows on the host: a mask contains both its end pixels and stays
-//     inside their bounding box, so the box grows by the hit pixels and, with free space on
-//     and at least one ray, by the origin's and the misses' pixels.
+//   * the kernels write grown copies of the cells (GridInsert2, grid2d.cu), installed after the
+//     insert's one synchronisation, when the flags and boxes are read back; a flag refuses the
+//     call and every handle keeps its cells, limits and box.
 #include <algorithm>
 #include <climits>
 #include <cmath>
+
+#include <cub/device/device_scan.cuh>
 
 #include "insert2d.cuh"
 
@@ -34,46 +47,153 @@ struct csm_range_inserter2d {
 
 namespace csm {
 
-__global__ void k_ins2_hits(const int* __restrict__ hit_flat, int n, uint16_t* cells,
-                            const uint16_t* __restrict__ hit_table) {
+enum : int { kIns2Outside = 1, kIns2TooManyPixels = 2 };   // flag bits in status[0]
+
+// One handle of an insert as the kernels see it.
+struct Ins2Target {
+  uint16_t* cells;        // what the insert writes: the handle's cells or their grown copy
+  Limits2 S;              // the grown limits, superscaled by kSubpixelScale
+  int pitch;
+  int2 begin;             // the origin's superscaled cell
+  long long slot_begin;   // the handle's slot range [slot_begin, slot_begin + slot_cap)
+  long long slot_cap;
+};
+
+// Status block: status[0] the flags, status[4 + 4h ..] handle h's touched box (min x, min y,
+// max x, max y).
+constexpr int kIns2BoxBase = 4;
+
+// One thread per (handle blockIdx.y, point i): points are the returns, then (with free space)
+// the misses; with free space point i is also ray i.
+__global__ void k_ins2_index(const Ins2Target* __restrict__ targets,
+                             const float2* __restrict__ pts, int num_points, int n, int num_rays,
+                             int* __restrict__ status, int* __restrict__ hit_flat,
+                             int2* __restrict__ ends, long long* __restrict__ counts) {
+  const int h = blockIdx.y;
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < n) ApplyTable(cells + hit_flat[i], hit_table);
+  const Ins2Target& t = targets[h];
+  const long long ray = static_cast<long long>(h) * num_rays + i;
+  bool in = false;
+  int x = 0, y = 0;
+  if (i < num_points) {
+    const float2 p = pts[i];
+    long long ix, iy;
+    t.S.CellIndex(p.x, p.y, &ix, &iy);
+    if (t.S.Contains(ix, iy)) {
+      in = true;
+      x = static_cast<int>(ix) / kSubpixelScale;
+      y = static_cast<int>(iy) / kSubpixelScale;
+      if (i < n) hit_flat[static_cast<long long>(h) * n + i] = y * t.pitch + x;
+      if (num_rays > 0) {
+        ends[ray] = make_int2(static_cast<int>(ix), static_cast<int>(iy));
+        counts[ray] = abs(x - t.begin.x / kSubpixelScale) + abs(y - t.begin.y / kSubpixelScale) + 1;
+      }
+    } else {
+      atomicOr(status, kIns2Outside);
+      if (num_rays > 0) counts[ray] = 0;
+    }
+  }
+  if (h == 0 && i == 0 && num_rays > 0)   // the sum's last entry: the total of every handle
+    counts[static_cast<long long>(gridDim.y) * num_rays] = 0;
+  const int lo_x = __reduce_min_sync(0xffffffffu, in ? x : INT_MAX);
+  const int lo_y = __reduce_min_sync(0xffffffffu, in ? y : INT_MAX);
+  const int hi_x = __reduce_max_sync(0xffffffffu, in ? x : INT_MIN);
+  const int hi_y = __reduce_max_sync(0xffffffffu, in ? y : INT_MIN);
+  if ((threadIdx.x & 31) == 0 && lo_x <= hi_x) {
+    int* box = status + kIns2BoxBase + 4 * h;
+    atomicMin(box + 0, lo_x);
+    atomicMin(box + 1, lo_y);
+    atomicMax(box + 2, hi_x);
+    atomicMax(box + 3, hi_y);
+  }
 }
 
-// RayToPixelMask(begin, end, kSubpixelScale) of ray r into slots [off[r], off[r + 1]) as flat
-// cell indices; the slots it does not fill stay -1.
-__global__ void k_ins2_rays(int2 begin, const int2* __restrict__ ends, const int* __restrict__ off,
-                            int num_rays, int pitch, int* __restrict__ slots) {
+// RayToPixelMask(begin, end, kSubpixelScale) of ray r of handle blockIdx.y into its slots as
+// flat cell indices; the slots it does not fill stay -1.  Writes nothing after an end outside
+// the limits, or for a handle whose exact total passes its slot range (which raises the flag).
+__global__ void k_ins2_rays(const Ins2Target* __restrict__ targets, const int2* __restrict__ ends,
+                            const long long* __restrict__ off, int num_rays, int* status,
+                            int* __restrict__ slots) {
+  const int h = blockIdx.y;
   const int r = blockIdx.x * blockDim.x + threadIdx.x;
-  if (r >= num_rays) return;
-  int* out = slots + off[r];
-  const int cap = off[r + 1] - off[r];
+  if (r >= num_rays || (*status & kIns2Outside)) return;
+  const Ins2Target& t = targets[h];
+  const long long* o = off + static_cast<long long>(h) * num_rays;
+  if (o[num_rays] - o[0] > t.slot_cap) {
+    if (r == 0) atomicOr(status, kIns2TooManyPixels);
+    return;
+  }
+  int* out = slots + t.slot_begin + (o[r] - o[0]);
+  const int cap = static_cast<int>(o[r + 1] - o[r]);
+  const int pitch = t.pitch;
   int count = 0;
-  RayToPixelMask2(begin, ends[r], [&](int x, int y) {
+  RayToPixelMask2(t.begin, ends[static_cast<long long>(h) * num_rays + r], [&](int x, int y) {
     if (count < cap) out[count] = y * pitch + x;
     ++count;
   });
   for (int k = count; k < cap; ++k) out[k] = -1;
 }
 
-__global__ void k_ins2_misses(const int* __restrict__ slots, int num_slots, uint16_t* cells,
+// The number of slots handle h's rays fill: its exact total.
+__device__ __forceinline__ long long HandleSlots(const long long* off, int h, int num_rays) {
+  return num_rays > 0 ? off[static_cast<long long>(h + 1) * num_rays] -
+                            off[static_cast<long long>(h) * num_rays]
+                      : 0;
+}
+
+__global__ void k_ins2_hits(const Ins2Target* __restrict__ targets, const int* __restrict__ hit_flat,
+                            int n, const int* status, const uint16_t* __restrict__ hit_table) {
+  if (*status) return;
+  const int h = blockIdx.y;
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n) ApplyTable(targets[h].cells + hit_flat[static_cast<long long>(h) * n + i], hit_table);
+}
+
+__global__ void k_ins2_misses(const Ins2Target* __restrict__ targets,
+                              const long long* __restrict__ off, int num_rays,
+                              const int* __restrict__ slots, const int* status,
                               const uint16_t* __restrict__ miss_table) {
-  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < num_slots; i += gridDim.x * blockDim.x) {
-    const int flat = slots[i];
+  if (*status) return;
+  const int h = blockIdx.y;
+  const long long num_slots = HandleSlots(off, h, num_rays);
+  const int* s = slots + targets[h].slot_begin;
+  uint16_t* cells = targets[h].cells;
+  for (long long i = blockIdx.x * blockDim.x + threadIdx.x; i < num_slots;
+       i += gridDim.x * blockDim.x) {
+    const int flat = s[i];
     if (flat >= 0) ApplyTable(cells + flat, miss_table);
   }
 }
 
 // FinishUpdate: clears the marker of every hit cell and mask pixel (the same cell may be
 // listed many times; neighbouring 16-bit cells share a word).
-__global__ void k_ins2_finish(const int* __restrict__ hit_flat, int n,
-                              const int* __restrict__ slots, int num_slots, uint16_t* cells) {
-  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n + num_slots;
+__global__ void k_ins2_finish(const Ins2Target* __restrict__ targets,
+                              const int* __restrict__ hit_flat, int n,
+                              const long long* __restrict__ off, int num_rays,
+                              const int* __restrict__ slots, const int* status) {
+  if (*status) return;
+  const int h = blockIdx.y;
+  const long long total = n + HandleSlots(off, h, num_rays);
+  const int* hits = hit_flat + static_cast<long long>(h) * n;
+  const int* s = slots + targets[h].slot_begin;
+  uint16_t* cells = targets[h].cells;
+  for (long long i = blockIdx.x * blockDim.x + threadIdx.x; i < total;
        i += gridDim.x * blockDim.x) {
-    const int flat = i < n ? hit_flat[i] : slots[i - n];
+    const int flat = i < n ? hits[i] : s[i - n];
     if (flat < 0) continue;
     ClearUpdateMarker(cells, flat);
   }
+}
+
+// The slots handle h reserves for rays whose L1 lengths sum to l1 (in metres), at
+// resolution res.  A point's pixel is floor((max - p) / res) per axis (the superscaled index
+// rounds within one subpixel of it and drops the subpixels), so a ray's |dx| + |dy| + 1 is
+// below its L1 length in cells + 3.  The relative and the + 1 margins absorb the double
+// rounding of the lengths and of the cell coordinates on exact cell borders.  Capped at
+// 2^31 - 1: an exact total past that is refused anyway ("too many ray pixels").
+long long SlotReservation(double l1, double res, int num_rays) {
+  const double bound = l1 / res * (1. + 1e-9) + 3. * num_rays + 1.;
+  return bound >= static_cast<double>(INT_MAX) ? INT_MAX : static_cast<long long>(bound);
 }
 
 }  // namespace csm
@@ -120,124 +240,185 @@ csm_status csm_range_inserter2d_destroy(csm_range_inserter2d* inserter) {
   return CSM_OK;
 }
 
+csm_status csm_range_inserter2d_insert_submaps(const csm_range_inserter2d* inserter,
+                                                const float origin[3], const float* returns,
+                                                int32_t num_returns, const float* misses,
+                                                int32_t num_misses, csm_rt_grid2d* const* grids,
+                                                int32_t num_grids, csm_stats* stats) {
+  CSM_REQUIRE(inserter && origin && grids, "null pointer");
+  CSM_REQUIRE(num_grids >= 1 && num_grids <= 65535, "num_grids");
+  CSM_REQUIRE(num_returns >= 0 && (num_returns == 0 || returns), "returns");
+  CSM_REQUIRE(num_misses >= 0 && (num_misses == 0 || misses), "misses");
+  const int H = num_grids;
+  for (int h = 0; h < H; ++h) {
+    CSM_REQUIRE(grids[h] != nullptr, "null grid");
+    for (int k = 0; k < h; ++k) CSM_REQUIRE(grids[k] != grids[h], "a grid appears twice");
+  }
+  Ctx* ctx = inserter->ctx;
+  for (int h = 0; h < H; ++h) {
+    CSM_REQUIRE(grids[h]->d_wcells == nullptr, "a TSDF2D handle takes the TSDF inserter");
+    CSM_REQUIRE(grids[h]->ctx == ctx, "grid on another device than the inserter");
+  }
+  const int n = num_returns, m = num_misses;
+  const bool free_space = inserter->options.insert_free_space != 0;
+  const int num_points = free_space ? n + m : n;   // what the kernels index
+  const int num_rays = free_space ? n + m : 0;
+  // ---- one pass over the points: finite, bounding box (GrowAsNeeded, :35-50), ray lengths ----
+  CSM_REQUIRE(Finite(origin, 3), "non-finite point");
+  float lo_x = origin[0], lo_y = origin[1], hi_x = origin[0], hi_y = origin[1];
+  double l1 = 0.;
+  bool finite = true;
+  auto scan = [&](const float* p, int k) {
+    for (int i = 0; i < k; ++i) {
+      const float* q = p + 3 * static_cast<size_t>(i);
+      finite = finite && std::isfinite(q[0]) && std::isfinite(q[1]) && std::isfinite(q[2]);
+      lo_x = std::min(lo_x, q[0]);
+      lo_y = std::min(lo_y, q[1]);
+      hi_x = std::max(hi_x, q[0]);
+      hi_y = std::max(hi_y, q[1]);
+      l1 += std::abs(static_cast<double>(q[0]) - origin[0]) +
+            std::abs(static_cast<double>(q[1]) - origin[1]);
+    }
+  };
+  scan(returns, n);
+  scan(misses, m);
+  CSM_REQUIRE(finite, "non-finite point");
+  if (!free_space) l1 = 0.;
+
+  std::lock_guard<std::mutex> lock(ctx->mu);
+  CSM_CUDA(cudaSetDevice(ctx->device));
+  // ---- every handle grows, and its origin is checked, before anything changes ----
+  std::vector<std::unique_ptr<GridInsert2>> tx(H);
+  std::vector<Ins2Target> targets(H);
+  long long num_slots = 0;
+  for (int h = 0; h < H; ++h) {
+    tx[h].reset(new GridInsert2(grids[h], h));
+    CSM_REQUIRE(tx[h]->Grow(lo_x, lo_y, hi_x, hi_y), "the grid would grow past 30000 cells");
+    const Limits2& L = tx[h]->L;
+    Ins2Target& t = targets[h];
+    // the superscaled limits (:58-65)
+    t.S = Limits2{L.resolution / kSubpixelScale, L.max_x, L.max_y, L.nx * kSubpixelScale,
+                  L.ny * kSubpixelScale};
+    long long ix, iy;
+    t.S.CellIndex(origin[0], origin[1], &ix, &iy);
+    CSM_REQUIRE(t.S.Contains(ix, iy), "origin outside the grown limits");
+    t.begin = make_int2(static_cast<int>(ix), static_cast<int>(iy));
+    t.pitch = tx[h]->arrays.pitch;
+    t.slot_begin = num_slots;
+    t.slot_cap = num_rays > 0 ? SlotReservation(l1, L.resolution, num_rays) : 0;
+    num_slots += t.slot_cap;
+  }
+
+  // ---- workspaces, before any transaction queues a copy into pinned memory ----
+  cudaStream_t s = ctx->stream;
+  auto align = [](size_t b) { return (b + 255) / 256 * 256; };
+  const size_t hn = static_cast<size_t>(H) * n, hr = static_cast<size_t>(H) * num_rays;
+  const size_t status_bytes = sizeof(int) * (kIns2BoxBase + 4 * static_cast<size_t>(H));
+  const size_t o_targets = align(status_bytes);
+  const size_t o_pts = o_targets + align(sizeof(Ins2Target) * H);
+  const size_t up_bytes = o_pts + align(sizeof(float2) * static_cast<size_t>(num_points));
+  const size_t o_hits = up_bytes;
+  const size_t o_ends = o_hits + align(sizeof(int) * hn);
+  const size_t o_counts = o_ends + align(sizeof(int2) * hr);
+  const size_t o_off = o_counts + align(sizeof(long long) * (hr + 1));
+  const size_t o_scan = o_off + align(sizeof(long long) * (hr + 1));
+  size_t scan_bytes = 0;
+  if (num_rays > 0)
+    CSM_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, scan_bytes, static_cast<long long*>(nullptr),
+                                           static_cast<long long*>(nullptr),
+                                           static_cast<long long>(hr + 1), s));
+  const size_t o_slots = o_scan + align(scan_bytes);
+  const size_t work_bytes = o_slots + sizeof(int) * static_cast<size_t>(num_slots);
+  PinnedBuf& up = ctx->P("ins2_upload");
+  PinnedBuf& down = ctx->P("ins2_status");
+  DevBuf& d_work = ctx->D("ins2_work");
+  CSM_TRY(up.Reserve(up_bytes));
+  CSM_TRY(down.Reserve(status_bytes));
+  CSM_TRY(d_work.Reserve(work_bytes));
+  CSM_TRY(ReserveKnownBoxSlots(ctx, H));
+
+  CSM_CUDA(cudaEventRecord(ctx->ev0, s));
+  for (int h = 0; h < H; ++h) {
+    CSM_TRY(tx[h]->Begin());
+    targets[h].cells = tx[h]->arrays.cells;
+  }
+  // ---- upload: status | targets | points ----
+  char* hp = up.as<char>();
+  int* h_status = reinterpret_cast<int*>(hp);
+  std::fill(h_status, h_status + kIns2BoxBase, 0);
+  for (int h = 0; h < H; ++h) {
+    int* box = h_status + kIns2BoxBase + 4 * h;
+    box[0] = box[1] = INT_MAX;
+    box[2] = box[3] = INT_MIN;
+  }
+  std::memcpy(hp + o_targets, targets.data(), sizeof(Ins2Target) * H);
+  float2* h_pts = reinterpret_cast<float2*>(hp + o_pts);
+  for (int i = 0; i < num_points; ++i) {
+    const float* q = i < n ? returns + 3 * static_cast<size_t>(i)
+                           : misses + 3 * static_cast<size_t>(i - n);
+    h_pts[i] = make_float2(q[0], q[1]);
+  }
+  CSM_CUDA(cudaMemcpyAsync(d_work.p, hp, up_bytes, cudaMemcpyHostToDevice, s));
+  char* d = d_work.as<char>();
+  int* d_status = reinterpret_cast<int*>(d);
+  const Ins2Target* d_targets = reinterpret_cast<const Ins2Target*>(d + o_targets);
+  int* d_hits = reinterpret_cast<int*>(d + o_hits);
+  int2* d_ends = reinterpret_cast<int2*>(d + o_ends);
+  long long* d_counts = reinterpret_cast<long long*>(d + o_counts);
+  long long* d_off = reinterpret_cast<long long*>(d + o_off);
+  int* d_slots = reinterpret_cast<int*>(d + o_slots);
+  if (num_points > 0) {
+    const dim3 per_point(DivUp(num_points, 256), H);
+    k_ins2_index<<<per_point, 256, 0, s>>>(d_targets, reinterpret_cast<const float2*>(d + o_pts),
+                                           num_points, n, num_rays, d_status, d_hits, d_ends,
+                                           d_counts);
+    CSM_LAUNCH_CHECK();
+    if (num_rays > 0) {
+      CSM_CUDA(cub::DeviceScan::ExclusiveSum(d + o_scan, scan_bytes, d_counts, d_off,
+                                             static_cast<long long>(hr + 1), s));
+      k_ins2_rays<<<per_point, 256, 0, s>>>(d_targets, d_ends, d_off, num_rays, d_status,
+                                            d_slots);
+      CSM_LAUNCH_CHECK();
+    }
+    if (n > 0) {
+      k_ins2_hits<<<dim3(DivUp(n, 256), H), 256, 0, s>>>(d_targets, d_hits, n, d_status,
+                                                         inserter->d_tables);
+      CSM_LAUNCH_CHECK();
+    }
+    long long max_cap = 0;
+    for (const Ins2Target& t : targets) max_cap = std::max(max_cap, t.slot_cap);
+    if (num_rays > 0) {
+      k_ins2_misses<<<dim3(Blocks(max_cap), H), 256, 0, s>>>(
+          d_targets, d_off, num_rays, d_slots, d_status, inserter->d_tables + kValueCount);
+      CSM_LAUNCH_CHECK();
+    }
+    k_ins2_finish<<<dim3(Blocks(n + max_cap), H), 256, 0, s>>>(d_targets, d_hits, n, d_off,
+                                                               num_rays, d_slots, d_status);
+    CSM_LAUNCH_CHECK();
+  }
+  CSM_CUDA(cudaMemcpyAsync(down.p, d_status, status_bytes, cudaMemcpyDeviceToHost, s));
+  CSM_CUDA(cudaEventRecord(ctx->ev1, s));
+  CSM_CUDA(cudaStreamSynchronize(s));
+  const int flags = down.as<int>()[0];
+  CSM_REQUIRE(!(flags & kIns2Outside), "a point outside the grown limits");
+  CSM_REQUIRE(!(flags & kIns2TooManyPixels), "too many ray pixels");
+  for (int h = 0; h < H; ++h) {
+    KnownBox2 touched = BoxFrom(down.as<int>() + kIns2BoxBase + 4 * h);
+    if (num_rays > 0)
+      touched.Extend(targets[h].begin.x / kSubpixelScale, targets[h].begin.y / kSubpixelScale);
+    CSM_TRY(tx[h]->Commit(touched, stats));
+  }
+  return CSM_OK;
+}
+
 csm_status csm_range_inserter2d_insert(const csm_range_inserter2d* inserter,
                                        const float origin[3], const float* returns,
                                        int32_t num_returns, const float* misses,
                                        int32_t num_misses, csm_rt_grid2d* grid,
                                        csm_stats* stats) {
-  CSM_REQUIRE(inserter && origin && grid, "null pointer");
-  CSM_REQUIRE(num_returns >= 0 && (num_returns == 0 || returns), "returns");
-  CSM_REQUIRE(num_misses >= 0 && (num_misses == 0 || misses), "misses");
-  CSM_REQUIRE(grid->d_wcells == nullptr, "a TSDF2D handle takes the TSDF inserter");
-  Ctx* ctx = inserter->ctx;
-  CSM_REQUIRE(grid->ctx == ctx, "grid on another device than the inserter");
-  const int n = num_returns, m = num_misses;
-  CSM_REQUIRE(Finite(origin, 3) && Finite(returns, 3 * static_cast<size_t>(n)) &&
-                  Finite(misses, 3 * static_cast<size_t>(m)),
-              "non-finite point");
-  const bool free_space = inserter->options.insert_free_space != 0;
-  std::lock_guard<std::mutex> lock(ctx->mu);
-  // ---- GrowAsNeeded (:35-50) on the limits, before anything changes ----
-  float lo_x = origin[0], lo_y = origin[1], hi_x = origin[0], hi_y = origin[1];
-  auto extend = [&](const float* p, int k) {
-    for (int i = 0; i < k; ++i) {
-      const float x = p[3 * static_cast<size_t>(i)], y = p[3 * static_cast<size_t>(i) + 1];
-      lo_x = std::min(lo_x, x);
-      lo_y = std::min(lo_y, y);
-      hi_x = std::max(hi_x, x);
-      hi_y = std::max(hi_y, y);
-    }
-  };
-  extend(returns, n);
-  extend(misses, m);
-  GridInsert2 tx(grid);
-  CSM_REQUIRE(tx.Grow(lo_x, lo_y, hi_x, hi_y), "the grid would grow past 30000 cells");
-  const Limits2& L = tx.L;
-  // ---- superscaled indices (:58-65) ----
-  Limits2 S{L.resolution / kSubpixelScale, L.max_x, L.max_y, L.nx * kSubpixelScale,
-            L.ny * kSubpixelScale};
-  auto superscaled = [&](const float* p, int2* out) -> bool {
-    long long ix, iy;
-    S.CellIndex(p[0], p[1], &ix, &iy);
-    if (!S.Contains(ix, iy)) return false;
-    *out = make_int2(static_cast<int>(ix), static_cast<int>(iy));
-    return true;
-  };
-  int2 begin;
-  CSM_REQUIRE(superscaled(origin, &begin), "origin outside the grown limits");
-  const int num_rays = free_space ? n + m : 0;
-  std::vector<int2> ends(std::max(n, num_rays));
-  std::vector<int> hit_flat(n), off(num_rays + 1, 0);
-  const int pitch = tx.arrays.pitch;
-  KnownBox2 touched;
-  for (int i = 0; i < n; ++i) {
-    CSM_REQUIRE(superscaled(returns + 3 * static_cast<size_t>(i), &ends[i]),
-                "return outside the grown limits");
-    const int x = ends[i].x / kSubpixelScale, y = ends[i].y / kSubpixelScale;
-    hit_flat[i] = y * pitch + x;
-    touched.Extend(x, y);
-  }
-  if (free_space) {
-    for (int i = 0; i < m; ++i) {
-      int2& e = ends[n + i];
-      CSM_REQUIRE(superscaled(misses + 3 * static_cast<size_t>(i), &e),
-                  "miss outside the grown limits");
-      touched.Extend(e.x / kSubpixelScale, e.y / kSubpixelScale);
-    }
-    if (num_rays > 0) touched.Extend(begin.x / kSubpixelScale, begin.y / kSubpixelScale);
-    const int bx = begin.x / kSubpixelScale, by = begin.y / kSubpixelScale;
-    long long total = 0;
-    for (int r = 0; r < num_rays; ++r) {
-      off[r] = static_cast<int>(total);
-      total += std::abs(ends[r].x / kSubpixelScale - bx) + std::abs(ends[r].y / kSubpixelScale - by) + 1;
-      CSM_REQUIRE(total < (1LL << 31), "too many ray pixels");
-    }
-    off[num_rays] = static_cast<int>(total);
-  }
-  const int num_slots = off[num_rays];
-
-  CSM_TRY(tx.Begin());
-  cudaStream_t s = ctx->stream;
-  uint16_t* cells = tx.arrays.cells;
-  // ---- upload: hit cells | ray ends | slot offsets ----
-  if (n > 0 || num_rays > 0) {
-    const size_t o_ends = (sizeof(int) * static_cast<size_t>(n) + 255) / 256 * 256;
-    const size_t o_off = o_ends + (sizeof(int2) * static_cast<size_t>(num_rays) + 255) / 256 * 256;
-    const size_t o_slots = o_off + (sizeof(int) * static_cast<size_t>(num_rays + 1) + 255) / 256 * 256;
-    const size_t up_bytes = o_slots;
-    PinnedBuf& up = ctx->P("ins2_upload");
-    DevBuf& d_up = ctx->D("ins2_upload");
-    CSM_TRY(up.Reserve(up_bytes));
-    CSM_TRY(d_up.Reserve(up_bytes + sizeof(int) * static_cast<size_t>(num_slots)));
-    char* h = up.as<char>();
-    std::memcpy(h, hit_flat.data(), sizeof(int) * static_cast<size_t>(n));
-    std::memcpy(h + o_ends, ends.data(), sizeof(int2) * static_cast<size_t>(num_rays));
-    std::memcpy(h + o_off, off.data(), sizeof(int) * static_cast<size_t>(num_rays + 1));
-    CSM_CUDA(cudaMemcpyAsync(d_up.p, h, up_bytes, cudaMemcpyHostToDevice, s));
-    char* d = d_up.as<char>();
-    const int* d_hits = reinterpret_cast<const int*>(d);
-    int* d_slots = reinterpret_cast<int*>(d + o_slots);
-    const uint16_t* hit_table = inserter->d_tables;
-    const uint16_t* miss_table = inserter->d_tables + kValueCount;
-    if (n > 0) {
-      k_ins2_hits<<<Blocks(n, 1LL << 30), 256, 0, s>>>(d_hits, n, cells, hit_table);
-      CSM_LAUNCH_CHECK();
-    }
-    if (num_rays > 0) {
-      k_ins2_rays<<<Blocks(num_rays, 1LL << 30), 256, 0, s>>>(
-          begin, reinterpret_cast<const int2*>(d + o_ends), reinterpret_cast<const int*>(d + o_off),
-          num_rays, pitch, d_slots);
-      CSM_LAUNCH_CHECK();
-      k_ins2_misses<<<Blocks(num_slots), 256, 0, s>>>(d_slots, num_slots, cells, miss_table);
-      CSM_LAUNCH_CHECK();
-    }
-    k_ins2_finish<<<Blocks(static_cast<long long>(n) + num_slots), 256, 0, s>>>(
-        d_hits, n, d_slots, num_slots, cells);
-    CSM_LAUNCH_CHECK();
-  }
-  CSM_CUDA(cudaEventRecord(ctx->ev1, s));
-  CSM_CUDA(cudaStreamSynchronize(s));
-  return tx.Commit(touched, stats);
+  CSM_REQUIRE(grid, "null pointer");
+  return csm_range_inserter2d_insert_submaps(inserter, origin, returns, num_returns, misses,
+                                             num_misses, &grid, 1, stats);
 }
 
 }  // extern "C"

@@ -417,8 +417,10 @@ csm_status csm_tsdf_inserter2d_insert(const csm_tsdf_inserter2d* inserter, const
   P.max_w = grid->max_weight;
   P.weight_resolution = ValueResolution(0.f, grid->max_weight);
 
-  CSM_TRY(tx.Begin());
   cudaStream_t s = ctx->stream;
+  CSM_CUDA(cudaSetDevice(ctx->device));
+  CSM_CUDA(cudaEventRecord(ctx->ev0, s));
+  CSM_TRY(tx.Begin());
   const CellArrays2& work = tx.arrays;
 
   // ---- upload: flags + box | ray records | slot offsets; workspace for slots and pairs ----

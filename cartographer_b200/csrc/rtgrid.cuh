@@ -101,12 +101,13 @@ csm_status UploadCells(csm_rt_grid2d* g, const uint16_t* cells, const uint16_t* 
 struct Limits2 {   // MapLimits (2d/map_limits.h)
   double resolution, max_x, max_y;
   int nx, ny;
-  // GetCellIndex (map_limits.h:69-76): the float point enters double arithmetic
-  void CellIndex(float px, float py, long long* ix, long long* iy) const {
-    *ix = std::llround((max_y - static_cast<double>(py)) / resolution - 0.5);
-    *iy = std::llround((max_x - static_cast<double>(px)) / resolution - 0.5);
+  // GetCellIndex (map_limits.h:69-76): the float point enters double arithmetic.  One
+  // definition for host and device: both llround round half away from zero.
+  __host__ __device__ void CellIndex(float px, float py, long long* ix, long long* iy) const {
+    *ix = llround((max_y - static_cast<double>(py)) / resolution - 0.5);
+    *iy = llround((max_x - static_cast<double>(px)) / resolution - 0.5);
   }
-  bool Contains(long long ix, long long iy) const {
+  __host__ __device__ bool Contains(long long ix, long long iy) const {
     return ix >= 0 && iy >= 0 && ix < nx && iy < ny;
   }
 };
@@ -118,19 +119,27 @@ struct CellArrays2 {
   int pitch = 0;
 };
 
+// Reserves the context's staging of `n` known-cells boxes, so that the transactions of one
+// insert (box_slot 0 .. n - 1) can start their box reductions without moving the buffers under
+// one another's pending copies.  Caller holds ctx->mu.
+csm_status ReserveKnownBoxSlots(Ctx* ctx, int n);
+
 // The part of one 2D insert that changes the handle (caller holds ctx->mu):
 //   1. Grow: Grid2D::GrowAsNeeded on the limits, from the bounding box of the insert's points;
-//   2. Begin: records ctx->ev0, starts the known-box reduction of a handle made from cells
-//      (before its cells move) and allocates the grown arrays, on the handle's stream;
-//   3. the caller's kernels write `arrays` at limits L; the caller records ctx->ev1 and
-//      synchronises the stream;
+//   2. Begin: starts the known-box reduction of a handle made from cells (before its cells
+//      move) into staging slot `box_slot`, and allocates the grown arrays, on the handle's
+//      stream;
+//   3. the caller's kernels write `arrays` at limits L; the caller records ctx->ev1 (ctx->ev0
+//      before its first device work) and synchronises the stream;
 //   4. Commit: installs grown arrays, moves the old known box by the growth and extends it by
-//      what the insert touched, and fills stats.
+//      what the insert touched, and fills stats (may be NULL).
 // Grown arrays not committed are freed when the transaction ends: the handle keeps its size
-// and its cells.
+// and its cells.  Several transactions make one when the caller grows all of them before it
+// begins any, gives each its own box slot (ReserveKnownBoxSlots first), and commits all of
+// them or none.
 class GridInsert2 {
  public:
-  explicit GridInsert2(csm_rt_grid2d* grid);
+  explicit GridInsert2(csm_rt_grid2d* grid, int box_slot = 0);
   ~GridInsert2();
   GridInsert2(const GridInsert2&) = delete;
   GridInsert2& operator=(const GridInsert2&) = delete;
@@ -144,6 +153,7 @@ class GridInsert2 {
 
  private:
   csm_rt_grid2d* grid_;
+  int box_slot_;
   int grow_x_ = 0, grow_y_ = 0;   // cell offset of the old cells in the grown arrays
   bool grown_ = false;            // `arrays` were allocated by Begin
   bool box_stale_ = false;

@@ -630,12 +630,133 @@ class ProbabilityGridRangeDataInserter2D:
         self.last_stats = stats.as_dict()
         grid._info()
 
+    def insert_submaps(self, grids, origin, returns, misses=None):
+        """Insert(range_data, grid) into every ProbabilityGrid RealTimeGrid2D of `grids`, in
+        one call (csm_range_inserter2d_insert_submaps), as ActiveSubmaps2D::InsertRangeData
+        inserts each scan into its active submaps: each grid ends as len(grids) Insert calls
+        in order would leave it, and a refused call leaves every grid unchanged."""
+        org = np.zeros(3, np.float32)
+        o = np.asarray(origin, np.float32).reshape(-1)
+        org[:len(o)] = o[:3]
+        ret = _f32(np.zeros((0, 3)) if returns is None else returns)
+        mis = _f32(np.zeros((0, 3)) if misses is None else misses)
+        handles = (C.c_void_p * len(grids))(*[g._h for g in grids])
+        stats = CsmStats()
+        check(lib().csm_range_inserter2d_insert_submaps(
+            self._h, ptr(org, C.c_float), ptr(ret, C.c_float), C.c_int32(len(ret)),
+            ptr(mis, C.c_float), C.c_int32(len(mis)), handles, C.c_int32(len(grids)),
+            C.byref(stats)))
+        self.last_stats = stats.as_dict()
+        for g in grids:
+            g._info()
+
     def close(self):
         if getattr(self, "_h", None):
             lib().csm_range_inserter2d_destroy(self._h)
             self._h = None
 
     __del__ = close
+
+
+# ===========================================================================
+# Submap2D and ActiveSubmaps2D (mapping/2d/submap_2d.h) over device grids
+# ===========================================================================
+@dataclass
+class SubmapsOptions2D:
+    """proto SubmapsOptions2D (mapping/proto/submaps_options_2d.proto) with its GridOptions2D
+    and RangeDataInserterOptions; defaults are configuration_files/trajectory_builder_2d.lua's
+    submaps.  `resolution` is the float grid option."""
+    num_range_data: int = 90
+    grid_type: str = "PROBABILITY_GRID"
+    resolution: float = 0.05
+    range_data_inserter_type: str = "PROBABILITY_GRID_INSERTER_2D"
+    probability_grid_range_data_inserter_options: ProbabilityGridRangeDataInserterOptions2D = \
+        field(default_factory=ProbabilityGridRangeDataInserterOptions2D)
+
+
+def create_grid_limits(origin, resolution):
+    """The MapLimits of ActiveSubmaps2D::CreateGrid (submap_2d.cc:192-204):
+    (resolution, max_x, max_y, 100, 100).  The float resolution option and the float origin
+    enter double arithmetic: max = origin.cast<double>() + 0.5 * 100 * resolution."""
+    r = float(np.float32(resolution))
+    o = np.asarray(origin, np.float32).reshape(-1)
+    return (r, float(o[0]) + 0.5 * 100 * r, float(o[1]) + 0.5 * 100 * r, 100, 100)
+
+
+class DeviceSubmap2D:
+    """A ProbabilityGrid Submap2D whose grid lives on the device: .grid (a RealTimeGrid2D, the
+    cropped grid once finished), .local_pose (x, y, 0, 1, 0, 0, 0) from the float origin,
+    .num_range_data and .insertion_finished: what pose_graph.OverlappingSubmapsTrimmer2D reads.
+    """
+
+    def __init__(self, origin, resolution, device=0):
+        o = np.asarray(origin, np.float32).reshape(-1)
+        self.local_pose = (float(o[0]), float(o[1]), 0.0, 1.0, 0.0, 0.0, 0.0)
+        res, max_x, max_y, nx, ny = create_grid_limits(o[:2], resolution)
+        self.grid = RealTimeGrid2D.empty(res, max_x, max_y, nx, ny, device)
+        self.num_range_data = 0
+        self.insertion_finished = False
+
+    def Finish(self):
+        """Submap2D::Finish (submap_2d.cc:146-151): the grid becomes its crop; the uncropped
+        handle is closed."""
+        assert not self.insertion_finished
+        cropped = self.grid.ComputeCroppedGrid()
+        self.grid.close()
+        self.grid = cropped
+        self.insertion_finished = True
+
+    def constraint_builder_submap(self):
+        """The constraint_builder.Submap2D view ConstraintBuilder2D reads of a finished submap:
+        the cropped grid and ComputeSubmapPose's (x, y, 0)."""
+        from .constraint_builder import Submap2D
+        if not self.insertion_finished:
+            raise ValueError("DeviceSubmap2D: only a finished submap closes loops")
+        return Submap2D(self.grid, (self.local_pose[0], self.local_pose[1], 0.0))
+
+
+class ActiveSubmaps2D:
+    """ActiveSubmaps2D (submap_2d.cc:153-236) over device grids: InsertRangeData writes each
+    scan into the (at most two) active submaps with one csm_range_inserter2d_insert_submaps
+    call.  ProbabilityGrid submaps only.  Evicted submaps are dropped from the list but stay
+    alive while the caller holds them."""
+
+    def __init__(self, options, device=0):
+        if options.num_range_data <= 0:
+            raise ValueError("num_range_data must be positive")
+        if (options.grid_type != "PROBABILITY_GRID" or
+                options.range_data_inserter_type != "PROBABILITY_GRID_INSERTER_2D"):
+            raise ValueError("ActiveSubmaps2D on the device takes ProbabilityGrid submaps only")
+        self.options = options
+        self.device = device
+        self.range_data_inserter = ProbabilityGridRangeDataInserter2D(
+            options.probability_grid_range_data_inserter_options, device)
+        self._submaps = []
+
+    def submaps(self):
+        return list(self._submaps)
+
+    def InsertRangeData(self, origin, returns, misses=None):
+        """origin (2 or 3), returns and misses (n x 3) in the local frame.  Returns the active
+        submaps."""
+        n = self.options.num_range_data
+        if not self._submaps or self._submaps[-1].num_range_data == n:
+            self._add_submap(np.asarray(origin, np.float32).reshape(-1)[:2])
+        for s in self._submaps:
+            assert not s.insertion_finished
+        self.range_data_inserter.insert_submaps([s.grid for s in self._submaps], origin,
+                                                returns, misses)
+        for s in self._submaps:
+            s.num_range_data += 1
+        if self._submaps[0].num_range_data == 2 * n:
+            self._submaps[0].Finish()
+        return self.submaps()
+
+    def _add_submap(self, origin):
+        if len(self._submaps) >= 2:
+            assert self._submaps[0].insertion_finished
+            del self._submaps[0]
+        self._submaps.append(DeviceSubmap2D(origin, self.options.resolution, self.device))
 
 
 # ===========================================================================

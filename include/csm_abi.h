@@ -1001,6 +1001,20 @@ csm_status csm_range_inserter2d_insert(const csm_range_inserter2d* inserter,
                                        int32_t num_returns, const float* misses,
                                        int32_t num_misses, csm_rt_grid2d* grid,
                                        csm_stats* stats /* may be NULL */);
+/* ActiveSubmaps2D::InsertRangeData's inserts (mapping/2d/submap_2d.cc:162-175): the range data
+ * into every handle of `grids`, in one call.  Every handle ends bit-equal to what num_grids
+ * csm_range_inserter2d_insert calls in order would leave it: cells, limits and known-cells box.
+ * CSM_E_INVALID, with every handle unchanged, for a null pointer (the list or an entry),
+ * num_grids outside [1, 65535], a handle that appears twice, or what csm_range_inserter2d_insert
+ * refuses for any handle: a TSDF2D handle, a handle on another device than the inserter, a
+ * non-finite input, or an insert that would grow a grid to 30000 cells or more per axis.  One
+ * stream synchronisation however many handles; stats (may be NULL) gets host_syncs and
+ * device_ms, which spans the whole call. */
+csm_status csm_range_inserter2d_insert_submaps(const csm_range_inserter2d* inserter,
+                                               const float origin[3], const float* returns,
+                                               int32_t num_returns, const float* misses,
+                                               int32_t num_misses, csm_rt_grid2d* const* grids,
+                                               int32_t num_grids, csm_stats* stats /* may be NULL */);
 /* ActiveSubmaps2D::CreateGrid (mapping/2d/submap_2d.cc): an all-unknown ProbabilityGrid of the
  * given limits with an empty known-cells box. */
 csm_status csm_rt_grid2d_create_empty(double resolution, double max_x, double max_y,
