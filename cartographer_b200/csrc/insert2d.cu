@@ -37,6 +37,7 @@
 #include <cub/device/device_scan.cuh>
 
 #include "insert2d.cuh"
+#include "resident2d.cuh"
 
 struct csm_range_inserter2d {
   csm::Ctx* ctx = nullptr;
@@ -200,6 +201,169 @@ long long SlotReservation(double l1, double res, int num_rays) {
 
 using namespace csm;
 
+namespace {
+
+// The handles of one insert: 1 .. 65535 distinct ProbabilityGrid handles on the inserter's device.
+csm_status CheckGrids(const csm_range_inserter2d* inserter, csm_rt_grid2d* const* grids,
+                      int32_t num_grids) {
+  CSM_REQUIRE(num_grids >= 1 && num_grids <= 65535, "num_grids");
+  const int H = num_grids;
+  for (int h = 0; h < H; ++h) {
+    CSM_REQUIRE(grids[h] != nullptr, "null grid");
+    for (int k = 0; k < h; ++k) CSM_REQUIRE(grids[k] != grids[h], "a grid appears twice");
+  }
+  for (int h = 0; h < H; ++h) {
+    CSM_REQUIRE(grids[h]->d_wcells == nullptr, "a TSDF2D handle takes the TSDF inserter");
+    CSM_REQUIRE(grids[h]->ctx == inserter->ctx, "grid on another device than the inserter");
+  }
+  return CSM_OK;
+}
+
+// Every handle's insert from the points' box and ray lengths: the host's points (returns,
+// misses) are uploaded, or points.d_pts already holds them on the device.
+csm_status InsertSubmaps(const csm_range_inserter2d* inserter, const float origin[3],
+                         const InsertPoints2& points, const float* returns, const float* misses,
+                         int n, int m, csm_rt_grid2d* const* grids, int32_t num_grids,
+                         csm_stats* stats) {
+  const int H = num_grids;
+  Ctx* ctx = inserter->ctx;
+  const bool free_space = inserter->options.insert_free_space != 0;
+  const int num_points = free_space ? n + m : n;   // what the kernels index
+  const int num_rays = free_space ? n + m : 0;
+  const float lo_x = points.lo_x, lo_y = points.lo_y, hi_x = points.hi_x, hi_y = points.hi_y;
+  const double l1 = free_space ? points.l1 : 0.;
+  std::lock_guard<std::mutex> lock(ctx->mu);
+  CSM_CUDA(cudaSetDevice(ctx->device));
+  // ---- every handle grows, and its origin is checked, before anything changes ----
+  std::vector<std::unique_ptr<GridInsert2>> tx(H);
+  std::vector<Ins2Target> targets(H);
+  long long num_slots = 0;
+  for (int h = 0; h < H; ++h) {
+    tx[h].reset(new GridInsert2(grids[h], h));
+    CSM_REQUIRE(tx[h]->Grow(lo_x, lo_y, hi_x, hi_y), "the grid would grow past 30000 cells");
+    const Limits2& L = tx[h]->L;
+    Ins2Target& t = targets[h];
+    // the superscaled limits (:58-65)
+    t.S = Limits2{L.resolution / kSubpixelScale, L.max_x, L.max_y, L.nx * kSubpixelScale,
+                  L.ny * kSubpixelScale};
+    long long ix, iy;
+    t.S.CellIndex(origin[0], origin[1], &ix, &iy);
+    CSM_REQUIRE(t.S.Contains(ix, iy), "origin outside the grown limits");
+    t.begin = make_int2(static_cast<int>(ix), static_cast<int>(iy));
+    t.pitch = tx[h]->arrays.pitch;
+    t.slot_begin = num_slots;
+    t.slot_cap = num_rays > 0 ? SlotReservation(l1, L.resolution, num_rays) : 0;
+    num_slots += t.slot_cap;
+  }
+
+  // ---- workspaces, before any transaction queues a copy into pinned memory ----
+  cudaStream_t s = ctx->stream;
+  auto align = [](size_t b) { return (b + 255) / 256 * 256; };
+  const size_t hn = static_cast<size_t>(H) * n, hr = static_cast<size_t>(H) * num_rays;
+  const size_t status_bytes = sizeof(int) * (kIns2BoxBase + 4 * static_cast<size_t>(H));
+  const size_t o_targets = align(status_bytes);
+  const size_t o_pts = o_targets + align(sizeof(Ins2Target) * H);
+  const size_t up_bytes =
+      o_pts + (points.d_pts ? 0 : align(sizeof(float2) * static_cast<size_t>(num_points)));
+  const size_t o_hits = up_bytes;
+  const size_t o_ends = o_hits + align(sizeof(int) * hn);
+  const size_t o_counts = o_ends + align(sizeof(int2) * hr);
+  const size_t o_off = o_counts + align(sizeof(long long) * (hr + 1));
+  const size_t o_scan = o_off + align(sizeof(long long) * (hr + 1));
+  size_t scan_bytes = 0;
+  if (num_rays > 0)
+    CSM_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, scan_bytes, static_cast<long long*>(nullptr),
+                                           static_cast<long long*>(nullptr),
+                                           static_cast<long long>(hr + 1), s));
+  const size_t o_slots = o_scan + align(scan_bytes);
+  const size_t work_bytes = o_slots + sizeof(int) * static_cast<size_t>(num_slots);
+  PinnedBuf& up = ctx->P("ins2_upload");
+  PinnedBuf& down = ctx->P("ins2_status");
+  DevBuf& d_work = ctx->D("ins2_work");
+  CSM_TRY(up.Reserve(up_bytes));
+  CSM_TRY(down.Reserve(status_bytes));
+  CSM_TRY(d_work.Reserve(work_bytes));
+  CSM_TRY(ReserveKnownBoxSlots(ctx, H));
+
+  CSM_CUDA(cudaEventRecord(ctx->ev0, s));
+  for (int h = 0; h < H; ++h) {
+    CSM_TRY(tx[h]->Begin());
+    targets[h].cells = tx[h]->arrays.cells;
+  }
+  // ---- upload: status | targets | points ----
+  char* hp = up.as<char>();
+  int* h_status = reinterpret_cast<int*>(hp);
+  std::fill(h_status, h_status + kIns2BoxBase, 0);
+  for (int h = 0; h < H; ++h) {
+    int* box = h_status + kIns2BoxBase + 4 * h;
+    box[0] = box[1] = INT_MAX;
+    box[2] = box[3] = INT_MIN;
+  }
+  std::memcpy(hp + o_targets, targets.data(), sizeof(Ins2Target) * H);
+  if (!points.d_pts) {
+    float2* h_pts = reinterpret_cast<float2*>(hp + o_pts);
+    for (int i = 0; i < num_points; ++i) {
+      const float* q = i < n ? returns + 3 * static_cast<size_t>(i)
+                             : misses + 3 * static_cast<size_t>(i - n);
+      h_pts[i] = make_float2(q[0], q[1]);
+    }
+  }
+  CSM_CUDA(cudaMemcpyAsync(d_work.p, hp, up_bytes, cudaMemcpyHostToDevice, s));
+  char* d = d_work.as<char>();
+  int* d_status = reinterpret_cast<int*>(d);
+  const Ins2Target* d_targets = reinterpret_cast<const Ins2Target*>(d + o_targets);
+  int* d_hits = reinterpret_cast<int*>(d + o_hits);
+  int2* d_ends = reinterpret_cast<int2*>(d + o_ends);
+  long long* d_counts = reinterpret_cast<long long*>(d + o_counts);
+  long long* d_off = reinterpret_cast<long long*>(d + o_off);
+  int* d_slots = reinterpret_cast<int*>(d + o_slots);
+  if (num_points > 0) {
+    const dim3 per_point(DivUp(num_points, 256), H);
+    k_ins2_index<<<per_point, 256, 0, s>>>(d_targets,
+                                           points.d_pts ? points.d_pts
+                                                        : reinterpret_cast<const float2*>(d + o_pts),
+                                           num_points, n, num_rays, d_status, d_hits, d_ends,
+                                           d_counts);
+    CSM_LAUNCH_CHECK();
+    if (num_rays > 0) {
+      CSM_CUDA(cub::DeviceScan::ExclusiveSum(d + o_scan, scan_bytes, d_counts, d_off,
+                                             static_cast<long long>(hr + 1), s));
+      k_ins2_rays<<<per_point, 256, 0, s>>>(d_targets, d_ends, d_off, num_rays, d_status,
+                                            d_slots);
+      CSM_LAUNCH_CHECK();
+    }
+    if (n > 0) {
+      k_ins2_hits<<<dim3(DivUp(n, 256), H), 256, 0, s>>>(d_targets, d_hits, n, d_status,
+                                                         inserter->d_tables);
+      CSM_LAUNCH_CHECK();
+    }
+    long long max_cap = 0;
+    for (const Ins2Target& t : targets) max_cap = std::max(max_cap, t.slot_cap);
+    if (num_rays > 0) {
+      k_ins2_misses<<<dim3(Blocks(max_cap), H), 256, 0, s>>>(
+          d_targets, d_off, num_rays, d_slots, d_status, inserter->d_tables + kValueCount);
+      CSM_LAUNCH_CHECK();
+    }
+    k_ins2_finish<<<dim3(Blocks(n + max_cap), H), 256, 0, s>>>(d_targets, d_hits, n, d_off,
+                                                               num_rays, d_slots, d_status);
+    CSM_LAUNCH_CHECK();
+  }
+  CSM_CUDA(cudaMemcpyAsync(down.p, d_status, status_bytes, cudaMemcpyDeviceToHost, s));
+  CSM_CUDA(cudaEventRecord(ctx->ev1, s));
+  CSM_CUDA(cudaStreamSynchronize(s));
+  const int flags = down.as<int>()[0];
+  CSM_REQUIRE(!(flags & kIns2Outside), "a point outside the grown limits");
+  CSM_REQUIRE(!(flags & kIns2TooManyPixels), "too many ray pixels");
+  for (int h = 0; h < H; ++h) {
+    KnownBox2 touched = BoxFrom(down.as<int>() + kIns2BoxBase + 4 * h);
+    if (num_rays > 0)
+      touched.Extend(targets[h].begin.x / kSubpixelScale, targets[h].begin.y / kSubpixelScale);
+    CSM_TRY(tx[h]->Commit(touched, stats));
+  }
+  return CSM_OK;
+}
+
+}  // namespace
 
 extern "C" {
 
@@ -246,23 +410,10 @@ csm_status csm_range_inserter2d_insert_submaps(const csm_range_inserter2d* inser
                                                 int32_t num_misses, csm_rt_grid2d* const* grids,
                                                 int32_t num_grids, csm_stats* stats) {
   CSM_REQUIRE(inserter && origin && grids, "null pointer");
-  CSM_REQUIRE(num_grids >= 1 && num_grids <= 65535, "num_grids");
   CSM_REQUIRE(num_returns >= 0 && (num_returns == 0 || returns), "returns");
   CSM_REQUIRE(num_misses >= 0 && (num_misses == 0 || misses), "misses");
-  const int H = num_grids;
-  for (int h = 0; h < H; ++h) {
-    CSM_REQUIRE(grids[h] != nullptr, "null grid");
-    for (int k = 0; k < h; ++k) CSM_REQUIRE(grids[k] != grids[h], "a grid appears twice");
-  }
-  Ctx* ctx = inserter->ctx;
-  for (int h = 0; h < H; ++h) {
-    CSM_REQUIRE(grids[h]->d_wcells == nullptr, "a TSDF2D handle takes the TSDF inserter");
-    CSM_REQUIRE(grids[h]->ctx == ctx, "grid on another device than the inserter");
-  }
+  CSM_TRY(CheckGrids(inserter, grids, num_grids));
   const int n = num_returns, m = num_misses;
-  const bool free_space = inserter->options.insert_free_space != 0;
-  const int num_points = free_space ? n + m : n;   // what the kernels index
-  const int num_rays = free_space ? n + m : 0;
   // ---- one pass over the points: finite, bounding box (GrowAsNeeded, :35-50), ray lengths ----
   CSM_REQUIRE(Finite(origin, 3), "non-finite point");
   float lo_x = origin[0], lo_y = origin[1], hi_x = origin[0], hi_y = origin[1];
@@ -283,134 +434,23 @@ csm_status csm_range_inserter2d_insert_submaps(const csm_range_inserter2d* inser
   scan(returns, n);
   scan(misses, m);
   CSM_REQUIRE(finite, "non-finite point");
-  if (!free_space) l1 = 0.;
-
-  std::lock_guard<std::mutex> lock(ctx->mu);
-  CSM_CUDA(cudaSetDevice(ctx->device));
-  // ---- every handle grows, and its origin is checked, before anything changes ----
-  std::vector<std::unique_ptr<GridInsert2>> tx(H);
-  std::vector<Ins2Target> targets(H);
-  long long num_slots = 0;
-  for (int h = 0; h < H; ++h) {
-    tx[h].reset(new GridInsert2(grids[h], h));
-    CSM_REQUIRE(tx[h]->Grow(lo_x, lo_y, hi_x, hi_y), "the grid would grow past 30000 cells");
-    const Limits2& L = tx[h]->L;
-    Ins2Target& t = targets[h];
-    // the superscaled limits (:58-65)
-    t.S = Limits2{L.resolution / kSubpixelScale, L.max_x, L.max_y, L.nx * kSubpixelScale,
-                  L.ny * kSubpixelScale};
-    long long ix, iy;
-    t.S.CellIndex(origin[0], origin[1], &ix, &iy);
-    CSM_REQUIRE(t.S.Contains(ix, iy), "origin outside the grown limits");
-    t.begin = make_int2(static_cast<int>(ix), static_cast<int>(iy));
-    t.pitch = tx[h]->arrays.pitch;
-    t.slot_begin = num_slots;
-    t.slot_cap = num_rays > 0 ? SlotReservation(l1, L.resolution, num_rays) : 0;
-    num_slots += t.slot_cap;
-  }
-
-  // ---- workspaces, before any transaction queues a copy into pinned memory ----
-  cudaStream_t s = ctx->stream;
-  auto align = [](size_t b) { return (b + 255) / 256 * 256; };
-  const size_t hn = static_cast<size_t>(H) * n, hr = static_cast<size_t>(H) * num_rays;
-  const size_t status_bytes = sizeof(int) * (kIns2BoxBase + 4 * static_cast<size_t>(H));
-  const size_t o_targets = align(status_bytes);
-  const size_t o_pts = o_targets + align(sizeof(Ins2Target) * H);
-  const size_t up_bytes = o_pts + align(sizeof(float2) * static_cast<size_t>(num_points));
-  const size_t o_hits = up_bytes;
-  const size_t o_ends = o_hits + align(sizeof(int) * hn);
-  const size_t o_counts = o_ends + align(sizeof(int2) * hr);
-  const size_t o_off = o_counts + align(sizeof(long long) * (hr + 1));
-  const size_t o_scan = o_off + align(sizeof(long long) * (hr + 1));
-  size_t scan_bytes = 0;
-  if (num_rays > 0)
-    CSM_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, scan_bytes, static_cast<long long*>(nullptr),
-                                           static_cast<long long*>(nullptr),
-                                           static_cast<long long>(hr + 1), s));
-  const size_t o_slots = o_scan + align(scan_bytes);
-  const size_t work_bytes = o_slots + sizeof(int) * static_cast<size_t>(num_slots);
-  PinnedBuf& up = ctx->P("ins2_upload");
-  PinnedBuf& down = ctx->P("ins2_status");
-  DevBuf& d_work = ctx->D("ins2_work");
-  CSM_TRY(up.Reserve(up_bytes));
-  CSM_TRY(down.Reserve(status_bytes));
-  CSM_TRY(d_work.Reserve(work_bytes));
-  CSM_TRY(ReserveKnownBoxSlots(ctx, H));
-
-  CSM_CUDA(cudaEventRecord(ctx->ev0, s));
-  for (int h = 0; h < H; ++h) {
-    CSM_TRY(tx[h]->Begin());
-    targets[h].cells = tx[h]->arrays.cells;
-  }
-  // ---- upload: status | targets | points ----
-  char* hp = up.as<char>();
-  int* h_status = reinterpret_cast<int*>(hp);
-  std::fill(h_status, h_status + kIns2BoxBase, 0);
-  for (int h = 0; h < H; ++h) {
-    int* box = h_status + kIns2BoxBase + 4 * h;
-    box[0] = box[1] = INT_MAX;
-    box[2] = box[3] = INT_MIN;
-  }
-  std::memcpy(hp + o_targets, targets.data(), sizeof(Ins2Target) * H);
-  float2* h_pts = reinterpret_cast<float2*>(hp + o_pts);
-  for (int i = 0; i < num_points; ++i) {
-    const float* q = i < n ? returns + 3 * static_cast<size_t>(i)
-                           : misses + 3 * static_cast<size_t>(i - n);
-    h_pts[i] = make_float2(q[0], q[1]);
-  }
-  CSM_CUDA(cudaMemcpyAsync(d_work.p, hp, up_bytes, cudaMemcpyHostToDevice, s));
-  char* d = d_work.as<char>();
-  int* d_status = reinterpret_cast<int*>(d);
-  const Ins2Target* d_targets = reinterpret_cast<const Ins2Target*>(d + o_targets);
-  int* d_hits = reinterpret_cast<int*>(d + o_hits);
-  int2* d_ends = reinterpret_cast<int2*>(d + o_ends);
-  long long* d_counts = reinterpret_cast<long long*>(d + o_counts);
-  long long* d_off = reinterpret_cast<long long*>(d + o_off);
-  int* d_slots = reinterpret_cast<int*>(d + o_slots);
-  if (num_points > 0) {
-    const dim3 per_point(DivUp(num_points, 256), H);
-    k_ins2_index<<<per_point, 256, 0, s>>>(d_targets, reinterpret_cast<const float2*>(d + o_pts),
-                                           num_points, n, num_rays, d_status, d_hits, d_ends,
-                                           d_counts);
-    CSM_LAUNCH_CHECK();
-    if (num_rays > 0) {
-      CSM_CUDA(cub::DeviceScan::ExclusiveSum(d + o_scan, scan_bytes, d_counts, d_off,
-                                             static_cast<long long>(hr + 1), s));
-      k_ins2_rays<<<per_point, 256, 0, s>>>(d_targets, d_ends, d_off, num_rays, d_status,
-                                            d_slots);
-      CSM_LAUNCH_CHECK();
-    }
-    if (n > 0) {
-      k_ins2_hits<<<dim3(DivUp(n, 256), H), 256, 0, s>>>(d_targets, d_hits, n, d_status,
-                                                         inserter->d_tables);
-      CSM_LAUNCH_CHECK();
-    }
-    long long max_cap = 0;
-    for (const Ins2Target& t : targets) max_cap = std::max(max_cap, t.slot_cap);
-    if (num_rays > 0) {
-      k_ins2_misses<<<dim3(Blocks(max_cap), H), 256, 0, s>>>(
-          d_targets, d_off, num_rays, d_slots, d_status, inserter->d_tables + kValueCount);
-      CSM_LAUNCH_CHECK();
-    }
-    k_ins2_finish<<<dim3(Blocks(n + max_cap), H), 256, 0, s>>>(d_targets, d_hits, n, d_off,
-                                                               num_rays, d_slots, d_status);
-    CSM_LAUNCH_CHECK();
-  }
-  CSM_CUDA(cudaMemcpyAsync(down.p, d_status, status_bytes, cudaMemcpyDeviceToHost, s));
-  CSM_CUDA(cudaEventRecord(ctx->ev1, s));
-  CSM_CUDA(cudaStreamSynchronize(s));
-  const int flags = down.as<int>()[0];
-  CSM_REQUIRE(!(flags & kIns2Outside), "a point outside the grown limits");
-  CSM_REQUIRE(!(flags & kIns2TooManyPixels), "too many ray pixels");
-  for (int h = 0; h < H; ++h) {
-    KnownBox2 touched = BoxFrom(down.as<int>() + kIns2BoxBase + 4 * h);
-    if (num_rays > 0)
-      touched.Extend(targets[h].begin.x / kSubpixelScale, targets[h].begin.y / kSubpixelScale);
-    CSM_TRY(tx[h]->Commit(touched, stats));
-  }
-  return CSM_OK;
+  const InsertPoints2 points{nullptr, lo_x, lo_y, hi_x, hi_y, l1};
+  return InsertSubmaps(inserter, origin, points, returns, misses, n, m, grids, num_grids, stats);
 }
 
+}  // extern "C"
+
+csm_status csm::InsertSubmapsResident(const csm_range_inserter2d* inserter, const float origin[3],
+                                      const InsertPoints2& points, int32_t num_returns,
+                                      int32_t num_misses, csm_rt_grid2d* const* grids,
+                                      int32_t num_grids, csm_stats* stats) {
+  CSM_REQUIRE(inserter && origin && grids && points.d_pts, "null pointer");
+  CSM_TRY(CheckGrids(inserter, grids, num_grids));
+  return InsertSubmaps(inserter, origin, points, nullptr, nullptr, num_returns, num_misses, grids,
+                       num_grids, stats);
+}
+
+extern "C" {
 csm_status csm_range_inserter2d_insert(const csm_range_inserter2d* inserter,
                                        const float origin[3], const float* returns,
                                        int32_t num_returns, const float* misses,

@@ -27,6 +27,7 @@
 // into a CPU harness (SIMT shims, one std::thread per CUDA thread) to check their control
 // flow against the oracle where no GPU is present; the library itself never defines it.
 #ifndef CSM_REFINE_DEVICE_ONLY
+#include "resident2d.cuh"
 #include "rtgrid.cuh"
 #endif
 #include "trust_region.cuh"
@@ -554,7 +555,72 @@ void FillJob(const csm_rt_grid2d* grid, int n, long long xyz_off, const double t
   }
 }
 
+// Uploads the staging buffer `up` (the jobs' clouds, then at off_jobs the jobs; only the jobs when
+// d_cloud is not null, whose clouds the jobs then index), solves every job in one launch and
+// reads the results back: one stream synchronisation.
+csm_status SolveJobs(Ctx* ctx, DevBuf& d_up, size_t off_jobs, size_t up_bytes, int num_jobs,
+                     const float* d_cloud, const RefOpts& P, csm_ceres_result2d* results,
+                     csm_stats* stats) {
+  cudaStream_t s = ctx->stream;
+  const char* h = ctx->P("ref_upload").as<char>();
+  DevBuf& d_out = ctx->D("ref_results");
+  PinnedBuf& rb = ctx->P("ref_readback");
+  CSM_TRY(d_out.Reserve(sizeof(RefResultDev) * num_jobs));
+  CSM_TRY(rb.Reserve(sizeof(RefResultDev) * num_jobs));
+  CSM_CUDA(cudaEventRecord(ctx->ev0, s));
+  if (d_cloud == nullptr)
+    CSM_CUDA(cudaMemcpyAsync(d_up.p, h, up_bytes, cudaMemcpyHostToDevice, s));
+  else
+    CSM_CUDA(cudaMemcpyAsync(d_up.as<char>() + off_jobs, h + off_jobs, up_bytes - off_jobs,
+                             cudaMemcpyHostToDevice, s));
+  ProfBegin(ctx);
+  k_ceres_match2d<<<num_jobs, kRefThreads, 0, s>>>(
+      reinterpret_cast<const RefJobDev*>(d_up.as<char>() + off_jobs), P,
+      d_cloud ? d_cloud : d_up.as<float>(), d_out.as<RefResultDev>());
+  CSM_LAUNCH_CHECK();
+  ProfEnd(ctx, "k_ceres_match2d", static_cast<double>(num_jobs));
+  CSM_CUDA(cudaEventRecord(ctx->ev1, s));
+  CSM_CUDA(cudaMemcpyAsync(rb.p, d_out.p, sizeof(RefResultDev) * num_jobs,
+                           cudaMemcpyDeviceToHost, s));
+  CSM_CUDA(cudaStreamSynchronize(s));
+  const RefResultDev* r = rb.as<RefResultDev>();
+  for (int j = 0; j < num_jobs; ++j) {
+    csm_ceres_result2d& o = results[j];
+    std::memset(&o, 0, sizeof(o));
+    std::memcpy(o.pose_estimate, r[j].pose, sizeof(double) * 3);
+    o.initial_cost = r[j].initial_cost;
+    o.final_cost = r[j].final_cost;
+    o.iterations = r[j].iterations;
+    o.num_successful_steps = r[j].num_successful_steps;
+    o.termination = r[j].termination;
+  }
+  if (stats) {
+    std::memset(stats, 0, sizeof(*stats));
+    float ms = 0.f;
+    cudaEventElapsedTime(&ms, ctx->ev0, ctx->ev1);
+    stats->device_ms = ms;
+    stats->host_syncs = 1;
+  }
+  return CSM_OK;
+}
+
 }  // namespace
+
+csm_status csm::CeresMatch2DResident(Ctx* ctx, const csm_rt_grid2d* grid, const float* d_xyz, int n,
+                                const double target[2], const double init[3],
+                                const csm_ceres_options2d* options, csm_ceres_result2d* result,
+                                csm_stats* stats) {
+  RefOpts P;
+  CSM_TRY(FillOpts(options, &P));
+  CSM_REQUIRE(grid != nullptr && n >= 1, "empty point cloud");
+  const size_t up_bytes = sizeof(RefJobDev);
+  PinnedBuf& up = ctx->P("ref_upload");
+  DevBuf& d_up = ctx->D("ref_upload");
+  CSM_TRY(up.Reserve(up_bytes));
+  CSM_TRY(d_up.Reserve(up_bytes));
+  FillJob(grid, n, 0, target, init, up.as<RefJobDev>());
+  return SolveJobs(ctx, d_up, 0, up_bytes, 1, d_xyz, P, result, stats);
+}
 
 extern "C" {
 
@@ -582,17 +648,12 @@ csm_status csm_ceres_match2d_batch(const csm_ceres_job2d* jobs, int32_t num_jobs
   CSM_TRY(AcquireLane(device, &guard));
   Ctx* ctx = guard.lane;
   CSM_CUDA(cudaSetDevice(ctx->device));
-  cudaStream_t s = ctx->stream;
   const size_t off_jobs = (static_cast<size_t>(floats) * 4 + 255) / 256 * 256;
   const size_t up_bytes = off_jobs + sizeof(RefJobDev) * num_jobs;
   PinnedBuf& up = ctx->P("ref_upload");
   DevBuf& d_up = ctx->D("ref_upload");
-  DevBuf& d_out = ctx->D("ref_results");
-  PinnedBuf& rb = ctx->P("ref_readback");
   CSM_TRY(up.Reserve(up_bytes));
   CSM_TRY(d_up.Reserve(up_bytes));
-  CSM_TRY(d_out.Reserve(sizeof(RefResultDev) * num_jobs));
-  CSM_TRY(rb.Reserve(sizeof(RefResultDev) * num_jobs));
   char* h = up.as<char>();
   RefJobDev* hj = reinterpret_cast<RefJobDev*>(h + off_jobs);
   long long off = 0;
@@ -603,37 +664,7 @@ csm_status csm_ceres_match2d_batch(const csm_ceres_job2d* jobs, int32_t num_jobs
             jobs[j].initial_pose, &hj[j]);
     off += 3LL * jobs[j].num_points;
   }
-  CSM_CUDA(cudaEventRecord(ctx->ev0, s));
-  CSM_CUDA(cudaMemcpyAsync(d_up.p, h, up_bytes, cudaMemcpyHostToDevice, s));
-  ProfBegin(ctx);
-  k_ceres_match2d<<<num_jobs, kRefThreads, 0, s>>>(
-      reinterpret_cast<const RefJobDev*>(d_up.as<char>() + off_jobs), P, d_up.as<float>(),
-      d_out.as<RefResultDev>());
-  CSM_LAUNCH_CHECK();
-  ProfEnd(ctx, "k_ceres_match2d", static_cast<double>(num_jobs));
-  CSM_CUDA(cudaEventRecord(ctx->ev1, s));
-  CSM_CUDA(cudaMemcpyAsync(rb.p, d_out.p, sizeof(RefResultDev) * num_jobs,
-                           cudaMemcpyDeviceToHost, s));
-  CSM_CUDA(cudaStreamSynchronize(s));
-  const RefResultDev* r = rb.as<RefResultDev>();
-  for (int j = 0; j < num_jobs; ++j) {
-    csm_ceres_result2d& o = results[j];
-    std::memset(&o, 0, sizeof(o));
-    std::memcpy(o.pose_estimate, r[j].pose, sizeof(double) * 3);
-    o.initial_cost = r[j].initial_cost;
-    o.final_cost = r[j].final_cost;
-    o.iterations = r[j].iterations;
-    o.num_successful_steps = r[j].num_successful_steps;
-    o.termination = r[j].termination;
-  }
-  if (stats) {
-    std::memset(stats, 0, sizeof(*stats));
-    float ms = 0.f;
-    cudaEventElapsedTime(&ms, ctx->ev0, ctx->ev1);
-    stats->device_ms = ms;
-    stats->host_syncs = 1;
-  }
-  return CSM_OK;
+  return SolveJobs(ctx, d_up, off_jobs, up_bytes, num_jobs, nullptr, P, results, stats);
 }
 
 csm_status csm_ceres_evaluate2d(const csm_rt_grid2d* grid, const float* xyz, int32_t num_points,

@@ -19,6 +19,7 @@
 #include <algorithm>
 #include <cmath>
 #include <cstring>
+#include <string>
 #include <vector>
 
 #include <cub/device/device_radix_sort.cuh>
@@ -28,6 +29,7 @@
 
 #include "common.cuh"
 #include "point_batch.cuh"
+#include "voxel_filter.cuh"
 
 namespace csm {
 namespace {
@@ -81,14 +83,18 @@ struct CloudState {
 
 // ---- range filter and the adaptive search --------------------------------------------------
 
+// A point outside `pre_active` (when given) is not in the cloud at all: the batch then filters
+// the subsequence of points it flags, in order.
 __global__ void k_vf_range(const float* __restrict__ xyz, const int* __restrict__ off, int nc,
-                           const float* __restrict__ max_range, int n, unsigned char* active,
-                           int* num_active) {
+                           const float* __restrict__ max_range,
+                           const unsigned char* __restrict__ pre_active, int n,
+                           unsigned char* active, int* num_active) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
   const int c = CloudOf(off, nc, i);
   const float x = xyz[3 * i], y = xyz[3 * i + 1], z = xyz[3 * i + 2];
-  const bool in = sqrtf((x * x + y * y) + z * z) <= max_range[c];   // FilterByMaxRange (:31-36)
+  const bool in = (pre_active == nullptr || pre_active[i]) &&
+                  sqrtf((x * x + y * y) + z * z) <= max_range[c];   // FilterByMaxRange (:31-36)
   active[i] = in;
   if (in) atomicAdd(&num_active[c], 1);
 }
@@ -400,16 +406,37 @@ csm_status ValidateClouds(const float* const* xyz, const int32_t* num_points, in
   return CSM_OK;
 }
 
-// The whole batch: `options` null for VoxelFilter at `resolution`, else the adaptive filter.
-csm_status Run(const float* const* xyz, const std::vector<int>& off, const float* resolution,
-               const csm_adaptive_voxel_filter_options* options, int32_t device,
-               int32_t* kept_indices, int32_t* num_kept, csm_stats* stats) {
+}  // namespace
+
+size_t VoxelFilterStateBytes() { return sizeof(CloudState); }
+
+csm_status VoxelFilterCheckStates(const void* states, int num_clouds) {
+  const CloudState* rst = static_cast<const CloudState*>(states);
+  for (int c = 0; c < num_clouds; ++c) {
+    if (rst[c].error) {
+      SetError("adaptive voxel filter: cloud %d did not settle in %d bisection steps", c,
+               kBisectionSteps);
+      return CSM_E_INTERNAL;
+    }
+    if (rst[c].phase != kDone) {
+      SetError("adaptive voxel filter: cloud %d did not finish its search", c);
+      return CSM_E_INTERNAL;
+    }
+  }
+  return CSM_OK;
+}
+
+// The whole batch on ctx's stream, up to its device outputs: `options` null for VoxelFilter at
+// `resolution`, else the adaptive filter.  The points come from the host clouds `xyz`, or are
+// already on the device at d_xyz (off.back() x {x, y, z}).
+csm_status VoxelFilterEnqueue(Ctx* ctx, const char* workspace, const float* const* xyz,
+                              const float* d_xyz, const std::vector<int>& off,
+                              const float* resolution,
+                              const csm_adaptive_voxel_filter_options* options,
+                              const unsigned char* d_pre_active, cudaEvent_t start,
+                              VoxelFilterDeviceOut* result) {
   const int nc = static_cast<int>(off.size()) - 1;
   const int n = off.back();
-  LaneGuard guard;
-  CSM_TRY(AcquireLane(device, &guard));
-  Ctx* ctx = guard.lane;
-  CSM_CUDA(cudaSetDevice(ctx->device));
   cudaStream_t s = ctx->stream;
   const bool adaptive = options != nullptr;
 
@@ -516,7 +543,7 @@ csm_status Run(const float* const* xyz, const std::vector<int>& off, const float
     return a;
   };
   lay(sizer);
-  DevBuf& ws = ctx->D("voxel_filter");
+  DevBuf& ws = ctx->D(workspace);
   CSM_TRY(ws.Reserve(sizer.at));
   Carver carver;
   carver.base = ws.as<char>();
@@ -528,12 +555,13 @@ csm_status Run(const float* const* xyz, const std::vector<int>& off, const float
   const size_t o_mr = o_st + Align(sizeof(CloudState) * std::max(nc, 1));
   const size_t o_to = o_mr + Align(sizeof(float) * std::max(nc, 1));
   const size_t up_bytes = o_to + sizeof(long long) * (nc + 1);
-  PinnedBuf& up = ctx->P("voxel_filter_up");
+  PinnedBuf& up = ctx->P((std::string(workspace) + "_up").c_str());
   CSM_TRY(up.Reserve(up_bytes));
   char* h = up.as<char>();
-  for (int c = 0; c < nc; ++c)
-    if (off[c + 1] > off[c])
-      std::memcpy(h + sizeof(float) * 3 * off[c], xyz[c], sizeof(float) * 3 * (off[c + 1] - off[c]));
+  if (d_xyz == nullptr)
+    for (int c = 0; c < nc; ++c)
+      if (off[c + 1] > off[c])
+        std::memcpy(h + sizeof(float) * 3 * off[c], xyz[c], sizeof(float) * 3 * (off[c + 1] - off[c]));
   std::memcpy(h + o_off, off.data(), sizeof(int) * (nc + 1));
   if (nc > 0) {
     std::memcpy(h + o_st, st.data(), sizeof(CloudState) * nc);
@@ -541,8 +569,10 @@ csm_status Run(const float* const* xyz, const std::vector<int>& off, const float
   }
   std::memcpy(h + o_to, table_off.data(), sizeof(long long) * (nc + 1));
 
-  CSM_CUDA(cudaEventRecord(ctx->ev0, s));
-  CSM_CUDA(cudaMemcpyAsync(a.xyz, h, o_off, cudaMemcpyHostToDevice, s));
+  if (start) CSM_CUDA(cudaEventRecord(start, s));
+  const float* pts = d_xyz ? d_xyz : a.xyz;
+  if (d_xyz == nullptr && n > 0)
+    CSM_CUDA(cudaMemcpyAsync(a.xyz, h, o_off, cudaMemcpyHostToDevice, s));
   CSM_CUDA(cudaMemcpyAsync(a.off, h + o_off, sizeof(int) * (nc + 1), cudaMemcpyHostToDevice, s));
   if (nc > 0) {
     CSM_CUDA(cudaMemcpyAsync(a.st, h + o_st, sizeof(CloudState) * nc, cudaMemcpyHostToDevice, s));
@@ -558,7 +588,8 @@ csm_status Run(const float* const* xyz, const std::vector<int>& off, const float
     CSM_CUDA(cudaMemsetAsync(a.distinct, 0, sizeof(int) * nc, s));
     CSM_CUDA(cudaMemsetAsync(a.empty_seen, 0, sizeof(int) * nc, s));
     if (n > 0) {
-      k_vf_range<<<nb, kThreads, 0, s>>>(a.xyz, a.off, nc, a.max_range, n, a.active, a.num_active);
+      k_vf_range<<<nb, kThreads, 0, s>>>(pts, a.off, nc, a.max_range, d_pre_active, n, a.active,
+                                         a.num_active);
       CSM_LAUNCH_CHECK();
     }
     k_vf_start<<<cb, kThreads, 0, s>>>(a.st, a.num_active, nc);
@@ -567,7 +598,7 @@ csm_status Run(const float* const* xyz, const std::vector<int>& off, const float
     for (int trial = 0; trial < 1 + kHalvingSteps + kBisectionSteps; ++trial) {
       if (n > 0) {
         CSM_CUDA(cudaMemsetAsync(a.table, 0xff, sizeof(unsigned long long) * table_slots, s));
-        k_vf_count<<<nb, kThreads, 0, s>>>(a.xyz, a.off, nc, a.active, n, a.st, a.table,
+        k_vf_count<<<nb, kThreads, 0, s>>>(pts, a.off, nc, a.active, n, a.st, a.table,
                                            a.table_off, a.empty_seen, a.distinct);
         CSM_LAUNCH_CHECK();
       }
@@ -578,7 +609,7 @@ csm_status Run(const float* const* xyz, const std::vector<int>& off, const float
 
   if (n > 0) {
     const unsigned char* active = adaptive ? a.active : nullptr;
-    k_vf_keys<<<nb, kThreads, 0, s>>>(a.xyz, a.off, nc, active, n, a.st, a.keys, a.vals, a.kept);
+    k_vf_keys<<<nb, kThreads, 0, s>>>(pts, a.off, nc, active, n, a.st, a.keys, a.vals, a.kept);
     CSM_LAUNCH_CHECK();
     size_t tb = temp_bytes;
     CSM_CUDA(cub::DeviceRadixSort::SortPairs(a.temp, tb, a.keys, a.keys_s, a.vals, a.vals_s, n,
@@ -633,31 +664,45 @@ csm_status Run(const float* const* xyz, const std::vector<int>& off, const float
   } else if (nc > 0) {
     CSM_CUDA(cudaMemsetAsync(a.counts, 0, sizeof(int) * nc, s));
   }
+  result->kept_indices = a.out;
+  result->num_kept = a.counts;
+  result->kept = a.kept;
+  result->states = a.st;
+  return CSM_OK;
+}
+
+namespace {
+
+// The whole batch from host clouds to host outputs, with one stream synchronisation.
+csm_status Run(const float* const* xyz, const std::vector<int>& off, const float* resolution,
+               const csm_adaptive_voxel_filter_options* options, int32_t device,
+               int32_t* kept_indices, int32_t* num_kept, csm_stats* stats) {
+  const int nc = static_cast<int>(off.size()) - 1;
+  const int n = off.back();
+  LaneGuard guard;
+  CSM_TRY(AcquireLane(device, &guard));
+  Ctx* ctx = guard.lane;
+  CSM_CUDA(cudaSetDevice(ctx->device));
+  cudaStream_t s = ctx->stream;
+  VoxelFilterDeviceOut a;
+  CSM_TRY(VoxelFilterEnqueue(ctx, "voxel_filter", xyz, nullptr, off, resolution, options,
+                             nullptr, ctx->ev0, &a));
   // ---- read-back: indices, counts, states (error flags) ----
   const size_t o_cnt = Align(sizeof(int) * std::max(n, 1));
   const size_t o_rst = o_cnt + Align(sizeof(int) * std::max(nc, 1));
   PinnedBuf& down = ctx->P("voxel_filter_down");
   CSM_TRY(down.Reserve(o_rst + sizeof(CloudState) * std::max(nc, 1)));
   char* d = down.as<char>();
-  if (n > 0) CSM_CUDA(cudaMemcpyAsync(d, a.out, sizeof(int) * n, cudaMemcpyDeviceToHost, s));
+  if (n > 0)
+    CSM_CUDA(cudaMemcpyAsync(d, a.kept_indices, sizeof(int) * n, cudaMemcpyDeviceToHost, s));
   if (nc > 0) {
-    CSM_CUDA(cudaMemcpyAsync(d + o_cnt, a.counts, sizeof(int) * nc, cudaMemcpyDeviceToHost, s));
-    CSM_CUDA(cudaMemcpyAsync(d + o_rst, a.st, sizeof(CloudState) * nc, cudaMemcpyDeviceToHost, s));
+    CSM_CUDA(cudaMemcpyAsync(d + o_cnt, a.num_kept, sizeof(int) * nc, cudaMemcpyDeviceToHost, s));
+    CSM_CUDA(cudaMemcpyAsync(d + o_rst, a.states, sizeof(CloudState) * nc, cudaMemcpyDeviceToHost,
+                             s));
   }
   CSM_CUDA(cudaEventRecord(ctx->ev1, s));
   CSM_CUDA(cudaStreamSynchronize(s));
-  const CloudState* rst = reinterpret_cast<const CloudState*>(d + o_rst);
-  for (int c = 0; c < nc; ++c) {
-    if (rst[c].error) {
-      SetError("adaptive voxel filter: cloud %d did not settle in %d bisection steps", c,
-               kBisectionSteps);
-      return CSM_E_INTERNAL;
-    }
-    if (rst[c].phase != kDone) {
-      SetError("adaptive voxel filter: cloud %d did not finish its search", c);
-      return CSM_E_INTERNAL;
-    }
-  }
+  CSM_TRY(VoxelFilterCheckStates(d + o_rst, nc));
   const int* counts = reinterpret_cast<const int*>(d + o_cnt);
   long long total = 0;
   for (int c = 0; c < nc; ++c) total += counts[c];

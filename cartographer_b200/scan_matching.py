@@ -739,13 +739,19 @@ class ActiveSubmaps2D:
     def InsertRangeData(self, origin, returns, misses=None):
         """origin (2 or 3), returns and misses (n x 3) in the local frame.  Returns the active
         submaps."""
+        return self.insert_with(origin, lambda grids: self.range_data_inserter.insert_submaps(
+            grids, origin, returns, misses))
+
+    def insert_with(self, origin, insert):
+        """InsertRangeData's lifecycle around insert(grids), which writes the scan whose local
+        origin is `origin` into the active submaps' grids (local_slam.LocalTrajectoryBuilder2D
+        inserts range data that stays on the device)."""
         n = self.options.num_range_data
         if not self._submaps or self._submaps[-1].num_range_data == n:
             self._add_submap(np.asarray(origin, np.float32).reshape(-1)[:2])
         for s in self._submaps:
             assert not s.insertion_finished
-        self.range_data_inserter.insert_submaps([s.grid for s in self._submaps], origin,
-                                                returns, misses)
+        insert([s.grid for s in self._submaps])
         for s in self._submaps:
             s.num_range_data += 1
         if self._submaps[0].num_range_data == 2 * n:

@@ -1281,6 +1281,109 @@ csm_status csm_cb_batch3d_run(csm_ctx* ctx, const csm_matcher3d* const* matchers
                               const int32_t* submap_owner, int32_t max_concurrency,
                               csm_result3d* results, csm_stats* stats /* may be NULL */);
 
+/* ---- local SLAM in 2D: LocalTrajectoryBuilder2D on the device ------------------------------ */
+/* LocalTrajectoryBuilder2D (mapping/internal/2d/local_trajectory_builder_2d.cc:65-300) from
+ * synchronized range data to the submap insert, with the range data in device memory between the
+ * stages.  The caller keeps the pose extrapolator, the range-data collator and the motion filter
+ * (double precision and libm on the host) and the ActiveSubmaps2D lifecycle; the handle runs
+ * every per-point stage.  Each stage equals the existing single-stage entry points on the same
+ * data: csm_voxel_filter_batch, csm_adaptive_voxel_filter_batch, csm_rt_match2d_batch,
+ * csm_ceres_match2d_batch and csm_range_inserter2d_insert_submaps.  Float options of the proto
+ * are floats here and compare as floats. */
+typedef struct csm_local_slam_options2d {   /* proto LocalTrajectoryBuilderOptions2D */
+  float min_range, max_range;
+  float min_z, max_z;
+  float missing_data_ray_length;
+  float voxel_filter_size;                   /* finite, > 0 */
+  int32_t num_accumulated_range_data;        /* >= 1; the caller decides when to match */
+  int32_t use_online_correlative_scan_matching;
+  csm_adaptive_voxel_filter_options adaptive_voxel_filter;
+  double linear_search_window;               /* real_time_correlative_scan_matcher */
+  double angular_search_window;
+  double translation_delta_cost_weight;
+  double rotation_delta_cost_weight;
+  csm_ceres_options2d ceres;                 /* ceres_scan_matcher */
+  csm_range_inserter_options2d inserter;     /* submaps.range_data_inserter */
+} csm_local_slam_options2d;
+typedef struct csm_local_slam2d csm_local_slam2d;
+csm_status csm_local_slam2d_create(const csm_local_slam_options2d* options, int32_t device,
+                                   csm_local_slam2d** out);
+csm_status csm_local_slam2d_destroy(csm_local_slam2d* handle);
+/* AddRangeData's per-point loop (:163-186) on one synchronized scan: hit i (hits, num_hits x
+ * {x, y, z}) and its origin origins[origin_index[i]] go through poses[pose_index[i]] (num_poses x
+ * {tx, ty, tz, qw, qx, qy, qz}, the Rigid3f range_data_poses the host extrapolated, with the
+ * backwards-time clamp applied); a hit at range >= min_range is a return if range <= max_range,
+ * else a miss at missing_data_ray_length along its ray.  Returns and misses are appended in input
+ * order to the accumulation, which the first call after a match starts afresh.  CSM_E_INVALID,
+ * with nothing changed, for a null pointer, an empty input, a non-finite point or pose, or an
+ * index out of range; CSM_E_CAPACITY, with nothing changed, when the grown accumulation does not
+ * fit the device.  No stream synchronisation (device_ms is not measured and reads 0).  The input
+ * is staged in one of two pinned buffers that alternate between calls: the call waits for the
+ * copy out of its buffer from two calls earlier (an event wait, normally long complete), and a
+ * staging buffer that has to grow is reallocated, which waits for the device. */
+csm_status csm_local_slam2d_accumulate(csm_local_slam2d* handle, const float* hits,
+                                       int32_t num_hits, const float* origins,
+                                       int32_t num_origins, const int32_t* origin_index,
+                                       const float* poses, int32_t num_poses,
+                                       const int32_t* pose_index, csm_stats* stats /* may be NULL */);
+enum {
+  CSM_LOCAL_SLAM_MATCHED = 0,
+  CSM_LOCAL_SLAM_DROPPED_EMPTY_RETURNS = 1,    /* :217-220, no return in [min_z, max_z] */
+  CSM_LOCAL_SLAM_DROPPED_EMPTY_FILTERED = 2    /* :231-233 */
+};
+typedef struct csm_local_slam_match2d {
+  int32_t status;             /* CSM_LOCAL_SLAM_* */
+  int32_t matched_submap;     /* 1 when a grid was given: the pose is the scan matchers' */
+  int32_t num_returns;        /* the voxel-filtered gravity-aligned range data */
+  int32_t num_misses;
+  int32_t num_filtered;       /* the adaptively filtered point cloud */
+  int32_t reserved;
+  double pose_estimate[3];    /* the 2D pose {x, y, angle} (the prediction without a grid) */
+  double rt_score;            /* the real-time matcher's score, 0 when it did not run */
+  csm_ceres_result2d ceres;   /* the refinement's summary, zero when it did not run */
+} csm_local_slam_match2d;
+/* TransformToGravityAlignedFrameAndFilter (:51-63) of the accumulation through to_gravity
+ * (gravity_alignment.cast<float>() * range_data_poses.back().inverse(), {t, q wxyz}), then
+ * AddAccumulatedRangeData up to the pose (:211-244): the adaptive voxel filter and ScanMatch
+ * against `grid` (the front active submap's ProbabilityGrid; NULL when there is none) with the
+ * prediction pose_prediction.  origin is the accumulated origin (range_data_poses.back()
+ * .translation()).  The call ends the accumulation.  A dropped scan is not an error and leaves
+ * every grid untouched.  CSM_E_INVALID, with nothing changed, for a null pointer, a non-finite
+ * pose or origin, nothing accumulated, a TSDF2D grid or a grid on another device.  Stream
+ * synchronisations: one when the cropped returns are empty, two when the filtered cloud is empty
+ * or there is no grid, three with a grid, four with the online matcher. */
+csm_status csm_local_slam2d_match(csm_local_slam2d* handle, const float to_gravity[7],
+                                  const float origin[3], const double pose_prediction[3],
+                                  const csm_rt_grid2d* grid, csm_local_slam_match2d* result,
+                                  csm_stats* stats /* may be NULL */);
+/* InsertIntoSubmap's insert (:245-252, 279-300) of the last matched scan: TransformRangeData of
+ * its voxel-filtered gravity-aligned range data through pose (Embed3D(pose_estimate_2d
+ * .cast<float>()), {t, q wxyz}) into the local frame, then what csm_range_inserter2d_insert_submaps
+ * does with it on `grids` (the active submaps), without an upload.  local_origin (may be NULL)
+ * receives range_data_in_local.origin.  CSM_E_INVALID, with every handle unchanged, for what
+ * csm_range_inserter2d_insert_submaps refuses, a non-finite pose, or no matched scan since the
+ * last insert.  Two stream synchronisations (the local range data's box and ray lengths, which
+ * decide the grids' growth, then the insert). */
+csm_status csm_local_slam2d_insert(csm_local_slam2d* handle, const float pose[7],
+                                   csm_rt_grid2d* const* grids, int32_t num_grids,
+                                   float local_origin[3], csm_stats* stats /* may be NULL */);
+/* Read-back hooks: the points of one stage of the current scan (n x {x, y, z}).  *count gets
+ * their number; with xyz != NULL they are copied (CSM_E_CAPACITY below it).  The filtered cloud is
+ * the host copy the match made (no synchronisation); the others take one. */
+enum {
+  CSM_LOCAL_SLAM_ACCUMULATED_RETURNS = 0,
+  CSM_LOCAL_SLAM_ACCUMULATED_MISSES = 1,
+  CSM_LOCAL_SLAM_CROPPED_RETURNS = 2,   /* gravity-aligned and cropped */
+  CSM_LOCAL_SLAM_CROPPED_MISSES = 3,
+  CSM_LOCAL_SLAM_FILTERED_RETURNS = 4,  /* + VoxelFilter: the gravity-aligned range data */
+  CSM_LOCAL_SLAM_FILTERED_MISSES = 5,
+  CSM_LOCAL_SLAM_FILTERED = 6,          /* AdaptiveVoxelFilter of the returns */
+  CSM_LOCAL_SLAM_LOCAL_RETURNS = 7,     /* range_data_in_local, after an insert */
+  CSM_LOCAL_SLAM_LOCAL_MISSES = 8
+};
+csm_status csm_local_slam2d_read(const csm_local_slam2d* handle, int32_t which, float* xyz,
+                                 int64_t capacity, int32_t* count);
+
 #ifdef __cplusplus
 }
 #endif
