@@ -472,6 +472,7 @@ csm_status csm_local_slam2d_match(csm_local_slam2d* h, const float to_gravity[7]
   h->n_crop_r = n_r;
   h->n_crop_m = n_m;
   h->n_vf_r = h->n_vf_m = h->n_filtered = 0;
+  h->h_filtered.clear();
   const Vec3f go = Rigid3Apply(T, Vec3f{origin[0], origin[1], origin[2]});
   h->ga_origin[0] = go.x;
   h->ga_origin[1] = go.y;
@@ -481,11 +482,6 @@ csm_status csm_local_slam2d_match(csm_local_slam2d* h, const float to_gravity[7]
     if (stats) *stats = st;
     return CSM_OK;
   };
-  if (n_r == 0) {   // :217-220
-    r.status = CSM_LOCAL_SLAM_DROPPED_EMPTY_RETURNS;
-    return finish();
-  }
-
   // ---- 2: VoxelFilter of both clouds, AdaptiveVoxelFilter of the filtered returns ----
   const int n = n_r + n_m;
   CSM_TRY(h->scan.Reserve(sizeof(float3) * n));
@@ -499,7 +495,11 @@ csm_status csm_local_slam2d_match(csm_local_slam2d* h, const float to_gravity[7]
   if (n_m > 0)
     CSM_CUDA(cudaMemcpyAsync(cropped + n_r, ga + bound, sizeof(float3) * n_m,
                              cudaMemcpyDeviceToDevice, s));
-  h->cropped_ready = true;
+  h->cropped_ready = true;   // a dropped scan's cropped misses stay readable too
+  if (n_r == 0) {   // :217-220
+    r.status = CSM_LOCAL_SLAM_DROPPED_EMPTY_RETURNS;
+    return finish();
+  }
   const float vs[2] = {h->o.voxel_filter_size, h->o.voxel_filter_size};
   VoxelFilterDeviceOut vf_out, avf_out;
   CSM_TRY(VoxelFilterEnqueue(ctx, "local_slam_vf", nullptr, reinterpret_cast<const float*>(cropped),
@@ -665,7 +665,7 @@ csm_status csm_local_slam2d_read(const csm_local_slam2d* h, int32_t which, float
     *count = h->n_filtered;
     CSM_REQUIRE(xyz || h->n_filtered == 0 || capacity == 0, "null xyz");
     if (xyz && capacity >= h->n_filtered) {
-      std::memcpy(xyz, h->h_filtered.data(), sizeof(float) * h->h_filtered.size());
+      std::memcpy(xyz, h->h_filtered.data(), sizeof(float) * 3 * h->n_filtered);
       return CSM_OK;
     }
     if (xyz) {
